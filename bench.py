@@ -15,8 +15,8 @@ three refinement iterations (6 views, 32^3 volume) -- BASELINE.json's full-estim
 
 N > 1 (torchrun): one process per GPU, each rank runs an independent replica on its own frames
 (weak scaling, no data-path collective; poses are all-gathered once at the end over NCCL).
-`--impl reference` times the CPU oracle port instead (the reference itself cannot travel to the
-GPU box: /root/reference does not exist there).
+`--impl reference` times the CPU oracle port instead (a torch-CPU restatement of the reference path).
+`--dump-outputs DIR` writes what the device-resident path returned for its last timed batch as DIR/<name>.npy.
 """
 import argparse
 import json
@@ -38,34 +38,22 @@ E2E_MAX_BATCH = 10
 
 
 def pick_batch(steps, workers):
-    """Frames per batched stage for a timed region of `steps` poses on `workers` lanes: the largest batch <= 10 that
-    deals every lane the same number of full batches (steps 20, 2 lanes -> 10; a ragged tail would leave one lane
-    idle for a whole batch), 4 when nothing divides.  Measured on B200 at 20 steps (2 lanes): batch 4 -> 164 poses/s
-    device-resident / 123-135 end to end, 5 -> 172 / 130, 10 -> 171-174 / 138-142; 1 lane x 20 -> 162 / 139;
-    4 lanes x 5 -> 171 / 135."""
+    """Frames per batched stage for a timed region of exactly `steps` poses on `workers` lanes; always a divisor of
+    `steps`, so the timed batches hold exactly `steps` poses.  Preferred: the largest batch <= 10 that deals every lane
+    the same number of full batches (steps 20, 2 lanes -> 10; a ragged tail would leave one lane idle for a whole
+    batch) if it is at least 4 or the whole per-lane share; otherwise the largest divisor of `steps` <= 10, the lanes
+    then running unequal numbers of batches (22 steps -> 11 batches of 2)."""
     if E2E_BATCH > 0:
-        return E2E_BATCH
+        return E2E_BATCH                         # main() rejects a G6D_E2E_BATCH that does not divide --steps
     if steps % workers == 0:
         per_lane = steps // workers
         for b in range(min(E2E_MAX_BATCH, per_lane), 0, -1):
             if per_lane % b == 0 and (b >= 4 or b == per_lane):
                 return b
-    return 4 if steps >= 4 * workers else 1      # very short runs: frame by frame (no batch larger than the run)
+    return max(b for b in range(1, min(E2E_MAX_BATCH, steps) + 1) if steps % b == 0)
 METRIC = 'poses/sec end-to-end (128^2 crop, 64 refs, 3 refine iters)'
 WORKLOAD = ('full estimator detect->select->3x refine: synthetic 480x640 frame, detector 32 refs x 4 scales, '
             'selector 64 refs x 5 angles, refiner 6 views 32^3 volume, seeded random weights')
-
-
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the roofline kernels, from the committed
-    `ncu --set full` captures of this round (profiles/ncu_traffic.json, written by tools/ncu_summary.py)."""
-    path = os.path.join(ROOT, 'profiles', 'ncu_traffic.json')
-    if os.path.exists(path):
-        try:
-            return json.load(open(path))
-        except Exception:
-            pass
-    return {}
 
 
 def read_peaks():
@@ -73,7 +61,7 @@ def read_peaks():
     if os.path.exists(path):
         d = json.load(open(path))
         return {'hbm_gbs': d['hbm_gbs'], 'bf16_tflops': d.get('bf16_tflops_sustained', d['bf16_tflops']), 'src': 'measured'}
-    return {'hbm_gbs': 6650.0, 'bf16_tflops': 1400.0, 'src': 'fallback'}
+    return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0, 'src': 'H100 SXM data-sheet (700 W)'}
 
 
 class ClockSampler:
@@ -126,7 +114,7 @@ def usable_cpus():
 def cpu_pose_fn(device='cpu'):
     """Returns (fn, describe): fn() runs ONE network-only pose of the oracle port (a functional torch
     restatement of the reference's three networks) on `device`: 'cpu' = the reference arm / cpu_baseline
-    on the host cores; 'cuda' = the same torch ops in eager mode on the B200 (cuDNN / cuBLAS fp32, TF32
+    on the host cores; 'cuda' = the same torch ops in eager mode on the GPU (cuDNN / cuBLAS fp32, TF32
     disabled) -- the same-box GPU comparison point BASELINE.md 4.6 asks for."""
     from gen6d_b200 import geometry as G
     from gen6d_b200 import synthetic as syn
@@ -172,7 +160,7 @@ def cpu_pose_fn(device='cpu'):
 
 
 def torch_cuda_baseline(steps=10, warm=3):
-    """PyTorch eager (cuDNN/cuBLAS fp32, allow_tf32 = False) on the same B200: the oracle port on CUDA
+    """PyTorch eager (cuDNN/cuBLAS fp32, allow_tf32 = False) on the same GPU: the oracle port on CUDA
     tensors, device-resident inputs, CUDA events.  A reported comparison point, not a target."""
     fn, info = cpu_pose_fn('cuda')
     for _ in range(warm):
@@ -334,6 +322,38 @@ def run_reference_arm(args, rank, world):
 
 
 # ---------------------------------------------------------------------------------------------
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, stage_outputs):
+    """Writes the outputs of the last timed batch (what the captured stages hand back to the estimator) as
+    out_dir/<stage>_<i>.npy (<stage>.<k>_<i> for the k-th repeat of a stage within the batch), float64 where the
+    stage returns float64, float32 otherwise; outputs that are not arrays are skipped.  An array beyond its share of
+    DUMP_LIMIT_BYTES is replaced by a fixed seeded sample of its flattened elements."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays, seen = [], {}
+    for name, outs in stage_outputs:
+        k = seen[name] = seen.get(name, -1) + 1
+        stem = name if k == 0 else f'{name}.{k}'
+        outs = outs if isinstance(outs, (tuple, list)) else (outs,)
+        for i, t in enumerate(outs):
+            if isinstance(t, torch.Tensor):
+                a = t.detach().cpu().numpy()
+            elif isinstance(t, np.ndarray):
+                a = t
+            else:
+                continue
+            if a.dtype.kind not in 'biuf':
+                continue
+            arrays.append((f'{stem}_{i}', a.astype(np.float64 if a.dtype == np.float64 else np.float32)))
+    share = DUMP_LIMIT_BYTES // max(len(arrays), 1)
+    for name, a in arrays:
+        if a.nbytes > share:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, share // a.itemsize, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + '.npy'), a)
+
+
 def run_ours(args, rank, world, local_rank):
     from gen6d_b200 import _lib, graphs, ops
     from gen6d_b200 import geometry as G
@@ -389,22 +409,25 @@ def run_ours(args, rank, world, local_rank):
     det, sel, rfr = est.detector, est.selector, est.refiner
 
     def device_batch(i=0, eager=False):
-        """One batch of Bt poses on lane i through the captured stage graphs (eager=True: kernel by kernel)."""
+        """One batch of Bt poses on lane i through the captured stage graphs (eager=True: kernel by kernel).
+        Returns [(stage name, outputs)] of the batch's stages."""
+        outs = []
         with torch.no_grad():
             for m, name, fn, inputs in recs[0 if eager else i % W]:
-                if eager:
-                    fn(*inputs)
-                else:
-                    m.stages.run(name, fn, inputs)
+                outs.append((name, fn(*inputs) if eager else m.stages.run(name, fn, inputs)))
+        return outs
+
+    last_outputs = []
 
     def device_steps(n):
-        """n poses = ceil(n / Bt) batches dealt round-robin to the lanes (a short last batch runs full)."""
+        """Exactly n poses = n / Bt batches dealt round-robin to the lanes."""
+        assert n % Bt == 0, f'{n} poses are not whole batches of {Bt}'
         main = torch.cuda.current_stream()
         for st in lanes:
             st.wait_stream(main)
         for i in range((n + Bt - 1) // Bt):
             with torch.cuda.stream(lanes[i % W]):
-                device_batch(i)
+                last_outputs[:] = device_batch(i)
         for st in lanes:
             main.wait_stream(st)
 
@@ -446,7 +469,9 @@ def run_ours(args, rank, world, local_rank):
     if rank == 0:
         sampler.start()
     note('stage graphs recorded')
-    dev_ms, _, launches = timed(device_steps, args.steps, max(args.warmup, 2 * W * Bt), batched=True)
+    dev_ms, _, launches = timed(device_steps, args.steps, Bt * -(-max(args.warmup, 2 * W * Bt) // Bt), batched=True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_outputs)
 
     note('device-resident timing done')
     # ---- end to end through the public API (numpy in, numpy out)
@@ -507,14 +532,10 @@ def run_ours(args, rank, world, local_rank):
     ffma = stats.get('g6d_conv', {'ms': 0, 'work': 0, 'n': 0})
     f16 = ops.conv_kind() == _lib.TC_F16
     split = 3.0 if f16 else 6.0             # bf16-peak units per fp32-equivalent flop: 3 fp16 MMAs, or 3 TF32 MMAs at half rate
-    traffic = ncu_traffic()
-    roof = {'kernel': 'conv_tc2_kernel / conv_tcflat_kernel (tcgen05 implicit-GEMM convolution, fp32-faithful 3-term operand split, '
-                      + ('fp16 hi + 2^11-scaled fp16 lo halves, kind::f16' if f16 else 'tf32 hi/lo halves, kind::tf32') + ')',
+    roof = {'kernel': 'conv_tc2_kernel / conv_tcflat_kernel (wgmma implicit-GEMM convolution, fp32-faithful 3-term operand split, '
+                      + ('fp16 hi + 2^11-scaled fp16 lo halves, f16 wgmma' if f16 else 'tf32 hi/lo halves, tf32 wgmma') + ')',
             'bound': 'tensor', 'achieved': conv['work'] / max(conv['ms'], 1e-9) / 1e9, 'peak': peaks['bf16_tflops'], 'unit': 'TFLOP/s',
-            'traffic': traffic.get('conv'),
-            'traffic_of': 'DRAM bytes of ONE launch of the 3x3 512->512 layer on a 120x160 map (tools/conv_one.py, ncu --set full): '
-                          'its 4.2 GB of operand reads are served from L2; activations + weights come from HBM once',
-            'peak_source': f"{peaks['src']} bf16 dense GEMM (sustained); achieved counts fp32-equivalent flops 2MNK, each issued as 3 "
+            'peak_source': f"{peaks['src']} bf16 dense GEMM" + (' (sustained)' if peaks['src'] == 'measured' else ' (not reached at a lower power limit)') + "; achieved counts fp32-equivalent flops 2MNK, each issued as 3 "
                            + ('fp16' if f16 else 'TF32') + f" MMAs, so 1/{split:g} of this peak is the ceiling of the parity mode",
             'launches_per_step': conv['n'] / Bt, 'ms_per_step': conv['ms'] / Bt,
             'share_of_step': conv['ms'] / max(eager_ms, 1e-9),
@@ -535,10 +556,7 @@ def run_ours(args, rank, world, local_rank):
             extra.append({'kernel': label, 'bound': 'hbm', 'achieved': ach, 'peak': peaks['hbm_gbs'], 'unit': 'GB/s',
                           'frac': ach / peaks['hbm_gbs'], 'us_per_launch': s['ms'] / s['n'] * 1e3,
                           'units_per_launch': units, 'unit_is': 'one query' if units == 1 else 'one pose-iteration (the batched refine stage fills all volumes of the batch in one launch)',
-                          'algorithmic_bytes_per_unit': s['work'] / s['n'] / units,
-                          'traffic': traffic.get('s2' if 'score3' in key else 'r2'),
-                          'traffic_of': 'dram__bytes_read.sum + dram__bytes_write.sum of one launch with ONE unit (ncu --set full on tools/profile_step.py)'
-                                        + ('' if units == 1 else '; the 50 MB the kernel writes per unit stay in L2 for the embed convolutions that read them next')})
+                          'algorithmic_bytes_per_unit': s['work'] / s['n'] / units})
     note('kernel timing done')
     accuracy = add_accuracy(est, db) if rank == 0 else None
     note('accuracy done')
@@ -552,9 +570,9 @@ def run_ours(args, rank, world, local_rank):
             'warmup': args.warmup, 'ms_per_step': dev_ms / args.steps, 'higher_is_better': True, 'scaling': 'weak',
             'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
             'config': {'workload': WORKLOAD, 'parallelism': f'replica x{world} (independent frames per GPU); per GPU {E2E_WORKERS} lanes (streams) x batches of '
-                                                            f'{Bt} frames through the batched stages = {E2E_WORKERS * Bt} frames in flight' + ('; camera algebra between the stages on the device, one captured graph per batch' if est.cfg['device_glue'] else '; stages sequenced by the host'),
+                                                            f'{Bt} frames through the batched stages = {min(E2E_WORKERS, args.steps // Bt) * Bt} frames in flight' + ('; camera algebra between the stages on the device, one captured graph per batch' if est.cfg['device_glue'] else '; stages sequenced by the host'),
                        'l2': 'per-step working set (220 MB selector reference stack + 300 MB weights + detector '
-                             'activations) exceeds the 126 MB L2; no explicit flush'},
+                             'activations) exceeds the 50 MB L2; no explicit flush'},
             'e2e': {'value': world * args.steps / (pipe_ms * 1e-3), 'unit': 'poses/s', 'ms_per_step': pipe_ms / args.steps,
                     'h2d_bytes_per_step': io['h2d'] // n_calls, 'd2h_bytes_per_step': io['d2h'] // n_calls,
                     'api': f'Gen6DEstimator.predict_many(numpy frames, Ks, workers={E2E_WORKERS}, batch={Bt}) -> numpy poses: {E2E_WORKERS} host threads '
@@ -591,6 +609,8 @@ def main():
     ap.add_argument('--steps', type=int, default=None)
     ap.add_argument('--warmup', type=int, default=None)
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference', 'torch-cuda'])
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed batch of the device-resident path as DIR/<name>.npy')
     args = ap.parse_args()
     rank, world = int(os.environ.get('RANK', 0)), int(os.environ.get('WORLD_SIZE', 1))
     local_rank = int(os.environ.get('LOCAL_RANK', 0))
@@ -606,6 +626,10 @@ def main():
         return
     args.steps = 20 if args.steps is None else args.steps
     args.warmup = 3 if args.warmup is None else max(3, args.warmup)
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
+    if E2E_BATCH > 0 and args.steps % E2E_BATCH:
+        ap.error(f'G6D_E2E_BATCH={E2E_BATCH} does not divide --steps {args.steps}: the timed region must be whole batches')
     run_ours(args, rank, world, local_rank)
     if world > 1:
         import torch.distributed as dist

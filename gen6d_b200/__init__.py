@@ -1,4 +1,4 @@
-"""gen6d_b200 -- B200-native (sm_100a) implementation of the Gen6D inference hot path.
+"""gen6d_b200 -- H100-native (sm_90a) implementation of the Gen6D inference hot path.
 
 Host side: Python classes that mirror the reference's `network.{detector,selector,refiner}` and
 `estimator.Gen6DEstimator` interfaces (same names, arguments, checkpoint format).

@@ -78,7 +78,7 @@ _SIGNATURES = {
     'g6d_pack_conv_weight': [P, P, I, I, I, I, P, P],
     'g6d_conv_tc_supported': [C.POINTER(ConvDesc), I],
     'g6d_conv_tc_debug': [C.POINTER(C.c_int)],
-    'g6d_debug_umma_shift': [P, I, I, P],
+    'g6d_debug_desc_shift': [P, I, I, P],
     'g6d_conv_tc_workspace_bytes': [C.POINTER(ConvDesc), I],
     'g6d_conv_tc': [C.POINTER(ConvDesc), P, P, P, I, I, P, P, P, P, P, P, L, P],
     'g6d_conv_tc_stats_supported': [C.POINTER(ConvDesc), I, L],

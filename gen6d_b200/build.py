@@ -1,4 +1,4 @@
-"""Builds libgen6d_b200.so in-tree with nvcc for sm_100a (no JIT cache, so the .so travels with
+"""Builds libgen6d_b200.so in-tree with nvcc for sm_90a (H100) (no JIT cache, so the .so travels with
 the repo snapshot to the GPU box).  `python -m gen6d_b200.build [--force] [-v]`"""
 import hashlib
 import os
@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libgen6d_b200.so')
 STAMP = os.path.join(HERE, '.libgen6d_b200.hash')
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC']
 NO_FMA = ('glue.cu',)
 
@@ -53,7 +53,7 @@ def build(force=False, verbose=False):
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError('nvcc failed building libgen6d_b200.so')
-    cmd = [nvcc, '-shared', '-o', LIB] + objs + ['-lcudart']
+    cmd = [nvcc, '-shared', NVCC_FLAGS[0], NVCC_FLAGS[1], '-o', LIB] + objs + ['-lcudart']
     subprocess.run(cmd, check=True)
     with open(STAMP, 'w') as f:
         f.write(dig)

@@ -1,4 +1,4 @@
-// Shared helpers for libgen6d_b200.so (sm_100a).
+// Shared helpers for libgen6d_b200.so (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -33,7 +33,7 @@ inline cudaStream_t as_stream(g6d_stream_t s) { return reinterpret_cast<cudaStre
         }                                 \
     } while (0)
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

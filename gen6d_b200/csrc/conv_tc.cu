@@ -1,17 +1,17 @@
-// Implicit-GEMM convolution on the 5th-generation tensor cores (tcgen05), fp32-faithful through a
+// Implicit-GEMM convolution on the Hopper tensor cores (wgmma, sm_90a), fp32-faithful through a
 // three-term operand split:  A*B ~= A_hi*B_hi + A_hi*B_lo + A_lo*B_hi, x_hi = round(x) to an 11-bit
 // significand, x_lo = x - x_hi (exact in fp32).  The dropped A_lo*B_lo term is O(2^-22) relative, so
 // index selections (detection cell, viewpoint) stay bit-exact against the fp32 reference while the
 // contraction runs on the tensor pipe instead of the FFMA pipe.  Two operand kinds share every kernel:
 //
-//   G6D_TC_TF32  hi/lo are tf32 (fp32 containers, 8-bit exponent): any fp32 range, kind::tf32 MMAs
+//   G6D_TC_TF32  hi/lo are tf32 (fp32 containers, 8-bit exponent): any fp32 range, tf32 wgmmas
 //                (K = 8 per instruction, 32 K-elements per 128-byte swizzle row);
 //   G6D_TC_F16   hi = fp16(x), lo = fp16((x - hi) * 2^11): the same 11 + 11 significand bits, but
-//                kind::f16 MMAs issue K = 16 per instruction at the same cycle cost and every operand
+//                f16 wgmmas issue K = 16 per instruction at twice the tf32 rate and every operand
 //                byte (shared-memory tile, TMA weight stream, operand re-read) carries twice the K:
 //                2x the tensor ceiling and half the shared-memory traffic per flop.  The lo halves are
 //                pre-scaled by 2^11 so that they live in the same exponent range as the hi halves (no
-//                fp16 subnormals); both cross terms accumulate in their own TMEM accumulator, which the
+//                fp16 subnormals); both cross terms accumulate in their own accumulator, which the
 //                epilogue folds in with an exact 2^-11.  Range contract: |x| <= 65504 for activations
 //                and weights (saturating conversion beyond that), full relative accuracy for |x| >=
 //                6.1e-5, absolute error <= ~2^-36 below.  Inside this network every tensor-core operand
@@ -19,22 +19,18 @@
 //                VGG feature, all O(1e-3 .. 1e3).  G6D_CONV_KIND=tf32 selects the wide-range kind.
 //
 // GEMM view (same as conv_ffma.cu): M = B*Do*Ho*Wo, N = Cout, K = taps*Cin, channels-last.
-// One CTA computes 128 x BLOCK_N output tiles (UMMA M=128, cta_group::1, accumulators in TMEM).
-//
-// conv_tc2_kernel (general strides / shapes): persistent, one CTA per SM loops over (M tile, N tile,
-// K split) work items.  14 warps:
+// One CTA computes 64 x BLOCK_N output tiles (wgmma M = 64, accumulators in registers).  12 warps:
 //   warps 0-7   A producers: gather the im2col rows of the K-block from global memory (coalesced
 //               128-bit loads, register prefetch ring), apply the folded InstanceNorm(+ReLU) /
 //               selector q(.)ref prologue to in-bounds elements, split into hi/lo and st.shared both
-//               tiles in the canonical K-major SWIZZLE_128B layout the UMMA descriptor expects;
-//   warp 8      B producer: one lane issues TMA (cp.async.bulk.tensor.2d, 128B swizzle) loads of the
-//               pre-split weight tiles W_hi / W_lo [Cout, K] (K-major) + an L2 prefetch running ahead;
-//   warp 9      MMA issuer (+ TMEM owner): 12 tcgen05.mma per K-block (4 K-steps x 3 split terms);
-//               tcgen05.commit releases the stage; two TMEM accumulator buffers so that
-//   warps 10-13 the epilogue (tcgen05.ld -> bias/activation -> global, or split-K partials) of tile i
-//               overlaps the MMAs of tile i+1.
-// conv_tcflat_kernel (stride-1 multi-tap convolutions whose halo fits in shared memory): A-operand
-// reuse across taps, see below.
+//               tiles in the canonical K-major SWIZZLE_128B layout the wgmma descriptor expects;
+//   warps 8-11  the consumer warpgroup: 12 wgmmas per K-block (4 K-steps x 3 split terms), one
+//               group in flight while the next stage is awaited, then the epilogue (bias / activation
+//               -> global, or split-K partials) straight from the accumulator registers.  Its first
+//               thread also streams the pre-split weight tiles W_hi / W_lo [Cout, K] (K-major) by TMA
+//               (cp.async.bulk.tensor.2d, 128B swizzle) into the stages it frees.
+// conv_tc2_kernel handles general strides / shapes (persistent); conv_tcflat_kernel (stride-1
+// multi-tap convolutions whose halo fits in shared memory) reuses the A operand across taps, see below.
 #include <stdlib.h>
 #include <string.h>
 
@@ -44,9 +40,10 @@
 
 namespace g6d {
 
-constexpr int TC_BM = 128;       // rows per tile (UMMA M)
+constexpr int TC_BM = 64;                                  // rows per tile (wgmma M)
 constexpr int TC_PRODUCER_WARPS = 8;
-constexpr int TC_THREADS = (TC_PRODUCER_WARPS + 2) * 32;   // flat kernel: producers double as epilogue
+constexpr int TC_THREADS = (TC_PRODUCER_WARPS + 4) * 32;   // producers + one consumer warpgroup
+constexpr int TC_ISSUER = TC_PRODUCER_WARPS * 32;          // consumer thread that also issues the weight TMA
 constexpr int TC_MAX_K_PER_CHAIN = 2048;                   // longest accumulate chain per CTA (see fill_tc_params)
 
 template <int KIND> struct KindCfg;
@@ -134,85 +131,112 @@ __device__ __forceinline__ float4 affine4(float4 x, const float4 sc, const float
 }
 
 // ------------------------------------------------------------------------------------------ MMA
-// cute::UMMA::InstrDescriptor, fp32 accumulate, both operands K-major: c_format F32 (1) at [4,6);
-// a_format / b_format at [7,10) / [10,13): TF32 = 2 for kind::tf32, F16 = 0 for kind::f16;
-// n_dim = N>>3 at [17,23); m_dim = M>>4 at [24,29).
-template <int KIND>
-__device__ __forceinline__ uint32_t umma_idesc(int M, int N) {
-    constexpr uint32_t fmt = KIND == G6D_TC_TF32 ? 2u : 0u;
-    return (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-template <int KIND>
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    if constexpr (KIND == G6D_TC_TF32) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-            ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-    } else {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-            ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-    }
-}
-__device__ __forceinline__ bool elect_one_sync() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-#define G6D_TMEM_LD16(r, taddr)                                                                                       \
-    asm volatile(                                                                                                     \
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"      \
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),             \
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])        \
-        : "r"(taddr))
+// One consumer warpgroup owns a 64 x BN output tile with every accumulator in registers: NMAIN
+// round-robin chains for the main (hi*hi) term and one for the two cross terms, BN / 2 registers each
+// (128 per thread for every BN).  Each tensor-core accumulate truncates to fp32; spreading the K-blocks
+// over several shorter, smaller-magnitude chains (summed in fp32 round-to-nearest by the epilogue)
+// divides the resulting bias on same-sign data by ~NMAIN at no cost.
+template <int BN> struct AccCfg {
+    static constexpr int NMAIN = BN == 32 ? 7 : (BN == 64 ? 3 : 1);
+    static constexpr int R = BN / 2;
+};
 
-// Fused InstanceNorm statistics of the convolution's OUTPUT (the reference normalises the raw conv
-// result and the next layer's loader applies it): each epilogue warp holds 32 output rows x 16 channels
-// of final values; a transposing butterfly (8+4+2+1+1 shuffles per quantity) leaves the 32-row sums of
-// channel (lane >> 1) in lanes 2c / 2c+1; even lanes add sum(y), odd lanes sum(y^2) to the per
-// (group, channel) fp64 accumulators the separate in_stats_partial pass used to produce.  All 32 rows of
-// a warp belong to one group (the host only enables this when stats_rows % 32 == 0 / whole planes).
-__device__ __forceinline__ void epilogue_stats(float (&v)[16], bool row_valid, double* __restrict__ ws, long long group,
-                                               int Cout, int n0, int lane) {
-    float q[16];
+// The 4 K steps x 3 split terms of one stage into the main accumulator `main` and the cross accumulator,
+// committed as one wgmma group; first_* start a chain.  The callers unroll their K-block loop by NMAIN so
+// that `main` is a compile-time register array (a runtime choice makes ptxas serialize the wgmmas).
+template <int BN, int KIND>
+__device__ __forceinline__ void mma_stage(float (&main)[BN / 2], float (&cross)[BN / 2], uint32_t a_hi, uint32_t a_lo,
+                                          uint32_t b_hi, uint32_t b_lo, bool first_cross, bool first_main) {
+    const uint64_t dah = gmma_desc_sw128(a_hi), dal = gmma_desc_sw128(a_lo);
+    const uint64_t dbh = gmma_desc_sw128(b_hi), dbl = gmma_desc_sw128(b_lo);
+    wgmma_fence();
 #pragma unroll
-    for (int j = 0; j < 16; ++j) { v[j] = row_valid ? v[j] : 0.f; q[j] = v[j] * v[j]; }
+    for (int ks = 0; ks < 4; ++ks) {             // 4 x 32 bytes of K per 128-byte row
+        const uint64_t adv = (uint64_t)((ks * 32) >> 4);
+        wgmma<BN, KIND>(cross, dal + adv, dbh + adv, (!first_cross || ks > 0) ? 1u : 0u);
+        wgmma<BN, KIND>(cross, dah + adv, dbl + adv, 1u);
+        wgmma<BN, KIND>(main, dah + adv, dbh + adv, (!first_main || ks > 0) ? 1u : 0u);
+    }
+    wgmma_commit();
+}
+
+// Epilogue of one consumer thread: rows r and r + 8 of the tile (dst0 / dst1 point at column n_base of
+// their output row, nullptr for rows outside the output), columns 8 i + 2 (lane & 3) + {0, 1}.  Folds the
+// cross terms (smallest magnitude first, scaled back by the lo pre-scale) and the main chains, adds
+// bias + activation unless the output is a split-K partial, stores, and -- when stats is given --
+// adds the InstanceNorm moments of the stored values to the per (group, channel) fp64 accumulators
+// (the reference normalises the raw conv result and the next layer's loader applies it).  All 16 rows
+// of a warp belong to one group (the host only enables this for groups of whole 32-row slices / planes).
+template <int BN, int KIND>
+__device__ __forceinline__ void epilogue_tile(float (&acc)[AccCfg<BN>::NMAIN][BN / 2], float (&cross)[BN / 2], int n_acc,
+                                              float* dst0, float* dst1, int n_base, int Cout, const float* __restrict__ bias,
+                                              int act, bool partial, bool vec2, double* __restrict__ stats, long long group,
+                                              int lane) {
+    constexpr int NMAIN = AccCfg<BN>::NMAIN;
+    const int cq = 2 * (lane & 3);
 #pragma unroll
-    for (int half = 8, off = 16; half >= 1; half >>= 1, off >>= 1) {
-        const bool upper = (lane & off) != 0;
+    for (int j = 0; j < BN / 2; ++j) {
+        float v = cross[j] * KindCfg<KIND>::CROSS;
 #pragma unroll
-        for (int j = 0; j < half; ++j) {
-            const float sv = upper ? v[j] : v[j + half], kv = upper ? v[j + half] : v[j];
-            const float sq = upper ? q[j] : q[j + half], kq = upper ? q[j + half] : q[j];
-            v[j] = kv + __shfl_xor_sync(0xffffffffu, sv, off);
-            q[j] = kq + __shfl_xor_sync(0xffffffffu, sq, off);
+        for (int a = 0; a < NMAIN; ++a)
+            if (a < n_acc) v += acc[a][j];
+        cross[j] = v;
+    }
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+        const int c = 8 * i + cq, n = n_base + c;
+        float b0 = 0.f, b1 = 0.f;
+        if (!partial && bias) {
+            if (n < Cout) b0 = __ldg(bias + n);
+            if (n + 1 < Cout) b1 = __ldg(bias + n + 1);
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            float& x0 = cross[4 * i + 2 * h];
+            float& x1 = cross[4 * i + 2 * h + 1];
+            if (!partial) { x0 = tc_act(x0 + b0, act); x1 = tc_act(x1 + b1, act); }
+            float* dst = h ? dst1 : dst0;
+            if (dst) {
+                if (vec2 && n + 2 <= Cout) {
+                    *reinterpret_cast<float2*>(dst + c) = make_float2(x0, x1);
+                } else {
+                    if (n < Cout) dst[c] = x0;
+                    if (n + 1 < Cout) dst[c + 1] = x1;
+                }
+            }
         }
     }
-    const float s1 = v[0] + __shfl_xor_sync(0xffffffffu, v[0], 1);
-    const float s2 = q[0] + __shfl_xor_sync(0xffffffffu, q[0], 1);
-    const int n = n0 + (lane >> 1);
-    if (n < Cout) atomicAdd(ws + (group * Cout + n) * 2 + (lane & 1), (double)((lane & 1) ? s2 : s1));
+    if (!stats || partial) return;
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const float y0 = dst0 ? cross[4 * i + e] : 0.f, y1 = dst1 ? cross[4 * i + 2 + e] : 0.f;
+            float s1 = y0 + y1, s2 = y0 * y0 + y1 * y1;
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) {                // the 8 lanes that share this column
+                s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+                s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+            }
+            const int n = n_base + 8 * i + cq + e;
+            if (lane < 4 && n < Cout) {
+                atomicAdd(stats + (group * Cout + n) * 2, (double)s1);
+                atomicAdd(stats + (group * Cout + n) * 2 + 1, (double)s2);
+            }
+        }
+    }
 }
 
 // ==========================================================================================
 // conv_tc2_kernel: persistent implicit-GEMM convolution.
 //   * one CTA per SM loops over (M tile, N tile, K split) work items, so there is no wave tail and
-//     the per-CTA set-up (TMEM allocation, barrier init, descriptor prefetch) is paid once;
-//   * two TMEM accumulator buffers: the MMA warp starts the next tile while four dedicated
-//     epilogue warps drain the previous one (tmem_full / tmem_empty barriers);
-//   * the eight producer warps keep a register prefetch ring (global loads of the next K-block(s)
-//     in flight while K-block it is transformed and stored);
-//   * the smem ring never drains between tiles (one global K-block counter).
-// TMEM accumulators per buffer: NMAIN round-robin chains for the main (hi*hi) term + one for the
-// cross terms.  Each tensor-core accumulate truncates to fp32; spreading the K-blocks over several
-// shorter, smaller-magnitude chains (summed in fp32 round-to-nearest by the epilogue) divides the
-// resulting bias on same-sign data by ~NMAIN at no cost.
-// NPW producer warps + TMA + MMA + 4 epilogue warps.  NPW = 8 is what ships: 16 producer warps (2 tile
-// rows per thread, one more K-block of loads in flight) were measured 25-30 % SLOWER on the large layers
-// (704 threads cap the kernel at 80 registers: the deeper ring spills into the same L1 data pipe).
-constexpr int tc2_threads(int npw) { return (npw + 6) * 32; }
+//     the per-CTA set-up (barrier init, descriptor prefetch) is paid once;
+//   * eight producer warps keep a register prefetch ring (global loads of the next K-block(s) in
+//     flight while K-block it is transformed and stored) and never drain the smem ring between tiles
+//     (one global K-block counter), so they fill the next tile's stages during the epilogue;
+//   * one consumer warpgroup issues the wgmmas of a stage, keeps one stage's group in flight while it
+//     waits for the next, releases each stage once its group has completed and runs the epilogue;
+//   * one consumer thread streams the weight tiles by TMA, STAGES K-blocks ahead of the MMAs.
 constexpr int TC2_PF_BYTES = 12 * 128;      // weight-tile L2 prefetch distance, in bytes of K per row
 
 template <int BN> struct Tc2Cfg {
@@ -221,30 +245,26 @@ template <int BN> struct Tc2Cfg {
     static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
     static constexpr int STAGES = (208 * 1024) / STAGE_BYTES > 6 ? 6 : (208 * 1024) / STAGE_BYTES;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
-    static constexpr int NMAIN = BN == 32 ? 7 : (BN == 64 ? 3 : 1);      // per accumulator buffer
-    static constexpr int BUF_COLS = (NMAIN + 1) * BN;                     // 256
-    static constexpr int TMEM_COLS = 2 * BUF_COLS;                        // 512: two buffers
 };
 
 struct Tc2Work { int m_tiles, n_tiles, total; };
 
-template <int BN, int KIND, int NPW>
-__global__ void __launch_bounds__(tc2_threads(NPW), 1)  // 448 threads x 128 registers, or 704 x 80 (warps allocate registers in units of 512)
+template <int BN, int KIND>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUtensorMap map_hi,
                 const __grid_constant__ CUtensorMap map_lo) {
     using Cfg = Tc2Cfg<BN>;
     using KC = KindCfg<KIND>;
+    constexpr int NPW = TC_PRODUCER_WARPS;
     constexpr int STAGES = Cfg::STAGES;
-    constexpr int NMAIN = Cfg::NMAIN;
+    constexpr int NMAIN = AccCfg<BN>::NMAIN;
     constexpr int BK = KC::BK, NV = KC::NV;
-    constexpr int ROWS = 32 / NPW;                       // tile rows per producer thread (4 or 2)
     constexpr int RSTEP = NPW * 4;                       // rows r0 + RSTEP*j
+    constexpr int ROWS = TC_BM / RSTEP;                  // tile rows per producer thread
     constexpr int RING = KC::RING;                       // register prefetch ring (K-blocks); RING-1 in flight
-    constexpr int W_TMA = NPW, W_MMA = NPW + 1;          // warp roles; epilogue = the four warps after W_MMA
-    constexpr int PF = TC2_PF_BYTES / 128;     // K-blocks
+    constexpr int PF = TC2_PF_BYTES / 128;               // K-blocks
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
     const uint32_t bar_base = base + STAGES * Cfg::STAGE_BYTES;
     auto a_hi = [&](int s) { return base + s * Cfg::STAGE_BYTES; };
     auto a_lo = [&](int s) { return base + s * Cfg::STAGE_BYTES + Cfg::A_BYTES; };
@@ -253,31 +273,19 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
     auto full_a = [&](int s) { return bar_base + 8 * s; };
     auto full_b = [&](int s) { return bar_base + 8 * (STAGES + s); };
     auto empty = [&](int s) { return bar_base + 8 * (2 * STAGES + s); };
-    auto tmem_full = [&](int b) { return bar_base + 8 * (3 * STAGES + b); };
-    auto tmem_empty = [&](int b) { return bar_base + 8 * (3 * STAGES + 2 + b); };
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(base_ptr + STAGES * Cfg::STAGE_BYTES + 8 * (3 * STAGES + 4));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (warp == W_TMA && lane == 0) {
+    if (threadIdx.x == TC_ISSUER) {
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(full_a(s), NPW);        // the producer warps
-            mbar_init(full_b(s), 1);
-            mbar_init(empty(s), 1);
+            mbar_init(full_b(s), 1);          // the TMA transaction
+            mbar_init(empty(s), 4);           // the consumer warps
         }
-        for (int b = 0; b < 2; ++b) { mbar_init(tmem_full(b), 1); mbar_init(tmem_empty(b), 4); }
         fence_barrier_init();
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_lo) : "memory");
     }
-    if (warp == W_MMA) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     ::"r"(smem_u32((const void*)tmem_slot)), "n"(Cfg::TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_acc = *tmem_slot;
 
     // work item -> (m tile, n tile, split); n fastest so neighbouring CTAs share the gathered A rows in L2
     auto decode = [&](int w, int& mt, int& nt, int& sp) {
@@ -285,6 +293,7 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
         mt = w % wk.m_tiles;
         sp = w / wk.m_tiles;
     };
+    auto kblocks_of = [&](int sp) { return min(p.kblocks, sp * p.kb_per_split + p.kb_per_split) - sp * p.kb_per_split; };
 
     if (warp < NPW) {
         // =============================== A producers ===============================
@@ -298,7 +307,7 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
             decode(w, mt, nt, sp);
             const int m_base = mt * TC_BM;
             const int kb_begin = sp * p.kb_per_split;
-            const int nkb = min(p.kblocks, kb_begin + p.kb_per_split) - kb_begin;
+            const int nkb = kblocks_of(sp);
             int rb[ROWS], rsp[ROWS], rc[ROWS];
             unsigned rvmask = 0;
             const long long plane_sz = (long long)p.D * p.H * p.W;
@@ -396,173 +405,89 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
             }
             git += nkb;
         }
-    } else if (warp == W_TMA) {
-        // =============================== B producer (TMA) ===============================
-        if (lane == 0) {
-            int git = 0;
-            for (int w = blockIdx.x; w < wk.total; w += gridDim.x) {
-                int mt, nt, sp;
-                decode(w, mt, nt, sp);
-                const int kb_begin = sp * p.kb_per_split;
-                const int nkb = min(p.kblocks, kb_begin + p.kb_per_split) - kb_begin;
-                // The weight tiles of a small-M layer are touched once and come from HBM: with only
-                // STAGES tiles in flight the ring is latency-bound (measured 5000 cycles per K-block
-                // at M = 660).  An L2 prefetch running PF K-blocks ahead costs no shared memory.
-                for (int it = 0; it < min(nkb, PF); ++it) {
-                    tma_prefetch_2d(&map_hi, (kb_begin + it) * BK, nt * BN);
-                    tma_prefetch_2d(&map_lo, (kb_begin + it) * BK, nt * BN);
-                }
-                for (int it = 0; it < nkb; ++it, ++git) {
-                    const int s = git % STAGES;
-                    if (it + PF < nkb) {
-                        tma_prefetch_2d(&map_hi, (kb_begin + it + PF) * BK, nt * BN);
-                        tma_prefetch_2d(&map_lo, (kb_begin + it + PF) * BK, nt * BN);
-                    }
-                    mbar_wait(empty(s), ((git / STAGES) & 1) ^ 1, 3, git);
-                    mbar_expect_tx(full_b(s), 2 * Cfg::B_BYTES);
-                    const int k = (kb_begin + it) * BK;
-                    tma_load_2d(b_hi(s), &map_hi, full_b(s), k, nt * BN);
-                    tma_load_2d(b_lo(s), &map_lo, full_b(s), k, nt * BN);
-                }
-            }
-        }
-    } else if (warp == W_MMA) {
-        // =============================== MMA issuer ===============================
-        if (elect_one_sync()) {
-            const uint32_t idesc = umma_idesc<KIND>(TC_BM, BN);
-            int git = 0, tile = 0;
-            for (int w = blockIdx.x; w < wk.total; w += gridDim.x, ++tile) {
-                int mt, nt, sp;
-                decode(w, mt, nt, sp);
-                const int kb_begin = sp * p.kb_per_split;
-                const int nkb = min(p.kblocks, kb_begin + p.kb_per_split) - kb_begin;
-                const int buf = tile & 1;
-                mbar_wait(tmem_empty(buf), ((tile >> 1) & 1) ^ 1, 6, tile);     // epilogue has drained this buffer
-                tc_fence_after();
-                const uint32_t acc0 = tmem_acc + (uint32_t)(buf * Cfg::BUF_COLS);
-                for (int it = 0; it < nkb; ++it, ++git) {
-                    const int s = git % STAGES;
-                    mbar_wait(full_a(s), (git / STAGES) & 1, 4, git);
-                    mbar_wait(full_b(s), (git / STAGES) & 1, 5, git);
-                    tc_fence_after();
-                    const uint64_t dah = umma_desc_sw128(a_hi(s)), dal = umma_desc_sw128(a_lo(s));
-                    const uint64_t dbh = umma_desc_sw128(b_hi(s)), dbl = umma_desc_sw128(b_lo(s));
-                    const uint32_t main_acc = acc0 + (uint32_t)((it % NMAIN) * BN);
-                    const uint32_t cross_acc = acc0 + (uint32_t)(NMAIN * BN);
-                    if constexpr (BN == 128 && NMAIN == 1) {
-                        // B_hi and B_lo sit back to back in the stage (a 256-row K-major tile) and the main and
-                        // cross accumulators back to back in TMEM: ONE N = 256 MMA forms A_hi * [B_hi | B_lo],
-                        // reading A_hi from shared memory once instead of twice (20 KB of operand reads per
-                        // K-step instead of 24; same 192 tensor cycles).  Then cross += A_lo * B_hi.
-                        const uint32_t idesc2 = umma_idesc<KIND>(TC_BM, 2 * BN);
-#pragma unroll
-                        for (int ks = 0; ks < 4; ++ks) {
-                            const uint64_t adv = (uint64_t)((ks * 32) >> 4);
-                            umma<KIND>(acc0, dah + adv, dbh + adv, idesc2, (it > 0 || ks > 0) ? 1u : 0u);
-                            umma<KIND>(cross_acc, dal + adv, dbh + adv, idesc, 1u);
-                        }
-                    } else {
-#pragma unroll
-                        for (int ks = 0; ks < 4; ++ks) {                 // 4 x 32 bytes of K per 128-byte row
-                            const uint64_t adv = (uint64_t)((ks * 32) >> 4);
-                            umma<KIND>(cross_acc, dal + adv, dbh + adv, idesc, (it > 0 || ks > 0) ? 1u : 0u);
-                            umma<KIND>(cross_acc, dah + adv, dbl + adv, idesc, 1u);
-                            umma<KIND>(main_acc, dah + adv, dbh + adv, idesc, (it >= NMAIN || ks > 0) ? 1u : 0u);
-                        }
-                    }
-                    umma_commit(empty(s));
-                }
-                umma_commit(tmem_full(buf));
-            }
-        }
     } else {
-        // =============================== epilogue (the 4 warps after the MMA warp) ===============================
-        const int quad = warp & 3;                     // TMEM lane quadrant = warp id % 4
-        int tile = 0;
-        for (int w = blockIdx.x; w < wk.total; w += gridDim.x, ++tile) {
+        // =============================== consumer warpgroup ===============================
+        const int cw = warp - NPW;                     // warp inside the warpgroup: rows 16 cw .. 16 cw + 15
+        const bool issuer = threadIdx.x == TC_ISSUER;
+        // weight-tile stream of the issuer: the next global K-block lg = K-block lit of work item lw
+        int lw = blockIdx.x, lit = 0, lg = 0;
+        auto load_next = [&]() {
+            int mt, nt, sp, nkb = 0;
+            for (; lw < wk.total; lw += gridDim.x, lit = 0) {
+                decode(lw, mt, nt, sp);
+                nkb = kblocks_of(sp);
+                if (lit < nkb) break;
+            }
+            if (lw >= wk.total) return;
+            const int kb_begin = sp * p.kb_per_split;
+            // The weight tiles of a small-M layer are touched once and come from HBM: with only STAGES
+            // tiles in flight the ring is latency-bound.  An L2 prefetch running PF K-blocks ahead costs
+            // no shared memory.
+            if (lit == 0) {
+                for (int i = 0; i < min(nkb, PF); ++i) {
+                    tma_prefetch_2d(&map_hi, (kb_begin + i) * BK, nt * BN);
+                    tma_prefetch_2d(&map_lo, (kb_begin + i) * BK, nt * BN);
+                }
+            } else if (lit + PF - 1 < nkb) {
+                tma_prefetch_2d(&map_hi, (kb_begin + lit + PF - 1) * BK, nt * BN);
+                tma_prefetch_2d(&map_lo, (kb_begin + lit + PF - 1) * BK, nt * BN);
+            }
+            const int s = lg % STAGES;
+            mbar_wait(empty(s), ((lg / STAGES) & 1) ^ 1, 3, lg);
+            mbar_expect_tx(full_b(s), 2 * Cfg::B_BYTES);
+            tma_load_2d(b_hi(s), &map_hi, full_b(s), (kb_begin + lit) * BK, nt * BN);
+            tma_load_2d(b_lo(s), &map_lo, full_b(s), (kb_begin + lit) * BK, nt * BN);
+            ++lit; ++lg;
+        };
+        // the wgmma group of global K-block g has completed: hand its stage back to the producers
+        auto release = [&](int g) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty(g % STAGES));
+            if (issuer) load_next();
+        };
+        if (issuer)
+            for (int i = 0; i < STAGES; ++i) load_next();
+
+        float acc[NMAIN][BN / 2];
+        float cross[BN / 2];
+        int g = 0;
+        for (int w = blockIdx.x; w < wk.total; w += gridDim.x) {
             int mt, nt, sp;
             decode(w, mt, nt, sp);
-            const int kb_begin = sp * p.kb_per_split;
-            const int nkb = min(p.kblocks, kb_begin + p.kb_per_split) - kb_begin;
-            const int buf = tile & 1;
-            mbar_wait(tmem_full(buf), (tile >> 1) & 1, 2, tile);
-            tc_fence_after();
-            const int m = mt * TC_BM + quad * 32 + lane;
-            const int n_base = nt * BN;
-            const bool partial = p.splits > 1;
-            // 128-bit stores need 16-byte aligned rows: channel strides / offsets multiples of 4 floats
-            const bool vec_ok = partial ? (p.Cout & 3) == 0
-                                        : ((p.ocs & 3) == 0 && (p.oco & 3) == 0 && (reinterpret_cast<uintptr_t>(p.y) & 15) == 0 &&
-                                           (!p.bias || (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0));
-            const int n_acc = nkb < NMAIN ? nkb : NMAIN;
-            const uint32_t tbase = tmem_acc + (uint32_t)(buf * Cfg::BUF_COLS) + ((uint32_t)(quad * 32) << 16);
-#pragma unroll 1
-            for (int cc = 0; cc < BN; cc += 16) {
-                float accv[16];
-                {   // cross terms first (smallest magnitude), scaled back by the lo pre-scale
-                    uint32_t r[16];
-                    G6D_TMEM_LD16(r, tbase + (uint32_t)(NMAIN * BN + cc));
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+            const int nkb = kblocks_of(sp);
+            for (int it0 = 0; it0 < nkb; it0 += NMAIN) {
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) accv[j] = __uint_as_float(r[j]) * KC::CROSS;
-                }
-#pragma unroll
-                for (int a = 0; a < NMAIN; ++a) {
-                    if (a < n_acc) {
-                        uint32_t r[16];
-                        G6D_TMEM_LD16(r, tbase + (uint32_t)(a * BN + cc));
-                        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) accv[j] += __uint_as_float(r[j]);
+                for (int a = 0; a < NMAIN; ++a) {              // K-block it uses main accumulator it % NMAIN
+                    const int it = it0 + a;
+                    if (it < nkb) {
+                        const int s = g % STAGES;
+                        mbar_wait(full_a(s), (g / STAGES) & 1, 4, g);
+                        mbar_wait(full_b(s), (g / STAGES) & 1, 5, g);
+                        mma_stage<BN, KIND>(acc[a], cross, a_hi(s), a_lo(s), b_hi(s), b_lo(s), it == 0, it < NMAIN);
+                        wgmma_wait<1>();
+                        if (it > 0) release(g - 1);
+                        ++g;
                     }
                 }
-                const int n0 = n_base + cc;
-                if (!partial) {
-                    if (p.bias) {
-                        if (vec_ok && n0 + 16 <= p.Cout) {          // 4 x 128-bit (L1-broadcast) bias loads
-#pragma unroll
-                            for (int j4 = 0; j4 < 4; ++j4) {
-                                const float4 bb = __ldg(reinterpret_cast<const float4*>(p.bias + n0) + j4);
-                                accv[j4 * 4] += bb.x; accv[j4 * 4 + 1] += bb.y; accv[j4 * 4 + 2] += bb.z; accv[j4 * 4 + 3] += bb.w;
-                            }
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 16; ++j)
-                                if (n0 + j < p.Cout) accv[j] += __ldg(p.bias + n0 + j);
-                        }
-                    }
-                    if (p.act != G6D_ACT_NONE) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) accv[j] = tc_act(accv[j], p.act);
-                    }
-                }
-                if (m < p.M) {
-                    float* dst = partial ? p.ws + ((long long)sp * p.M + m) * p.Cout + n0
-                                         : p.y + (long long)m * p.ocs + p.oco + n0;
-                    if (vec_ok && n0 + 16 <= p.Cout) {      // 4 x 128-bit stores per thread instead of 16 scalar ones
-#pragma unroll
-                        for (int j4 = 0; j4 < 4; ++j4)
-                            reinterpret_cast<float4*>(dst)[j4] = make_float4(accv[j4 * 4], accv[j4 * 4 + 1], accv[j4 * 4 + 2], accv[j4 * 4 + 3]);
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j)
-                            if (n0 + j < p.Cout) dst[j] = accv[j];
-                    }
-                }
-                if (p.stats && !partial)
-                    epilogue_stats(accv, m < p.M, p.stats, (long long)(mt * TC_BM + quad * 32) / p.stats_rows, p.Cout, n0, lane);
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tmem_empty(buf));
+            wgmma_wait<0>();
+            if (nkb > 0) release(g - 1);
+
+            const bool partial = p.splits > 1;
+            const int n_base = nt * BN;
+            const int m0 = mt * TC_BM + 16 * cw + (lane >> 2), m1 = m0 + 8;
+            float* out = partial ? p.ws + (long long)sp * p.M * p.Cout + n_base : p.y + p.oco + n_base;
+            const long long ld = partial ? p.Cout : p.ocs;
+            // 64-bit stores need 8-byte aligned column pairs
+            const bool vec2 = partial ? (p.Cout & 1) == 0
+                                      : ((p.ocs & 1) == 0 && (p.oco & 1) == 0 && (reinterpret_cast<uintptr_t>(p.y) & 7) == 0);
+            epilogue_tile<BN, KIND>(acc, cross, nkb < NMAIN ? nkb : NMAIN, m0 < p.M ? out + m0 * ld : nullptr,
+                                    m1 < p.M ? out + m1 * ld : nullptr, n_base, p.Cout, p.bias, p.act, partial, vec2,
+                                    p.stats, (long long)(mt * TC_BM + 16 * cw) / p.stats_rows, lane);
         }
     }
-    __syncthreads();
-    if (warp == W_MMA) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_acc), "n"(Cfg::TMEM_COLS) : "memory");
-    }
 }
+
 
 // Split-K epilogue: y = act(sum_s ws[s] + bias); one thread per output element.
 __global__ void conv_tc_reduce_kernel(const float* __restrict__ ws, const float* __restrict__ bias,
@@ -699,19 +624,21 @@ static int fill_tc_params(const g6d_conv_desc* d, int kind, ConvTcP& p) {
     const int min_kb = 256 / bk;                     // never split below 256 K-elements per item
     int splits = 1;
     if (ctas < kNumSMs && p.kblocks >= 2 * min_kb) {
-        // as many K splits as still fit in ONE wave of the 148 persistent CTAs (a second, partial wave
+        // as many K splits as still fit in ONE wave of the persistent CTAs (a second, partial wave
         // of long items costs more than the parallelism it adds)
         splits = (int)(kNumSMs / ctas);
         splits = splits > p.kblocks / min_kb ? p.kblocks / min_kb : splits;
         splits = splits < 1 ? 1 : splits;
     }
-    // The tensor core adds each K-step into the fp32 accumulator with truncation; over very long
-    // K chains of same-sign products (detector correlation: K = 115200 of post-ReLU features)
-    // that is a systematic bias of ~4e-5 relative.  For long-K problems (K > 8192) the chain per
-    // CTA is bounded to 2048 terms and the partials are summed in fp32 round-to-nearest.
+    // The tensor core adds each K-step into the fp32 accumulator with truncation; over long K chains
+    // of same-sign products that is a systematic bias (detector correlation, K = 115200 of post-ReLU
+    // features: ~4e-5 relative; on Hopper it already shows in the 3x3x512 VGG layers and compounds
+    // through the pyramid: 3.4e-5 on the detector's raw correlation, 2.2e-5 with the split, at +0.9 %
+    // detection time, see DESIGN.md section 3).  For K > 2048 the chain per accumulator is bounded to
+    // 2048 terms and the partials are summed in fp32 round-to-nearest.
     // d->max_chain_k bounds the K-elements per ACCUMULATOR; a split rotates over NMAIN of them
-    const int nmain = bn == 32 ? Tc2Cfg<32>::NMAIN : (bn == 64 ? Tc2Cfg<64>::NMAIN : Tc2Cfg<128>::NMAIN);
-    const int chain = d->max_chain_k > 0 ? d->max_chain_k * nmain : (K > 8192 ? TC_MAX_K_PER_CHAIN : 0);
+    const int nmain = bn == 32 ? AccCfg<32>::NMAIN : (bn == 64 ? AccCfg<64>::NMAIN : AccCfg<128>::NMAIN);
+    const int chain = d->max_chain_k > 0 ? d->max_chain_k * nmain : (K > TC_MAX_K_PER_CHAIN ? TC_MAX_K_PER_CHAIN * nmain : 0);
     const int max_kb = chain > bk ? chain / bk : 1;
     const int min_splits = chain > 0 ? (p.kblocks + max_kb - 1) / max_kb : 1;
     splits = splits < min_splits ? min_splits : splits;
@@ -721,12 +648,12 @@ static int fill_tc_params(const g6d_conv_desc* d, int kind, ConvTcP& p) {
     return G6D_OK;
 }
 
-template <int BN, int KIND, int NPW = 8>
+template <int BN, int KIND>
 static int launch_tc2(const ConvTcP& p, const CUtensorMap& mh, const CUtensorMap& ml, cudaStream_t st) {
     using Cfg = Tc2Cfg<BN>;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN, KIND, NPW>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+        cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) { set_error("g6d_conv_tc: cannot opt in to %d B of shared memory: %s", Cfg::SMEM_BYTES, cudaGetErrorString(e)); return G6D_ECUDA; }
         configured = true;
     }
@@ -735,7 +662,7 @@ static int launch_tc2(const ConvTcP& p, const CUtensorMap& mh, const CUtensorMap
     const long long total = (long long)wk.m_tiles * wk.n_tiles * p.splits;
     wk.total = (int)total;
     const int grid = total < kNumSMs ? (int)total : kNumSMs;
-    conv_tc2_kernel<BN, KIND, NPW><<<grid, tc2_threads(NPW), Cfg::SMEM_BYTES, st>>>(p, wk, mh, ml);
+    conv_tc2_kernel<BN, KIND><<<grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(p, wk, mh, ml);
     G6D_CHECK_LAUNCH("g6d_conv_tc");
     return G6D_OK;
 }
@@ -794,15 +721,16 @@ __global__ void pack_conv_weight_tc_kernel(const float* __restrict__ w, void* __
 //
 // The output positions of one image plane are enumerated over the PADDED width Wp = W + 2*pw:
 // f = y*Wp + x.  Tap (ky,kx) of output f reads padded-input position f + ky*Wp + kx, so for a
-// tile of 128 consecutive f the A operand of EVERY tap is a window of 128 consecutive rows of
-// one shared-memory buffer holding padded-input positions [f0, f0 + 127 + (kh-1)*Wp + kw-1]:
-// the tap is selected by the UMMA descriptor's start address (+shift*128 B; the 128B swizzle is a
-// function of the absolute smem address, verified by g6d_debug_umma_shift).  The producers
+// tile of 64 consecutive f the A operand of EVERY tap is a window of 64 consecutive rows of
+// one shared-memory buffer holding padded-input positions [f0, f0 + 63 + (kh-1)*Wp + kw-1]:
+// the tap is selected by the wgmma descriptor's start address (+shift*128 B; the 128B swizzle is a
+// function of the absolute smem address, checked by g6d_debug_desc_shift).  The producers
 // therefore gather (and prologue-transform, and hi/lo split) each input element ONCE per channel
 // block instead of once per tap: 9x less producer work / L2 traffic for 3x3 ("FLAT" mode).  When
 // the halo (kh-1)*Wp does not fit in shared memory (wide images, 15x15 correlation kernels) the
 // buffer holds one kernel row at a time ("ROW" mode: kw-fold reuse).  Columns x >= Wo of the
-// padded enumeration are computed and dropped.  B tiles stream by TMA per (channel block, tap).
+// padded enumeration are computed and dropped.  B tiles stream by TMA per (channel block, tap),
+// issued by one consumer thread b_stages blocks ahead of the MMAs.
 struct ConvFlatP {
     const float* x; const float* bias; const float* ps; const float* pb; float* y; float* ws;
     int B, D, H, W, Cin, ics, ico, Cout, kd, kh, kw, pd, ph, pw, Do, Ho, Wo, ocs, oco, pro, act;
@@ -812,19 +740,15 @@ struct ConvFlatP {
     double* stats; long long stats_rows;
 };
 
-template <int BN> struct FlatCfg {
-    static constexpr int NMAIN = BN == 32 ? 7 : (BN == 256 ? 1 : 3);
-    static constexpr int TMEM_COLS = (NMAIN + 1) * BN;             // 256 / 256 / 512 columns
-};
-
 template <int BN, int KIND>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo) {
     using KC = KindCfg<KIND>;
-    constexpr int NMAIN = FlatCfg<BN>::NMAIN;
-    constexpr int TMEM_COLS = FlatCfg<BN>::TMEM_COLS;
+    constexpr int NMAIN = AccCfg<BN>::NMAIN;
     constexpr int B_BYTES = BN * 128;
     constexpr int BK = KC::BK, NV = KC::NV;
+    constexpr int RSTEP = TC_PRODUCER_WARPS * 4;         // rows r0 + RSTEP*j of a trip
+    constexpr int ROWS = TC_BM / RSTEP;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
@@ -840,9 +764,7 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
     auto a_empty = [&](int s) { return bar_base + 8 * (4 + s); };
     auto b_full = [&](int s) { return bar_base + 8 * (8 + s); };
     auto b_empty = [&](int s) { return bar_base + 8 * (12 + s); };
-    const uint32_t tmem_full = bar_base + 8 * 16;
     const uint32_t bar_off = (bar_base - base);
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(base_ptr + bar_off + 8 * 17);
     int* rowtab = reinterpret_cast<int*>(base_ptr + bar_off + 256);   // [ntab][seg_rows]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -864,46 +786,37 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
         const int yy = g / p.Wp - p.ph, xx = g % p.Wp - p.pw;
         rowtab[e] = ((unsigned)yy < (unsigned)p.H && (unsigned)xx < (unsigned)p.W) ? yy * p.W + xx : -1;
     }
-    if (warp == TC_PRODUCER_WARPS && lane == 0) {
+    if (threadIdx.x == TC_ISSUER) {
         for (int s = 0; s < 4; ++s) {
             mbar_init(a_full(s), TC_PRODUCER_WARPS);
-            mbar_init(a_empty(s), 1);
+            mbar_init(a_empty(s), 4);             // the consumer warps
             mbar_init(b_full(s), 1);
-            mbar_init(b_empty(s), 1);
+            mbar_init(b_empty(s), 4);
         }
-        mbar_init(tmem_full, 1);
         fence_barrier_init();
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_lo) : "memory");
     }
-    if (warp == TC_PRODUCER_WARPS + 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     ::"r"(smem_u32((const void*)tmem_slot)), "n"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_acc = *tmem_slot;
 
     if (warp < TC_PRODUCER_WARPS) {
         // =============================== A producers ===============================
         const int chunk = threadIdx.x & 7;
         const int cofs = chunk * 4;                             // channels [cofs, cofs+4) (+32 for the 2nd load), see f16_k_source
-        const int r0 = threadIdx.x >> 3;                        // rows r0 + 32*j
+        const int r0 = threadIdx.x >> 3;                        // rows r0 + RSTEP*j
         const long long plane = (long long)p.H * p.W;
         const long long gi = (long long)b / p.group_rows;
         const bool relu = p.pro == G6D_PRO_AFFINE_RELU;
-        // Software pipeline over (unit, 128-row trip) with a ring of NB register slots: the global loads of
+        // Software pipeline over (unit, TC_BM-row trip) with a ring of NB register slots: the global loads of
         // the next NB-1 trips (possibly of the next unit: they only touch registers, so they do not wait for
         // the stage to be free) are in flight while a trip is transformed and stored.  Without it every trip
         // paid a full L2 round trip before its first st.shared.
         constexpr int NB = 3;
-        const int trips = (p.seg_rows + 127) / 128;
+        const int trips = (p.seg_rows + TC_BM - 1) / TC_BM;
         const int total = nunits * trips;
-        float4 v[NB][4][NV]; int off[NB][4];
+        float4 v[NB][ROWS][NV]; int off[NB][ROWS];
         auto unit_of = [&](int tt, int& u, int& rbase, int& cb, int& kz, int& tb) {
-            u = tt / trips; rbase = (tt - u * trips) * 128;
+            u = tt / trips; rbase = (tt - u * trips) * TC_BM;
             cb = cb_begin + u / p.nseg;
             const int seg = u % p.nseg;
             // FLAT: seg = kz, table 0.  ROW: seg = kz*kh + ky, table ky.
@@ -918,8 +831,8 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
             const float* xplane = p.x + ((long long)b * p.D + (zok ? zz : 0)) * plane * p.ics + p.ico + cb * BK + cofs;
             const int* tab = rowtab + tb * p.seg_rows;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int r = rbase + r0 + 32 * j;
+            for (int j = 0; j < ROWS; ++j) {
+                const int r = rbase + r0 + RSTEP * j;
                 off[q][j] = (r < p.seg_rows && zok) ? tab[r] : -1;
 #pragma unroll
                 for (int e = 0; e < NV; ++e) v[q][j][e] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -938,8 +851,8 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
             const int c = cb * BK + cofs;
             if (rbase == 0) mbar_wait(a_empty(s), ((u / p.a_stages) & 1) ^ 1, 1, u);
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const int r = rbase + r0 + 32 * j;
+            for (int j = 0; j < ROWS; ++j) {
+                const int r = rbase + r0 + RSTEP * j;
                 if (r >= p.rows_pad) continue;
                 if (p.pro != G6D_PRO_NONE && off[q][j] >= 0) {
                     const float4* scp; const float4* shp;
@@ -957,7 +870,7 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
                 const uint32_t so = r * 128 + ((chunk ^ (r & 7)) << 4);
                 split_store<KIND>(a_hi(s) + so, a_lo(s) + so, v[q][j]);
             }
-            if (rbase + 128 >= p.seg_rows) {          // last trip of the unit: publish the stage
+            if (rbase + TC_BM >= p.seg_rows) {          // last trip of the unit: publish the stage
                 fence_proxy_async();
                 __syncwarp();
                 if (lane == 0) mbar_arrive(a_full(s));
@@ -975,142 +888,86 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
                 }
             }
         }
-
-        // =============================== epilogue ===============================
-        mbar_wait(tmem_full, 0, 2, nunits);
-        tc_fence_after();
-        const int quad = warp & 3;
-        const int row = quad * 32 + lane;
-        const int f = f0 + row;
-        const int yo = f / p.Wp, xo = f % p.Wp;
-        const bool valid = yo < p.Ho && xo < p.Wo;
-        const long long m = (((long long)b * p.Do + zo) * p.Ho + yo) * p.Wo + xo;
-        constexpr int HALF = BN / 2;
-        const int col0 = (warp >> 2) * HALF;
-        const bool partial = p.splits > 1;
-        const bool vec_ok = partial ? (p.Cout & 3) == 0
-                                    : ((p.ocs & 3) == 0 && (p.oco & 3) == 0 && (reinterpret_cast<uintptr_t>(p.y) & 15) == 0 &&
-                                       (!p.bias || (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0));
-        const int total_mm = nunits * p.taps_per_seg;
-        const int n_acc = total_mm < NMAIN ? total_mm : NMAIN;
-#pragma unroll
-        for (int cc = 0; cc < HALF; cc += 16) {
-            float accv[16];
-            const uint32_t taddr = tmem_acc + ((uint32_t)(quad * 32) << 16) + (uint32_t)(col0 + cc);
-            {
-                uint32_t r[16];
-                G6D_TMEM_LD16(r, taddr + (uint32_t)(NMAIN * BN));
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                for (int j = 0; j < 16; ++j) accv[j] = __uint_as_float(r[j]) * KC::CROSS;
+    } else {
+        // =============================== consumer warpgroup ===============================
+        const int cw = warp - TC_PRODUCER_WARPS;
+        const bool issuer = threadIdx.x == TC_ISSUER;
+        const int taps = p.taps_per_seg;
+        const int nb_total = nunits * taps;
+        int lb = 0;                                    // next B block the issuer loads
+        auto load_b = [&]() {
+            if (lb >= nb_total) return;
+            const int u = lb / taps, t = lb % taps;
+            const int cb = cb_begin + u / p.nseg, seg = u % p.nseg;
+            const int s = lb % p.b_stages;
+            mbar_wait(b_empty(s), ((lb / p.b_stages) & 1) ^ 1, 3, lb);
+            mbar_expect_tx(b_full(s), 2 * B_BYTES);
+            const int k = (seg * taps + t) * p.Cin + cb * BK;
+            tma_load_2d(b_hi(s), &map_hi, b_full(s), k, n_base);
+            tma_load_2d(b_lo(s), &map_lo, b_full(s), k, n_base);
+            ++lb;
+        };
+        // the wgmma group of B block q has completed: free its B stage and, after a unit's last tap, its A stage
+        auto release = [&](int q) {
+            __syncwarp();
+            if (lane == 0) {
+                mbar_arrive(b_empty(q % p.b_stages));
+                if (q % taps == taps - 1) mbar_arrive(a_empty((q / taps) % p.a_stages));
             }
+            if (issuer) load_b();
+        };
+        if (issuer)
+            for (int i = 0; i < p.b_stages; ++i) load_b();
+
+        float acc[NMAIN][BN / 2];
+        float cross[BN / 2];
+        // B block bi = (unit u, tap t) = (bi / taps, bi % taps) uses main accumulator bi % NMAIN
+        for (int b0 = 0; b0 < nb_total; b0 += NMAIN) {
 #pragma unroll
             for (int a = 0; a < NMAIN; ++a) {
-                if (a < n_acc) {
-                    uint32_t r[16];
-                    G6D_TMEM_LD16(r, taddr + (uint32_t)(a * BN));
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) accv[j] += __uint_as_float(r[j]);
-                }
-            }
-            const int n0 = n_base + col0 + cc;
-            if (!partial) {
-                if (p.bias) {
-                    if (vec_ok && n0 + 16 <= p.Cout) {
-#pragma unroll
-                        for (int j4 = 0; j4 < 4; ++j4) {
-                            const float4 bb = __ldg(reinterpret_cast<const float4*>(p.bias + n0) + j4);
-                            accv[j4 * 4] += bb.x; accv[j4 * 4 + 1] += bb.y; accv[j4 * 4 + 2] += bb.z; accv[j4 * 4 + 3] += bb.w;
-                        }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j)
-                            if (n0 + j < p.Cout) accv[j] += __ldg(p.bias + n0 + j);
-                    }
-                }
-                if (p.act != G6D_ACT_NONE) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) accv[j] = tc_act(accv[j], p.act);
-                }
-            }
-            if (valid) {
-                float* dst = partial ? p.ws + ((long long)split * p.M + m) * p.Cout + n0 : p.y + m * p.ocs + p.oco + n0;
-                if (vec_ok && n0 + 16 <= p.Cout) {
-#pragma unroll
-                    for (int j4 = 0; j4 < 4; ++j4)
-                        reinterpret_cast<float4*>(dst)[j4] = make_float4(accv[j4 * 4], accv[j4 * 4 + 1], accv[j4 * 4 + 2], accv[j4 * 4 + 3]);
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (n0 + j < p.Cout) dst[j] = accv[j];
-                }
-            }
-            if (p.stats && !partial)      // tiles never span planes and a group is made of whole planes
-                epilogue_stats(accv, valid, p.stats, (((long long)b * p.Do + zo) * p.Ho * p.Wo) / p.stats_rows, p.Cout, n0, lane);
-        }
-        tc_fence_before();
-    } else if (warp == TC_PRODUCER_WARPS) {
-        // =============================== B producer (TMA) ===============================
-        if (lane == 0) {
-            int bi = 0;
-            for (int u = 0; u < nunits; ++u) {
-                const int cb = cb_begin + u / p.nseg, seg = u % p.nseg;
-                for (int t = 0; t < p.taps_per_seg; ++t, ++bi) {
-                    const int s = bi % p.b_stages;
-                    const uint32_t n_use = bi / p.b_stages;
-                    mbar_wait(b_empty(s), (n_use & 1) ^ 1, 3, bi);
-                    mbar_expect_tx(b_full(s), 2 * B_BYTES);
-                    const int k = (seg * p.taps_per_seg + t) * p.Cin + cb * BK;
-                    tma_load_2d(b_hi(s), &map_hi, b_full(s), k, n_base);
-                    tma_load_2d(b_lo(s), &map_lo, b_full(s), k, n_base);
-                }
-            }
-        }
-    } else {
-        // =============================== MMA issuer ===============================
-        if (elect_one_sync()) {
-            const uint32_t idesc = umma_idesc<KIND>(TC_BM, BN);
-            int bi = 0;
-            for (int u = 0; u < nunits; ++u) {
-                const int sa = u % p.a_stages;
-                mbar_wait(a_full(sa), (u / p.a_stages) & 1, 4, u);
-                tc_fence_after();
-                for (int t = 0; t < p.taps_per_seg; ++t, ++bi) {
-                    const int sb = bi % p.b_stages;
+                const int bi = b0 + a;
+                if (bi < nb_total) {
+                    const int u = bi / taps, t = bi - u * taps;
+                    const int sa = u % p.a_stages, sb = bi % p.b_stages;
+                    if (t == 0) mbar_wait(a_full(sa), (u / p.a_stages) & 1, 4, u);
                     mbar_wait(b_full(sb), (bi / p.b_stages) & 1, 5, bi);
-                    tc_fence_after();
                     const int shift = p.mode == 1 ? t : (t / p.kw) * p.Wp + (t % p.kw);     // rows
-                    const uint64_t dah = umma_desc_sw128(a_hi(sa) + shift * 128), dal = umma_desc_sw128(a_lo(sa) + shift * 128);
-                    const uint64_t dbh = umma_desc_sw128(b_hi(sb)), dbl = umma_desc_sw128(b_lo(sb));
-                    const uint32_t main_acc = tmem_acc + (uint32_t)((bi % NMAIN) * BN);
-                    const uint32_t cross_acc = tmem_acc + (uint32_t)(NMAIN * BN);
-#pragma unroll
-                    for (int ks = 0; ks < 4; ++ks) {
-                        const uint64_t adv = (uint64_t)((ks * 32) >> 4);
-                        umma<KIND>(cross_acc, dal + adv, dbh + adv, idesc, (bi > 0 || ks > 0) ? 1u : 0u);
-                        umma<KIND>(cross_acc, dah + adv, dbl + adv, idesc, 1u);
-                        umma<KIND>(main_acc, dah + adv, dbh + adv, idesc, (bi >= NMAIN || ks > 0) ? 1u : 0u);
-                    }
-                    umma_commit(b_empty(sb));
+                    mma_stage<BN, KIND>(acc[a], cross, a_hi(sa) + shift * 128, a_lo(sa) + shift * 128, b_hi(sb), b_lo(sb),
+                                        bi == 0, bi < NMAIN);
+                    wgmma_wait<1>();
+                    if (bi > 0) release(bi - 1);
                 }
-                umma_commit(a_empty(sa));
             }
-            umma_commit(tmem_full);
         }
-    }
-    __syncthreads();
-    if (warp == TC_PRODUCER_WARPS + 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_acc), "n"(TMEM_COLS) : "memory");
+        wgmma_wait<0>();
+        if (nb_total > 0) release(nb_total - 1);
+
+        // =============================== epilogue ===============================
+        const bool partial = p.splits > 1;
+        const long long m_plane = ((long long)b * p.Do + zo) * p.Ho * p.Wo;
+        float* dst[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int f = f0 + 16 * cw + (lane >> 2) + 8 * h;
+            const int yo = f / p.Wp, xo = f % p.Wp;
+            const long long m = m_plane + (long long)yo * p.Wo + xo;
+            dst[h] = (yo < p.Ho && xo < p.Wo) ? (partial ? p.ws + ((long long)split * p.M + m) * p.Cout + n_base
+                                                         : p.y + m * p.ocs + p.oco + n_base)
+                                              : nullptr;
+        }
+        const bool vec2 = partial ? (p.Cout & 1) == 0
+                                  : ((p.ocs & 1) == 0 && (p.oco & 1) == 0 && (reinterpret_cast<uintptr_t>(p.y) & 7) == 0);
+        // tiles never span planes and a group is made of whole planes
+        epilogue_tile<BN, KIND>(acc, cross, nb_total < NMAIN ? nb_total : NMAIN, dst[0], dst[1], n_base, p.Cout, p.bias,
+                                p.act, partial, vec2, p.stats, m_plane / p.stats_rows, lane);
     }
 }
 
+
 // G6D_CONV_FLAT: 0 = never use the A-reuse kernel, 1 = FLAT mode only (default), 2 = FLAT and ROW.
-// Measured on B200 (tools/conv_breakdown.py): the MMAs are shared-memory-bandwidth bound
-// (every MMA re-reads 4 KB of A and N*32 B of B; at N = 128 that alone is 128 B/clk/SM), so the
-// 3x-reuse ROW mode does not pay for its junk columns, while FLAT (9x reuse, and the prologue
-// applied once per element instead of once per tap) gains 26 % on the selector's first tower conv.
+// The MMAs re-read their A and B tiles from shared memory, so the 3x-reuse ROW mode computes junk
+// columns without saving operand traffic; FLAT (9x reuse, and the prologue applied once per element
+// instead of once per tap) saves the producers most of their work.
 static int flat_level() {
     static int v = -1;
     if (v < 0) { const char* e = getenv("G6D_CONV_FLAT"); v = (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1; }
@@ -1165,8 +1022,8 @@ static int fill_flat_params(const g6d_conv_desc* d, int kind, ConvFlatP& p, int*
     const long long K = (long long)d->Cin * d->kd * d->kh * d->kw;
     int splits = 1;
     if (ctas < kNumSMs && p.cblocks >= 2) splits = (int)((kNumSMs + ctas - 1) / ctas);
-    const int nmain = bn == 32 ? FlatCfg<32>::NMAIN : (bn == 64 ? FlatCfg<64>::NMAIN : FlatCfg<128>::NMAIN);
-    const long long chain = d->max_chain_k > 0 ? (long long)d->max_chain_k * nmain : (K > 8192 ? TC_MAX_K_PER_CHAIN : 0);
+    const int nmain = bn == 32 ? AccCfg<32>::NMAIN : (bn == 64 ? AccCfg<64>::NMAIN : AccCfg<128>::NMAIN);
+    const long long chain = d->max_chain_k > 0 ? (long long)d->max_chain_k * nmain : (K > TC_MAX_K_PER_CHAIN ? TC_MAX_K_PER_CHAIN * nmain : 0);
     if (chain > 0) { const int ms = (int)((K + chain - 1) / chain); splits = splits < ms ? ms : splits; }
     splits = splits > p.cblocks ? p.cblocks : splits;
     splits = splits < 1 ? 1 : splits;
@@ -1207,7 +1064,7 @@ static int dispatch_tc2(int bn, const ConvTcP& p, const CUtensorMap& mh, const C
 using namespace g6d;
 
 // Debug aid: copies the 8-int timeout record (0 = no timeout; else [1]=waiter role 1 A-producer/empty,
-// 2 epilogue/tmem_full, 3 B-producer/empty, 4 MMA/full_a, 5 MMA/full_b, 6 MMA/tmem_empty; [2]=iteration;
+// 3 weight-TMA issuer/empty, 4 MMA/full_a, 5 MMA/full_b; [2]=iteration;
 // [3]=parity; [4..6]=block; [7]=thread) and clears it.  Synchronises the device.
 extern "C" int g6d_conv_tc_debug(int* host_out8) {
     G6D_REQUIRE(host_out8 != nullptr, "g6d_conv_tc_debug: null");
@@ -1345,20 +1202,18 @@ extern "C" int g6d_pack_conv_weight_tc(const float* w, void* out_hi, void* out_l
 // ------------------------------------------------------------------------------------------
 // Probe (debug/test only): does a K-major SWIZZLE_128B A operand tolerate a start address that is
 // shifted by `shift` rows (shift*128 B, not 1024-aligned) when the data was written with the
-// swizzle phase of its ABSOLUTE shared-memory row?  D[128 x 32] = A[shift .. shift+128) x B^T with
-// K = 32, A[r][k] = r + k/64 (exactly representable), B = 32x32 identity.  `mode` selects how the
-// descriptor's base_offset field is set: 0 -> 0, 1 -> (start_address >> 7) & 7.
+// swizzle phase of its ABSOLUTE shared-memory row?  D[64 x 32] = A[shift .. shift+64) x B^T with
+// K = 32, A[r][k] = r + k/64 (exactly representable), B = 32x32 identity, so D[i][n] = shift + i + n/64.
+// `mode` selects the descriptor's base_offset field: 0 -> 0, 1 -> (start_address >> 7) & 7.
 namespace g6d {
-__global__ void __launch_bounds__(128) umma_shift_probe_kernel(float* out, int shift, int mode) {
+__global__ void __launch_bounds__(128) desc_shift_probe_kernel(float* out, int shift, int mode) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* bp = smem_raw + (base - smem_u32(smem_raw));
-    const uint32_t a_base = base;                 // 160 rows x 128 B
-    const uint32_t b_base = base + 160 * 128;     // 32 rows x 128 B (20480 is 1024-aligned)
-    const uint32_t bar = b_base + 32 * 128;
-    volatile uint32_t* slot = reinterpret_cast<volatile uint32_t*>(bp + 160 * 128 + 32 * 128 + 16);
+    const uint32_t a_base = base;                 // 96 rows x 128 B
+    const uint32_t b_base = base + 96 * 128;      // 32 rows x 128 B (12288 is 1024-aligned)
     const int t = threadIdx.x;
-    for (int r = t; r < 160; r += 128)
+    for (int r = t; r < 96; r += 128)
         for (int c = 0; c < 8; ++c) {
             float4 v = make_float4(r + (c * 4 + 0) / 64.f, r + (c * 4 + 1) / 64.f, r + (c * 4 + 2) / 64.f, r + (c * 4 + 3) / 64.f);
             *reinterpret_cast<float4*>(bp + r * 128 + ((c ^ (r & 7)) << 4)) = v;
@@ -1366,45 +1221,32 @@ __global__ void __launch_bounds__(128) umma_shift_probe_kernel(float* out, int s
     for (int r = t; r < 32; r += 128)
         for (int c = 0; c < 8; ++c) {
             float4 v = make_float4(r == c * 4 ? 1.f : 0.f, r == c * 4 + 1 ? 1.f : 0.f, r == c * 4 + 2 ? 1.f : 0.f, r == c * 4 + 3 ? 1.f : 0.f);
-            *reinterpret_cast<float4*>(bp + 160 * 128 + r * 128 + ((c ^ (r & 7)) << 4)) = v;
+            *reinterpret_cast<float4*>(bp + 96 * 128 + r * 128 + ((c ^ (r & 7)) << 4)) = v;
         }
     fence_proxy_async();
-    if (t == 0) { mbar_init(bar, 1); fence_barrier_init(); }
-    if (t < 32) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 32;" ::"r"(smem_u32((const void*)slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *slot;
-    if (t == 0) {
-        const uint32_t start = a_base + shift * 128;
-        uint64_t da = umma_desc_sw128(start);
-        if (mode == 1) da |= (uint64_t)((start >> 7) & 7) << 49;
-        const uint64_t db = umma_desc_sw128(b_base);
-        const uint32_t idesc = umma_idesc<G6D_TC_TF32>(128, 32);
-        for (int ks = 0; ks < 4; ++ks) umma<G6D_TC_TF32>(tmem, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), idesc, ks > 0);
-        umma_commit(bar);
-    }
-    mbar_wait(bar, 0, 9, 0);
-    tc_fence_after();
+    const uint32_t start = a_base + shift * 128;
+    uint64_t da = gmma_desc_sw128(start);
+    if (mode == 1) da |= (uint64_t)((start >> 7) & 7) << 49;
+    const uint64_t db = gmma_desc_sw128(b_base);
+    float d[16];
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) wgmma<32, G6D_TC_TF32>(d, da + (uint64_t)(ks * 2), db + (uint64_t)(ks * 2), ks > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
     const int warp = t >> 5, lane = t & 31;
-    for (int cc = 0; cc < 32; cc += 16) {
-        uint32_t r[16];
-        G6D_TMEM_LD16(r, tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)cc);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        for (int j = 0; j < 16; ++j) out[(warp * 32 + lane) * 32 + cc + j] = __uint_as_float(r[j]);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+        const int row = 16 * warp + (lane >> 2) + 8 * ((j >> 1) & 1), col = 8 * (j >> 2) + 2 * (lane & 3) + (j & 1);
+        out[row * 32 + col] = d[j];
     }
-    tc_fence_before();
-    __syncthreads();
-    if (t < 32) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 32;" ::"r"(tmem) : "memory");
 }
 }  // namespace g6d
 
-extern "C" int g6d_debug_umma_shift(float* out, int shift, int mode, g6d_stream_t stream) {
-    G6D_REQUIRE(out && shift >= 0 && shift <= 31, "g6d_debug_umma_shift: bad args");
-    g6d::umma_shift_probe_kernel<<<1, 128, 160 * 128 + 32 * 128 + 1024 + 64, g6d::as_stream(stream)>>>(out, shift, mode);
-    G6D_CHECK_LAUNCH("g6d_debug_umma_shift");
+extern "C" int g6d_debug_desc_shift(float* out, int shift, int mode, g6d_stream_t stream) {
+    G6D_REQUIRE(out && shift >= 0 && shift <= 31, "g6d_debug_desc_shift: bad args");
+    g6d::desc_shift_probe_kernel<<<1, 128, 96 * 128 + 32 * 128 + 1024, g6d::as_stream(stream)>>>(out, shift, mode);
+    G6D_CHECK_LAUNCH("g6d_debug_desc_shift");
     return G6D_OK;
 }

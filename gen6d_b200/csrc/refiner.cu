@@ -24,8 +24,8 @@ struct VolParams {
 //            mean / unbiased two-pass std / query sample are written as full 512 B rows with
 //            streaming stores.
 // Feature maps (3.7 MB / pose) are L2/L1 resident; algorithmic HBM traffic is the 50 MB of output.
-// The floor of this formulation is the L1 gather: 28 taps x 512 B per voxel = 14 KB through a
-// 128 B/clk L1 -> ~13 us per pose on 148 SMs, above the 8.2 us pure-HBM time (see DESIGN.md).
+// The floor of this formulation is the L1 gather: 28 taps x 512 B per voxel = 14 KB through the
+// 128 B/clk L1 of each SM.
 constexpr int kViewsMax = kMaxRefViews;   // views = R references + the query (view index R) <= 8
 
 template <int RT>   // RT > 0: number of reference views known at compile time (6 on the estimator path); 0: runtime

@@ -1,4 +1,4 @@
-"""Gen6DEstimator on the B200 networks: same constructor / build / predict contract as the
+"""Gen6DEstimator on the H100 networks: same constructor / build / predict contract as the
 reference's estimator.py:94-216 (numpy images and poses in, numpy pose out; `ref_info`, `cfg`).
 
 The stage sequencing is inherently serial per frame (crop depends on the detection, refinement

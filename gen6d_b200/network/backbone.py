@@ -1,4 +1,4 @@
-"""VGG11-BN feature pyramid on the sm_100a kernels (reference: network/pretrain_models.py:17-31
+"""VGG11-BN feature pyramid on the sm_90a kernels (reference: network/pretrain_models.py:17-31
 VGGBNPretrain and :61-72 VGGBNPretrainV3; layer table :86-111).
 
 Eval-mode BatchNorm is folded into the packed conv weights/bias at pack time

@@ -113,7 +113,7 @@ class PackedModule(nn.Module):
 class Branches:
     """Fork/join of independent sub-graphs onto side streams (the four detector scales, the three
     selector towers, the refiner's feature branches).  At batch 1 most of their kernels launch far
-    fewer CTAs than the 148 SMs, so running the branches concurrently is what fills the machine.
+    fewer CTAs than the GPU has SMs, so running the branches concurrently is what fills the machine.
     Works eagerly and under CUDA-graph capture (the side streams fork from and join back into the
     capturing stream, so the captured graph gets parallel branches).  Branch results must be kept
     alive by the caller until they have been consumed on the main stream.  G6D_BRANCH_STREAMS=0

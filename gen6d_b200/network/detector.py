@@ -1,4 +1,4 @@
-"""Detector on the sm_100a kernels.  Mirrors network/detector.py of the reference: same class
+"""Detector on the sm_90a kernels.  Mirrors network/detector.py of the reference: same class
 name, cfg keys, checkpoint keys and method contracts (load_ref_imgs / detect_que_imgs numpy API,
 load_impl / detect_impl / forward tensor API)."""
 import numpy as np

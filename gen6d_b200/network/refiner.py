@@ -1,4 +1,4 @@
-"""Volume refiner on the sm_100a kernels.  Mirrors network/refiner.py of the reference: class
+"""Volume refiner on the sm_90a kernels.  Mirrors network/refiner.py of the reference: class
 name, cfg keys, checkpoint keys, forward(data) tensor API and the load_ref_imgs /
 refine_que_imgs numpy API.
 

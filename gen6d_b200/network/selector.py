@@ -1,4 +1,4 @@
-"""Viewpoint selector on the sm_100a kernels.  Mirrors network/selector.py (+ attention.py) of the
+"""Viewpoint selector on the sm_90a kernels.  Mirrors network/selector.py (+ attention.py) of the
 reference: class name, cfg keys, checkpoint keys, load_ref_imgs / select_que_imgs numpy API and
 extract_ref_feats / compute_view_point_feats / forward tensor API.
 

@@ -272,7 +272,7 @@ class PackedConv:
 
 
 def conv_path():
-    """'tc' (tcgen05 split-operand kernels, default) or 'ffma' (fp32 CUDA-core fallback for A/B checks): env G6D_CONV_PATH."""
+    """'tc' (wgmma split-operand kernels, default) or 'ffma' (fp32 CUDA-core fallback for A/B checks): env G6D_CONV_PATH."""
     return os.environ.get('G6D_CONV_PATH', 'tc')
 
 

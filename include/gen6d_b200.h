@@ -1,5 +1,5 @@
 /*
- * gen6d_b200.h -- C ABI of libgen6d_b200.so: the sm_100a kernels behind the Gen6D inference
+ * gen6d_b200.h -- C ABI of libgen6d_b200.so: the sm_90a (H100) kernels behind the Gen6D inference
  * hot path (detector correlation head, selector similarity scoring, refiner feature volume +
  * conv stacks).
  *
@@ -182,7 +182,7 @@ typedef struct g6d_conv_desc {
     int prologue;             /* G6D_PRO_* applied to in-bounds input elements before the MAC */
     long long group_rows;     /* G6D_PRO_AFFINE*: input batch items per norm group */
     int act;                  /* G6D_ACT_* epilogue after bias */
-    int max_chain_k;          /* tensor-core path: 0 = default; > 0 bounds the K-elements accumulated into one TMEM
+    int max_chain_k;          /* tensor-core path: 0 = default; > 0 bounds the K-elements accumulated into one
                                  accumulator (longer problems are split and summed in fp32 round-to-nearest).  The tensor
                                  core truncates on every accumulate, which biases long chains of SAME-SIGN products
                                  (detector correlation: post-ReLU features x post-ReLU features) by ~5e-8 per step. */
@@ -216,22 +216,22 @@ int g6d_vgg_first_block(const float* x, const float* w, const float* bias, float
  * (eval-mode BatchNorm fold). */
 int g6d_pack_conv_weight(const float* w, float* out, int Cout, int Cin, int Cin_pad, int taps,
                          const float* cout_scale, g6d_stream_t stream);
-/* ---- tensor-core path (tcgen05, three-term operand split: fp32-faithful on the tensor pipe) ------
+/* ---- tensor-core path (wgmma, three-term operand split: fp32-faithful on the tensor pipe) --------
  * Same contract as g6d_conv, for problems g6d_conv_tc_supported accepts (Cin a multiple of the
  * kind's K-block, Cout >= 16).  A*B ~= A_hi*B_hi + A_hi*B_lo + A_lo*B_hi with 11-bit-significand
  * halves; `kind` selects their container:
- *   G6D_TC_TF32: hi = tf32(x), lo = tf32(x - hi), fp32 arrays, K-block 32, tcgen05.mma kind::tf32;
- *   G6D_TC_F16 : hi = fp16(x), lo = fp16((x - hi) * 2^11), __half arrays, K-block 64, kind::f16 (twice
+ *   G6D_TC_TF32: hi = tf32(x), lo = tf32(x - hi), fp32 arrays, K-block 32, tf32 wgmma;
+ *   G6D_TC_F16 : hi = fp16(x), lo = fp16((x - hi) * 2^11), __half arrays, K-block 64, f16 wgmma (twice
  *                the K per instruction and per operand byte; the kernels undo the 2^11 in the epilogue).
  *                Range contract: |x| <= 65504 (saturating), full accuracy for |x| >= 6.1e-5.
  * Weights are pre-split [w_rows >= Cout, K] K-major arrays (K = tap*Cin + c), see
  * g6d_pack_conv_weight_tc / g6d_split_operand.  A tiles are gathered + transformed + split by
- * producer warps, B tiles arrive by TMA, accumulators live in TMEM. */
+ * producer warps, B tiles arrive by TMA, accumulators live in the consumer warpgroup's registers. */
 #define G6D_TC_TF32 0
 #define G6D_TC_F16 1
 int g6d_conv_tc_supported(const g6d_conv_desc* desc, int kind);
-/* debug probe: D[128x32] = A[shift..shift+128) x I for a row-shifted SWIZZLE_128B descriptor (mode: base_offset rule) */
-int g6d_debug_umma_shift(float* out, int shift, int mode, g6d_stream_t stream);
+/* debug probe: D[64x32] = A[shift..shift+64) x I for a row-shifted SWIZZLE_128B descriptor (mode: base_offset rule) */
+int g6d_debug_desc_shift(float* out, int shift, int mode, g6d_stream_t stream);
 /* debug: host_out8[0] != 0 if a pipeline wait inside g6d_conv_tc timed out (kernel bailed out); syncs */
 int g6d_conv_tc_debug(int* host_out8);
 long long g6d_conv_tc_workspace_bytes(const g6d_conv_desc* desc, int kind);

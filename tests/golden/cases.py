@@ -78,7 +78,7 @@ def detector_case(seed=11, rfn=4, hq=96, wq=128, qn=1):
 
 def detector_case_full(seed=111):
     """BASELINE configs[1], detector half: 480x640 frame, 32 reference views (the estimator default):
-    rfn >= 16 routes the correlation through the tcgen05 kernel."""
+    rfn >= 16 routes the correlation through the tensor-core kernel."""
     return detector_case(seed=seed, rfn=32, hq=480, wq=640)
 
 

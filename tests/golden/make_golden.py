@@ -1,8 +1,7 @@
 """Generate the golden vectors under tests/golden/ by running the UNMODIFIED reference
-(/root/reference, imported through ref_shims) on the seeded cases of cases.py.
-
-Run in the build container only (the GPU box has no /root/reference):
-    python tests/golden/make_golden.py
+(a liuyuan-pal/Gen6D checkout named by GEN6D_REFERENCE, imported through ref_shims) on the seeded
+cases of cases.py.  Needs no GPU:
+    GEN6D_REFERENCE=/path/to/Gen6D python tests/golden/make_golden.py
 Outputs: net_golden.npz (network-level taps), state_dict_spec.json (checkpoint keys/shapes).
 The estimator-level vectors are produced by make_golden_estimator.py.
 """

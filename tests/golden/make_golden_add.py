@@ -2,8 +2,9 @@
 synthetic inputs"), produced by the UNMODIFIED reference: estimator.Gen6DEstimator.build/predict
 (CPU, via ref_shims) over N_FRAMES frames of the synthetic object database with the seeded
 checkpoints, scored with the reference's utils/pose_utils.py:149-215 (compute_pose_errors /
-compute_metrics_impl) against the database's ground-truth poses.  Build container only:
-    python tests/golden/make_golden_add.py
+compute_metrics_impl) against the database's ground-truth poses.  Needs a reference checkout
+named by GEN6D_REFERENCE, no GPU:
+    GEN6D_REFERENCE=/path/to/Gen6D python tests/golden/make_golden_add.py
 Outputs tests/golden/add_golden.npz."""
 import os
 import sys

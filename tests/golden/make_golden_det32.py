@@ -1,10 +1,11 @@
 """Golden vectors for BASELINE configs[1]'s detector half at full size, produced by the UNMODIFIED
 reference (network/detector.py via ref_shims): 480x640 frame, 32 reference views -> the raw sliding
 inner products of detector.py:222-224 (tap D2, BEFORE normalize_scores) for each of the 4 detection
-scales and 3 pyramid levels, plus the final maps / argmax.  With rfn = 32 the B200 build routes
-the correlation through the tcgen05 kernel (network/detector.py: rfn >= 16), which the rfn = 4
-case of make_golden.py does not.  Build container only:
-    python tests/golden/make_golden_det32.py
+scales and 3 pyramid levels, plus the final maps / argmax.  With rfn = 32 the build routes
+the correlation through the tensor-core kernel (network/detector.py: rfn >= 16), which the rfn = 4
+case of make_golden.py does not.  Needs a reference checkout
+named by GEN6D_REFERENCE, no GPU:
+    GEN6D_REFERENCE=/path/to/Gen6D python tests/golden/make_golden_det32.py
 Outputs tests/golden/det32_golden.npz (strided subsamples of the big maps, see `sub`)."""
 import os
 import sys

@@ -1,7 +1,8 @@
 """Golden vectors for the host geometry and the full estimator, produced by the UNMODIFIED
 reference (estimator.py, utils/*.py, network/*.py via ref_shims) on the synthetic in-memory
-object database and the seeded checkpoints.  Build container only:
-    python tests/golden/make_golden_estimator.py
+object database and the seeded checkpoints.  Needs a reference checkout
+named by GEN6D_REFERENCE, no GPU:
+    GEN6D_REFERENCE=/path/to/Gen6D python tests/golden/make_golden_estimator.py
 Outputs tests/golden/est_golden.npz."""
 import os
 import sys

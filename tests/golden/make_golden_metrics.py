@@ -1,6 +1,7 @@
 """Golden vectors for the evaluation metrics (SURVEY §8 row f4) from the UNMODIFIED reference
-(utils/pose_utils.py:149-215 compute_pose_errors / compute_metrics_impl).  Build container only:
-    python tests/golden/make_golden_metrics.py
+(utils/pose_utils.py:149-215 compute_pose_errors / compute_metrics_impl).  Needs a reference checkout
+named by GEN6D_REFERENCE, no GPU:
+    GEN6D_REFERENCE=/path/to/Gen6D python tests/golden/make_golden_metrics.py
 Outputs tests/golden/metrics_golden.npz."""
 import os
 import sys

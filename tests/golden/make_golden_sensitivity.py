@@ -5,7 +5,9 @@ pose).  This script measures that amplification on the reference itself (CPU, vi
 golden frame's refinement chain from the golden initial pose, and from that pose perturbed by a rotation
 of 1e-3 rad and a 1e-3 relative translation -- the size of difference that fp32 summation order in the
 detector / selector produces.  tests/test_estimator_gpu.py bounds the GPU path's deviation by the
-reference's own gain.  Build container only:  python tests/golden/make_golden_sensitivity.py
+reference's own gain.  Needs a reference checkout
+named by GEN6D_REFERENCE, no GPU:
+    GEN6D_REFERENCE=/path/to/Gen6D python tests/golden/make_golden_sensitivity.py
 Outputs tests/golden/sens_golden.npz."""
 import os
 import sys

@@ -1,13 +1,15 @@
-"""Import shims that let the UNMODIFIED reference (/root/reference) run on this CPU-only
-container.  Used only by tests/golden/make_golden.py (golden-vector generation); nothing on
-the GPU box imports this file.  See SURVEY.md section 8(c) for why each shim exists.
+"""Import shims that let the UNMODIFIED reference (a liuyuan-pal/Gen6D checkout, located by the
+GEN6D_REFERENCE environment variable) run on a CPU-only machine.  Used by the golden-vector
+generators under tests/golden/; no test imports it.  See SURVEY.md section 8(c) for why each shim exists.
 """
 import sys
 import types
 
 import numpy as np
 
-REFERENCE_ROOT = '/root/reference'
+import os
+
+REFERENCE_ROOT = os.environ.get('GEN6D_REFERENCE', '')
 
 
 def _euler_axis_rotation(axis, ang):
@@ -70,8 +72,10 @@ def mat2quat(mat):
 def install(networks=True):
     """Put stub modules in sys.modules, neutralise .cuda(), patch the VGG download.
     networks=False: only the stubs for the absent third-party packages (the reference's own `network`
-    package is not imported and torch is left untouched) -- used by tests/test_dropin.py, which puts
-    gen6d_b200.network in its place."""
+    package is not imported and torch is left untouched), for a caller that puts gen6d_b200.network in
+    its place."""
+    if not os.path.isfile(os.path.join(REFERENCE_ROOT, 'estimator.py')) or not os.path.isdir(os.path.join(REFERENCE_ROOT, 'network')):
+        raise RuntimeError(f'GEN6D_REFERENCE={REFERENCE_ROOT!r} is not a liuyuan-pal/Gen6D checkout')
     if REFERENCE_ROOT not in sys.path:
         sys.path.insert(0, REFERENCE_ROOT)
 

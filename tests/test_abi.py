@@ -47,8 +47,9 @@ def test_compute_fails_loudly_without_cuda():
 
 
 def test_bench_batch_choice_deals_lanes_evenly():
-    """bench.py's pick_batch: the timed region of `steps` poses is dealt to the lanes as equal numbers of full batches
-    whenever the step count allows it (the driver's 20 steps on 2 lanes -> 2 x 10)."""
+    """bench.py's pick_batch: the timed region of `steps` poses is always whole batches (the batch divides `steps`, so
+    exactly `steps` poses are timed), dealt to the lanes as equal numbers of full batches whenever the step count
+    allows it (20 steps on 2 lanes -> 2 x 10)."""
     import importlib.util
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     spec = importlib.util.spec_from_file_location('g6d_bench', os.path.join(root, 'bench.py'))
@@ -56,9 +57,12 @@ def test_bench_batch_choice_deals_lanes_evenly():
     spec.loader.exec_module(bench)
     if bench.E2E_BATCH > 0:
         pytest.skip('G6D_E2E_BATCH overrides the choice')
-    want = {(20, 2): 10, (16, 2): 8, (24, 2): 6, (14, 2): 7, (20, 1): 10, (4, 2): 2, (2, 2): 1, (22, 2): 4, (5, 2): 1,
-            (9, 2): 4, (40, 2): 10, (30, 3): 10}
+    want = {(20, 2): 10, (16, 2): 8, (24, 2): 6, (14, 2): 7, (20, 1): 10, (4, 2): 2, (2, 2): 1, (22, 2): 2, (5, 2): 5,
+            (9, 2): 9, (40, 2): 10, (30, 3): 10, (13, 2): 1, (1, 2): 1}
     for (steps, lanes), b in want.items():
         assert bench.pick_batch(steps, lanes) == b, (steps, lanes)
+    for steps in range(1, 64):
+        for lanes in (1, 2, 3, 4):
+            assert steps % bench.pick_batch(steps, lanes) == 0, (steps, lanes)      # exactly `steps` poses timed
         if steps % lanes == 0 and (steps // lanes) % b == 0:
             assert (steps // b) % lanes == 0          # every lane runs the same number of batches

@@ -1,4 +1,4 @@
-"""The tcgen05 split-operand convolution (g6d_conv_tc) against torch fp64 CPU and against the FFMA
+"""The wgmma split-operand convolution (g6d_conv_tc) against torch fp64 CPU and against the FFMA
 path, for both operand kinds (G6D_TC_F16: fp16 hi + 2^11-scaled fp16 lo, the default; G6D_TC_TF32: tf32
 hi/lo): it must be fp32-faithful (error ~1e-6 relative; a single TF32 or fp16 product would be ~5e-4)."""
 import os
@@ -191,13 +191,13 @@ def test_tc_fused_output_statistics(ops, case):
     np.testing.assert_allclose(pb.cpu().numpy(), (-mean / torch.sqrt(var + 1e-5)).float().numpy(), rtol=1e-4, atol=2e-5)
 
 
-@pytest.mark.parametrize('B,hw,cin,cout', [(320, 8, 128, 128),    # 160 tiles on 148 CTAs
+@pytest.mark.parametrize('B,hw,cin,cout', [(320, 8, 128, 128),    # 160 tiles on the persistent grid
                                            (320, 4, 256, 256),    # 80 tiles
                                            (150, 8, 128, 192),    # 75 x 2 tiles, the second N tile half empty
                                            (80, 4, 256, 256),     # 20 tiles -> uniform split-K
                                            (1, 8, 512, 512)])     # one M tile, four N tiles (uniform split-K)
 def test_tc_tile_counts_that_do_not_divide_the_grid(ops, B, hw, cin, cout):
-    """Persistent kernel with tile counts that do not divide over its 148 CTAs (a partial last round, or a short
+    """Persistent kernel with tile counts that do not divide over its persistent CTAs (a partial last round, or a short
     grid with uniform split-K + the reduce kernel), InstanceNorm prologue and fused output moments: fp32-faithful
     and bit-reproducible."""
     x = torch.randn(B, cin, hw, hw, generator=g(70)) * 2 + 1

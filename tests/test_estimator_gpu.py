@@ -1,4 +1,4 @@
-"""End-to-end: Gen6DEstimator.build + predict on the B200 networks vs the golden run of the
+"""End-to-end: Gen6DEstimator.build + predict on the H100 networks vs the golden run of the
 unmodified reference estimator (CPU) on the same synthetic database and seeded checkpoints."""
 import os
 

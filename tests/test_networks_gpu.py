@@ -90,8 +90,8 @@ def test_detector_maps_argmax_positions(det):
 
 def test_detector_tcgen05_correlation_480x640_32refs():
     """BASELINE configs[1], detector half, at full size: 480x640 frame x 32 reference views.  With
-    rfn >= 16 the sliding inner product of detector.py:222-224 runs on the tcgen05 kernel (refs as the
-    K-major B operand, K = 15*15*512 split into <= 2048-term chains); its raw output per scale and
+    rfn >= 16 the sliding inner product of detector.py:222-224 runs on the tensor-core kernel (refs as the
+    K-major B operand, split into short accumulate chains); its raw output per scale and
     level, the final argmax and the decoded position are pinned to the golden run of the unmodified
     reference (tests/golden/make_golden_det32.py)."""
     from gen6d_b200 import ops

@@ -1,4 +1,4 @@
-"""Time one conv shape across M for the tcgen05 kernels (G6D_CONV_TC_V=1|2 chooses v1/v2)."""
+"""Time one conv shape across M for the tensor-core kernels (G6D_CONV_TC_V=1|2 chooses v1/v2)."""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from gen6d_b200 import ops

@@ -1,4 +1,4 @@
-"""Detector correlation shapes (refs as kernels, Cout = 32): default tcgen05 kernel vs the A-reuse
+"""Detector correlation shapes (refs as kernels, Cout = 32): default tensor-core kernel vs the A-reuse
 ROW mode (G6D_CONV_FLAT=2).  Spawns one process per setting (the switch is read once per process)."""
 import os, subprocess, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,5 +1,5 @@
 """Aggregate an `ncu --metrics gpu__time_duration.sum --csv` launch list by kernel (markdown table):
-    python tools/launch_summary.py profiles/launches_r02.csv [top_n]"""
+    python tools/launch_summary.py launches.csv [top_n]"""
 import collections
 import csv
 import sys
