@@ -19,16 +19,24 @@
 //                VGG feature, all O(1e-3 .. 1e3).  G6D_CONV_KIND=tf32 selects the wide-range kind.
 //
 // GEMM view (same as conv_ffma.cu): M = B*Do*Ho*Wo, N = Cout, K = taps*Cin, channels-last.
-// One CTA computes 64 x BLOCK_N output tiles (wgmma M = 64, accumulators in registers).  12 warps:
+// One CTA computes 128 x BLOCK_N output tiles, 64 rows per consumer warpgroup (wgmma M = 64,
+// accumulators in registers).  16 warps:
 //   warps 0-7   A producers: gather the im2col rows of the K-block from global memory (coalesced
-//               128-bit loads, register prefetch ring), apply the folded InstanceNorm(+ReLU) /
-//               selector q(.)ref prologue to in-bounds elements, split into hi/lo and st.shared both
-//               tiles in the canonical K-major SWIZZLE_128B layout the wgmma descriptor expects;
-//   warps 8-11  the consumer warpgroup: 12 wgmmas per K-block (4 K-steps x 3 split terms), one
-//               group in flight while the next stage is awaited, then the epilogue (bias / activation
-//               -> global, or split-K partials) straight from the accumulator registers.  Its first
-//               thread also streams the pre-split weight tiles W_hi / W_lo [Cout, K] (K-major) by TMA
-//               (cp.async.bulk.tensor.2d, 128B swizzle) into the stages it frees.
+//               128-bit loads, register prefetch ring; 16 rows per warp), apply the folded
+//               InstanceNorm(+ReLU) / selector q(.)ref prologue to in-bounds elements, split into hi/lo
+//               and st.shared both tiles in the canonical K-major SWIZZLE_128B layout the wgmma
+//               descriptor expects;
+//   warps 8-15  two consumer warpgroups, rows 0-63 and 64-127 of the tile, both reading the same
+//               weight tiles of a stage: 12 wgmmas per K-block each (4 K-steps x 3 split terms),
+//               one group in flight while the next stage is awaited, then the
+//               epilogue (bias / activation -> global, or split-K partials) straight from the
+//               accumulator registers.  The first consumer thread also streams the pre-split weight
+//               tiles W_hi / W_lo [Cout, K] (K-major) by TMA (cp.async.bulk.tensor.2d, 128B swizzle)
+//               into the stages the consumers free.
+// A consumer's accumulators alone take 128 registers, the launch bound of 512 threads allows 128 per
+// thread: the producer warpgroups give registers up (setmaxnreg.dec to TC_PRODUCER_REGS) and the
+// consumer warpgroups take them (setmaxnreg.inc to TC_CONSUMER_REGS); ptxas allocates the code after
+// each setmaxnreg within its new count.
 // conv_tc2_kernel handles general strides / shapes (persistent); conv_tcflat_kernel (stride-1
 // multi-tap convolutions whose halo fits in shared memory) reuses the A operand across taps, see below.
 #include <stdlib.h>
@@ -40,26 +48,33 @@
 
 namespace g6d {
 
-constexpr int TC_BM = 64;                                  // rows per tile (wgmma M)
+constexpr int TC_BM = 128;                                 // rows per tile: 64 (wgmma M) per consumer warpgroup
 constexpr int TC_PRODUCER_WARPS = 8;
-constexpr int TC_THREADS = (TC_PRODUCER_WARPS + 4) * 32;   // producers + one consumer warpgroup
+constexpr int TC_CONSUMER_WARPS = 8;                       // two warpgroups
+constexpr int TC_THREADS = (TC_PRODUCER_WARPS + TC_CONSUMER_WARPS) * 32;
 constexpr int TC_ISSUER = TC_PRODUCER_WARPS * 32;          // consumer thread that also issues the weight TMA
+constexpr int TC_PRODUCER_REGS = 96, TC_CONSUMER_REGS = 160;
+static_assert(TC_PRODUCER_WARPS * TC_PRODUCER_REGS + TC_CONSUMER_WARPS * TC_CONSUMER_REGS <= 65536 / 32, "register file of one SM");
+static_assert(TC_BM == 64 * (TC_CONSUMER_WARPS / 4), "one 64-row wgmma tile per consumer warpgroup");
 constexpr int TC_MAX_K_PER_CHAIN = 2048;                   // longest accumulate chain per CTA (see fill_tc_params)
 
 template <int KIND> struct KindCfg;
 template <> struct KindCfg<G6D_TC_TF32> {
     static constexpr int BK = 32;          // K elements per 128-byte swizzle row
     static constexpr int NV = 1;           // float4 loads per (thread, row) chunk of 16 smem bytes
-    static constexpr int RING = 3;         // register prefetch ring (K-blocks)
     static constexpr float CROSS = 1.f;    // scale of the cross-term accumulator
 };
 template <> struct KindCfg<G6D_TC_F16> {
     static constexpr int BK = 64;
     static constexpr int NV = 2;
-    static constexpr int RING = 2;
     static constexpr float CROSS = 1.f / 2048.f;
 };
 constexpr float F16_LO_SCALE = 2048.f;
+// The producers' register prefetch ring holds one float4 column (ROWS rows x 16 bytes of fp32 input) per
+// slot, i.e. a K-block of fp32 or half a K-block of fp16 operands; RING - 1 slots are in flight while one
+// is transformed and stored.  The persistent kernel's producers also keep per-row coordinates, so within
+// TC_PRODUCER_REGS they hold two slots (16 KB in flight per SM) and the A-reuse kernel's three (32 KB).
+constexpr int TC2_RING = 2, FLAT_RING = 3;
 // K order inside a 64-element fp16 K-block.  A producer thread fills one 16-byte shared-memory chunk
 // (8 halves) of a tile row from two 128-bit global loads; to keep BOTH loads of a warp fully coalesced
 // (8 lanes x 16 B = one 128-byte line per row) lane c reads channels [4c, 4c+4) and [32+4c, 32+4c+4), so
@@ -106,22 +121,24 @@ __device__ __forceinline__ void split_tf32x4(const float4 v, float4& hi, float4&
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
     asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
-// one 16-byte chunk of a tile row: NV float4 of fp32 input -> hi and lo tiles
+__device__ __forceinline__ void st_shared_v2(uint32_t addr, uint32_t a, uint32_t b) {
+    asm volatile("st.shared.v2.b32 [%0], {%1,%2};" ::"r"(addr), "r"(a), "r"(b) : "memory");
+}
+// float4 e (< NV) of the 16-byte chunk of a tile row: fp32 input -> hi and lo tiles (all 16 bytes for tf32,
+// bytes [8e, 8e + 8) for fp16)
 template <int KIND>
-__device__ __forceinline__ void split_store(uint32_t hi_addr, uint32_t lo_addr, const float4 (&v)[KindCfg<KIND>::NV]) {
+__device__ __forceinline__ void split_store(uint32_t hi_addr, uint32_t lo_addr, const float4 v, int e) {
     if constexpr (KIND == G6D_TC_TF32) {
         float4 hi, lo;
-        split_tf32x4(v[0], hi, lo);
+        split_tf32x4(v, hi, lo);
         st_shared_v4(hi_addr, __float_as_uint(hi.x), __float_as_uint(hi.y), __float_as_uint(hi.z), __float_as_uint(hi.w));
         st_shared_v4(lo_addr, __float_as_uint(lo.x), __float_as_uint(lo.y), __float_as_uint(lo.z), __float_as_uint(lo.w));
     } else {
-        uint32_t h[4], l[4];
-        split_f16x2(v[0].x, v[0].y, h[0], l[0]);
-        split_f16x2(v[0].z, v[0].w, h[1], l[1]);
-        split_f16x2(v[1].x, v[1].y, h[2], l[2]);
-        split_f16x2(v[1].z, v[1].w, h[3], l[3]);
-        st_shared_v4(hi_addr, h[0], h[1], h[2], h[3]);
-        st_shared_v4(lo_addr, l[0], l[1], l[2], l[3]);
+        uint32_t h[2], l[2];
+        split_f16x2(v.x, v.y, h[0], l[0]);
+        split_f16x2(v.z, v.w, h[1], l[1]);
+        st_shared_v2(hi_addr + 8 * e, h[0], h[1]);
+        st_shared_v2(lo_addr + 8 * e, l[0], l[1]);
     }
 }
 __device__ __forceinline__ float4 affine4(float4 x, const float4 sc, const float4 sh, bool relu) {
@@ -131,31 +148,46 @@ __device__ __forceinline__ float4 affine4(float4 x, const float4 sc, const float
 }
 
 // ------------------------------------------------------------------------------------------ MMA
-// One consumer warpgroup owns a 64 x BN output tile with every accumulator in registers: NMAIN
-// round-robin chains for the main (hi*hi) term and one for the two cross terms, BN / 2 registers each
-// (128 per thread for every BN).  Each tensor-core accumulate truncates to fp32; spreading the K-blocks
-// over several shorter, smaller-magnitude chains (summed in fp32 round-to-nearest by the epilogue)
-// divides the resulting bias on same-sign data by ~NMAIN at no cost.
+// Each consumer warpgroup owns 64 rows x BN columns of the tile with every accumulator in registers:
+// NMAIN round-robin chains for the main (hi*hi) term and one for the two cross terms, BN / 2 registers
+// each (128 per thread for every BN).  Each tensor-core accumulate truncates to fp32; spreading the
+// K-blocks over several shorter, smaller-magnitude chains (summed in fp32 round-to-nearest by the
+// epilogue) divides the resulting bias on same-sign data by ~NMAIN at no cost.  The accumulators are
+// zeroed in registers at the start of a tile and every wgmma accumulates.
 template <int BN> struct AccCfg {
     static constexpr int NMAIN = BN == 32 ? 7 : (BN == 64 ? 3 : 1);
     static constexpr int R = BN / 2;
 };
 
-// The 4 K steps x 3 split terms of one stage into the main accumulator `main` and the cross accumulator,
-// committed as one wgmma group; first_* start a chain.  The callers unroll their K-block loop by NMAIN so
-// that `main` is a compile-time register array (a runtime choice makes ptxas serialize the wgmmas).
+template <int BN, int NMAIN>
+__device__ __forceinline__ void zero_acc(float (&acc)[NMAIN][BN / 2], float (&cross)[BN / 2]) {
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) {
+        cross[j] = 0.f;
+#pragma unroll
+        for (int a = 0; a < NMAIN; ++a) acc[a][j] = 0.f;
+    }
+}
+
+// The 4 K steps x 3 split terms of one stage of a warpgroup's 64 rows into the main accumulator `main`
+// and the cross accumulator, committed as one wgmma group.  The callers unroll their K-block loop by
+// NMAIN so that `main` is a compile-time register array (a runtime choice makes ptxas serialize the
+// wgmmas).  A_hi*B_hi and A_hi*B_lo are not merged into one wgmma of width 2 BN over the adjacent B
+// tiles: its accumulator registers would have to be `main` followed by `cross`, which ptxas cannot
+// arrange for NMAIN > 1 main chains, and for BN = 128 ptxas rejects the n256 instruction under the
+// 128-register launch budget (it checks the instruction against that count, not the setmaxnreg one).
 template <int BN, int KIND>
 __device__ __forceinline__ void mma_stage(float (&main)[BN / 2], float (&cross)[BN / 2], uint32_t a_hi, uint32_t a_lo,
-                                          uint32_t b_hi, uint32_t b_lo, bool first_cross, bool first_main) {
+                                          uint32_t b_hi, uint32_t b_lo) {
     const uint64_t dah = gmma_desc_sw128(a_hi), dal = gmma_desc_sw128(a_lo);
     const uint64_t dbh = gmma_desc_sw128(b_hi), dbl = gmma_desc_sw128(b_lo);
     wgmma_fence();
 #pragma unroll
     for (int ks = 0; ks < 4; ++ks) {             // 4 x 32 bytes of K per 128-byte row
         const uint64_t adv = (uint64_t)((ks * 32) >> 4);
-        wgmma<BN, KIND>(cross, dal + adv, dbh + adv, (!first_cross || ks > 0) ? 1u : 0u);
+        wgmma<BN, KIND>(cross, dal + adv, dbh + adv, 1u);
         wgmma<BN, KIND>(cross, dah + adv, dbl + adv, 1u);
-        wgmma<BN, KIND>(main, dah + adv, dbh + adv, (!first_main || ks > 0) ? 1u : 0u);
+        wgmma<BN, KIND>(main, dah + adv, dbh + adv, 1u);
     }
     wgmma_commit();
 }
@@ -231,11 +263,12 @@ __device__ __forceinline__ void epilogue_tile(float (&acc)[AccCfg<BN>::NMAIN][BN
 // conv_tc2_kernel: persistent implicit-GEMM convolution.
 //   * one CTA per SM loops over (M tile, N tile, K split) work items, so there is no wave tail and
 //     the per-CTA set-up (barrier init, descriptor prefetch) is paid once;
-//   * eight producer warps keep a register prefetch ring (global loads of the next K-block(s) in
+//   * the eight producer warps keep a register prefetch ring (global loads of the next K-block(s) in
 //     flight while K-block it is transformed and stored) and never drain the smem ring between tiles
 //     (one global K-block counter), so they fill the next tile's stages during the epilogue;
-//   * one consumer warpgroup issues the wgmmas of a stage, keeps one stage's group in flight while it
-//     waits for the next, releases each stage once its group has completed and runs the epilogue;
+//   * each of the two consumer warpgroups issues the wgmmas of its 64 rows of a stage, keeps one
+//     stage's group in flight while it waits for the next, releases each stage once its group has
+//     completed (a stage is free when all 8 consumer warps have released it) and runs the epilogue;
 //   * one consumer thread streams the weight tiles by TMA, STAGES K-blocks ahead of the MMAs.
 constexpr int TC2_PF_BYTES = 12 * 128;      // weight-tile L2 prefetch distance, in bytes of K per row
 
@@ -261,7 +294,7 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
     constexpr int BK = KC::BK, NV = KC::NV;
     constexpr int RSTEP = NPW * 4;                       // rows r0 + RSTEP*j
     constexpr int ROWS = TC_BM / RSTEP;                  // tile rows per producer thread
-    constexpr int RING = KC::RING;                       // register prefetch ring (K-blocks); RING-1 in flight
+    constexpr int RING = TC2_RING;                       // register prefetch ring (float4 columns); RING-1 in flight
     constexpr int PF = TC2_PF_BYTES / 128;               // K-blocks
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -279,7 +312,7 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(full_a(s), NPW);        // the producer warps
             mbar_init(full_b(s), 1);          // the TMA transaction
-            mbar_init(empty(s), 4);           // the consumer warps
+            mbar_init(empty(s), TC_CONSUMER_WARPS);
         }
         fence_barrier_init();
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_hi) : "memory");
@@ -296,6 +329,7 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
     auto kblocks_of = [&](int sp) { return min(p.kblocks, sp * p.kb_per_split + p.kb_per_split) - sp * p.kb_per_split; };
 
     if (warp < NPW) {
+        setmaxnreg_dec<TC_PRODUCER_REGS>();
         // =============================== A producers ===============================
         // All producer warps fill every K-block: ROWS rows x one 16-byte smem chunk (4 or 8 channels) per thread.
         const int chunk = threadIdx.x & 7;
@@ -332,31 +366,30 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
                 if (p.K != p.Cin) { tap = k / p.Cin; c0 = k - tap * p.Cin; }
                 kx = tap % p.kw; const int tq = tap / p.kw; ky = tq % p.kh; kz = tq / p.kh;
             }
-            // prefetch ring: slot q holds K-block (it % RING == q)
-            float4 v[RING][ROWS][NV];
+            // prefetch ring: slot q holds float4 column e = u % NV of K-block u / NV, u % RING == q
+            float4 v[RING][ROWS];
             unsigned okm[RING]; int kc[RING]; int ksp[RING];
-            auto issue_loads = [&](int q) {
+            auto issue_loads = [&](int q, int e) {
                 const int tap_sp = (kz * p.H + ky) * p.W + kx;
-                okm[q] = 0; kc[q] = c0 + cofs; ksp[q] = tap_sp;
-                const float* xb = p.x + p.ico + cofs + c0;
+                okm[q] = 0; kc[q] = c0 + cofs + 32 * e; ksp[q] = tap_sp;
+                const float* xb = p.x + p.ico + kc[q];
 #pragma unroll
                 for (int j = 0; j < ROWS; ++j) {
                     const int z = ((rc[j] >> 24) & 0xff) - 8 + kz, y = ((rc[j] >> 12) & 0xfff) - 8 + ky, x = (rc[j] & 0xfff) - 8 + kx;
                     const bool inb = ((rvmask >> j) & 1u) && (unsigned)z < (unsigned)p.D && (unsigned)y < (unsigned)p.H &&
                                      (unsigned)x < (unsigned)p.W;
-#pragma unroll
-                    for (int e = 0; e < NV; ++e) v[q][j][e] = make_float4(0.f, 0.f, 0.f, 0.f);
+                    v[q][j] = make_float4(0.f, 0.f, 0.f, 0.f);
                     if (inb) {
-                        const float4* src = reinterpret_cast<const float4*>(xb + ((long long)rb[j] * plane_sz + rsp[j] + tap_sp) * p.ics);
-#pragma unroll
-                        for (int e = 0; e < NV; ++e) v[q][j][e] = __ldg(src + e * 8);
+                        v[q][j] = __ldg(reinterpret_cast<const float4*>(xb + ((long long)rb[j] * plane_sz + rsp[j] + tap_sp) * p.ics));
                         okm[q] |= 1u << j;
                     }
                 }
-                c0 += BK;
-                if (c0 == p.Cin) { c0 = 0; if (++kx == p.kw) { kx = 0; if (++ky == p.kh) { ky = 0; ++kz; } } }
+                if (e == NV - 1) {
+                    c0 += BK;
+                    if (c0 == p.Cin) { c0 = 0; if (++kx == p.kw) { kx = 0; if (++ky == p.kh) { ky = 0; ++kz; } } }
+                }
             };
-            auto process = [&](int q, int it) {
+            auto process = [&](int q, int e, int it) {
                 const int g_it = git + it;
                 const int s = g_it % STAGES;
                 const uint32_t n_use = g_it / STAGES;
@@ -374,40 +407,45 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
                                 scp = reinterpret_cast<const float4*>(p.ps + g * p.Cin + kc[q]);
                                 shp = reinterpret_cast<const float4*>(p.pb + g * p.Cin + kc[q]);
                             }
-#pragma unroll
-                            for (int e = 0; e < NV; ++e) v[q][j][e] = affine4(v[q][j][e], __ldg(scp + e * 8), __ldg(shp + e * 8), relu);
+                            v[q][j] = affine4(v[q][j], __ldg(scp), __ldg(shp), relu);
                         }
                     }
                 }
-                mbar_wait(empty(s), (n_use & 1) ^ 1, 1, g_it);
+                if (e == 0) mbar_wait(empty(s), (n_use & 1) ^ 1, 1, g_it);
 #pragma unroll
                 for (int j = 0; j < ROWS; ++j) {
                     const int r = r0 + RSTEP * j;
                     const uint32_t so = r * 128 + ((chunk ^ (r & 7)) << 4);        // Swizzle<3,4,3>
-                    split_store<KIND>(a_hi(s) + so, a_lo(s) + so, v[q][j]);
+                    split_store<KIND>(a_hi(s) + so, a_lo(s) + so, v[q][j], e);
                 }
-                fence_proxy_async();          // generic-proxy smem writes -> visible to the tensor core (async proxy)
-                __syncwarp();
-                if (lane == 0) mbar_arrive(full_a(s));
+                if (e == NV - 1) {
+                    fence_proxy_async();      // generic-proxy smem writes -> visible to the tensor core (async proxy)
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(full_a(s));
+                }
             };
-            // software pipeline, unrolled by RING so the ring slots are compile-time register names
+            // software pipeline over the nkb * NV columns, unrolled by RING so that the ring slots are
+            // compile-time register names
+            const int ncol = nkb * NV;
 #pragma unroll
             for (int q = 0; q < RING - 1; ++q)
-                if (q < nkb) issue_loads(q);
-            for (int it = 0; it < nkb; it += RING) {
+                if (q < ncol) issue_loads(q, q % NV);
+            for (int u = 0; u < ncol; u += RING) {
 #pragma unroll
                 for (int q = 0; q < RING; ++q) {
-                    if (it + q < nkb) {
-                        if (it + q + RING - 1 < nkb) issue_loads((q + RING - 1) % RING);
-                        process(q, it + q);
+                    if (u + q < ncol) {
+                        if (u + q + RING - 1 < ncol) issue_loads((q + RING - 1) % RING, (u + q + RING - 1) % NV);
+                        process(q, (u + q) % NV, (u + q) / NV);
                     }
                 }
             }
             git += nkb;
         }
     } else {
-        // =============================== consumer warpgroup ===============================
-        const int cw = warp - NPW;                     // warp inside the warpgroup: rows 16 cw .. 16 cw + 15
+        // =============================== consumer warpgroups ===============================
+        setmaxnreg_inc<TC_CONSUMER_REGS>();
+        const int cw = warp - NPW;                     // consumer warp: rows 16 cw .. 16 cw + 15 of the tile
+        const uint32_t a_row = (cw >> 2) * 64 * 128;   // this warpgroup's 64 rows of the A tiles
         const bool issuer = threadIdx.x == TC_ISSUER;
         // weight-tile stream of the issuer: the next global K-block lg = K-block lit of work item lw
         int lw = blockIdx.x, lit = 0, lg = 0;
@@ -455,6 +493,7 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
             int mt, nt, sp;
             decode(w, mt, nt, sp);
             const int nkb = kblocks_of(sp);
+            zero_acc<BN, NMAIN>(acc, cross);
             for (int it0 = 0; it0 < nkb; it0 += NMAIN) {
 #pragma unroll
                 for (int a = 0; a < NMAIN; ++a) {              // K-block it uses main accumulator it % NMAIN
@@ -463,7 +502,7 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
                         const int s = g % STAGES;
                         mbar_wait(full_a(s), (g / STAGES) & 1, 4, g);
                         mbar_wait(full_b(s), (g / STAGES) & 1, 5, g);
-                        mma_stage<BN, KIND>(acc[a], cross, a_hi(s), a_lo(s), b_hi(s), b_lo(s), it == 0, it < NMAIN);
+                        mma_stage<BN, KIND>(acc[a], cross, a_hi(s) + a_row, a_lo(s) + a_row, b_hi(s), b_lo(s));
                         wgmma_wait<1>();
                         if (it > 0) release(g - 1);
                         ++g;
@@ -721,8 +760,8 @@ __global__ void pack_conv_weight_tc_kernel(const float* __restrict__ w, void* __
 //
 // The output positions of one image plane are enumerated over the PADDED width Wp = W + 2*pw:
 // f = y*Wp + x.  Tap (ky,kx) of output f reads padded-input position f + ky*Wp + kx, so for a
-// tile of 64 consecutive f the A operand of EVERY tap is a window of 64 consecutive rows of
-// one shared-memory buffer holding padded-input positions [f0, f0 + 63 + (kh-1)*Wp + kw-1]:
+// tile of 128 consecutive f the A operand of EVERY tap is a window of 128 consecutive rows of
+// one shared-memory buffer holding padded-input positions [f0, f0 + 127 + (kh-1)*Wp + kw-1]:
 // the tap is selected by the wgmma descriptor's start address (+shift*128 B; the 128B swizzle is a
 // function of the absolute smem address, checked by g6d_debug_desc_shift).  The producers
 // therefore gather (and prologue-transform, and hi/lo split) each input element ONCE per channel
@@ -789,9 +828,9 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
     if (threadIdx.x == TC_ISSUER) {
         for (int s = 0; s < 4; ++s) {
             mbar_init(a_full(s), TC_PRODUCER_WARPS);
-            mbar_init(a_empty(s), 4);             // the consumer warps
+            mbar_init(a_empty(s), TC_CONSUMER_WARPS);
             mbar_init(b_full(s), 1);
-            mbar_init(b_empty(s), 4);
+            mbar_init(b_empty(s), TC_CONSUMER_WARPS);
         }
         fence_barrier_init();
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_hi) : "memory");
@@ -800,6 +839,7 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
     __syncthreads();
 
     if (warp < TC_PRODUCER_WARPS) {
+        setmaxnreg_dec<TC_PRODUCER_REGS>();
         // =============================== A producers ===============================
         const int chunk = threadIdx.x & 7;
         const int cofs = chunk * 4;                             // channels [cofs, cofs+4) (+32 for the 2nd load), see f16_k_source
@@ -811,11 +851,13 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
         // the next NB-1 trips (possibly of the next unit: they only touch registers, so they do not wait for
         // the stage to be free) are in flight while a trip is transformed and stored.  Without it every trip
         // paid a full L2 round trip before its first st.shared.
-        constexpr int NB = 3;
+        // A slot holds one float4 column (e = tt % NV) of a trip, see FLAT_RING.
+        constexpr int NB = FLAT_RING;
         const int trips = (p.seg_rows + TC_BM - 1) / TC_BM;
-        const int total = nunits * trips;
-        float4 v[NB][ROWS][NV]; int off[NB][ROWS];
+        const int total = nunits * trips * NV;
+        float4 v[NB][ROWS]; int off[NB][ROWS];
         auto unit_of = [&](int tt, int& u, int& rbase, int& cb, int& kz, int& tb) {
+            tt /= NV;
             u = tt / trips; rbase = (tt - u * trips) * TC_BM;
             cb = cb_begin + u / p.nseg;
             const int seg = u % p.nseg;
@@ -823,33 +865,28 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
             kz = p.mode == 1 ? seg / p.kh : seg;
             tb = p.mode == 1 ? seg % p.kh : 0;
         };
-        auto issue = [&](int tt, int q) {
+        auto issue = [&](int tt, int q, int e) {
             int u, rbase, cb, kz, tb;
             unit_of(tt, u, rbase, cb, kz, tb);
             const int zz = zo + kz - p.pd;
             const bool zok = (unsigned)zz < (unsigned)p.D;
-            const float* xplane = p.x + ((long long)b * p.D + (zok ? zz : 0)) * plane * p.ics + p.ico + cb * BK + cofs;
+            const float* xplane = p.x + ((long long)b * p.D + (zok ? zz : 0)) * plane * p.ics + p.ico + cb * BK + cofs + 32 * e;
             const int* tab = rowtab + tb * p.seg_rows;
 #pragma unroll
             for (int j = 0; j < ROWS; ++j) {
                 const int r = rbase + r0 + RSTEP * j;
                 off[q][j] = (r < p.seg_rows && zok) ? tab[r] : -1;
-#pragma unroll
-                for (int e = 0; e < NV; ++e) v[q][j][e] = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (off[q][j] >= 0) {
-                    const float4* src = reinterpret_cast<const float4*>(xplane + (long long)off[q][j] * p.ics);
-#pragma unroll
-                    for (int e = 0; e < NV; ++e) v[q][j][e] = __ldg(src + e * 8);
-                }
+                v[q][j] = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (off[q][j] >= 0) v[q][j] = __ldg(reinterpret_cast<const float4*>(xplane + (long long)off[q][j] * p.ics));
             }
         };
-        auto store = [&](int tt, int q) {
+        auto store = [&](int tt, int q, int e) {
             int u, rbase, cb, kz, tb;
             unit_of(tt, u, rbase, cb, kz, tb);
             const int s = u % p.a_stages;
             const int zz = zo + kz - p.pd;
-            const int c = cb * BK + cofs;
-            if (rbase == 0) mbar_wait(a_empty(s), ((u / p.a_stages) & 1) ^ 1, 1, u);
+            const int c = cb * BK + cofs + 32 * e;
+            if (rbase == 0 && e == 0) mbar_wait(a_empty(s), ((u / p.a_stages) & 1) ^ 1, 1, u);
 #pragma unroll
             for (int j = 0; j < ROWS; ++j) {
                 const int r = rbase + r0 + RSTEP * j;
@@ -864,13 +901,12 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
                         scp = reinterpret_cast<const float4*>(p.ps + gi * p.Cin + c);
                         shp = reinterpret_cast<const float4*>(p.pb + gi * p.Cin + c);
                     }
-#pragma unroll
-                    for (int e = 0; e < NV; ++e) v[q][j][e] = affine4(v[q][j][e], __ldg(scp + e * 8), __ldg(shp + e * 8), relu);
+                    v[q][j] = affine4(v[q][j], __ldg(scp), __ldg(shp), relu);
                 }
                 const uint32_t so = r * 128 + ((chunk ^ (r & 7)) << 4);
-                split_store<KIND>(a_hi(s) + so, a_lo(s) + so, v[q][j]);
+                split_store<KIND>(a_hi(s) + so, a_lo(s) + so, v[q][j], e);
             }
-            if (rbase + TC_BM >= p.seg_rows) {          // last trip of the unit: publish the stage
+            if (rbase + TC_BM >= p.seg_rows && e == NV - 1) {     // last column of the unit: publish the stage
                 fence_proxy_async();
                 __syncwarp();
                 if (lane == 0) mbar_arrive(a_full(s));
@@ -878,19 +914,21 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
         };
 #pragma unroll
         for (int q = 0; q < NB - 1; ++q)
-            if (q < total) issue(q, q);
+            if (q < total) issue(q, q, q % NV);
         for (int tt = 0; tt < total; tt += NB) {
 #pragma unroll
             for (int q = 0; q < NB; ++q) {
                 if (tt + q < total) {
-                    if (tt + q + NB - 1 < total) issue(tt + q + NB - 1, (q + NB - 1) % NB);
-                    store(tt + q, q);
+                    if (tt + q + NB - 1 < total) issue(tt + q + NB - 1, (q + NB - 1) % NB, (tt + q + NB - 1) % NV);
+                    store(tt + q, q, (tt + q) % NV);
                 }
             }
         }
     } else {
-        // =============================== consumer warpgroup ===============================
+        // =============================== consumer warpgroups ===============================
+        setmaxnreg_inc<TC_CONSUMER_REGS>();
         const int cw = warp - TC_PRODUCER_WARPS;
+        const uint32_t a_row = (cw >> 2) * 64 * 128;   // this warpgroup's 64 rows of the A window
         const bool issuer = threadIdx.x == TC_ISSUER;
         const int taps = p.taps_per_seg;
         const int nb_total = nunits * taps;
@@ -921,6 +959,7 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
 
         float acc[NMAIN][BN / 2];
         float cross[BN / 2];
+        zero_acc<BN, NMAIN>(acc, cross);
         // B block bi = (unit u, tap t) = (bi / taps, bi % taps) uses main accumulator bi % NMAIN
         for (int b0 = 0; b0 < nb_total; b0 += NMAIN) {
 #pragma unroll
@@ -932,8 +971,8 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
                     if (t == 0) mbar_wait(a_full(sa), (u / p.a_stages) & 1, 4, u);
                     mbar_wait(b_full(sb), (bi / p.b_stages) & 1, 5, bi);
                     const int shift = p.mode == 1 ? t : (t / p.kw) * p.Wp + (t % p.kw);     // rows
-                    mma_stage<BN, KIND>(acc[a], cross, a_hi(sa) + shift * 128, a_lo(sa) + shift * 128, b_hi(sb), b_lo(sb),
-                                        bi == 0, bi < NMAIN);
+                    mma_stage<BN, KIND>(acc[a], cross, a_hi(sa) + shift * 128 + a_row, a_lo(sa) + shift * 128 + a_row, b_hi(sb),
+                                        b_lo(sb));
                     wgmma_wait<1>();
                     if (bi > 0) release(bi - 1);
                 }

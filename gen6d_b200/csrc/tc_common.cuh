@@ -134,6 +134,11 @@ template <> __device__ __forceinline__ void wgmma<128, G6D_TC_F16>(float (&d)[64
         : "l"(da), "l"(db), "r"(acc) : "memory");
 }
 
+// Warpgroup-wide register re-allocation: every warp of the warpgroup executes it with the same count.
+// ptxas allocates the code after it within the new count.
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
 __device__ __forceinline__ float to_tf32(float v) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
