@@ -39,9 +39,6 @@
 // each setmaxnreg within its new count.
 // conv_tc2_kernel handles general strides / shapes (persistent); conv_tcflat_kernel (stride-1
 // multi-tap convolutions whose halo fits in shared memory) reuses the A operand across taps, see below.
-#include <stdlib.h>
-#include <string.h>
-
 #include <cuda_fp16.h>
 
 #include "tc_common.cuh"
@@ -627,6 +624,7 @@ static int make_weight_map(CUtensorMap* map, const void* w, int rows, int K, int
 }
 
 static int tc_block_n(int Cout) { return Cout > 64 ? 128 : (Cout > 32 ? 64 : 32); }
+static int tc_nmain(int bn) { return bn == 32 ? AccCfg<32>::NMAIN : (bn == 64 ? AccCfg<64>::NMAIN : AccCfg<128>::NMAIN); }
 
 // the persistent kernel packs (z, y, x) + 8 into 8/12/12 bits and uses 32-bit spatial offsets and group indices
 static bool tc2_dims_ok(const g6d_conv_desc* d) {
@@ -637,7 +635,8 @@ static bool tc2_dims_ok(const g6d_conv_desc* d) {
 static int fill_tc_params(const g6d_conv_desc* d, int kind, ConvTcP& p) {
     G6D_REQUIRE(d != nullptr, "g6d_conv_tc: null desc");
     G6D_REQUIRE(kind == G6D_TC_TF32 || kind == G6D_TC_F16, "g6d_conv_tc: bad operand kind %d", kind);
-    G6D_REQUIRE(d->B > 0 && d->D > 0 && d->H > 0 && d->W > 0 && d->Cin > 0 && d->Cout > 0, "g6d_conv_tc: bad dims");
+    G6D_REQUIRE(d->B > 0 && d->D > 0 && d->H > 0 && d->W > 0 && d->Cin > 0, "g6d_conv_tc: bad dims");
+    G6D_REQUIRE(d->Cout >= 16, "g6d_conv_tc: Cout (%d) must be at least 16", d->Cout);
     G6D_REQUIRE(d->kd > 0 && d->kh > 0 && d->kw > 0 && d->stride > 0, "g6d_conv_tc: bad kernel/stride");
     const int bk = kind_bk(kind);
     G6D_REQUIRE((d->Cin % bk) == 0, "g6d_conv_tc: Cin (%d) must be a multiple of %d", d->Cin, bk);
@@ -648,7 +647,7 @@ static int fill_tc_params(const g6d_conv_desc* d, int kind, ConvTcP& p) {
     const int Do = (d->D + 2 * d->pd - d->kd) / d->stride + 1;
     const int Ho = (d->H + 2 * d->ph - d->kh) / d->stride + 1;
     const int Wo = (d->W + 2 * d->pw - d->kw) / d->stride + 1;
-    G6D_REQUIRE(Do == d->Do && Ho == d->Ho && Wo == d->Wo, "g6d_conv_tc: output dims mismatch");
+    G6D_REQUIRE(Do > 0 && Ho > 0 && Wo > 0 && Do == d->Do && Ho == d->Ho && Wo == d->Wo, "g6d_conv_tc: output dims mismatch");
     G6D_REQUIRE(d->prologue >= 0 && d->prologue <= 3 && d->act >= 0 && d->act <= 2, "g6d_conv_tc: bad prologue/act");
     const long long M = (long long)d->B * Do * Ho * Wo;
     const long long K = (long long)d->kd * d->kh * d->kw * d->Cin;
@@ -676,7 +675,7 @@ static int fill_tc_params(const g6d_conv_desc* d, int kind, ConvTcP& p) {
     // detection time, see DESIGN.md section 3).  For K > 2048 the chain per accumulator is bounded to
     // 2048 terms and the partials are summed in fp32 round-to-nearest.
     // d->max_chain_k bounds the K-elements per ACCUMULATOR; a split rotates over NMAIN of them
-    const int nmain = bn == 32 ? AccCfg<32>::NMAIN : (bn == 64 ? AccCfg<64>::NMAIN : AccCfg<128>::NMAIN);
+    const int nmain = tc_nmain(bn);
     const int chain = d->max_chain_k > 0 ? d->max_chain_k * nmain : (K > TC_MAX_K_PER_CHAIN ? TC_MAX_K_PER_CHAIN * nmain : 0);
     const int max_kb = chain > bk ? chain / bk : 1;
     const int min_splits = chain > 0 ? (p.kblocks + max_kb - 1) / max_kb : 1;
@@ -765,16 +764,14 @@ __global__ void pack_conv_weight_tc_kernel(const float* __restrict__ w, void* __
 // the tap is selected by the wgmma descriptor's start address (+shift*128 B; the 128B swizzle is a
 // function of the absolute smem address, checked by g6d_debug_desc_shift).  The producers
 // therefore gather (and prologue-transform, and hi/lo split) each input element ONCE per channel
-// block instead of once per tap: 9x less producer work / L2 traffic for 3x3 ("FLAT" mode).  When
-// the halo (kh-1)*Wp does not fit in shared memory (wide images, 15x15 correlation kernels) the
-// buffer holds one kernel row at a time ("ROW" mode: kw-fold reuse).  Columns x >= Wo of the
-// padded enumeration are computed and dropped.  B tiles stream by TMA per (channel block, tap),
-// issued by one consumer thread b_stages blocks ahead of the MMAs.
+// block instead of once per tap: 9x less producer work / L2 traffic for 3x3.  Columns x >= Wo of the
+// padded enumeration are computed and dropped.  A unit is one (channel block, kz) pair; B tiles stream
+// by TMA per (unit, tap), issued by one consumer thread b_stages blocks ahead of the MMAs.
 struct ConvFlatP {
     const float* x; const float* bias; const float* ps; const float* pb; float* y; float* ws;
     int B, D, H, W, Cin, ics, ico, Cout, kd, kh, kw, pd, ph, pw, Do, Ho, Wo, ocs, oco, pro, act;
     long long group_rows;
-    int Wp, tiles_per_plane, mode, nseg, taps_per_seg, seg_rows, rows_pad, ntab, cblocks;
+    int Wp, tiles_per_plane, seg_rows, rows_pad, cblocks;
     int a_stages, b_stages, splits, cb_per_split, M;
     double* stats; long long stats_rows;
 };
@@ -804,7 +801,7 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
     auto b_full = [&](int s) { return bar_base + 8 * (8 + s); };
     auto b_empty = [&](int s) { return bar_base + 8 * (12 + s); };
     const uint32_t bar_off = (bar_base - base);
-    int* rowtab = reinterpret_cast<int*>(base_ptr + bar_off + 256);   // [ntab][seg_rows]
+    int* rowtab = reinterpret_cast<int*>(base_ptr + bar_off + 256);   // [seg_rows]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     int tile = blockIdx.x;
@@ -816,14 +813,13 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
     const int split = blockIdx.z;
     const int cb_begin = split * p.cb_per_split;
     const int cb_end = min(p.cblocks, cb_begin + p.cb_per_split);
-    const int nunits = (cb_end - cb_begin) * p.nseg;
+    const int nunits = (cb_end - cb_begin) * p.kd;
 
-    // ---- setup: row tables (element offset of each gathered row inside its image plane, -1 = zero)
-    for (int e = threadIdx.x; e < p.ntab * p.seg_rows; e += blockDim.x) {
-        const int tb = e / p.seg_rows, i = e % p.seg_rows;
-        const int g = f0 + (p.mode == 1 ? tb * p.Wp : 0) + i;     // padded-input flat position
+    // ---- setup: row table (element offset of each gathered row inside its image plane, -1 = zero)
+    for (int i = threadIdx.x; i < p.seg_rows; i += blockDim.x) {
+        const int g = f0 + i;                                     // padded-input flat position
         const int yy = g / p.Wp - p.ph, xx = g % p.Wp - p.pw;
-        rowtab[e] = ((unsigned)yy < (unsigned)p.H && (unsigned)xx < (unsigned)p.W) ? yy * p.W + xx : -1;
+        rowtab[i] = ((unsigned)yy < (unsigned)p.H && (unsigned)xx < (unsigned)p.W) ? yy * p.W + xx : -1;
     }
     if (threadIdx.x == TC_ISSUER) {
         for (int s = 0; s < 4; ++s) {
@@ -856,33 +852,29 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
         const int trips = (p.seg_rows + TC_BM - 1) / TC_BM;
         const int total = nunits * trips * NV;
         float4 v[NB][ROWS]; int off[NB][ROWS];
-        auto unit_of = [&](int tt, int& u, int& rbase, int& cb, int& kz, int& tb) {
+        auto unit_of = [&](int tt, int& u, int& rbase, int& cb, int& kz) {
             tt /= NV;
             u = tt / trips; rbase = (tt - u * trips) * TC_BM;
-            cb = cb_begin + u / p.nseg;
-            const int seg = u % p.nseg;
-            // FLAT: seg = kz, table 0.  ROW: seg = kz*kh + ky, table ky.
-            kz = p.mode == 1 ? seg / p.kh : seg;
-            tb = p.mode == 1 ? seg % p.kh : 0;
+            cb = cb_begin + u / p.kd;
+            kz = u % p.kd;
         };
         auto issue = [&](int tt, int q, int e) {
-            int u, rbase, cb, kz, tb;
-            unit_of(tt, u, rbase, cb, kz, tb);
+            int u, rbase, cb, kz;
+            unit_of(tt, u, rbase, cb, kz);
             const int zz = zo + kz - p.pd;
             const bool zok = (unsigned)zz < (unsigned)p.D;
             const float* xplane = p.x + ((long long)b * p.D + (zok ? zz : 0)) * plane * p.ics + p.ico + cb * BK + cofs + 32 * e;
-            const int* tab = rowtab + tb * p.seg_rows;
 #pragma unroll
             for (int j = 0; j < ROWS; ++j) {
                 const int r = rbase + r0 + RSTEP * j;
-                off[q][j] = (r < p.seg_rows && zok) ? tab[r] : -1;
+                off[q][j] = (r < p.seg_rows && zok) ? rowtab[r] : -1;
                 v[q][j] = make_float4(0.f, 0.f, 0.f, 0.f);
                 if (off[q][j] >= 0) v[q][j] = __ldg(reinterpret_cast<const float4*>(xplane + (long long)off[q][j] * p.ics));
             }
         };
         auto store = [&](int tt, int q, int e) {
-            int u, rbase, cb, kz, tb;
-            unit_of(tt, u, rbase, cb, kz, tb);
+            int u, rbase, cb, kz;
+            unit_of(tt, u, rbase, cb, kz);
             const int s = u % p.a_stages;
             const int zz = zo + kz - p.pd;
             const int c = cb * BK + cofs + 32 * e;
@@ -930,17 +922,17 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
         const int cw = warp - TC_PRODUCER_WARPS;
         const uint32_t a_row = (cw >> 2) * 64 * 128;   // this warpgroup's 64 rows of the A window
         const bool issuer = threadIdx.x == TC_ISSUER;
-        const int taps = p.taps_per_seg;
+        const int taps = p.kh * p.kw;
         const int nb_total = nunits * taps;
         int lb = 0;                                    // next B block the issuer loads
         auto load_b = [&]() {
             if (lb >= nb_total) return;
             const int u = lb / taps, t = lb % taps;
-            const int cb = cb_begin + u / p.nseg, seg = u % p.nseg;
+            const int cb = cb_begin + u / p.kd, kz = u % p.kd;
             const int s = lb % p.b_stages;
             mbar_wait(b_empty(s), ((lb / p.b_stages) & 1) ^ 1, 3, lb);
             mbar_expect_tx(b_full(s), 2 * B_BYTES);
-            const int k = (seg * taps + t) * p.Cin + cb * BK;
+            const int k = (kz * taps + t) * p.Cin + cb * BK;
             tma_load_2d(b_hi(s), &map_hi, b_full(s), k, n_base);
             tma_load_2d(b_lo(s), &map_lo, b_full(s), k, n_base);
             ++lb;
@@ -970,7 +962,7 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
                     const int sa = u % p.a_stages, sb = bi % p.b_stages;
                     if (t == 0) mbar_wait(a_full(sa), (u / p.a_stages) & 1, 4, u);
                     mbar_wait(b_full(sb), (bi / p.b_stages) & 1, 5, bi);
-                    const int shift = p.mode == 1 ? t : (t / p.kw) * p.Wp + (t % p.kw);     // rows
+                    const int shift = (t / p.kw) * p.Wp + (t % p.kw);     // rows
                     mma_stage<BN, KIND>(acc[a], cross, a_hi(sa) + shift * 128 + a_row, a_lo(sa) + shift * 128 + a_row, b_hi(sb),
                                         b_lo(sb));
                     wgmma_wait<1>();
@@ -1003,72 +995,52 @@ conv_tcflat_kernel(const ConvFlatP p, const __grid_constant__ CUtensorMap map_hi
 }
 
 
-// G6D_CONV_FLAT: 0 = never use the A-reuse kernel, 1 = FLAT mode only (default), 2 = FLAT and ROW.
-// The MMAs re-read their A and B tiles from shared memory, so the 3x-reuse ROW mode computes junk
-// columns without saving operand traffic; FLAT (9x reuse, and the prologue applied once per element
-// instead of once per tap) saves the producers most of their work.
-static int flat_level() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("G6D_CONV_FLAT"); v = (e && e[0] >= '0' && e[0] <= '2') ? e[0] - '0' : 1; }
-    return v;
-}
-static bool flat_disabled() { return flat_level() == 0; }
-
-static int fill_flat_params(const g6d_conv_desc* d, int kind, ConvFlatP& p, int* smem_bytes) {
-    const int bk = kind_bk(kind);
-    if (!d || d->stride != 1 || (d->Cin % bk) != 0 || d->Cout < 16 || (d->in_cstride & 3) || (d->in_coff & 3)) return -1;
-    const int Do = d->D + 2 * d->pd - d->kd + 1, Ho = d->H + 2 * d->ph - d->kh + 1, Wo = d->W + 2 * d->pw - d->kw + 1;
-    if (Do != d->Do || Ho != d->Ho || Wo != d->Wo || Do < 1 || Ho < 1 || Wo < 1) return -1;
-    if (d->kd * d->kh * d->kw == 1) return -1;                        // 1x1: nothing to reuse, persistent kernel
+// The A-reuse kernel's parameters for a descriptor that fill_tc_params has accepted, or false when the
+// shape does not suit that kernel: it needs stride 1, more than one tap, image planes that fill most of
+// their 128-row tiles, and room for two A stages of the full halo and three B stages.
+static bool fill_flat_params(const g6d_conv_desc* d, int kind, ConvFlatP& p, int* smem_bytes) {
+    if (d->stride != 1 || d->kd * d->kh * d->kw == 1) return false;       // 1x1: nothing to reuse
+    const int Do = d->Do, Ho = d->Ho, Wo = d->Wo;
     const int bn = tc_block_n(d->Cout);
     const int Wp = d->W + 2 * d->pw;
-    const int flat_rows = TC_BM + (d->kh - 1) * Wp + d->kw - 1;
-    const int row_rows = TC_BM + d->kw - 1;
+    const int rows = TC_BM + (d->kh - 1) * Wp + d->kw - 1;
     const int budget = 220 * 1024;
     const int b_stage = 2 * bn * 128;
     // tiles never span image planes: small planes (selector 4x4 / 8x8 maps) would leave most of a
     // 128-row tile empty -> keep those on the batch-flattened kernel
     {
         const long long tiles = ((long long)Ho * Wp + TC_BM - 1) / TC_BM;
-        if ((long long)Ho * Wo * 100 < tiles * TC_BM * 60) return -1;
+        if ((long long)Ho * Wo * 100 < tiles * TC_BM * 60) return false;
     }
-    auto a_stage = [](int rows) { return 2 * ((rows + 7) / 8 * 8) * 128; };
-    int mode, rows, ntab;
-    // FLAT when two A stages of the full halo + >= 3 B stages fit
-    if (2 * a_stage(flat_rows) + 3 * b_stage + 4 * flat_rows + 2048 <= budget) { mode = 0; rows = flat_rows; ntab = 1; }
-    else if (d->kw > 1 && flat_level() >= 2) { mode = 1; rows = row_rows; ntab = d->kh; }
-    else return -1;
+    const long long a_stage = 2ll * ((rows + 7) / 8 * 8) * 128;
+    const int tab_bytes = 4 * rows;
+    int a_st = 2, b_st = 3;
+    long long used = a_st * a_stage + b_st * b_stage + tab_bytes + 2048;
+    if (used > budget) return false;
+    while (b_st < 4 && used + b_stage <= budget) { ++b_st; used += b_stage; }
+    while (a_st < 4 && used + a_stage <= budget) { ++a_st; used += a_stage; }
     p.B = d->B; p.D = d->D; p.H = d->H; p.W = d->W; p.Cin = d->Cin; p.ics = d->in_cstride; p.ico = d->in_coff;
     p.Cout = d->Cout; p.kd = d->kd; p.kh = d->kh; p.kw = d->kw; p.pd = d->pd; p.ph = d->ph; p.pw = d->pw;
     p.Do = Do; p.Ho = Ho; p.Wo = Wo; p.ocs = d->out_cstride; p.oco = d->out_coff; p.pro = d->prologue; p.act = d->act;
     p.group_rows = d->group_rows > 0 ? d->group_rows : 1;
-    p.Wp = Wp; p.tiles_per_plane = (Ho * Wp + TC_BM - 1) / TC_BM; p.mode = mode;
-    p.nseg = mode == 0 ? d->kd : d->kd * d->kh; p.taps_per_seg = mode == 0 ? d->kh * d->kw : d->kw;
-    p.seg_rows = rows; p.rows_pad = (rows + 7) / 8 * 8; p.ntab = ntab; p.cblocks = d->Cin / bk;
-    const long long M = (long long)d->B * Do * Ho * Wo;
-    if (M >= (1ll << 31)) return -1;
-    p.M = (int)M;
-    const int tab_bytes = 4 * ntab * rows;
-    int a_st = 2, b_st = 3;
-    int used = a_st * a_stage(rows) + b_st * b_stage + tab_bytes + 2048;
-    while (b_st < 4 && used + b_stage <= budget) { ++b_st; used += b_stage; }
-    while (a_st < 4 && used + a_stage(rows) <= budget) { ++a_st; used += a_stage(rows); }
-    if (used > budget) return -1;
+    p.Wp = Wp; p.tiles_per_plane = (Ho * Wp + TC_BM - 1) / TC_BM;
+    p.seg_rows = rows; p.rows_pad = (rows + 7) / 8 * 8; p.cblocks = d->Cin / kind_bk(kind);
+    p.M = d->B * Do * Ho * Wo;
     p.a_stages = a_st; p.b_stages = b_st;
-    *smem_bytes = a_st * a_stage(rows) + b_st * b_stage + 256 + tab_bytes + 1024 + 64;
+    *smem_bytes = (int)(a_st * a_stage) + b_st * b_stage + 256 + tab_bytes + 1024 + 64;
     // split over channel blocks when the tile grid cannot fill the machine, or to bound accumulate chains
     const long long ctas = (long long)d->B * Do * p.tiles_per_plane * ((d->Cout + bn - 1) / bn);
     const long long K = (long long)d->Cin * d->kd * d->kh * d->kw;
     int splits = 1;
     if (ctas < kNumSMs && p.cblocks >= 2) splits = (int)((kNumSMs + ctas - 1) / ctas);
-    const int nmain = bn == 32 ? AccCfg<32>::NMAIN : (bn == 64 ? AccCfg<64>::NMAIN : AccCfg<128>::NMAIN);
+    const int nmain = tc_nmain(bn);
     const long long chain = d->max_chain_k > 0 ? (long long)d->max_chain_k * nmain : (K > TC_MAX_K_PER_CHAIN ? TC_MAX_K_PER_CHAIN * nmain : 0);
     if (chain > 0) { const int ms = (int)((K + chain - 1) / chain); splits = splits < ms ? ms : splits; }
     splits = splits > p.cblocks ? p.cblocks : splits;
     splits = splits < 1 ? 1 : splits;
     p.cb_per_split = (p.cblocks + splits - 1) / splits;
     p.splits = (p.cblocks + p.cb_per_split - 1) / p.cb_per_split;
-    return 0;
+    return true;
 }
 
 template <int BN, int KIND>
@@ -1085,17 +1057,48 @@ static int launch_flat(const ConvFlatP& p, int smem, const CUtensorMap& mh, cons
     return G6D_OK;
 }
 
-template <int KIND>
-static int dispatch_flat(int bn, const ConvFlatP& p, int smem, const CUtensorMap& mh, const CUtensorMap& ml, cudaStream_t st) {
-    if (bn == 128) return launch_flat<128, KIND>(p, smem, mh, ml, st);
-    if (bn == 64) return launch_flat<64, KIND>(p, smem, mh, ml, st);
-    return launch_flat<32, KIND>(p, smem, mh, ml, st);
+// What runs for one descriptor.  fill_tc_params validates it; the A-reuse kernel then takes the shapes it
+// suits and the persistent kernel the rest.  Every entry point below is built on make_plan, so they all
+// accept the same descriptors and agree on the kernel and its splits.
+struct ConvPlan {
+    ConvTcP tc;                // the validated descriptor; the persistent kernel's parameters
+    ConvFlatP flat;            // the A-reuse kernel's parameters when use_flat
+    bool use_flat;
+    int bn, splits, flat_smem;
+};
+
+static int make_plan(const g6d_conv_desc* d, int kind, ConvPlan& pl) {
+    const int rc = fill_tc_params(d, kind, pl.tc);
+    if (rc != G6D_OK) return rc;
+    pl.use_flat = fill_flat_params(d, kind, pl.flat, &pl.flat_smem);
+    pl.bn = tc_block_n(d->Cout);
+    pl.splits = pl.use_flat ? pl.flat.splits : pl.tc.splits;
+    return G6D_OK;
+}
+
+// fused output statistics are possible when every 32-row epilogue slice lies in one group; the A-reuse
+// kernel's tiles never span image planes, so its groups must also be made of whole planes
+static bool stats_ok(const ConvPlan& pl, long long stats_rows) {
+    if (stats_rows <= 0 || stats_rows % 32 != 0 || pl.tc.M % stats_rows != 0) return false;
+    return !pl.use_flat || stats_rows % ((long long)pl.flat.Ho * pl.flat.Wo) == 0;
+}
+
+template <class P>
+static void bind_tensors(P& p, const float* x, const float* bias, const float* ps, const float* pb, float* y, void* ws,
+                         double* stats, long long stats_rows) {
+    p.x = x; p.bias = bias; p.ps = ps; p.pb = pb; p.y = y; p.ws = static_cast<float*>(ws);
+    p.stats = stats; p.stats_rows = stats ? stats_rows : 1;
+}
+
+template <int BN, int KIND>
+static int launch_plan(const ConvPlan& pl, const CUtensorMap& mh, const CUtensorMap& ml, cudaStream_t st) {
+    return pl.use_flat ? launch_flat<BN, KIND>(pl.flat, pl.flat_smem, mh, ml, st) : launch_tc2<BN, KIND>(pl.tc, mh, ml, st);
 }
 template <int KIND>
-static int dispatch_tc2(int bn, const ConvTcP& p, const CUtensorMap& mh, const CUtensorMap& ml, cudaStream_t st) {
-    if (bn == 128) return launch_tc2<128, KIND>(p, mh, ml, st);
-    if (bn == 64) return launch_tc2<64, KIND>(p, mh, ml, st);
-    return launch_tc2<32, KIND>(p, mh, ml, st);
+static int dispatch(const ConvPlan& pl, const CUtensorMap& mh, const CUtensorMap& ml, cudaStream_t st) {
+    if (pl.bn == 128) return launch_plan<128, KIND>(pl, mh, ml, st);
+    if (pl.bn == 64) return launch_plan<64, KIND>(pl, mh, ml, st);
+    return launch_plan<32, KIND>(pl, mh, ml, st);
 }
 
 }  // namespace g6d
@@ -1117,95 +1120,48 @@ extern "C" int g6d_conv_tc_debug(int* host_out8) {
 }
 
 extern "C" int g6d_conv_tc_supported(const g6d_conv_desc* d, int kind) {
-    if (!d || (kind != G6D_TC_TF32 && kind != G6D_TC_F16)) return 0;
-    return (d->Cin % kind_bk(kind)) == 0 && d->Cout >= 16 && (d->in_cstride & 3) == 0 && (d->in_coff & 3) == 0 &&
-           tc2_dims_ok(d) ? 1 : 0;
+    ConvPlan pl{};
+    return make_plan(d, kind, pl) == G6D_OK ? 1 : 0;
 }
 
 extern "C" long long g6d_conv_tc_workspace_bytes(const g6d_conv_desc* desc, int kind) {
-    {
-        ConvFlatP fp{}; int smem = 0;
-        if (!flat_disabled() && (kind == G6D_TC_TF32 || kind == G6D_TC_F16) && fill_flat_params(desc, kind, fp, &smem) == 0)
-            return fp.splits > 1 ? (long long)fp.splits * fp.M * fp.Cout * (long long)sizeof(float) : 0;
-    }
-    ConvTcP p{};
-    if (fill_tc_params(desc, kind, p) != G6D_OK) return -1;
-    return p.splits > 1 ? (long long)p.splits * p.M * p.Cout * (long long)sizeof(float) : 0;
-}
-
-// fused output statistics are possible when every 32-row epilogue slice lies in one group
-static bool stats_ok_tc2(long long stats_rows, long long M) { return stats_rows > 0 && stats_rows % 32 == 0 && M % stats_rows == 0; }
-static bool stats_ok_flat(const ConvFlatP& fp, long long stats_rows) {
-    return stats_rows > 0 && stats_rows % 32 == 0 && stats_rows % ((long long)fp.Ho * fp.Wo) == 0 && (long long)fp.M % stats_rows == 0;
+    ConvPlan pl{};
+    if (make_plan(desc, kind, pl) != G6D_OK) return -1;
+    return pl.splits > 1 ? (long long)pl.splits * pl.tc.M * pl.tc.Cout * (long long)sizeof(float) : 0;
 }
 
 extern "C" int g6d_conv_tc_stats_supported(const g6d_conv_desc* desc, int kind, long long stats_rows) {
-    if (!g6d_conv_tc_supported(desc, kind)) return 0;
-    ConvFlatP fp{}; int smem = 0;
-    if (!flat_disabled() && fill_flat_params(desc, kind, fp, &smem) == 0) return stats_ok_flat(fp, stats_rows) ? 1 : 0;
-    const long long M = (long long)desc->B * desc->Do * desc->Ho * desc->Wo;
-    return stats_ok_tc2(stats_rows, M) ? 1 : 0;
+    ConvPlan pl{};
+    return make_plan(desc, kind, pl) == G6D_OK && stats_ok(pl, stats_rows) ? 1 : 0;
 }
 
 extern "C" int g6d_conv_tc(const g6d_conv_desc* desc, const float* x, const void* w_hi, const void* w_lo, int w_rows,
                            int kind, const float* bias, const float* pro_scale, const float* pro_shift, float* y,
                            void* ws, double* stats, long long stats_rows, g6d_stream_t stream) {
-    G6D_REQUIRE(kind == G6D_TC_TF32 || kind == G6D_TC_F16, "g6d_conv_tc: bad operand kind %d", kind);
-    if (stats) {
-        G6D_REQUIRE(g6d_conv_tc_stats_supported(desc, kind, stats_rows), "g6d_conv_tc: fused statistics need groups of whole 32-row slices / planes (stats_rows %lld)", stats_rows);
-        const long long M = (long long)desc->B * desc->Do * desc->Ho * desc->Wo;
-        cudaError_t e = cudaMemsetAsync(stats, 0, sizeof(double) * 2 * (M / stats_rows) * desc->Cout, as_stream(stream));
-        if (e != cudaSuccess) { set_error("g6d_conv_tc: memset: %s", cudaGetErrorString(e)); return G6D_ECUDA; }
-    }
-    {   // stride-1 multi-tap convolutions: A-reuse kernel
-        ConvFlatP fp{}; int smem = 0;
-        if (!flat_disabled() && fill_flat_params(desc, kind, fp, &smem) == 0) {
-            G6D_REQUIRE(x && w_hi && w_lo && y, "g6d_conv_tc: null tensor pointer");
-            G6D_REQUIRE(w_rows >= fp.Cout, "g6d_conv_tc: weight rows (%d) < Cout (%d)", w_rows, fp.Cout);
-            if (fp.pro != G6D_PRO_NONE) G6D_REQUIRE(pro_scale && pro_shift, "g6d_conv_tc: prologue operands missing");
-            if (fp.splits > 1) G6D_REQUIRE(ws != nullptr, "g6d_conv_tc: split workspace required (%d splits)", fp.splits);
-            fp.x = x; fp.bias = bias; fp.ps = pro_scale; fp.pb = pro_shift; fp.y = y; fp.ws = (float*)ws;
-            fp.stats = stats; fp.stats_rows = stats ? stats_rows : 1;
-            const int bn = tc_block_n(fp.Cout);
-            const int K = fp.kd * fp.kh * fp.kw * fp.Cin;
-            CUtensorMap mh, ml;
-            int rc2;
-            if ((rc2 = make_weight_map(&mh, w_hi, w_rows, K, bn, kind)) != G6D_OK) return rc2;
-            if ((rc2 = make_weight_map(&ml, w_lo, w_rows, K, bn, kind)) != G6D_OK) return rc2;
-            cudaStream_t st = as_stream(stream);
-            rc2 = kind == G6D_TC_F16 ? dispatch_flat<G6D_TC_F16>(bn, fp, smem, mh, ml, st)
-                                     : dispatch_flat<G6D_TC_TF32>(bn, fp, smem, mh, ml, st);
-            if (rc2 != G6D_OK) return rc2;
-            if (fp.splits > 1) {
-                const long long n = (long long)fp.M * fp.Cout;
-                (void)n;
-                launch_reduce(fp.ws, bias, y, fp.M, fp.Cout, fp.splits, fp.ocs, fp.oco, fp.act, fp.stats, fp.stats_rows, st);
-                G6D_CHECK_LAUNCH("g6d_conv_tc(flat reduce)");
-            }
-            return G6D_OK;
-        }
-    }
-    ConvTcP p{};
-    int rc = fill_tc_params(desc, kind, p);
+    ConvPlan pl{};
+    int rc = make_plan(desc, kind, pl);
     if (rc != G6D_OK) return rc;
+    const ConvTcP& p = pl.tc;
+    if (stats) G6D_REQUIRE(stats_ok(pl, stats_rows), "g6d_conv_tc: fused statistics need groups of whole 32-row slices / planes (stats_rows %lld)", stats_rows);
     G6D_REQUIRE(x && w_hi && w_lo && y, "g6d_conv_tc: null tensor pointer");
     G6D_REQUIRE(w_rows >= p.Cout, "g6d_conv_tc: weight rows (%d) < Cout (%d)", w_rows, p.Cout);
     if (p.pro != G6D_PRO_NONE) G6D_REQUIRE(pro_scale && pro_shift, "g6d_conv_tc: prologue operands missing");
-    if (p.splits > 1) G6D_REQUIRE(ws != nullptr, "g6d_conv_tc: split-K workspace required (%d splits)", p.splits);
-    p.x = x; p.bias = bias; p.ps = pro_scale; p.pb = pro_shift; p.y = y; p.ws = (float*)ws;
-    p.stats = stats; p.stats_rows = stats ? stats_rows : 1;
-    const int bn = tc_block_n(p.Cout);
-    CUtensorMap mh, ml;
-    if ((rc = make_weight_map(&mh, w_hi, w_rows, p.K, bn, kind)) != G6D_OK) return rc;
-    if ((rc = make_weight_map(&ml, w_lo, w_rows, p.K, bn, kind)) != G6D_OK) return rc;
+    if (pl.splits > 1) G6D_REQUIRE(ws != nullptr, "g6d_conv_tc: split workspace required (%d splits)", pl.splits);
     cudaStream_t st = as_stream(stream);
-    rc = kind == G6D_TC_F16 ? dispatch_tc2<G6D_TC_F16>(bn, p, mh, ml, st) : dispatch_tc2<G6D_TC_TF32>(bn, p, mh, ml, st);
+    if (stats) {
+        cudaError_t e = cudaMemsetAsync(stats, 0, sizeof(double) * 2 * (p.M / stats_rows) * p.Cout, st);
+        if (e != cudaSuccess) { set_error("g6d_conv_tc: memset: %s", cudaGetErrorString(e)); return G6D_ECUDA; }
+    }
+    if (pl.use_flat) bind_tensors(pl.flat, x, bias, pro_scale, pro_shift, y, ws, stats, stats_rows);
+    else bind_tensors(pl.tc, x, bias, pro_scale, pro_shift, y, ws, stats, stats_rows);
+    CUtensorMap mh, ml;
+    if ((rc = make_weight_map(&mh, w_hi, w_rows, p.K, pl.bn, kind)) != G6D_OK) return rc;
+    if ((rc = make_weight_map(&ml, w_lo, w_rows, p.K, pl.bn, kind)) != G6D_OK) return rc;
+    rc = kind == G6D_TC_F16 ? dispatch<G6D_TC_F16>(pl, mh, ml, st) : dispatch<G6D_TC_TF32>(pl, mh, ml, st);
     if (rc != G6D_OK) return rc;
-    if (p.splits > 1) {
-        const long long n = (long long)p.M * p.Cout;
-        (void)n;
-        launch_reduce(p.ws, bias, y, p.M, p.Cout, p.splits, p.ocs, p.oco, p.act, p.stats, p.stats_rows, st);
-        G6D_CHECK_LAUNCH("g6d_conv_tc(splitk reduce)");
+    if (pl.splits > 1) {
+        launch_reduce(static_cast<float*>(ws), bias, y, p.M, p.Cout, pl.splits, p.ocs, p.oco, p.act, stats, stats_rows, st);
+        G6D_CHECK_LAUNCH("g6d_conv_tc(split reduce)");
     }
     return G6D_OK;
 }
@@ -1242,7 +1198,7 @@ extern "C" int g6d_pack_conv_weight_tc(const float* w, void* out_hi, void* out_l
 // Probe (debug/test only): does a K-major SWIZZLE_128B A operand tolerate a start address that is
 // shifted by `shift` rows (shift*128 B, not 1024-aligned) when the data was written with the
 // swizzle phase of its ABSOLUTE shared-memory row?  D[64 x 32] = A[shift .. shift+64) x B^T with
-// K = 32, A[r][k] = r + k/64 (exactly representable), B = 32x32 identity, so D[i][n] = shift + i + n/64.
+// K = 32, A[r][k] = r + k/64 (exact in fp32), B = 32x32 identity, so D[i][n] = shift + i + n/64.
 // `mode` selects the descriptor's base_offset field: 0 -> 0, 1 -> (start_address >> 7) & 7.
 namespace g6d {
 __global__ void __launch_bounds__(128) desc_shift_probe_kernel(float* out, int shift, int mode) {

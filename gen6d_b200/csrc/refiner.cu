@@ -1,6 +1,4 @@
 // Refiner-specific kernels: the unproject-and-aggregate volume fill (R2) and the pose heads.
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace g6d {
@@ -336,9 +334,7 @@ extern "C" int g6d_ref_volume_fill(const float* ref_feats, const float* que_feat
                 Q, R, fh, fw, C, sn, img_h, img_w};
     G6D_REQUIRE(R <= 7, "g6d_ref_volume_fill: at most 7 reference views (7 + query fill the 8 projection lanes x 4 voxels)");
     const long long bricks = (long long)((sn + 1) / 2) * ((sn + 3) / 4) * ((sn + 7) / 8);
-    static int v3 = -1;
-    if (v3 < 0) { const char* e = getenv("G6D_R2_V"); v3 = (e && e[0] == '2') ? 0 : 1; }
-    if (R == 6 && C == 128 && v3) ref_volume_fill_c128_kernel<6><<<(unsigned)(Q * bricks), 256, 0, as_stream(stream)>>>(p);
+    if (R == 6 && C == 128) ref_volume_fill_c128_kernel<6><<<(unsigned)(Q * bricks), 256, 0, as_stream(stream)>>>(p);
     else if (R == 6) ref_volume_fill_kernel<6><<<(unsigned)(Q * bricks), 256, 0, as_stream(stream)>>>(p);
     else ref_volume_fill_kernel<0><<<(unsigned)(Q * bricks), 256, 0, as_stream(stream)>>>(p);
     G6D_CHECK_LAUNCH("g6d_ref_volume_fill");

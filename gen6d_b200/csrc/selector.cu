@@ -1,7 +1,5 @@
 // Selector-specific kernels: the HBM-bound correlation + rotated-similarity score (S2), the
 // closed-form first-InstanceNorm statistics, and the small latency-bound tail ops (S4).
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace g6d {
@@ -475,21 +473,18 @@ extern "C" int g6d_sel_corr_score3(const float* ref0, const float* ref1, const f
     L.row_end[0] = (long long)S * P0; L.row_end[1] = L.row_end[0] + (long long)S * P1;
     L.row_end[2] = L.row_end[1] + (long long)S * P2;
     cudaStream_t st = as_stream(stream);
-    static int fused = -1;
-    if (fused < 0) { const char* e = getenv("G6D_S2_FUSED"); fused = (e && e[0] == '0') ? 0 : 1; }
     // one wave: as many CTAs per SM as are actually resident (the chunked kernel must not need a second wave)
-    static int occ[2] = {0, 0};
-    if (occ[fused] == 0) {
+    static int occ = 0;
+    if (occ == 0) {
         int n = 0;
-        cudaError_t e = fused ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, sel_corr_dots_kernel<512, true>, 256, 0)
-                              : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, sel_corr_dots_kernel<512, false>, 256, 0);
-        occ[fused] = (e == cudaSuccess && n > 0) ? n : 4;
+        cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, sel_corr_dots_kernel<512, true>, 256, 0);
+        occ = (e == cudaSuccess && n > 0) ? n : 4;
     }
     const long long pairs = (L.row_end[2] + 1) / 2;
     long long grid = (pairs + 7) / 8;                    // 8 warps per CTA, one row pair per warp per trip
-    const long long full = (long long)occ[fused] * kNumSMs;
+    const long long full = (long long)occ * kNumSMs;
     if (grid > full) grid = full;
-    if (fused && counters) {
+    if (counters) {
         int* done = counters;
         long long chunk = (L.row_end[2] + grid - 1) / grid;
         chunk += chunk & 1;                                  // even: row pairs never straddle two CTAs

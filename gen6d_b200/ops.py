@@ -374,8 +374,7 @@ def conv(x, pc, prologue=PRO_NONE, pro_scale=None, pro_shift=None, group_rows=1,
         if nbytes < 0:
             _lib.check(-1, 'g6d_conv_tc_workspace_bytes')
         ws = torch.empty(nbytes // 4, device=x.device, dtype=torch.float32) if nbytes > 0 else None
-        fuse = (stats_rows is not None and fused_stats_enabled() and
-                _lib.lib().g6d_conv_tc_stats_supported(C.byref(d), pc.kind, stats_rows))
+        fuse = stats_rows is not None and _lib.lib().g6d_conv_tc_stats_supported(C.byref(d), pc.kind, stats_rows)
         if fuse:
             stats = torch.empty(M // stats_rows, pc.cout, 2, device=x.device, dtype=torch.float64)
         _call('g6d_conv_tc', C.byref(d), _p(x), _p(pc.w_hi, pc.w_hi.dtype), _p(pc.w_lo, pc.w_lo.dtype), pc.w_hi.shape[0],
@@ -396,11 +395,6 @@ def conv(x, pc, prologue=PRO_NONE, pro_scale=None, pro_shift=None, group_rows=1,
     if stats is None:       # not fusable here (FFMA path, groups smaller than an epilogue slice): separate pass over the output
         stats = instnorm_partial(out, rows_per_group=stats_rows, channels=pc.cout, coff=out_coff)
     return out, stats
-
-
-def fused_stats_enabled():
-    """G6D_FUSED_STATS=0 computes every InstanceNorm statistic with the separate g6d_instnorm_partial pass (A/B checks)."""
-    return os.environ.get('G6D_FUSED_STATS', '1') != '0'
 
 
 def vgg_first_block(x, pc):

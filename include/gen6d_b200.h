@@ -218,8 +218,8 @@ int g6d_pack_conv_weight(const float* w, float* out, int Cout, int Cin, int Cin_
                          const float* cout_scale, g6d_stream_t stream);
 /* ---- tensor-core path (wgmma, three-term operand split: fp32-faithful on the tensor pipe) --------
  * Same contract as g6d_conv, for problems g6d_conv_tc_supported accepts (Cin a multiple of the
- * kind's K-block, Cout >= 16).  A*B ~= A_hi*B_hi + A_hi*B_lo + A_lo*B_hi with 11-bit-significand
- * halves; `kind` selects their container:
+ * kind's K-block, Cout >= 16, and every other descriptor check g6d_conv_tc makes).
+ * A*B ~= A_hi*B_hi + A_hi*B_lo + A_lo*B_hi with 11-bit-significand halves; `kind` selects their container:
  *   G6D_TC_TF32: hi = tf32(x), lo = tf32(x - hi), fp32 arrays, K-block 32, tf32 wgmma;
  *   G6D_TC_F16 : hi = fp16(x), lo = fp16((x - hi) * 2^11), __half arrays, K-block 64, f16 wgmma (twice
  *                the K per instruction and per operand byte; the kernels undo the 2^11 in the epilogue).
