@@ -160,12 +160,16 @@ class Gen6DEstimator:
         else:
             poses = np.stack(pose_inits, 0)
         if self.refiner is not None:
-            chain = [poses]
-            for _ in range(self.cfg['refine_iter']):
-                poses = self.refiner.refine_batch(frames, que_Ks, poses, size=128, ref_num=6, ref_even=True)
-                chain.append(poses)
-            inter['refine_poses'] = chain
+            poses, inter['refine_poses'] = self._refine_batch_host(frames, que_Ks, poses, self.cfg['refine_iter'])
         return poses, inter
+
+    def _refine_batch_host(self, frames, que_Ks, poses, iters):
+        """`iters` host-sequenced batched refinements from poses [qn,3,4] -> (poses, [poses, refined 1, ..., refined iters])."""
+        chain = [poses]
+        for _ in range(iters):
+            poses = self.refiner.refine_batch(frames, que_Ks, poses, size=128, ref_num=6, ref_even=True)
+            chain.append(poses)
+        return poses, chain
 
     # ------------------------------------------------------------------ device-resident prediction
     def _glue_possible(self):
@@ -225,6 +229,31 @@ class Gen6DEstimator:
                  'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': logits, 'sel_ref_idx': idx,
                  'refine_poses': [poses0] + refined}
         return (refined[-1] if refined else poses0), inter
+
+    # ------------------------------------------------------------------ video tracking (predict.py)
+    def tracker(self, num_sequences=1, refine_iter=1, smooth_num=5, smooth_std=2.5, bbox_3d=None):
+        """A Tracker for `num_sequences` videos stepped in lockstep (gen6d_b200/track.py): the first step is a full
+        prediction with cfg['refine_iter'] refinements, every later step `refine_iter` refinements from the previous
+        frame's pose, each followed by predict.py's box smoothing (`smooth_num` frames, `smooth_std`; defaults of
+        predict.py's --num / --std).  bbox_3d: the object's 8 box corners [8,3]; None: from the database's point cloud.
+        cfg['refine_iter'] is left untouched."""
+        from .track import Tracker
+        return Tracker(self, num_sequences, refine_iter=refine_iter, smooth_num=smooth_num, smooth_std=smooth_std,
+                       bbox_3d=bbox_3d)
+
+    def track(self, que_imgs, que_K, **tracker_kwargs):
+        """predict.py's loop over one video: que_imgs uint8 [h,w,3] frames of one size, que_K [3,3] (or one per frame).
+        Returns [(pose, smoothed_pose, inter)] per frame: the raw pose [3,4], the smoothed pose [3,4] (float64, as
+        pose_utils.pnp returns it) and that frame's intermediate results."""
+        trk = self.tracker(num_sequences=1, **tracker_kwargs)
+        Ks = np.asarray(que_K)
+        out = []
+        for t, img in enumerate(que_imgs):
+            K = Ks[t] if Ks.ndim == 3 else Ks
+            poses, smoothed, inter = trk.step([img], [K])
+            one = {k: ([p[0] for p in v] if k == 'refine_poses' else v[0]) for k, v in inter.items()}
+            out.append((poses[0], smoothed[0], one))
+        return out
 
     # ------------------------------------------------------------------ throughput API
     def worker_clone(self):

@@ -142,6 +142,21 @@ def glue_apply_refinements(views_struct, que_pose, que_K, rect, net_out):
     return poses
 
 
+def track_smooth(poses, poses_are_f32, bbox, Ks, ring, count, weights):
+    """One smoothing step for S tracked sequences (g6d_track_smooth): poses float64 [S,12] (raw), bbox float32 [8,3],
+    Ks float64 [S,9], ring float32 [S,num,8,2] and count int32 [S] (updated in place), weights float64 [num] ->
+    (smoothed poses float64 [S,12], averaged corners float64 [S,8,2])."""
+    S, num = poses.shape[0], ring.shape[1]
+    if ring.shape != (S, num, 8, 2) or count.shape != (S,) or weights.shape != (num,) or bbox.shape != (8, 3):
+        raise ValueError(f'track_smooth: inconsistent shapes ring {tuple(ring.shape)}, count {tuple(count.shape)}, '
+                         f'weights {tuple(weights.shape)}, bbox {tuple(bbox.shape)} for {S} sequences')
+    smoothed = torch.empty(S, 12, device=poses.device, dtype=torch.float64)
+    avg = torch.empty(S, 8, 2, device=poses.device, dtype=torch.float64)
+    _call('g6d_track_smooth', _p(poses, torch.float64), int(poses_are_f32), _p(bbox), _p(Ks, torch.float64), _p(ring),
+          _p(count, torch.int32), num, _p(weights, torch.float64), S, _p(smoothed, torch.float64), _p(avg, torch.float64), _stream())
+    return smoothed, avg
+
+
 def imagenet_norm(x, out_c=4):
     out = torch.empty(*x.shape[:-1], out_c, device=x.device, dtype=torch.float32)
     _call('g6d_imagenet_norm', _p(x), _p(out), x.numel() // x.shape[-1], x.shape[-1], out_c, _stream())

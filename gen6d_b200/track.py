@@ -1,0 +1,266 @@
+"""Video tracking (the reference's predict.py:47-70): a full prediction on the first frame, then `refine_iter`
+refinements per frame starting from the previous frame's pose, and predict.py's temporal smoothing (the object's 3-D
+box projected with every raw pose, an exponentially weighted average of the last `smooth_num` frames' corners, and a
+PnP solve back to a pose).
+
+With cfg['device_glue'] a tracking step for S sequences in lockstep is ONE captured graph -- the refinement chain
+(csrc/glue.cu + the refiner) followed by the smoothing kernel (csrc/track.cu) -- and one synchronising read; the
+previous poses and the corner histories stay on the device between steps.  Otherwise the host sequences the step
+with predict_batch's host path and runs the smoothing through g6d_track_smooth_host (same code, on the CPU).
+"""
+import numpy as np
+import torch
+
+from . import _lib
+from . import glue
+from . import ops
+from .graphs import StageCache
+
+
+# ------------------------------------------------------------------------------------------ smoothing inputs
+def smoothing_weights(num, std):
+    """predict.py:19 weighted_pts' weights, oldest frame first (the expression the reference evaluates)."""
+    return np.ascontiguousarray(np.exp(-(np.arange(num) / std) ** 2)[::-1])
+
+
+def bbox_from_points(pts):
+    """utils/draw_utils.py pts_range_to_bbox_pts(max(pts), min(pts)): the 8 corners (float32, the reference's order).
+    A box with zero extent along an axis (coplanar corners) is rejected: the smoothing's PnP solves the non-planar case
+    only, where the reference would fall back to OpenCV's homography initialisation."""
+    pts = np.asarray(pts)
+    hi, lo = np.max(pts, 0), np.min(pts, 0)
+    (maxx, maxy, maxz), (minx, miny, minz) = hi, lo
+    box = np.asarray([[minx, miny, minz], [minx, maxy, minz], [maxx, maxy, minz], [maxx, miny, minz],
+                      [minx, miny, maxz], [minx, maxy, maxz], [maxx, maxy, maxz], [maxx, miny, maxz]], np.float32)
+    check_bbox(box)
+    return box
+
+
+def check_bbox(box):
+    box = np.asarray(box, np.float32)
+    if box.shape != (8, 3) or not np.isfinite(box).all():
+        raise ValueError(f'bbox_3d must be 8 finite corners [8,3], got shape {box.shape}')
+    ext = box.max(0) - box.min(0)
+    if (ext <= 0).any():
+        raise ValueError(f'bbox_3d has zero extent along an axis ({ext.tolist()}): its corners are coplanar, and the '
+                         'smoothing solves the PnP for non-coplanar corners only')
+    return np.ascontiguousarray(box)
+
+
+def object_bbox(database):
+    """The box predict.py smooths with: from the database's object point cloud (`object_point_cloud`, as on this
+    package's SyntheticObjectDatabase and the reference's CustomDatabase), or, for a wrapped reference database, the
+    reference's get_ref_point_cloud.  None when neither exists."""
+    pc = getattr(database, 'object_point_cloud', None)
+    if pc is None and hasattr(database, 'db'):          # database.ReferenceDatabaseAdapter
+        pc = getattr(database.db, 'object_point_cloud', None)
+        if pc is None:
+            try:
+                from dataset.database import get_ref_point_cloud   # reference package
+                pc = get_ref_point_cloud(database.db)
+            except (ImportError, NotImplementedError, AttributeError):
+                pc = None
+    return None if pc is None else bbox_from_points(pc)
+
+
+def host_smooth(poses, poses_are_f32, bbox, Ks, ring, count, weights):
+    """g6d_track_smooth_host on numpy arrays: poses [S,3,4] / [S,12], Ks [S,3,3]; ring float32 [S,num,8,2] and count
+    int32 [S] are updated in place.  Returns (smoothed float64 [S,3,4], averaged corners float64 [S,8,2])."""
+    S = len(poses)
+    p = np.ascontiguousarray(np.asarray(poses, np.float64).reshape(S, 12))
+    K = np.ascontiguousarray(np.asarray(Ks, np.float64).reshape(S, 9))
+    box = np.ascontiguousarray(bbox, np.float32)
+    w = np.ascontiguousarray(weights, np.float64)
+    for a, dt in ((ring, np.float32), (count, np.int32)):
+        if a.dtype != dt or not a.flags.c_contiguous:
+            raise ValueError(f'host_smooth: ring / count must be contiguous {dt.__name__} arrays (updated in place)')
+    smoothed, avg = np.zeros((S, 12), np.float64), np.zeros((S, 8, 2), np.float64)
+    _lib.check(_lib.lib().g6d_track_smooth_host(p.ctypes.data, int(poses_are_f32), box.ctypes.data, K.ctypes.data,
+                                                ring.ctypes.data, count.ctypes.data, ring.shape[1] if ring.ndim > 1 else 0,
+                                                w.ctypes.data, S, smoothed.ctypes.data, avg.ctypes.data),
+               'g6d_track_smooth_host')
+    return smoothed.reshape(S, 3, 4), avg
+
+
+# ------------------------------------------------------------------------------------------ the tracker
+class Tracker:
+    """S sequences tracked in lockstep (one frame each per step); see Gen6DEstimator.tracker()."""
+
+    def __init__(self, est, num_sequences, refine_iter=1, smooth_num=5, smooth_std=2.5, bbox_3d=None):
+        if int(num_sequences) < 1:
+            raise ValueError(f'num_sequences must be >= 1, got {num_sequences}')
+        if int(refine_iter) < 1:
+            raise ValueError(f'refine_iter must be >= 1, got {refine_iter}')
+        if int(smooth_num) < 1:
+            raise ValueError(f'smooth_num must be >= 1, got {smooth_num}')
+        if not float(smooth_std) > 0:
+            raise ValueError(f'smooth_std must be > 0, got {smooth_std}')
+        if est.refiner is None:
+            raise ValueError('tracking refines from the previous pose: the estimator needs a refiner')
+        if bbox_3d is None:
+            bbox_3d = object_bbox(est.refiner.ref_database)
+            if bbox_3d is None:
+                raise ValueError('the database has no object point cloud: pass bbox_3d (the 8 corners of the object box)')
+        self.est = est
+        self.S, self.refine_iter = int(num_sequences), int(refine_iter)
+        self.num, self.std = int(smooth_num), float(smooth_std)
+        self.bbox = check_bbox(bbox_3d)
+        self.weights = smoothing_weights(self.num, self.std)
+        self._gen = est._generation()
+        self.stages = StageCache()       # this tracker's step graphs (they capture its device state)
+        self._dev = None                 # device copies of bbox / weights
+        self.reset()
+
+    # -------------------------------------------------------------- state
+    def reset(self):
+        """The next step is a full prediction (detect -> select -> cfg['refine_iter'] refinements) for every sequence,
+        and the smoothing histories restart."""
+        self._prev, self._prev_f32 = None, True
+        self._ring = np.zeros((self.S, self.num, 8, 2), np.float32)
+        self._count = np.zeros(self.S, np.int32)
+
+    def start(self, poses):
+        """Begin (or restart) every sequence from known poses [S,3,4]: the next step refines from them, and the
+        smoothing histories restart."""
+        poses = np.asarray(poses)
+        if poses.shape != (self.S, 3, 4):
+            raise ValueError(f'start: expected poses [{self.S},3,4], got {poses.shape}')
+        self.reset()
+        self._prev, self._prev_f32 = poses.copy(), poses.dtype == np.float32
+
+    def _check(self):
+        if self.est._generation() != self._gen:
+            raise RuntimeError('this tracker is stale: the estimator was rebuilt (build() on another object) or its weights '
+                               'changed since the tracker was created; create a new one with est.tracker()')
+
+    def _device_path(self):
+        return bool(self.est.cfg['device_glue']) and self.est._glue_possible()
+
+    def _to(self, device):
+        """Move the previous poses and the histories to the device (torch tensors) or the host (numpy)."""
+        if device:
+            if not isinstance(self._ring, torch.Tensor):
+                dev = self.est.detector.device
+                self._ring, self._count = torch.from_numpy(self._ring).to(dev), torch.from_numpy(self._count).to(dev)
+                if self._prev is not None:
+                    self._prev = torch.from_numpy(np.asarray(self._prev, np.float64).reshape(self.S, 12)).to(dev)
+        elif isinstance(self._ring, torch.Tensor):
+            self._ring, self._count = self._ring.cpu().numpy(), self._count.cpu().numpy()
+            if self._prev is not None:
+                p = self._prev.cpu().numpy().reshape(self.S, 3, 4)
+                self._prev = p.astype(np.float32) if self._prev_f32 else p
+
+    # -------------------------------------------------------------- one step
+    def step(self, frames, Ks):
+        """frames: S uint8 [h,w,3] of one size; Ks: [S,3,3].  Returns (raw poses float32 [S,3,4], smoothed poses float64
+        [S,3,4], inter): inter['refine_poses'] is this step's chain, inter['bbox_pts'] the projected box corners
+        [S,8,2], inter['smoothed_pts'] their weighted average [S,8,2]; a full-prediction step adds the detection and
+        selection entries of predict_batch."""
+        self._check()
+        if len(frames) != self.S or len(Ks) != self.S:
+            raise ValueError(f'step: this tracker follows {self.S} sequences, got {len(frames)} frames and {len(Ks)} Ks')
+        Ks = np.stack([np.asarray(K) for K in Ks], 0)
+        if self._device_path():
+            return self._step_device(frames, Ks)
+        return self._step_host(frames, Ks)
+
+    def _step_host(self, frames, Ks):
+        est = self.est
+        self._to(False)
+        if self._prev is None:
+            poses, inter = est.predict_batch(frames, list(Ks))
+        else:
+            dev_frames = est.detector.upload_frame([np.asarray(f) for f in frames])
+            poses, chain = est._refine_batch_host(dev_frames, list(Ks), np.stack(list(self._prev), 0), self.refine_iter)
+            inter = {'refine_poses': chain}
+        poses = np.asarray(poses)
+        smoothed, avg = host_smooth(poses, poses.dtype == np.float32, self.bbox, Ks, self._ring, self._count, self.weights)
+        self._prev, self._prev_f32 = poses, poses.dtype == np.float32
+        inter['bbox_pts'] = self._ring[np.arange(self.S), self._count - 1].copy()
+        inter['smoothed_pts'] = avg
+        return poses, smoothed, inter
+
+    def _device_consts(self):
+        if self._dev is None:
+            dev = self.est.detector.device
+            self._dev = {'bbox': torch.from_numpy(self.bbox).to(dev), 'weights': torch.from_numpy(self.weights.copy()).to(dev)}
+        return self._dev
+
+    def _full_fn(self, st):
+        predict, c = self.est._predict_device_fn(st), self._device_consts()
+
+        def fn(frames, cams, ring, count):
+            chain, det, crop, idx, sel_out, logits = predict(frames, cams)
+            poses = chain[-1]
+            smoothed, avg = ops.track_smooth(poses, chain.shape[0] > 1, c['bbox'], cams[:, :9].contiguous(), ring, count, c['weights'])
+            packed = torch.cat([t.reshape(-1).to(torch.float64) for t in (chain, smoothed, avg, ring, count, det, idx, sel_out, logits)])
+            return torch.cat([packed.view(torch.uint8), crop.reshape(-1)]), poses, ring, count
+        return fn
+
+    def _refine_fn(self, st, first_f32):
+        est, iters, c = self.est, self.refine_iter, self._device_consts()
+        R, refine = st['tables']['ref_num'], est.refiner._refine_warped(128)
+
+        def fn(frames, cams, prev, ring, count):
+            poses, chain = prev, [prev]
+            for it in range(iters):
+                jobs, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems(st['views'], R, cams, frames, poses,
+                                                                                             first_f32 or it > 0)
+                out = refine(jobs, que_K, que_pose, ref_Ks, ref_poses)
+                poses = ops.glue_apply_refinements(st['views'], que_pose, que_K, rect, out)
+                chain.append(poses)
+            smoothed, avg = ops.track_smooth(poses, True, c['bbox'], cams[:, :9].contiguous(), ring, count, c['weights'])
+            packed = torch.cat([t.reshape(-1).to(torch.float64) for t in (torch.stack(chain, 0), smoothed, avg, ring, count)])
+            return packed.view(torch.uint8), poses, ring, count
+        return fn
+
+    def _step_device(self, frames, Ks):
+        est, S, num = self.est, self.S, self.num
+        st = est._glue_state()
+        self._to(True)
+        full = self._prev is None
+        with torch.no_grad():
+            dev_frames = est.detector.upload_frame([np.asarray(f) for f in frames])
+            cams = est.detector._to_dev(glue.cameras(Ks))
+            if full:
+                outs = self.stages.run('track_full', self._full_fn(st), [dev_frames, cams, self._ring, self._count])
+            else:
+                outs = self.stages.run(f'track_refine{int(self._prev_f32)}', self._refine_fn(st, self._prev_f32),
+                                       [dev_frames, cams, self._prev, self._ring, self._count])
+            buf, poses_dev, ring, count = outs
+            prev_f32 = self._prev_f32
+            self._prev = poses_dev.clone()
+            self._ring.copy_(ring)
+            self._count.copy_(count)
+            host = est.detector._to_host(buf)                        # the step's one synchronising read
+        self._prev_f32 = True
+        n_chain = (est.cfg['refine_iter'] if full else self.refine_iter) + 1
+        sizes = [('chain', n_chain * S * 12), ('smoothed', S * 12), ('avg', S * 16), ('ring', S * num * 16), ('count', S)]
+        if full:
+            res = est.cfg['ref_resolution']
+            crop_bytes = S * res * res * 3
+            f64 = host[:len(host) - crop_bytes].view(np.float64)
+            crop = host[len(host) - crop_bytes:].reshape(S, res, res, 3)
+            sizes += [('det', S * 4), ('idx', S), ('sel_out', S * 2)]
+            sizes.append(('logits', len(f64) - sum(n for _, n in sizes)))
+        else:
+            f64 = host.view(np.float64)
+        vals, off = {}, 0
+        for name, n in sizes:
+            vals[name] = f64[off:off + n]
+            off += n
+        chain = vals['chain'].reshape(n_chain, S, 3, 4)
+        refined = [c.astype(np.float32) for c in chain[1:]]
+        first = chain[0].astype(np.float32) if (not full and prev_f32) else chain[0].copy()
+        inter = {}
+        if full:
+            det = vals['det'].reshape(S, 4).astype(np.float32)
+            sel_out = vals['sel_out'].reshape(S, 2).astype(np.float32)
+            inter.update({'det_position': det[:, :2].copy(), 'det_scale_r2q': det[:, 2].copy(), 'det_que_img': crop,
+                          'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': vals['logits'].reshape(S, -1).astype(np.float32),
+                          'sel_ref_idx': vals['idx'].astype(np.int64)})
+        ring_h, count_h = vals['ring'].reshape(S, num, 8, 2).astype(np.float32), vals['count'].astype(np.int64)
+        inter['refine_poses'] = [first] + refined
+        inter['bbox_pts'] = ring_h[np.arange(S), count_h - 1].copy()
+        inter['smoothed_pts'] = vals['avg'].reshape(S, 8, 2).copy()
+        return (refined[-1] if refined else first), vals['smoothed'].reshape(S, 3, 4).copy(), inter

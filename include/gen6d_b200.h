@@ -122,6 +122,19 @@ int g6d_glue_apply_refinements(const g6d_glue_views* views, const float* que_pos
                                const float* net_out, int qn, double* poses, g6d_stream_t stream);
 int g6d_glue_apply_refinements_host(const g6d_glue_views* views, const float* que_pose, const float* que_K, const float* rect,
                                     const float* net_out, int qn, double* poses);
+/* ---- temporal smoothing of tracked poses (predict.py:18-26,61-70; utils/base_utils.py:256-265 project_points;
+ * utils/pose_utils.py:246-279 pnp).  Per sequence s: project the object's bounding box bbox [8,3] (float32) with the raw
+ * pose poses[s] [12] (float64 storage; poses_are_f32: float32 values, projected in float32 like numpy does with
+ * predict.py's float32 K) and Ks[s] [9] (float64 values), append the corners to the history ring[s] [num,8,2]
+ * (oldest first; count[s] frames held, 0..num, advanced by the call), average the newest count[s] frames with
+ * weights [num] (np.exp(-(np.arange(num)/std)**2)[::-1]: oldest first, the newest count[s] of them used) -> avg_pts[s]
+ * [8,2] float64, and solve cv2.solvePnP(SOLVEPNP_ITERATIVE) for non-coplanar corners -> smoothed[s] [12] = [R | t]
+ * float64.  One thread per sequence.  The *_host variant runs the identical code on host memory and also rejects a
+ * count beyond the ring. */
+int g6d_track_smooth(const double* poses, int poses_are_f32, const float* bbox, const double* Ks, float* ring, int* count, int num,
+                     const double* weights, int S, double* smoothed, double* avg_pts, g6d_stream_t stream);
+int g6d_track_smooth_host(const double* poses, int poses_are_f32, const float* bbox, const double* Ks, float* ring, int* count,
+                          int num, const double* weights, int S, double* smoothed, double* avg_pts);
 /* (x - mean) / std on f32 [n_pixels, in_c] -> [n_pixels, out_c] (in_c, out_c in {3,4})
  * (network/detector.py:189, selector.py:115, refiner.py:65) */
 int g6d_imagenet_norm(const float* in, float* out, long long n_pixels, int in_c, int out_c, g6d_stream_t stream);
