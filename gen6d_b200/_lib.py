@@ -91,6 +91,7 @@ _SIGNATURES = {
     'g6d_det_score_fuse': [C.POINTER(DetMaps), I, P, P, P, P, P, P],
     'g6d_det_parse': [P, P, P, I, I, I, I, P, P, P],
     'g6d_det_corr_rowsum': [P, P, I, I, I, I, I, P],
+    'g6d_det_corr_rowsum_objects': [P, P, I, I, I, I, I, I, P],
     'g6d_sel_ref_sums': [P, I, I, I, P, P, P],
     'g6d_sel_corr_prologue': [P, P, P, I, I, I, F, P, P, P],
     'g6d_sel_corr_score': [P, P, I, I, I, P, P],

@@ -169,6 +169,31 @@ __global__ void det_corr_rowsum_kernel(const float4* __restrict__ partial, float
     out[i] = acc;
 }
 
+// Several objects' correlations from ONE 1 x k convolution whose output channels are the objects' kernel rows
+// concatenated: channel = (obj*k + ky)*rfn + r.  out is object-major [n_obj, qn, H, W, rfn]; each output element adds
+// its k rows in det_corr_rowsum_kernel's order, so n_obj = 1 gives that kernel's bits.  k = 1 only regroups
+// [qn, H, W, n_obj*rfn] into [n_obj, qn, H, W, rfn] (the direct, not row-decomposed, correlation).
+__global__ void det_corr_rowsum_objects_kernel(const float4* __restrict__ partial, float4* __restrict__ out, long long total,
+                                               int qn, int H, int W, int k, int rfn4, int n_obj) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const int r = (int)(i % rfn4);
+    long long t = i / rfn4;
+    const int x = (int)(t % W); t /= W;
+    const int y = (int)(t % H); t /= H;
+    const long long q = t % qn;
+    const int obj = (int)(t / qn);
+    const long long pix_stride = (long long)n_obj * k * rfn4;         // float4 per partial pixel (all objects)
+    const long long row_stride = (long long)W * pix_stride;           // float4 per partial row y'
+    const float4* p = partial + (q * (H + k - 1) + y) * row_stride + (long long)x * pix_stride + (long long)obj * k * rfn4 + r;
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int ky = 0; ky < k; ++ky) {
+        const float4 v = __ldg(p + ky * row_stride + ky * rfn4);
+        acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
+    }
+    out[i] = acc;
+}
+
 }  // namespace g6d
 
 using namespace g6d;
@@ -181,6 +206,17 @@ extern "C" int g6d_det_corr_rowsum(const float* partial, float* out, int qn, int
     det_corr_rowsum_kernel<<<ceil_div(total, 256), 256, 0, as_stream(stream)>>>(
         reinterpret_cast<const float4*>(partial), reinterpret_cast<float4*>(out), total, H, W, k, rfn / 4);
     G6D_CHECK_LAUNCH("g6d_det_corr_rowsum");
+    return G6D_OK;
+}
+
+extern "C" int g6d_det_corr_rowsum_objects(const float* partial, float* out, int n_obj, int qn, int H, int W, int k, int rfn,
+                                           g6d_stream_t stream) {
+    G6D_REQUIRE(partial && out && n_obj > 0 && qn > 0 && H > 0 && W > 0 && k > 0 && rfn > 0 && (rfn & 3) == 0,
+                "g6d_det_corr_rowsum_objects: bad args (n_obj, qn, H, W, k must be positive, rfn a positive multiple of 4)");
+    const long long total = (long long)n_obj * qn * H * W * (rfn / 4);
+    det_corr_rowsum_objects_kernel<<<ceil_div(total, 256), 256, 0, as_stream(stream)>>>(
+        reinterpret_cast<const float4*>(partial), reinterpret_cast<float4*>(out), total, qn, H, W, k, rfn / 4, n_obj);
+    G6D_CHECK_LAUNCH("g6d_det_corr_rowsum_objects");
     return G6D_OK;
 }
 

@@ -72,6 +72,16 @@ class Gen6DEstimator:
         from .database import as_object_database
         database = as_object_database(database)       # reference-repo databases are wrapped on the fly
         self._drop_workers()                           # clones made for a previous object are stale now
+        v = self._reference_views(database)
+        self.detector.load_ref_imgs(v['imgs'][:self.cfg['det_ref_view_num']])
+        self.selector.load_ref_imgs(v['ref_imgs'], v['poses'], v['center'], v['vert'])
+        self.ref_info = {k: v[k] for k in ('imgs', 'ref_imgs', 'Ks', 'poses', 'center', 'ref_ids')}
+        if self.refiner is not None:
+            self.refiner.load_ref_imgs(database, v['ids_all'])
+        torch.cuda.current_stream().synchronize()      # reference state complete before any other stream reads it
+
+    def _reference_views(self, database):
+        """The object-specific part of build(): FPS reference views, their normalised crops and rotated copies."""
         center, vert = database.object_center(), database.object_vert()
         ids_all = database.get_img_ids()
         ref_ids = G.select_views_fps(database, ids_all, self.cfg['ref_view_num'])
@@ -93,13 +103,8 @@ class Gen6DEstimator:
             rots = [np.stack([cv2.warpPerspective(database.get_image(i), Hs[k], (res, res), flags=cv2.INTER_LINEAR)
                               for k, i in enumerate(ref_ids)], 0) for Hs in rot_Hs]
         ref_imgs_rots = np.stack(rots, 0)  # an,rfn,h,w,3
-        self.detector.load_ref_imgs(ref_imgs[:self.cfg['det_ref_view_num']])
-        self.selector.load_ref_imgs(ref_imgs_rots, ref_poses, center, vert)
-        self.ref_info = {'imgs': ref_imgs, 'ref_imgs': ref_imgs_rots, 'Ks': ref_Ks, 'poses': ref_poses,
-                         'center': center, 'ref_ids': ref_ids}
-        if self.refiner is not None:
-            self.refiner.load_ref_imgs(database, ids_all)
-        torch.cuda.current_stream().synchronize()      # reference state complete before any other stream reads it
+        return {'imgs': ref_imgs, 'ref_imgs': ref_imgs_rots, 'Ks': ref_Ks, 'poses': ref_poses, 'center': center,
+                'ref_ids': ref_ids, 'vert': vert, 'ids_all': ids_all}
 
     def predict(self, que_img, que_K, pose_init=None):
         """estimator.py:173-216.  que_img uint8 [h,w,3], que_K [3,3] -> (pose [3,4], inter_results)."""
@@ -179,23 +184,28 @@ class Gen6DEstimator:
         """Device tables of the camera algebra (glue.py), rebuilt when any module's state changed."""
         gen = self._generation()
         if self._glue is None or self._glue['gen'] != gen:
-            dev = self.detector.device
-            up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-            refs = glue.selector_refs(self.ref_info)
-            refs_dev = {k: up(refs[k]) for k in ('poses', 'cen', 'f', 'dist')}
-            tables = glue.refiner_views(self.refiner.ref_database, self.refiner.ref_ids, 128, 6)
-            src = self.refiner._ref_sources(self.refiner.ref_ids)
-            views_dev = {k: up(tables[k]) for k in ('poses', 'R_look', 'RlookR', 'f', 'Kinv', 'even_idx', 'even_dirs')}
-            views_dev['src'] = up(np.asarray([s[0] for s in src], np.uint64).view(np.int64))
-            views_dev['rows'], views_dev['cols'] = up(np.asarray([s[1] for s in src], np.int32)), up(np.asarray([s[2] for s in src], np.int32))
-            torch.cuda.current_stream().synchronize()
-            ptr = lambda d: {k: t.data_ptr() for k, t in d.items()}
-            self._glue = {'gen': gen, 'keep': (refs_dev, views_dev), 'tables': tables,
-                          'refs': glue.refs_struct({**ptr(refs_dev), 'center': refs['center']}),
-                          'views': glue.views_struct(ptr(views_dev), tables, views_dev['src'].data_ptr(), views_dev['rows'].data_ptr(),
-                                                     views_dev['cols'].data_ptr())}
+            self._glue = {'gen': gen, **self._device_tables(self.ref_info, self.refiner.refs)}
             self.stages.clear()
         return self._glue
+
+    def _device_tables(self, ref_info, refiner_refs):
+        """Device copies of one object's glue tables (selector references from `ref_info`, the refiner's views and
+        resident images from `refiner_refs`) and the g6d_glue_refs / g6d_glue_views structs pointing at them."""
+        dev = self.detector.device
+        up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+        refs = glue.selector_refs(ref_info)
+        refs_dev = {k: up(refs[k]) for k in ('poses', 'cen', 'f', 'dist')}
+        tables = glue.refiner_views(refiner_refs.database, refiner_refs.ids, 128, 6)
+        src = self.refiner._ref_sources(refiner_refs.ids, refiner_refs)
+        views_dev = {k: up(tables[k]) for k in ('poses', 'R_look', 'RlookR', 'f', 'Kinv', 'even_idx', 'even_dirs')}
+        views_dev['src'] = up(np.asarray([s[0] for s in src], np.uint64).view(np.int64))
+        views_dev['rows'], views_dev['cols'] = up(np.asarray([s[1] for s in src], np.int32)), up(np.asarray([s[2] for s in src], np.int32))
+        torch.cuda.current_stream().synchronize()
+        ptr = lambda d: {k: t.data_ptr() for k, t in d.items()}
+        return {'keep': (refs_dev, views_dev), 'tables': tables,
+                'refs': glue.refs_struct({**ptr(refs_dev), 'center': refs['center']}),
+                'views': glue.views_struct(ptr(views_dev), tables, views_dev['src'].data_ptr(), views_dev['rows'].data_ptr(),
+                                           views_dev['cols'].data_ptr())}
 
     def _predict_device_fn(self, st):
         """frames u8 [qn,h,w,3], cams f64 [qn,20] -> every stage of predict_batch, enqueued back to back."""
@@ -255,6 +265,14 @@ class Gen6DEstimator:
             out.append((poses[0], smoothed[0], one))
         return out
 
+    # ------------------------------------------------------------------ several objects (gen6d_b200/objects.py)
+    def object_set(self):
+        """An ObjectSet over this estimator's networks (weights shared, loaded once): objects are added with their own
+        reference state, and ObjectSet.predict poses every object on the same frames in one captured graph.  The
+        estimator's own object (build) and the set's objects never affect each other."""
+        from .objects import ObjectSet
+        return ObjectSet(self)
+
     # ------------------------------------------------------------------ throughput API
     def worker_clone(self):
         import copy
@@ -268,6 +286,10 @@ class Gen6DEstimator:
     def _generation(self):
         mods = (self.detector, self.selector, self.refiner)
         return tuple(m.generation for m in mods if m is not None)
+
+    def _weights_generation(self):
+        mods = (self.detector, self.selector, self.refiner)
+        return tuple(m.weights_generation for m in mods if m is not None)
 
     def _drop_workers(self):
         pool = getattr(self, '_pool', None)

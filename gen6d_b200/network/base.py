@@ -20,6 +20,7 @@ class PackedModule(nn.Module):
         self.stages = StageCache()      # CUDA graphs of the fixed-shape numpy-API stages
         self._pinned, self._pinned_next = {}, {}
         self.generation = 0             # bumped whenever weights or cached reference state change (worker clones go stale)
+        self.weights_generation = 0     # bumped whenever the weights change (reference state computed with them goes stale)
         self.register_load_state_dict_post_hook(lambda module, keys: module.invalidate_packed())
 
     def bump_generation(self):
@@ -30,10 +31,12 @@ class PackedModule(nn.Module):
 
     def invalidate_packed(self):
         self._packed = None
+        self.weights_generation += 1
         self.bump_generation()
 
     def _apply(self, fn, *args, **kwargs):
         self._packed = None
+        self.weights_generation += 1
         self.bump_generation()
         return super()._apply(fn, *args, **kwargs)
 

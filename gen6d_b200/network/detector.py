@@ -1,6 +1,8 @@
 """Detector on the sm_90a kernels.  Mirrors network/detector.py of the reference: same class
 name, cfg keys, checkpoint keys and method contracts (load_ref_imgs / detect_que_imgs numpy API,
 load_impl / detect_impl / forward tensor API)."""
+from dataclasses import dataclass
+
 import numpy as np
 import torch
 
@@ -8,6 +10,18 @@ from .. import ops
 from .backbone import pack_vgg, vgg_v1
 from .base import Branches, PackedModule
 from .params import VGG11BNParams, detector_heads
+
+
+@dataclass
+class DetectorRefs:
+    """One object's reference state of the detector (detector.py:199-205)."""
+    center_feats: list      # 3 x [rfn, k, k, 512] channels-last (reference keeps NCHW)
+    kernels: list           # the same features packed as correlation kernels (Detector.pack_kernels)
+    shape: tuple = (120, 120)
+
+    @property
+    def rfn(self):
+        return self.center_feats[0].shape[0]
 
 
 class Detector(PackedModule):
@@ -25,9 +39,11 @@ class Detector(PackedModule):
         for name, mod in detector_heads(64, 3 * len(self.cfg['detection_scales'])).items():
             setattr(self, name, mod)
         self.pool_ratio = 8
-        self.ref_center_feats = None   # 3 x [rfn, k, k, 512] channels-last (reference keeps NCHW)
-        self.ref_kernels = None        # the same features packed as correlation kernels
-        self.ref_shape = None
+        self.refs = None               # DetectorRefs of the object load_ref_imgs / load_impl loaded
+
+    ref_center_feats = property(lambda self: None if self.refs is None else self.refs.center_feats)
+    ref_kernels = property(lambda self: None if self.refs is None else self.refs.kernels)
+    ref_shape = property(lambda self: None if self.refs is None else list(self.refs.shape))
 
     # ------------------------------------------------------------------ weights
     def _pack(self):
@@ -47,35 +63,43 @@ class Detector(PackedModule):
         """imgs01 [n,h,w,3] in [0,1] -> VGG features (detector.py:188-197)."""
         return vgg_v1(self.packed()['vgg'], ops.imagenet_norm(imgs01, out_c=4))
 
-    def _load_nhwc(self, ref01):
-        """detector.py:199-205: nearest resize to 120x120, features, cache (and pack as kernels)."""
+    def make_refs(self, ref01):
+        """detector.py:199-205: nearest resize to 120x120, features, packed as kernels -> DetectorRefs (not stored)."""
         ref01 = ops.resize_nearest(ref01, 120, 120)
         feats = self._features(ref01)
-        self.ref_center_feats = feats
-        self.ref_shape = [120, 120]
+        return DetectorRefs(feats, self.pack_kernels([feats]), (120, 120))
+
+    def _load_nhwc(self, ref01):
+        self.refs = self.make_refs(ref01)
+        self.bump_generation()          # captured graphs / worker clones hold pointers to the previous reference set
+
+    def pack_kernels(self, feats_objs):
+        """The correlation kernels of one or more objects: feats_objs[o] = 3 x [rfn, k, k, c] (equal shapes over the
+        objects).  Per level ONE PackedConv whose output channels are the objects' kernels concatenated, object-major."""
         kernels = []
-        for f in feats:
-            rfn, k, _, c = f.shape
+        for fs in zip(*feats_objs):
+            rfn, k, _, c = fs[0].shape
+            n_obj = len(fs)
+            cat = lambda flats: flats[0] if n_obj == 1 else torch.cat(flats, 0)
             kind = ops.tc_kind_for(c)
             if rfn >= 16 and rfn % 4 == 0 and kind is not None and ops.conv_path() == 'tc' and self.cfg.get('corr_rows', True):
                 # Tensor-core path, row-decomposed: the k x k kernels become a 1 x k convolution with
                 # k*rfn output channels (channel = ky*rfn + r) whose per-row results g6d_det_corr_rowsum
                 # adds up.  N = k*rfn (480 at 15 x 15 x 32 refs) fills full 128-wide MMA tiles; the direct
                 # form's N = rfn = 32 pays 40 cycles per MMA against a 16-cycle tensor floor.
-                flat = f.permute(1, 0, 2, 3).reshape(k * rfn, k * c).contiguous()      # [(ky, r), (kx, c)], K-major B operand
-                pc = ops.PackedConv(None, None, c, k * rfn, (1, 1, k), 1, (0, k // 2, k // 2))
+                flat = cat([f.permute(1, 0, 2, 3).reshape(k * rfn, k * c).contiguous() for f in fs])   # [(obj, ky, r), (kx, c)], K-major B operand
+                pc = ops.PackedConv(None, None, c, n_obj * k * rfn, (1, 1, k), 1, (0, k // 2, k // 2))
                 pc.w_hi, pc.w_lo, pc.kind = ops.split_operand(flat, kind)
                 pc.rows = (k, rfn)
                 pc.max_chain_k = 640        # post-ReLU features x post-ReLU features: same-sign products
             else:
-                flat = f.reshape(rfn, k * k * c)
-                pc = ops.PackedConv(ops.transpose_to_packed(flat), None, c, rfn, (1, k, k), 1, (0, k // 2, k // 2))
+                flat = cat([f.reshape(rfn, k * k * c) for f in fs])
+                pc = ops.PackedConv(ops.transpose_to_packed(flat), None, c, n_obj * rfn, (1, k, k), 1, (0, k // 2, k // 2))
                 if rfn >= 16 and kind is not None:   # channels-last features [rfn, (ky,kx,c)] are already the K-major B operand
                     pc.w_hi, pc.w_lo, pc.kind = ops.split_operand(flat, kind)
                     pc.max_chain_k = 640
             kernels.append(pc)
-        self.ref_kernels = kernels
-        self.bump_generation()          # captured graphs / worker clones hold pointers to the previous reference set
+        return kernels
 
     def scale_sizes(self, hq, wq):
         """detector.py:236-239: round(h * 2**s), rounded UP to a multiple of 32."""
@@ -99,10 +123,31 @@ class Detector(PackedModule):
             out.append(ops.det_corr_rowsum(y, *rows) if rows is not None else y)
         return out
 
+    def _raw_correlation_objects(self, que01, kernels, n_obj, rfn):
+        """_raw_correlation for n_obj objects (pack_kernels of their features): the query's features once, ONE
+        correlation GEMM per level over all objects -> per level the object-major maps [n_obj * qn, H, W, rfn]."""
+        feats = self._features(que01)
+        out = []
+        for f, pc in zip(feats, kernels):
+            y = ops.conv(f, pc)
+            k = pc.rows[0] if pc.rows is not None else 1
+            m = ops.det_corr_rowsum_objects(y, n_obj, k, rfn)
+            out.append(m.reshape(n_obj * m.shape[1], *m.shape[2:]))
+        return out
+
     def _detect_nhwc(self, que01, return_taps=False):
         """detector.py:232-266 on [qn,h,w,3] in [0,1].  Returns channels-last maps."""
         if self.ref_kernels is None:
             raise RuntimeError('Detector: load_ref_imgs / load_impl must be called first')
+        return self._detect_maps(que01, self._raw_correlation, que01.shape[0], self.refs.rfn, return_taps)
+
+    def _detect_objects_nhwc(self, que01, kernels, n_obj, rfn, return_taps=False):
+        """_detect_nhwc for n_obj objects sharing the query pyramid: maps of n_obj * qn rows, object-major."""
+        return self._detect_maps(que01, lambda cur: self._raw_correlation_objects(cur, kernels, n_obj, rfn),
+                                 n_obj * que01.shape[0], rfn, return_taps)
+
+    def _detect_maps(self, que01, correlate, rows, rfn, return_taps):
+        """Scale pyramid (correlate(scaled query) -> 3 raw maps of `rows` rows), fused score_conv and the three heads."""
         p = self.packed()
         qn, hq, wq, _ = que01.shape
         hs, ws = hq // 8, wq // 8
@@ -111,14 +156,13 @@ class Detector(PackedModule):
 
         def one_scale(ht, wt):
             cur = que01 if (ht, wt) == (hq, wq) else ops.resize_bilinear(que01, ht, wt)
-            return self._raw_correlation(cur)
+            return correlate(cur)
 
         maps = [br.run(i, lambda ht=ht, wt=wt: one_scale(ht, wt)) for i, (ht, wt) in enumerate(scales)]
         br.join()
         sizes = [[(r.shape[1], r.shape[2]) for r in raw] for raw in maps]
-        rfn = self.ref_center_feats[0].shape[0]
         feats = ops.det_score_fuse(maps, sizes, rfn, hs, ws, self.cfg['vgg_score_stats'], self.cfg['vgg_score_max'],
-                                   p['w1'], p['b1'], p['w2'], p['b2'], qn)
+                                   p['w1'], p['b1'], p['w2'], p['b2'], rows)
         outs = {}
         heads = ('score_predict', 'scale_predict', 'offset_predict')
         hb = Branches(len(heads))
@@ -167,9 +211,14 @@ class Detector(PackedModule):
     # ------------------------------------------------------------------ reference numpy API
     def load_ref_imgs(self, ref_imgs):
         """@param ref_imgs: uint8 [rfn,h,w,3] (detector.py:277-289)"""
+        self.refs = self.make_refs_u8(ref_imgs)
+        self.bump_generation()          # captured graphs / worker clones hold pointers to the previous reference set
+
+    def make_refs_u8(self, ref_imgs):
+        """What load_ref_imgs computes, returned as a DetectorRefs instead of stored."""
         with torch.no_grad():
             u8 = self._to_dev(ref_imgs)
-            self._load_nhwc(ops.preprocess_u8(u8, out_c=3, imagenet_norm=False))
+            return self.make_refs(ops.preprocess_u8(u8, out_c=3, imagenet_norm=False))
 
     def detect_que_imgs(self, que_imgs, que_dev=None):
         """@param que_imgs: uint8 [qn,h,w,3] -> {'positions': f32 [qn,2], 'scales': f32 [qn]} (detector.py:291-304)

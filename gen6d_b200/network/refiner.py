@@ -7,6 +7,7 @@ qn*(rfn+1) images, the volume fill on all qn volumes, the 3-D conv stack on [qn,
 InstanceNorm groups are per image / per pose, exactly as in the reference (no cross-pose term).
 """
 import threading
+from dataclasses import dataclass, field
 
 import numpy as np
 import torch
@@ -20,6 +21,16 @@ IN_EPS = 1e-5
 _UPLOAD_LOCK = threading.Lock()
 
 
+@dataclass
+class RefinerRefs:
+    """One object's reference state of the refiner (refiner.py:271-273): its database, the reference ids, and the
+    database images resident on the device (uploaded on first use)."""
+    database: object
+    ids: list
+    dev: dict = field(default_factory=dict)     # image id -> device uint8 [rows, cols, 3]
+    src: dict = field(default_factory=dict)     # image id -> geometry.warp_source() of that tensor
+
+
 class VolumeRefiner(PackedModule):
     default_cfg = {'refiner_sample_num': 32}
 
@@ -29,10 +40,10 @@ class VolumeRefiner(PackedModule):
         self.feature_net = RefineFeatureParams()
         self.volume_net = RefineVolumeParams()
         self.regressor = RefineRegressorParams()
-        self.ref_database = None
-        self.ref_ids = None
-        self._ref_dev = {}
-        self._ref_src = {}
+        self.refs = None              # RefinerRefs of the object load_ref_imgs loaded
+
+    ref_database = property(lambda self: None if self.refs is None else self.refs.database)
+    ref_ids = property(lambda self: None if self.refs is None else self.refs.ids)
 
     # ------------------------------------------------------------------ weights
     def _pack(self):
@@ -182,33 +193,38 @@ class VolumeRefiner(PackedModule):
         database of the reference repo (dataset/database.py BaseDatabase), exactly as the reference's
         estimator.py:171 passes it: the latter is wrapped on the fly (the reference reads the object's
         centre / diameter / up vector through free functions, database.py:311-397)."""
-        from ..database import as_object_database
-        self.ref_database = as_object_database(ref_database)
-        self.ref_ids = ref_ids
-        self._ref_dev = {}          # image id -> device uint8 [rows, cols, 3] (filled on first use)
-        self._ref_src = {}          # image id -> geometry.warp_source() of that tensor
+        self.refs = self.make_refs(ref_database, ref_ids)
         self.bump_generation()
 
-    def _ref_images_dev(self, ids):
+    @staticmethod
+    def make_refs(ref_database, ref_ids):
+        """What load_ref_imgs stores, returned as a RefinerRefs (the images are uploaded on first use)."""
+        from ..database import as_object_database
+        return RefinerRefs(as_object_database(ref_database), ref_ids)
+
+    def _ref_images_dev(self, ids, refs=None):
         """The database images the look-at crops are cut from, resident on the device: all of them
         are uploaded on first use (once per object) and then shared read-only by every worker
-        clone / stream, hence the lock and the synchronise before anyone else may see them."""
-        if not self._ref_dev:
+        clone / stream, hence the lock and the synchronise before anyone else may see them.
+        refs: the RefinerRefs to read (default: the module's own)."""
+        refs = self.refs if refs is None else refs
+        if not refs.dev:
             with _UPLOAD_LOCK:
-                if not self._ref_dev:
-                    dev = {i: torch.from_numpy(np.ascontiguousarray(self.ref_database.get_image(i))).to(self.device)
-                           for i in self.ref_ids}
+                if not refs.dev:
+                    dev = {i: torch.from_numpy(np.ascontiguousarray(refs.database.get_image(i))).to(self.device)
+                           for i in refs.ids}
                     torch.cuda.current_stream().synchronize()
-                    self._ref_dev.update(dev)
-        return [self._ref_dev[i] for i in ids]
+                    refs.dev.update(dev)
+        return [refs.dev[i] for i in ids]
 
-    def _ref_sources(self, ids):
+    def _ref_sources(self, ids, refs=None):
         """warp_source() triples of the resident database images `ids` (described once per object)."""
-        if not self._ref_src:
+        refs = self.refs if refs is None else refs
+        if not refs.src:
             from .. import geometry as G
-            dev = self._ref_images_dev(self.ref_ids)
-            self._ref_src.update({i: G.warp_source(t) for i, t in zip(self.ref_ids, dev)})
-        return [self._ref_src[i] for i in ids]
+            dev = self._ref_images_dev(refs.ids, refs)
+            refs.src.update({i: G.warp_source(t) for i, t in zip(refs.ids, dev)})
+        return [refs.src[i] for i in ids]
 
     def _refine_warped(self, size):
         """jobs: per pose one query crop followed by its rfn reference crops (qn * (rfn + 1) records)."""

@@ -8,6 +8,8 @@ slice-major, ref[l] = [S = rfn*an (r-major, a-minor), h_l, w_l, 512], which is s
  * the input tensor of the first tower convolution, whose loader forms the (never
    materialised) correlation volume q (.) ref with the first InstanceNorm3d folded in.
 """
+from dataclasses import dataclass
+
 import numpy as np
 import torch
 
@@ -36,6 +38,16 @@ class LocalComm:
 FEAT_PAD = 516  # 512 correlation features + 3 similarity scores, padded to a multiple of 4
 
 
+@dataclass
+class SelectorRefs:
+    """One object's reference state of the selector (selector.py:121-148), this rank's shard of it."""
+    feats_cache: list       # 3 x [S_local, h, w, 512]
+    sums: list              # per level (sum, sum of squares) over ALL S, float64 [h*w, 512]
+    pose_embed: torch.Tensor  # [rfn_local, 512]
+    shape: tuple            # (rfn_local, an)
+    rfn_total: int          # references over all shards
+
+
 class ViewpointSelector(PackedModule):
     default_cfg = {'selector_angle_num': 5}
 
@@ -45,12 +57,14 @@ class ViewpointSelector(PackedModule):
         self.backbone = VGG11BNParams()
         for name, mod in selector_modules(self.cfg['selector_angle_num']).items():
             setattr(self, name, mod)
-        self.ref_feats_cache = None   # 3 x [S_local, h, w, 512]
-        self.ref_sums = None          # per level (sum, sum of squares) over ALL S, float64 [h*w, 512]
-        self.ref_pose_embed = None    # [rfn_local, 512]
-        self.ref_shape = None         # (rfn_local, an)
-        self.rfn_total = None         # references over all shards
+        self.refs = None              # SelectorRefs of the object load_ref_imgs / extract_ref_feats loaded
         self.comm = LocalComm()       # gen6d_b200.dist.Comm when the reference axis is sharded over GPUs
+
+    ref_feats_cache = property(lambda self: None if self.refs is None else self.refs.feats_cache)
+    ref_sums = property(lambda self: None if self.refs is None else self.refs.sums)
+    ref_pose_embed = property(lambda self: None if self.refs is None else self.refs.pose_embed)
+    ref_shape = property(lambda self: None if self.refs is None else self.refs.shape)
+    rfn_total = property(lambda self: None if self.refs is None else self.refs.rfn_total)
 
     # ------------------------------------------------------------------ weights
     def _pack(self):
@@ -114,11 +128,16 @@ class ViewpointSelector(PackedModule):
         return cam / torch.clamp(torch.linalg.norm(cam, dim=1, keepdim=True), min=1e-12)
 
     def _load_nhwc(self, ref_norm4, rfn, an, ref_poses, object_center, object_vert, chunk=64):
+        self.refs = self._make_refs(ref_norm4, rfn, an, ref_poses, object_center, object_vert, chunk)
+        self.bump_generation()          # captured graphs / worker clones hold pointers to the previous reference set
+
+    def _make_refs(self, ref_norm4, rfn, an, ref_poses, object_center, object_vert, chunk=64):
         """ref_norm4: this rank's references [r0, r1) of the rfn in total, [S_local = (r1-r0)*an (r-major), h, w, 4]
         ImageNet-normalised (selector.py:121-148); ref_poses are those of ALL rfn references.  The callers
-        slice the image set BEFORE it is uploaded / converted, so a rank never holds more than its shard."""
+        slice the image set BEFORE it is uploaded / converted, so a rank never holds more than its shard.
+        -> SelectorRefs (not stored)."""
         p = self.packed()
-        self.rfn_total = rfn
+        rfn_total = rfn
         r0, r1 = self.comm.shard_range(rfn)
         assert ref_norm4.shape[0] == (r1 - r0) * an
         vp_all = self.viewpoints(ref_poses, object_center, object_vert)   # frame anchored on GLOBAL ref 0
@@ -128,18 +147,22 @@ class ViewpointSelector(PackedModule):
         for s0 in range(0, S, chunk):
             for l, f in enumerate(self._feats(ref_norm4[s0:s0 + chunk])):
                 levels[l].append(f)
-        self.ref_feats_cache = [torch.cat(lv, 0) if len(lv) > 1 else lv[0] for lv in levels]
-        sums = [ops.sel_ref_sums(f.reshape(S, -1, f.shape[-1])) for f in self.ref_feats_cache]
+        feats_cache = [torch.cat(lv, 0) if len(lv) > 1 else lv[0] for lv in levels]
+        sums = [ops.sel_ref_sums(f.reshape(S, -1, f.shape[-1])) for f in feats_cache]
         # closed-form first-InstanceNorm statistics need the sums over ALL references: one all-reduce at load
-        self.ref_sums = [(self.comm.all_reduce_sum(a), self.comm.all_reduce_sum(b)) for a, b in sums]
-        self.ref_shape = (rfn, an)
+        sums = [(self.comm.all_reduce_sum(a), self.comm.all_reduce_sum(b)) for a, b in sums]
         vp = torch.zeros(rfn, 4, dtype=torch.float32)
         vp[:, :3] = vp_all[r0:r1]
         x = vp.to(self.device).reshape(rfn, 1, 1, 4)
         for i, pc in enumerate(p['vpe']):
             x = ops.conv(x, pc, act=ops.ACT_RELU if i < 2 else ops.ACT_NONE)
-        self.ref_pose_embed = x.reshape(rfn, 512)
-        self.bump_generation()          # captured graphs / worker clones hold pointers to the previous reference set
+        return SelectorRefs(feats_cache, sums, x.reshape(rfn, 512), (rfn, an), rfn_total)
+
+    @staticmethod
+    def s2_counters_for(refs, device):
+        """Fresh completion counters of the fused S2 kernel for one reference record (zero; the kernel leaves them
+        zero).  Every record selected against concurrently needs its own."""
+        return torch.zeros(3 * refs.shape[0] * refs.shape[1], device=device, dtype=torch.int32)
 
     def comm_stats(self):
         """Collectives issued per query by the sharded path (counted on the last eager / capture pass)."""
@@ -161,7 +184,7 @@ class ViewpointSelector(PackedModule):
         exact, not per-shard."""
         return ops.instnorm_finalize(self.comm.all_reduce_sum(ws), rows_total, IN_EPS)
 
-    def _tower(self, level, ref, scale, shift, cat_buf, S):
+    def _tower(self, level, ref, scale, shift, cat_buf, S, refs):
         """corr_conv_list[level] (selector.py:27-69) on the implicit correlation volume."""
         convs = self.packed()['towers'][level]
         x, pro, ps, pb = ref, ops.PRO_CORR, scale, shift
@@ -175,11 +198,11 @@ class ViewpointSelector(PackedModule):
             # InstanceNorm3d statistics over (S, h, w) of the raw conv output; the normalisation
             # itself (and the ReLU) is applied by the next conv's loader.  MaxPool commutes with
             # the positive-slope affine, so pooling the raw tensor first is exact.
-            ps, pb = self._finalize(ws, rows // self.ref_shape[0] * self.rfn_total)
+            ps, pb = self._finalize(ws, rows // refs.shape[0] * refs.rfn_total)
             pro = ops.PRO_AFFINE_RELU if 'r' in post else ops.PRO_AFFINE
             x = ops.maxpool2x2(y) if 'p' in post else y
 
-    def _towers_sharded(self, q_feats, cat_buf, S, S_total):
+    def _towers_sharded(self, q_feats, cat_buf, S, S_total, refs):
         """The three towers with the reference axis sharded over GPUs, ROUND-synchronous: round r runs the
         r-th convolution of every tower that still has one (concurrently, on branch streams), then ONE
         all-reduce carries the InstanceNorm moments of all of them (5 rounds for the 6 + 4 + 2 convolutions
@@ -187,7 +210,7 @@ class ViewpointSelector(PackedModule):
         towers = self.packed()['towers']
         nbr = 3 if self.comm.capturable else 1
         state, keep = [], []
-        for l, (q, ref, (s1, s2)) in enumerate(zip(q_feats, self.ref_feats_cache, self.ref_sums)):
+        for l, (q, ref, (s1, s2)) in enumerate(zip(q_feats, refs.feats_cache, refs.sums)):
             h, w, c = q.shape
             scale, shift = ops.sel_corr_prologue(q.reshape(h * w, c), s1, s2, S_total, IN_EPS)
             state.append({'x': ref, 'pro': ops.PRO_CORR, 'ps': scale, 'pb': shift, 'i': 0})
@@ -221,24 +244,30 @@ class ViewpointSelector(PackedModule):
             o = 0
             for st, post, (y, ws, rows) in pend:
                 n = ws.numel()
-                ps, pb = ops.instnorm_finalize(flat[o:o + n].reshape(ws.shape), rows // self.ref_shape[0] * self.rfn_total, IN_EPS)
+                ps, pb = ops.instnorm_finalize(flat[o:o + n].reshape(ws.shape), rows // refs.shape[0] * refs.rfn_total, IN_EPS)
                 o += n
                 keep.append((y, ws))
                 st['ps'], st['pb'] = ps, pb
                 st['pro'] = ops.PRO_AFFINE_RELU if 'r' in post else ops.PRO_AFFINE
                 st['x'] = ops.maxpool2x2(y) if 'p' in post else y
 
-    def _select_one(self, q_feats):
-        """selector.py:177-215 for one query.  q_feats: 3 x [h, w, 512].  -> logits [rfn], angles [rfn]"""
+    def _select_one(self, q_feats, refs=None, counters=None):
+        """selector.py:177-215 for one query.  q_feats: 3 x [h, w, 512].  -> logits [rfn], angles [rfn]
+        refs: the SelectorRefs to select against (default: the module's own); with any other record, `counters` are
+        that record's own S2 counters (s2_counters_for), never the module's or another record's."""
         p = self.packed()
-        rfn, an = self.ref_shape
+        if refs is None:
+            refs, counters = self.refs, self._s2_counters()
+        rfn, an = refs.shape
         S = rfn * an
-        S_total = self.rfn_total * an
+        S_total = refs.rfn_total * an
+        if counters is None or counters.numel() != 3 * S:
+            raise ValueError('_select_one: a reference record other than the module\'s needs its own S2 counters [3*S]')
         dev = self.device
         cat_buf = torch.empty(S, 4, 4, 768, device=dev, dtype=torch.float32)
         feats = torch.empty(S, FEAT_PAD, device=dev, dtype=torch.float32)      # cols 0-511: cf3, 512-514 + pad: vp_norm
-        scores = ops.sel_corr_score3([r.reshape(S, -1, r.shape[-1]) for r in self.ref_feats_cache],
-                                     [q.reshape(-1, q.shape[-1]) for q in q_feats], counters=self._s2_counters())
+        scores = ops.sel_corr_score3([r.reshape(S, -1, r.shape[-1]) for r in refs.feats_cache],
+                                     [q.reshape(-1, q.shape[-1]) for q in q_feats], counters=counters)
         if self.comm.world == 1:
             br = Branches(3)                                # the three towers only meet in cat_buf
             keep = []
@@ -247,13 +276,13 @@ class ViewpointSelector(PackedModule):
                 h, w, c = q.shape
                 scale, shift = ops.sel_corr_prologue(q.reshape(h * w, c), s1, s2, S_total, IN_EPS)
                 keep.append((scale, shift))
-                self._tower(l, ref, scale, shift, cat_buf, S)
+                self._tower(l, ref, scale, shift, cat_buf, S, refs)
 
-            for l, (q, ref, (s1, s2)) in enumerate(zip(q_feats, self.ref_feats_cache, self.ref_sums)):
+            for l, (q, ref, (s1, s2)) in enumerate(zip(q_feats, refs.feats_cache, refs.sums)):
                 br.run(l, lambda l=l, q=q, ref=ref, s1=s1, s2=s2: one_level(l, q, ref, s1, s2))
             br.join()
         else:
-            self._towers_sharded(q_feats, cat_buf, S, S_total)
+            self._towers_sharded(q_feats, cat_buf, S, S_total, refs)
         # corr_feats_conv (selector.py:71-77): 1x1 768->512, IN, ReLU, 1x1 512->512, AvgPool(4,4).
         # The second 1x1 conv is linear, so the 4x4 average is taken first (16x less work).
         y, ws = ops.conv(cat_buf, p['cf0'], stats_rows=S * 16)
@@ -266,15 +295,15 @@ class ViewpointSelector(PackedModule):
             all_scores = self.comm.all_gather_cat(scores, dim=1).contiguous()
             tmp = torch.empty(S_total, 4, device=dev, dtype=torch.float32)
             ops.sel_vp_norm(all_scores, tmp, 0, IN_EPS)
-            r0, _ = self.comm.shard_range(self.rfn_total)
+            r0, _ = self.comm.shard_range(refs.rfn_total)
             feats[:, 512:516] = tmp[r0 * an:r0 * an + S]
         x = ops.conv(feats.reshape(S, 1, 1, FEAT_PAD), p['sp0'], act=ops.ACT_RELU)
         x = ops.conv(x, p['sp2']).reshape(rfn, an, 512)
-        sf = ops.sel_max_angle_add(x, self.ref_pose_embed)              # selector.py:203-204
+        sf = ops.sel_max_angle_add(x, refs.pose_embed)                  # selector.py:203-204
         # everything below couples all references (attention, InstanceNorm1d over rfn): gather the
         # per-reference score features once ([rfn,512] = 128 KB at 64 refs) and run the tail replicated
         sf = self.comm.all_gather_cat(sf, dim=0).contiguous()
-        rfn_local, rfn = rfn, self.rfn_total
+        rfn_local, rfn = rfn, refs.rfn_total
         for att, (m0, m3) in zip(p['atts'], p['mlps']):
             x4 = sf.reshape(rfn, 1, 1, 512)
             qv = ops.conv(x4, att['conv_query']).reshape(rfn, 512)
@@ -344,14 +373,19 @@ class ViewpointSelector(PackedModule):
     def load_ref_imgs(self, ref_imgs, ref_poses, object_center, object_vert):
         """@param ref_imgs: uint8 [an,rfn,h,w,3]; ref_poses [rfn,3,4]; object_center [3]; object_vert [3]
         (selector.py:150-163)"""
+        self.refs = self.make_refs(ref_imgs, ref_poses, object_center, object_vert)
+        self.bump_generation()          # captured graphs / worker clones hold pointers to the previous reference set
+
+    def make_refs(self, ref_imgs, ref_poses, object_center, object_vert):
+        """What load_ref_imgs computes, returned as a SelectorRefs instead of stored."""
         with torch.no_grad():
             an, rfn, h, w, _ = ref_imgs.shape
             r0, r1 = self.comm.shard_range(rfn)
             u8 = torch.from_numpy(np.ascontiguousarray(ref_imgs[:, r0:r1].transpose(1, 0, 2, 3, 4))).to(self.device)
             u8 = u8.reshape((r1 - r0) * an, h, w, 3)            # one-off load: no pinned staging ring for ~100s of MB
             x = ops.preprocess_u8(u8, out_c=4, imagenet_norm=True)
-            self._load_nhwc(x, rfn, an, ref_poses.astype(np.float32), object_center.astype(np.float32),
-                            object_vert.astype(np.float32))
+            return self._make_refs(x, rfn, an, ref_poses.astype(np.float32), object_center.astype(np.float32),
+                                   object_vert.astype(np.float32))
 
     def _select_warped(self, size):
         def fn(jobs):

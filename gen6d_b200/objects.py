@@ -1,0 +1,216 @@
+"""Several objects per frame over one set of networks.
+
+Gen6D is model-free: one checkpoint serves every object, and an object is only its reference state (the detector's
+correlation kernels, the selector's reference stack, the refiner's database images).  An ObjectSet
+(Gen6DEstimator.object_set()) keeps that state per object, next to the estimator's own, and poses every object on the
+same frames as ONE captured graph with one synchronising read:
+
+  upload -> ONE detection stage for all objects (the query's VGG pyramid once per scale, one correlation GEMM per level
+  over the objects' concatenated kernels, g6d_det_corr_rowsum_objects, then score fusion / heads / argmax on K*qn
+  "queries") -> the K*qn selector crops in one warp and one crop VGG, each object's selection against its own reference
+  stack -> refine_iter x (per-object refinement problems, ONE refiner stage over all K*qn poses, per-object update).
+
+Rows are object-major (object, frame) everywhere after the correlation, so each object's detections, crops and poses are
+a contiguous slice whose row i is frame i, which is the layout the g6d_glue_* kernels take.
+"""
+import numpy as np
+import torch
+
+from . import glue
+from . import ops
+from .graphs import StageCache
+
+
+class _Object:
+    """One object's reference state: a record per network module plus its glue tables on the device."""
+
+    def __init__(self, det, sel, ref, ref_info, tables, counters, weights_gen):
+        self.det, self.sel, self.ref = det, sel, ref
+        self.ref_info, self.tables, self.counters = ref_info, tables, counters
+        self.weights_gen = weights_gen
+
+
+class ObjectSet:
+    """Objects sharing one estimator's networks; see Gen6DEstimator.object_set().
+
+    Per object the device holds about the selector's reference stack (220 MB at 64 views x 5 angles), the detector's
+    kernels (tens of MB) and the object's database images (66 MB for a 72-view 480x640 object)."""
+
+    def __init__(self, est):
+        if est.refiner is None:
+            raise ValueError('an object set refines every pose: the estimator needs a refiner')
+        if getattr(est.selector.comm, 'world', 1) > 1:
+            raise ValueError('an object set does not shard the selector: the estimator\'s selector is sharded over GPUs')
+        if est.cfg['host_warps']:
+            raise ValueError("an object set cuts its crops on the device: cfg['host_warps'] must be False")
+        self.est = est
+        self._objects = {}
+        self._kernels = None            # the objects' detector kernels concatenated (rebuilt when membership changes)
+        self.stages = StageCache()      # the set's prediction graph
+
+    # -------------------------------------------------------------- membership
+    @property
+    def names(self):
+        return list(self._objects)
+
+    def __len__(self):
+        return len(self._objects)
+
+    def __contains__(self, name):
+        return name in self._objects
+
+    def add(self, name, database):
+        """Compute `database`'s reference state (what est.build(database, 'all') computes) and store it under `name`.
+        A reference-repo database is wrapped as build() does; cfg['device_build'] is honoured."""
+        from .database import as_object_database
+        if name in self._objects:
+            raise ValueError(f'object {name!r} is already in the set')
+        est = self.est
+        database = as_object_database(database)
+        v = est._reference_views(database)
+        det_imgs = v['imgs'][:est.cfg['det_ref_view_num']]
+        if self._objects:
+            rfn = next(iter(self._objects.values())).det.rfn
+            if len(det_imgs) != rfn:
+                raise ValueError(f'object {name!r} has {len(det_imgs)} detector reference views, the set\'s objects have {rfn}: '
+                                 'the detection correlation concatenates the objects\' kernels, so every object needs '
+                                 f"det_ref_view_num ({est.cfg['det_ref_view_num']}) views; a database with fewer views "
+                                 'than that gives fewer')
+        weights_gen = est._weights_generation()
+        det = est.detector.make_refs_u8(det_imgs)
+        sel = est.selector.make_refs(v['ref_imgs'], v['poses'], v['center'], v['vert'])
+        ref = est.refiner.make_refs(database, v['ids_all'])
+        ref_info = {k: v[k] for k in ('imgs', 'ref_imgs', 'Ks', 'poses', 'center', 'ref_ids')}
+        tables = est._device_tables(ref_info, ref)          # synchronises: the state is complete before any use
+        counters = est.selector.s2_counters_for(sel, est.selector.device)
+        self._objects[name] = _Object(det, sel, ref, ref_info, tables, counters, weights_gen)
+        self._membership_changed()
+
+    def remove(self, name):
+        if name not in self._objects:
+            raise ValueError(f'object {name!r} is not in the set (objects: {self.names})')
+        del self._objects[name]
+        self._membership_changed()
+
+    def _membership_changed(self):
+        self._kernels = None
+        self.stages.clear()             # the graph captured the previous objects' state
+
+    def _check(self):
+        if not self._objects:
+            raise ValueError('the object set is empty: add objects first')
+        gen = self.est._weights_generation()
+        stale = [n for n, o in self._objects.items() if o.weights_gen != gen]
+        if stale:
+            raise RuntimeError(f'objects {stale} are stale: the networks\' weights changed since they were added, and their '
+                               'reference features were computed with the old weights; remove and add them again')
+
+    def _detector_kernels(self):
+        if self._kernels is None:
+            with torch.no_grad():
+                self._kernels = self.est.detector.pack_kernels([o.det.center_feats for o in self._objects.values()])
+        return self._kernels
+
+    # -------------------------------------------------------------- prediction
+    def _detect(self, u8, return_taps=False):
+        """uint8 frames [qn,h,w,3] -> detector outputs of K*qn object-major rows (and taps)."""
+        objs = list(self._objects.values())
+        det = self.est.detector
+        o = det._detect_objects_nhwc(ops.preprocess_u8(u8, out_c=3, imagenet_norm=False), self._detector_kernels(),
+                                     len(objs), objs[0].det.rfn, return_taps)
+        out, _ = ops.det_parse(o['score_predict'], o['scale_predict'], o['offset_predict'], det.pool_ratio)
+        return out, o
+
+    def _predict_fn(self):
+        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> (packed results f64 as bytes ++ crops u8): every stage, back to back."""
+        est = self.est
+        objs = list(self._objects.values())
+        K, res, iters = len(objs), est.cfg['ref_resolution'], est.cfg['refine_iter']
+        R = objs[0].tables['tables']['ref_num']
+        sel, refine = est.selector, est.refiner._refine_warped(128)
+
+        def fn(frames, cams):
+            qn = frames.shape[0]
+            rows = lambda t, o: t[o * qn:(o + 1) * qn]
+            cat = lambda ts: ts[0] if len(ts) == 1 else torch.cat(ts, 0)
+            det, _ = self._detect(frames)                                            # [K*qn,4]: x, y, scale, score
+            jobs = cat([ops.glue_detection_jobs(rows(det, o), frames, res) for o in range(K)])
+            crop = ops.warp_affine_u8(jobs, K * qn, res, res)
+            feats = sel._feats(ops.preprocess_u8(crop, out_c=4, imagenet_norm=True))  # the crop VGG once for all objects
+            poses, sels = [], []
+            for o, ob in enumerate(objs):
+                lg, ang = [], []
+                for qi in range(qn):
+                    l, a, _ = sel._select_one([f[o * qn + qi] for f in feats], ob.sel, ob.counters)
+                    lg.append(l)
+                    ang.append(a)
+                logits = torch.stack(lg, 0)
+                idx, sel_out = ops.sel_parse(logits, torch.stack(ang, 0))
+                sels.append((idx, sel_out, logits))
+                poses.append(ops.glue_initial_poses(rows(det, o), idx, sel_out, ob.tables['refs'], cams))
+            chains = [[p] for p in poses]
+            for it in range(iters):
+                probs = [ops.glue_refine_problems(ob.tables['views'], R, cams, frames, poses[o], it > 0) for o, ob in enumerate(objs)]
+                jobs_r, que_K, que_pose, ref_Ks, ref_poses = [cat([p[i] for p in probs]) for i in (0, 1, 2, 4, 5)]
+                out = refine(jobs_r, que_K, que_pose, ref_Ks, ref_poses)              # one refiner stage for all K*qn poses
+                poses = [ops.glue_apply_refinements(ob.tables['views'], probs[o][2], probs[o][1], probs[o][3], rows(out, o))
+                         for o, ob in enumerate(objs)]
+                for o in range(K):
+                    chains[o].append(poses[o])
+            parts = []
+            for o in range(K):
+                idx, sel_out, logits = sels[o]
+                parts += [torch.stack(chains[o], 0), rows(det, o), idx, sel_out, logits]
+            packed = torch.cat([t.reshape(-1).to(torch.float64) for t in parts])
+            return torch.cat([packed.view(torch.uint8), crop.reshape(-1)])
+        return fn
+
+    def predict(self, que_imgs, que_Ks):
+        """Every object's pose on the same qn frames (uint8 [h,w,3] of one size; que_Ks [qn,3,3]).
+        Returns {name: (poses [qn,3,4], inter)}: inter has the keys and shapes of predict_batch's device-glue inter, plus
+        'det_score' [qn], the maximum of that object's detection score map (is the object in the frame at all)."""
+        self._check()
+        est = self.est
+        qn, res, iters = len(que_imgs), est.cfg['ref_resolution'], est.cfg['refine_iter']
+        if qn == 0 or len(que_Ks) != qn:
+            raise ValueError(f'predict: {qn} frames and {len(que_Ks)} intrinsics; need one K per frame and at least one frame')
+        det = est.detector
+        with torch.no_grad():
+            frames = det.upload_frame([np.asarray(f) for f in que_imgs])
+            cams = det._to_dev(glue.cameras(np.stack([np.asarray(K) for K in que_Ks], 0)))
+            buf = self.stages.run('predict', self._predict_fn(), [frames, cams])
+            host = det._to_host(buf)                                       # the call's one synchronising read
+        crop_bytes = len(self._objects) * qn * res * res * 3
+        f64 = host[:len(host) - crop_bytes].view(np.float64)
+        crops = host[len(host) - crop_bytes:].reshape(len(self._objects), qn, res, res, 3)
+        out, off = {}, 0
+        for o, (name, ob) in enumerate(self._objects.items()):
+            n_sel = len(ob.ref_info['poses'])
+
+            def take(n):
+                nonlocal off
+                off += n
+                return f64[off - n:off]
+            chain = take((iters + 1) * qn * 12).reshape(iters + 1, qn, 3, 4)
+            d = take(qn * 4).reshape(qn, 4).astype(np.float32)
+            idx = take(qn).astype(np.int64)
+            sel_out = take(qn * 2).reshape(qn, 2).astype(np.float32)
+            logits = take(qn * n_sel).reshape(qn, n_sel).astype(np.float32)
+            refined = [c.astype(np.float32) for c in chain[1:]]
+            inter = {'det_position': d[:, :2].copy(), 'det_scale_r2q': d[:, 2].copy(), 'det_score': d[:, 3].copy(),
+                     'det_que_img': crops[o].copy(), 'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': logits,
+                     'sel_ref_idx': idx, 'refine_poses': [chain[0].copy()] + refined}
+            out[name] = (refined[-1] if refined else chain[0].copy(), inter)
+        return out
+
+    def raw_correlation(self, que_imgs):
+        """The detector's raw correlation maps for inspection: {name: [scale][level] float32 [qn, H, W, rfn]} (the maps
+        _detect_nhwc(return_taps=True)['raw'] holds for a single object), computed eagerly with the shared pyramid."""
+        self._check()
+        det = self.est.detector
+        qn = len(que_imgs)
+        with torch.no_grad():
+            frames = det.upload_frame([np.asarray(f) for f in que_imgs])
+            _, taps = self._detect(frames, return_taps=True)
+        return {name: [[m[o * qn:(o + 1) * qn] for m in scale] for scale in taps['raw']]
+                for o, name in enumerate(self._objects)}

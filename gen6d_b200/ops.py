@@ -456,6 +456,18 @@ def det_corr_rowsum(partial, k, rfn):
     return out
 
 
+def det_corr_rowsum_objects(partial, n_obj, k, rfn):
+    """partial [qn, H+k-1, W, n_obj*k*rfn] (one 1 x k convolution over n_obj objects' kernels, channel = (obj*k + ky)*rfn + r)
+    -> object-major k x k correlations [n_obj, qn, H, W, rfn].  k = 1: a direct correlation [qn, H, W, n_obj*rfn] regrouped."""
+    qn, Hp, W, Cc = partial.shape
+    if Cc != n_obj * k * rfn:
+        raise ValueError(f'det_corr_rowsum_objects: {Cc} channels, expected n_obj*k*rfn = {n_obj}*{k}*{rfn}')
+    H = Hp - (k - 1)
+    out = torch.empty(n_obj, qn, H, W, rfn, device=partial.device, dtype=torch.float32)
+    _call('g6d_det_corr_rowsum_objects', _p(partial), _p(out), n_obj, qn, H, W, k, rfn, _stream())
+    return out
+
+
 def det_parse(scores, scales, offsets, pool_ratio=8):
     """scores/scales [qn,hs,ws,1], offsets [qn,hs,ws,2] -> (out [qn,4] = x,y,scale,score; idx [qn] int64)."""
     qn, hs, ws, _ = scores.shape

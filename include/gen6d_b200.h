@@ -292,6 +292,13 @@ int g6d_det_score_fuse(const g6d_det_maps* host_maps, int qn, const float* w1, c
  * contribution of kernel row ky to input row y'; out[q,y,x,r] = sum_ky partial[q, y+ky, x, ky*rfn + r]
  * is the k x k correlation map [qn, H, W, rfn].  rfn % 4 == 0. */
 int g6d_det_corr_rowsum(const float* partial, float* out, int qn, int H, int W, int k, int rfn, g6d_stream_t stream);
+/* g6d_det_corr_rowsum for n_obj objects at once: partial [qn, H+k-1, W, n_obj*k*rfn] is ONE 1 x k convolution with
+ * the objects' kernels concatenated along its output channels (channel = (obj*k + ky)*rfn + r);
+ * out[obj,q,y,x,r] = sum_ky partial[q, y+ky, x, (obj*k + ky)*rfn + r] is object-major [n_obj, qn, H, W, rfn], the k
+ * rows added in g6d_det_corr_rowsum's order.  k = 1 regroups a direct correlation [qn, H, W, n_obj*rfn].
+ * n_obj > 0, rfn % 4 == 0. */
+int g6d_det_corr_rowsum_objects(const float* partial, float* out, int n_obj, int qn, int H, int W, int k, int rfn,
+                                g6d_stream_t stream);
 /* detector.py:85-121: first-max flat argmax of scores [qn,hs,ws,1], then
  * position = ((x,y) + offset[y,x] + 0.5)*pool - 0.5, scale = 2**scale[y,x].
  * out [qn, 4] = (x, y, scale, score); out_idx [qn] (int64 flat index y*ws + x). */
