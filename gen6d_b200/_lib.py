@@ -84,6 +84,7 @@ _SIGNATURES = {
     'g6d_conv_tc_workspace_bytes': [C.POINTER(ConvDesc), I],
     'g6d_conv_tc': [C.POINTER(ConvDesc), P, P, P, I, I, P, P, P, P, P, P, L, P],
     'g6d_conv_tc_stats_supported': [C.POINTER(ConvDesc), I, L],
+    'g6d_conv_tc_plan': [C.POINTER(ConvDesc), I, C.POINTER(C.c_int)],
     'g6d_pack_conv_weight_tc': [P, P, P, I, I, I, I, I, P, I, P],
     'g6d_split_operand': [P, P, P, L, I, P],
     'g6d_transpose2d': [P, P, I, I, P],

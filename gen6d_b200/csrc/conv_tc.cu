@@ -25,7 +25,8 @@
 //               128-bit loads, register prefetch ring; 16 rows per warp), apply the folded
 //               InstanceNorm(+ReLU) / selector q(.)ref prologue to in-bounds elements, split into hi/lo
 //               and st.shared both tiles in the canonical K-major SWIZZLE_128B layout the wgmma
-//               descriptor expects;
+//               descriptor expects (conv_tc2_kernel with a split input: one thread loads the same tiles
+//               by TMA im2col instead, see split_input_ok);
 //   warps 8-15  two consumer warpgroups, rows 0-63 and 64-127 of the tile, both reading the same
 //               weight tiles of a stage: 12 wgmmas per K-block each (4 K-steps x 3 split terms),
 //               one group in flight while the next stage is awaited, then the
@@ -40,6 +41,7 @@
 // conv_tc2_kernel handles general strides / shapes (persistent); conv_tcflat_kernel (stride-1
 // multi-tap convolutions whose halo fits in shared memory) reuses the A operand across taps, see below.
 #include <cuda_fp16.h>
+#include <string.h>
 
 #include "tc_common.cuh"
 
@@ -91,6 +93,7 @@ struct ConvTcP {
     long long group_rows;
     int M, K, kblocks, splits, kb_per_split;
     double* stats; long long stats_rows;      // fused InstanceNorm statistics of the OUTPUT (see epilogue_stats)
+    int split_in;                             // A tiles by TMA im2col from the pre-split input (see split_input_ok)
 };
 
 // ------------------------------------------------------------------------------------------ operand split
@@ -138,6 +141,16 @@ __device__ __forceinline__ void split_store(uint32_t hi_addr, uint32_t lo_addr, 
         st_shared_v2(lo_addr + 8 * e, l[0], l[1]);
     }
 }
+// 128 pixels x 64 fp16 channels of a 4-D NHWC tensor by TMA im2col: the pixels the traversal of the map's
+// bounding box reaches from (w, h, n), each shifted by the filter tap (ox, oy), one 128-byte swizzled row each;
+// pixels outside the tensor arrive as zeros
+__device__ __forceinline__ void tma_im2col_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c, int w, int h, int n,
+                                              uint16_t ox, uint16_t oy) {
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
+        ::"r"(dst), "l"(map), "r"(bar), "r"(c), "r"(w), "r"(h), "r"(n), "h"(ox), "h"(oy) : "memory");
+}
+
 __device__ __forceinline__ float4 affine4(float4 x, const float4 sc, const float4 sh, bool relu) {
     x.x = fmaf(x.x, sc.x, sh.x); x.y = fmaf(x.y, sc.y, sh.y); x.z = fmaf(x.z, sc.z, sh.z); x.w = fmaf(x.w, sc.w, sh.w);
     if (relu) { x.x = fmaxf(x.x, 0.f); x.y = fmaxf(x.y, 0.f); x.z = fmaxf(x.z, 0.f); x.w = fmaxf(x.w, 0.f); }
@@ -282,7 +295,7 @@ struct Tc2Work { int m_tiles, n_tiles, total; };
 template <int BN, int KIND>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUtensorMap map_hi,
-                const __grid_constant__ CUtensorMap map_lo) {
+                const __grid_constant__ CUtensorMap map_lo, const __grid_constant__ CUtensorMap map_a) {
     using Cfg = Tc2Cfg<BN>;
     using KC = KindCfg<KIND>;
     constexpr int NPW = TC_PRODUCER_WARPS;
@@ -307,13 +320,14 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == TC_ISSUER) {
         for (int s = 0; s < STAGES; ++s) {
-            mbar_init(full_a(s), NPW);        // the producer warps
+            mbar_init(full_a(s), p.split_in ? 1 : NPW);   // the A TMA transaction, or the producer warps
             mbar_init(full_b(s), 1);          // the TMA transaction
             mbar_init(empty(s), TC_CONSUMER_WARPS);
         }
         fence_barrier_init();
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_lo) : "memory");
+        if (p.split_in) asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
     }
     __syncthreads();
 
@@ -327,6 +341,38 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
 
     if (warp < NPW) {
         setmaxnreg_dec<TC_PRODUCER_REGS>();
+        if (p.split_in) {
+            // =========================== A by TMA im2col ===========================
+            // The input is already split (hi / lo of channel block cb at channels [128 cb, 128 cb + 64) /
+            // [128 cb + 64, 128 cb + 128) of each pixel, in f16_k_source order), so a K-block of tap (kx, ky)
+            // is two im2col boxes of the 128 output pixels of the tile: byte for byte what the producers
+            // below would store.  One thread issues them; the other producer warps have nothing to do.
+            if (threadIdx.x == 0) {
+                int g = 0;
+                for (int w = blockIdx.x; w < wk.total; w += gridDim.x) {
+                    int mt, nt, sp;
+                    decode(w, mt, nt, sp);
+                    const int nkb = kblocks_of(sp);
+                    int m = mt * TC_BM;
+                    const int xo = m % p.Wo; m /= p.Wo;
+                    const int yo = m % p.Ho;
+                    const int b = m / p.Ho;
+                    const int k = sp * p.kb_per_split * BK;
+                    int tap = k / p.Cin, c0 = k - tap * p.Cin;
+                    for (int it = 0; it < nkb; ++it, ++g) {
+                        const int s = g % STAGES;
+                        mbar_wait(empty(s), ((g / STAGES) & 1) ^ 1, 1, g);
+                        mbar_expect_tx(full_a(s), 2 * Cfg::A_BYTES);
+                        const uint16_t ox = (uint16_t)(tap % p.kw), oy = (uint16_t)(tap / p.kw);
+                        tma_im2col_4d(a_hi(s), &map_a, full_a(s), 2 * c0, xo - p.pw, yo - p.ph, b, ox, oy);
+                        tma_im2col_4d(a_lo(s), &map_a, full_a(s), 2 * c0 + BK, xo - p.pw, yo - p.ph, b, ox, oy);
+                        c0 += BK;
+                        if (c0 == p.Cin) { c0 = 0; ++tap; }
+                    }
+                }
+            }
+            return;
+        }
         // =============================== A producers ===============================
         // All producer warps fill every K-block: ROWS rows x one 16-byte smem chunk (4 or 8 channels) per thread.
         const int chunk = threadIdx.x & 7;
@@ -623,6 +669,43 @@ static int make_weight_map(CUtensorMap* map, const void* w, int rows, int K, int
     return G6D_OK;
 }
 
+typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                   const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*, CUtensorMapInterleave,
+                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+static EncodeIm2colFn get_encode_im2col_fn() {
+    static EncodeIm2colFn fn = nullptr;
+    static bool tried = false;
+    if (!tried) {
+        tried = true;
+        void* sym = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &sym, cudaEnableDefault, &qres) == cudaSuccess &&
+            qres == cudaDriverEntryPointSuccess)
+            fn = reinterpret_cast<EncodeIm2colFn>(sym);
+    }
+    return fn;
+}
+
+// im2col map over the split input [B, H, W, 2 Cin] fp16: 64 channels x 128 pixels per box (one 128-byte swizzle
+// row per pixel); the bounding box of filter origins runs from -pad to dim - 1 + pad - (k - 1), i.e. the output
+// plane of a stride-1 convolution, and taps outside the tensor are filled with zeros (the padding)
+static int make_split_input_map(CUtensorMap* map, const void* xs, const g6d_conv_desc* d) {
+    EncodeIm2colFn enc = get_encode_im2col_fn();
+    if (!enc) { set_error("g6d_conv_tc: cuTensorMapEncodeIm2col unavailable"); return G6D_ECUDA; }
+    const cuuint64_t C2 = 2ull * d->Cin;
+    cuuint64_t dims[4] = {C2, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->B};
+    cuuint64_t strides[3] = {C2 * 2, C2 * 2 * d->W, C2 * 2 * d->W * d->H};
+    int lower[2] = {-d->pw, -d->ph};
+    int upper[2] = {d->pw - (d->kw - 1), d->ph - (d->kh - 1)};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(xs), dims, strides, lower, upper, 64, TC_BM, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_error("g6d_conv_tc: cuTensorMapEncodeIm2col failed (%d)", (int)r); return G6D_ECUDA; }
+    return G6D_OK;
+}
+
 static int tc_block_n(int Cout) { return Cout > 64 ? 128 : (Cout > 32 ? 64 : 32); }
 static int tc_nmain(int bn) { return bn == 32 ? AccCfg<32>::NMAIN : (bn == 64 ? AccCfg<64>::NMAIN : AccCfg<128>::NMAIN); }
 
@@ -687,7 +770,7 @@ static int fill_tc_params(const g6d_conv_desc* d, int kind, ConvTcP& p) {
 }
 
 template <int BN, int KIND>
-static int launch_tc2(const ConvTcP& p, const CUtensorMap& mh, const CUtensorMap& ml, cudaStream_t st) {
+static int launch_tc2(const ConvTcP& p, const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& ma, cudaStream_t st) {
     using Cfg = Tc2Cfg<BN>;
     static bool configured = false;
     if (!configured) {
@@ -700,7 +783,7 @@ static int launch_tc2(const ConvTcP& p, const CUtensorMap& mh, const CUtensorMap
     const long long total = (long long)wk.m_tiles * wk.n_tiles * p.splits;
     wk.total = (int)total;
     const int grid = total < kNumSMs ? (int)total : kNumSMs;
-    conv_tc2_kernel<BN, KIND><<<grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(p, wk, mh, ml);
+    conv_tc2_kernel<BN, KIND><<<grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(p, wk, mh, ml, ma);
     G6D_CHECK_LAUNCH("g6d_conv_tc");
     return G6D_OK;
 }
@@ -725,6 +808,30 @@ __global__ void split_f16_kernel(const float* __restrict__ in, __half* __restric
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     split_f16_scalar(in[(i & ~63ll) + f16_k_source((int)(i & 63))], hi[i], lo[i]);
+}
+
+// Activation [rows, ics] (channels [ico, ico + Cin)) -> split form [rows, 2 Cin] fp16 for the im2col A loads: channel
+// block cb of a row holds hi at [128 cb, 128 cb + 64) and lo at [128 cb + 64, 128 cb + 128), position p from channel
+// 64 cb + f16_k_source(p).  A thread makes one 16-byte chunk of each from the same two float4 loads and the same
+// split_f16x2 calls as a producer thread of conv_tc2_kernel, so the tiles are bit-identical.
+__global__ void split_input_f16_kernel(const float* __restrict__ x, int ics, int ico, int Cin, long long rows,
+                                       __half* __restrict__ out) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int chunks = Cin / 8;
+    if (i >= rows * chunks) return;
+    const long long r = i / chunks;
+    const int q = (int)(i - r * chunks), cb = q >> 3, c = q & 7;
+    const float* src = x + r * ics + ico + cb * 64 + 4 * c;
+    const float4 a = __ldg(reinterpret_cast<const float4*>(src));
+    const float4 b = __ldg(reinterpret_cast<const float4*>(src + 32));
+    uint4 h, l;
+    split_f16x2(a.x, a.y, h.x, l.x);
+    split_f16x2(a.z, a.w, h.y, l.y);
+    split_f16x2(b.x, b.y, h.z, l.z);
+    split_f16x2(b.z, b.w, h.w, l.w);
+    __half* row = out + r * 2 * Cin + cb * 128;
+    *reinterpret_cast<uint4*>(row + 8 * c) = h;
+    *reinterpret_cast<uint4*>(row + 64 + 8 * c) = l;
 }
 
 // [Cout, Cin, taps] (reference layout) -> hi/lo [rows_pad, taps*Cin_pad], K index = tap*Cin_pad + c
@@ -1065,7 +1172,18 @@ struct ConvPlan {
     ConvFlatP flat;            // the A-reuse kernel's parameters when use_flat
     bool use_flat;
     int bn, splits, flat_smem;
+    long long split_in_off;    // byte offset of the split input in the workspace (tc.split_in)
+    long long ws_bytes;        // workspace: split-K partials, then the split input
 };
+
+// The persistent kernel loads A by TMA im2col from a pre-split copy of the input for fp16 multi-tap 2-D
+// convolutions with stride 1 and no prologue: the gather, split and swizzle of 8 producer warps (each input
+// element once per tap, 16 KB in flight per SM) become two bulk copies per K-block.  The split pass reads and
+// writes the input once.  The bounding box of the im2col map is the output plane shifted by the padding.
+static bool split_input_ok(const g6d_conv_desc* d, int kind, bool use_flat) {
+    return !use_flat && kind == G6D_TC_F16 && d->prologue == G6D_PRO_NONE && d->stride == 1 && d->kd == 1 && d->D == 1 &&
+           d->kh * d->kw > 1 && d->kw <= 64 && d->kh <= 64 && d->pw < 64 && d->ph < 64;
+}
 
 static int make_plan(const g6d_conv_desc* d, int kind, ConvPlan& pl) {
     const int rc = fill_tc_params(d, kind, pl.tc);
@@ -1073,6 +1191,11 @@ static int make_plan(const g6d_conv_desc* d, int kind, ConvPlan& pl) {
     pl.use_flat = fill_flat_params(d, kind, pl.flat, &pl.flat_smem);
     pl.bn = tc_block_n(d->Cout);
     pl.splits = pl.use_flat ? pl.flat.splits : pl.tc.splits;
+    pl.tc.split_in = split_input_ok(d, kind, pl.use_flat) ? 1 : 0;
+    const long long partials = pl.splits > 1 ? (long long)pl.splits * pl.tc.M * pl.tc.Cout * (long long)sizeof(float) : 0;
+    pl.split_in_off = (partials + 255) / 256 * 256;
+    pl.ws_bytes = pl.tc.split_in ? pl.split_in_off + (long long)d->B * d->H * d->W * d->Cin * 2 * (long long)sizeof(__half)
+                                 : partials;
     return G6D_OK;
 }
 
@@ -1091,14 +1214,14 @@ static void bind_tensors(P& p, const float* x, const float* bias, const float* p
 }
 
 template <int BN, int KIND>
-static int launch_plan(const ConvPlan& pl, const CUtensorMap& mh, const CUtensorMap& ml, cudaStream_t st) {
-    return pl.use_flat ? launch_flat<BN, KIND>(pl.flat, pl.flat_smem, mh, ml, st) : launch_tc2<BN, KIND>(pl.tc, mh, ml, st);
+static int launch_plan(const ConvPlan& pl, const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& ma, cudaStream_t st) {
+    return pl.use_flat ? launch_flat<BN, KIND>(pl.flat, pl.flat_smem, mh, ml, st) : launch_tc2<BN, KIND>(pl.tc, mh, ml, ma, st);
 }
 template <int KIND>
-static int dispatch(const ConvPlan& pl, const CUtensorMap& mh, const CUtensorMap& ml, cudaStream_t st) {
-    if (pl.bn == 128) return launch_plan<128, KIND>(pl, mh, ml, st);
-    if (pl.bn == 64) return launch_plan<64, KIND>(pl, mh, ml, st);
-    return launch_plan<32, KIND>(pl, mh, ml, st);
+static int dispatch(const ConvPlan& pl, const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& ma, cudaStream_t st) {
+    if (pl.bn == 128) return launch_plan<128, KIND>(pl, mh, ml, ma, st);
+    if (pl.bn == 64) return launch_plan<64, KIND>(pl, mh, ml, ma, st);
+    return launch_plan<32, KIND>(pl, mh, ml, ma, st);
 }
 
 }  // namespace g6d
@@ -1127,12 +1250,24 @@ extern "C" int g6d_conv_tc_supported(const g6d_conv_desc* d, int kind) {
 extern "C" long long g6d_conv_tc_workspace_bytes(const g6d_conv_desc* desc, int kind) {
     ConvPlan pl{};
     if (make_plan(desc, kind, pl) != G6D_OK) return -1;
-    return pl.splits > 1 ? (long long)pl.splits * pl.tc.M * pl.tc.Cout * (long long)sizeof(float) : 0;
+    return pl.ws_bytes;
 }
 
 extern "C" int g6d_conv_tc_stats_supported(const g6d_conv_desc* desc, int kind, long long stats_rows) {
     ConvPlan pl{};
     return make_plan(desc, kind, pl) == G6D_OK && stats_ok(pl, stats_rows) ? 1 : 0;
+}
+
+extern "C" int g6d_conv_tc_plan(const g6d_conv_desc* desc, int kind, int* out4) {
+    G6D_REQUIRE(out4 != nullptr, "g6d_conv_tc_plan: null output");
+    ConvPlan pl{};
+    const int rc = make_plan(desc, kind, pl);
+    if (rc != G6D_OK) return rc;
+    out4[0] = pl.use_flat ? 1 : 0;
+    out4[1] = pl.bn;
+    out4[2] = pl.splits;
+    out4[3] = pl.tc.split_in;
+    return G6D_OK;
 }
 
 extern "C" int g6d_conv_tc(const g6d_conv_desc* desc, const float* x, const void* w_hi, const void* w_lo, int w_rows,
@@ -1146,7 +1281,7 @@ extern "C" int g6d_conv_tc(const g6d_conv_desc* desc, const float* x, const void
     G6D_REQUIRE(x && w_hi && w_lo && y, "g6d_conv_tc: null tensor pointer");
     G6D_REQUIRE(w_rows >= p.Cout, "g6d_conv_tc: weight rows (%d) < Cout (%d)", w_rows, p.Cout);
     if (p.pro != G6D_PRO_NONE) G6D_REQUIRE(pro_scale && pro_shift, "g6d_conv_tc: prologue operands missing");
-    if (pl.splits > 1) G6D_REQUIRE(ws != nullptr, "g6d_conv_tc: split workspace required (%d splits)", pl.splits);
+    if (pl.ws_bytes > 0) G6D_REQUIRE(ws != nullptr, "g6d_conv_tc: workspace required (%lld bytes)", pl.ws_bytes);
     cudaStream_t st = as_stream(stream);
     if (stats) {
         cudaError_t e = cudaMemsetAsync(stats, 0, sizeof(double) * 2 * (p.M / stats_rows) * p.Cout, st);
@@ -1154,10 +1289,18 @@ extern "C" int g6d_conv_tc(const g6d_conv_desc* desc, const float* x, const void
     }
     if (pl.use_flat) bind_tensors(pl.flat, x, bias, pro_scale, pro_shift, y, ws, stats, stats_rows);
     else bind_tensors(pl.tc, x, bias, pro_scale, pro_shift, y, ws, stats, stats_rows);
-    CUtensorMap mh, ml;
+    CUtensorMap mh, ml, ma;
     if ((rc = make_weight_map(&mh, w_hi, w_rows, p.K, pl.bn, kind)) != G6D_OK) return rc;
     if ((rc = make_weight_map(&ml, w_lo, w_rows, p.K, pl.bn, kind)) != G6D_OK) return rc;
-    rc = kind == G6D_TC_F16 ? dispatch<G6D_TC_F16>(pl, mh, ml, st) : dispatch<G6D_TC_TF32>(pl, mh, ml, st);
+    memset(&ma, 0, sizeof(ma));
+    if (p.split_in) {
+        __half* xs = reinterpret_cast<__half*>(static_cast<char*>(ws) + pl.split_in_off);
+        if ((rc = make_split_input_map(&ma, xs, desc)) != G6D_OK) return rc;
+        const long long rows = (long long)p.B * p.H * p.W, n = rows * (p.Cin / 8);
+        split_input_f16_kernel<<<ceil_div(n, 256), 256, 0, st>>>(x, p.ics, p.ico, p.Cin, rows, xs);
+        G6D_CHECK_LAUNCH("g6d_conv_tc(split input)");
+    }
+    rc = kind == G6D_TC_F16 ? dispatch<G6D_TC_F16>(pl, mh, ml, ma, st) : dispatch<G6D_TC_TF32>(pl, mh, ml, ma, st);
     if (rc != G6D_OK) return rc;
     if (pl.splits > 1) {
         launch_reduce(static_cast<float*>(ws), bias, y, p.M, p.Cout, pl.splits, p.ocs, p.oco, p.act, stats, stats_rows, st);

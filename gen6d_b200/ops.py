@@ -62,7 +62,7 @@ def collect_profile(prof):
     out = {k: {'ms': sum(r[0].elapsed_time(r[1]) for r in v), 'work': float(sum(r[2] for r in v)), 'n': len(v)}
            for k, v in prof.items() if k != '#calls'}
     if '#calls' in prof:
-        out['#calls'] = [(r[0].elapsed_time(r[1]), r[2], r[3], r[4]) for r in prof['#calls']]
+        out['#calls'] = [(r[0].elapsed_time(r[1]), r[2], r[3], r[4]() if callable(r[4]) else r[4]) for r in prof['#calls']]
     return out
 
 
@@ -392,10 +392,14 @@ def conv(x, pc, prologue=PRO_NONE, pro_scale=None, pro_shift=None, group_rows=1,
         fuse = stats_rows is not None and _lib.lib().g6d_conv_tc_stats_supported(C.byref(d), pc.kind, stats_rows)
         if fuse:
             stats = torch.empty(M // stats_rows, pc.cout, 2, device=x.device, dtype=torch.float64)
+        def tag(d=d, kind=pc.kind):        # formatted by collect_profile, outside the timed launches
+            plan = (C.c_int * 4)()
+            _lib.check(_lib.lib().g6d_conv_tc_plan(C.byref(d), kind, plan), 'g6d_conv_tc_plan')
+            return (f'M={M} N={pc.cout} K={kd * kh * kw * pc.cin} k={kd}x{kh}x{kw} s={s} pro={prologue} '
+                    f'{"reuse" if plan[0] else "persist"} BN={plan[1]} splits={plan[2]}{" im2col" if plan[3] else ""}')
         _call('g6d_conv_tc', C.byref(d), _p(x), _p(pc.w_hi, pc.w_hi.dtype), _p(pc.w_lo, pc.w_lo.dtype), pc.w_hi.shape[0],
               pc.kind, _p(pc.bias), _p(pro_scale), _p(pro_shift), _p(out), _p(ws), _p(stats, torch.float64), stats_rows or 0,
-              _stream(), work=work,
-              tag=f'M={M} N={pc.cout} K={kd * kh * kw * pc.cin} k={kd}x{kh}x{kw} s={s} pro={prologue}')
+              _stream(), work=work, tag=tag)
     else:
         if pc.w is None:
             raise _lib.Gen6DLibraryError('this operand was packed for the tensor-core path only and the problem is not supported there')

@@ -253,6 +253,11 @@ long long g6d_conv_tc_workspace_bytes(const g6d_conv_desc* desc, int kind);
  * g6d_instnorm_partial computes in a separate pass over y; feed them to g6d_instnorm_finalize.  Zeroed by
  * the call.  Allowed when g6d_conv_tc_stats_supported (groups made of whole 32-row slices / image planes). */
 int g6d_conv_tc_stats_supported(const g6d_conv_desc* desc, int kind, long long stats_rows);
+/* What g6d_conv_tc would launch for desc (no launch): out4 = {kernel (0 persistent, 1 A-reuse), BN, K splits,
+ * split input (1: the persistent kernel loads A by TMA im2col from an fp16 hi/lo copy of x that the call writes
+ * into the workspace -- fp16 kind, stride 1, no prologue, 2-D multi-tap)}.  G6D_EINVAL with g6d_conv_tc's
+ * message when the descriptor is rejected. */
+int g6d_conv_tc_plan(const g6d_conv_desc* desc, int kind, int* out4);
 int g6d_conv_tc(const g6d_conv_desc* desc, const float* x, const void* w_hi, const void* w_lo, int w_rows, int kind,
                 const float* bias, const float* pro_scale, const float* pro_shift, float* y, void* ws,
                 double* stats, long long stats_rows, g6d_stream_t stream);

@@ -1,26 +1,141 @@
-"""Per-call time / TFLOP/s of every tensor-core convolution in one pose step (eager, CUDA events)."""
-import os, sys, collections
-import numpy as np, torch
+"""Time / TFLOP/s of every tensor-core convolution in one batched pose step, per shape.
+
+    python tools/conv_breakdown.py [--batch B] [--refine-iter N] [--reps C] [--repeat R]
+
+The stages of one `predict_batch` over B synthetic frames (detect -> select -> N refinements; bench.py's
+workload is B = 10, N = 3) are recorded with their device inputs and replayed once eagerly to collect the
+arguments of every convolution.  Each distinct call is then timed on its own: a CUDA graph of C copies of
+it, replayed R times, median per copy (timing the calls inside the eager replay would measure the host
+whenever a kernel is shorter than its launch).  Each line aggregates the calls of one tag; the tag names
+the kernel the planner picked (persist: the persistent kernel, reuse: the A-reuse kernel), the prologue,
+BN and the K splits.  Times are per step of B poses."""
+import argparse
+import collections
+import os
+import sys
+
+import torch
+
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from gen6d_b200 import geometry as G, ops, synthetic as syn
-est, db = syn.build_estimator()
-ids = db.get_img_ids(); K = db.K
-img = db.get_image(ids[7])
-pose0, inter = est.predict(img, K)
-dev = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
-frame, crop = dev(img[None]), dev(inter['det_que_img'][None])
-pr = G.refine_problem(db, ids, img, K, inter['refine_poses'][0], 128, 6, True)
-prob = [dev(pr[k][None]) for k in ('que_img', 'que_K', 'que_pose', 'ref_imgs', 'ref_Ks', 'ref_poses')]
-def step():
-    with torch.no_grad():
-        est.detector._detect_u8(frame); est.selector._select_u8(crop); est.refiner._refine_u8(*prob)
-step(); torch.cuda.synchronize()
-prof = ops.enable_profiling(); step(); st = ops.collect_profile(prof)
-calls = st['#calls']
-tot = sum(c[0] for c in calls)
-print(f'conv_tc calls {len(calls)} total {tot:.2f} ms, {sum(c[1] for c in calls)/tot/1e9:.1f} TFLOP/s')
-agg = collections.OrderedDict()
-for ms, work, name, tag in calls:
-    a = agg.setdefault(tag, [0, 0.0, 0.0]); a[0] += 1; a[1] += ms; a[2] += work
-for tag, (n, ms, work) in sorted(agg.items(), key=lambda kv: -kv[1][1])[:40]:
-    print(f'{ms:7.3f} ms x{n:2d} {work/ms/1e9:6.1f} TF/s  {tag}')
+from gen6d_b200 import ops, synthetic as syn  # noqa: E402
+
+
+def record_step(batch, refine_iter):
+    """(estimator, [(stage fn, inputs)]) of one predict_batch over `batch` frames."""
+    est, db = syn.build_estimator(refine_iter=refine_iter)
+    ids = db.get_img_ids()
+    imgs = [db.get_image(ids[(7 + 3 * i) % len(ids)]) for i in range(batch)]
+    rec, mods = [], [m for m in (est, est.detector, est.selector, est.refiner) if m is not None]
+    for m in mods:
+        def wrapped(name, fn, inputs, _o=m.stages.run):
+            rec.append((fn, list(inputs)))
+            return _o(name, fn, inputs)
+        m.stages.run = wrapped
+    try:
+        est.predict_batch(imgs, [db.K] * batch)
+    finally:
+        for m in mods:
+            del m.stages.run
+    torch.cuda.synchronize()
+    return est, rec
+
+
+def conv_calls(rec):
+    """The arguments of every ops.conv call of one eager replay of the recorded stages (the tensors stay alive)."""
+    calls, orig = [], ops.conv
+
+    def wrapped(*a, **k):
+        calls.append((a, k))
+        return orig(*a, **k)
+    ops.conv = wrapped
+    try:
+        with torch.no_grad():
+            for fn, inputs in rec:
+                fn(*inputs)
+    finally:
+        ops.conv = orig
+    torch.cuda.synchronize()
+    return calls
+
+
+def time_call(a, k, reps, repeat):
+    """(tag, flop, ms) of one tensor-core ops.conv call: the median over `repeat` replays of a graph of `reps`
+    back-to-back copies of the call, per copy.  None for a call that does not take the tensor-core path."""
+    prof = ops.enable_profiling()
+    ops.conv(*a, **k)
+    calls = ops.collect_profile(prof).get('#calls')
+    if not calls:
+        return None
+    _, work, _, tag = calls[0]
+    g = torch.cuda.CUDAGraph()
+    with torch.no_grad(), torch.cuda.graph(g):
+        for _ in range(reps):
+            ops.conv(*a, **k)
+    g.replay()
+    times = []
+    for _ in range(repeat):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(); g.replay(); e1.record()
+        torch.cuda.synchronize()
+        times.append(e0.elapsed_time(e1) / reps)
+    del g
+    return tag, work, sorted(times)[len(times) // 2]
+
+
+def breakdown(calls, reps=10, repeat=5):
+    """{tag: [calls, ms, flop]} per step.  Calls with the same tag are timed once (the first of them)."""
+    agg, timed = collections.OrderedDict(), {}
+    for a, k in calls:
+        prof = ops.enable_profiling()
+        ops.conv(*a, **k)
+        c = ops.collect_profile(prof).get('#calls')
+        if not c:
+            continue
+        tag = c[0][3]
+        if tag not in timed:
+            timed[tag] = time_call(a, k, reps, repeat)
+        _, work, ms = timed[tag]
+        e = agg.setdefault(tag, [0, 0.0, 0.0])
+        e[0] += 1; e[1] += ms; e[2] += work
+    return agg
+
+
+def no_prologue_3x3_persistent(tag):
+    """The layers whose A operand could come from a split activation: stride-1 3x3, no prologue, persistent kernel."""
+    return ' k=1x3x3 s=1 pro=0 persist ' in f' {tag} '
+
+
+def report(agg, top=40):
+    tot_ms, tot_w = sum(a[1] for a in agg.values()), sum(a[2] for a in agg.values())
+    print(f'conv_tc calls {sum(a[0] for a in agg.values())} total {tot_ms:.2f} ms, {tot_w / tot_ms / 1e9:.1f} TFLOP/s')
+    classes = collections.OrderedDict()
+    for tag, (n, ms, w) in agg.items():
+        key = ' '.join(t for t in tag.split() if t.startswith(('pro=', 'persist', 'reuse')))
+        c = classes.setdefault(key, [0, 0.0, 0.0]); c[0] += n; c[1] += ms; c[2] += w
+    for key, (n, ms, w) in sorted(classes.items(), key=lambda kv: -kv[1][1]):
+        print(f'  {ms:7.3f} ms x{n:3d} {w / ms / 1e9:6.1f} TF/s  [{key}]')
+    sel = [a for t, a in agg.items() if no_prologue_3x3_persistent(t)]
+    if sel:
+        ms, w = sum(a[1] for a in sel), sum(a[2] for a in sel)
+        print(f'  {ms:7.3f} ms x{sum(a[0] for a in sel):3d} {w / ms / 1e9:6.1f} TF/s  [3x3 stride 1, no prologue, persistent]')
+    for tag, (n, ms, w) in sorted(agg.items(), key=lambda kv: -kv[1][1])[:top]:
+        print(f'{ms:7.3f} ms x{n:3d} {w / ms / 1e9:6.1f} TF/s  {tag}')
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument('--batch', type=int, default=10, help='frames per predict_batch (bench.py: 10)')
+    ap.add_argument('--refine-iter', type=int, default=3, help='refinements per pose (bench.py: 3)')
+    ap.add_argument('--reps', type=int, default=10, help='copies of a call per captured graph')
+    ap.add_argument('--repeat', type=int, default=5, help='timed graph replays per call (median)')
+    ap.add_argument('--top', type=int, default=40, help='shapes listed')
+    a = ap.parse_args()
+    ops.require_cuda()
+    _, rec = record_step(a.batch, a.refine_iter)
+    print(f'{torch.cuda.get_device_name()}: batch {a.batch}, {a.refine_iter} refinements, '
+          f'median of {a.repeat} replays of {a.reps} copies per shape')
+    report(breakdown(conv_calls(rec), a.reps, a.repeat), a.top)
+
+
+if __name__ == '__main__':
+    main()
