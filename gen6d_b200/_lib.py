@@ -16,6 +16,7 @@ G6D_DET_MAX_SCALES = 8
 PRO_NONE, PRO_AFFINE, PRO_AFFINE_RELU, PRO_CORR = 0, 1, 2, 3
 ACT_NONE, ACT_RELU, ACT_LEAKY01 = 0, 1, 2
 TC_TF32, TC_F16 = 0, 1
+TC_PRENORM = 1          # g6d_conv_tc_ex flags
 
 
 class ConvDesc(C.Structure):
@@ -85,6 +86,9 @@ _SIGNATURES = {
     'g6d_conv_tc': [C.POINTER(ConvDesc), P, P, P, I, I, P, P, P, P, P, P, L, P],
     'g6d_conv_tc_stats_supported': [C.POINTER(ConvDesc), I, L],
     'g6d_conv_tc_plan': [C.POINTER(ConvDesc), I, C.POINTER(C.c_int)],
+    'g6d_conv_tc_plan_ex': [C.POINTER(ConvDesc), I, I, C.POINTER(C.c_int)],
+    'g6d_conv_tc_workspace_bytes_ex': [C.POINTER(ConvDesc), I, I],
+    'g6d_conv_tc_ex': [C.POINTER(ConvDesc), P, P, P, I, I, P, P, P, P, P, P, L, I, P],
     'g6d_pack_conv_weight_tc': [P, P, P, I, I, I, I, I, P, I, P],
     'g6d_split_operand': [P, P, P, L, I, P],
     'g6d_transpose2d': [P, P, I, I, P],
@@ -109,7 +113,7 @@ _SIGNATURES = {
     'g6d_pose_errors_workspace_bytes': [I, I],
     'g6d_pose_errors': [P, I, P, P, P, I, I, P, P, P],
 }
-_RESTYPE = {'g6d_pose_errors_workspace_bytes': L, 'g6d_sel_corr_score3_workspace_bytes': L, 'g6d_conv_workspace_bytes': L, 'g6d_conv_tc_workspace_bytes': L, 'g6d_launch_count': L, 'g6d_last_error': C.c_char_p}
+_RESTYPE = {'g6d_pose_errors_workspace_bytes': L, 'g6d_sel_corr_score3_workspace_bytes': L, 'g6d_conv_workspace_bytes': L, 'g6d_conv_tc_workspace_bytes': L, 'g6d_conv_tc_workspace_bytes_ex': L, 'g6d_launch_count': L, 'g6d_last_error': C.c_char_p}
 
 _lib = None
 

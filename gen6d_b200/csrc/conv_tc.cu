@@ -156,6 +156,23 @@ __device__ __forceinline__ float4 affine4(float4 x, const float4 sc, const float
     if (relu) { x.x = fmaxf(x.x, 0.f); x.y = fmaxf(x.y, 0.f); x.z = fmaxf(x.z, 0.f); x.w = fmaxf(x.w, 0.f); }
     return x;
 }
+// The prologue (pro != G6D_PRO_NONE) of input channels [c, c + 4) of an in-bounds element of image b at spatial
+// offset sp (within its plane): G6D_PRO_CORR scales by ps[sp, c] and shifts by pb[c], G6D_PRO_AFFINE(_RELU) by
+// ps / pb[b / group_rows, c].  The persistent kernel's producers and split_input_f16_kernel both transform
+// their elements here, so a pre-normalised split input holds the bytes the producers would store.
+__device__ __forceinline__ float4 prologue4(float4 x, int pro, const float* __restrict__ ps, const float* __restrict__ pb,
+                                            int Cin, long long group_rows, long long b, long long sp, int c) {
+    const float4* scp; const float4* shp;
+    if (pro == G6D_PRO_CORR) {
+        scp = reinterpret_cast<const float4*>(ps + sp * Cin + c);
+        shp = reinterpret_cast<const float4*>(pb + c);
+    } else {
+        const long long g = (int)b / (int)group_rows;               // 32-bit divide (the host checks the range)
+        scp = reinterpret_cast<const float4*>(ps + g * Cin + c);
+        shp = reinterpret_cast<const float4*>(pb + g * Cin + c);
+    }
+    return affine4(x, __ldg(scp), __ldg(shp), pro == G6D_PRO_AFFINE_RELU);
+}
 
 // ------------------------------------------------------------------------------------------ MMA
 // Each consumer warpgroup owns 64 rows x BN columns of the tile with every accumulator in registers:
@@ -437,22 +454,10 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
                 const int s = g_it % STAGES;
                 const uint32_t n_use = g_it / STAGES;
                 if (p.pro != G6D_PRO_NONE) {
-                    const bool relu = p.pro == G6D_PRO_AFFINE_RELU;
 #pragma unroll
-                    for (int j = 0; j < ROWS; ++j) {
-                        if (okm[q] & (1u << j)) {
-                            const float4* scp; const float4* shp;
-                            if (p.pro == G6D_PRO_CORR) {
-                                scp = reinterpret_cast<const float4*>(p.ps + (long long)(rsp[j] + ksp[q]) * p.Cin + kc[q]);
-                                shp = reinterpret_cast<const float4*>(p.pb + kc[q]);
-                            } else {
-                                const long long g = rb[j] / (int)p.group_rows;       // 32-bit divide (host checks the range)
-                                scp = reinterpret_cast<const float4*>(p.ps + g * p.Cin + kc[q]);
-                                shp = reinterpret_cast<const float4*>(p.pb + g * p.Cin + kc[q]);
-                            }
-                            v[q][j] = affine4(v[q][j], __ldg(scp), __ldg(shp), relu);
-                        }
-                    }
+                    for (int j = 0; j < ROWS; ++j)
+                        if (okm[q] & (1u << j))
+                            v[q][j] = prologue4(v[q][j], p.pro, p.ps, p.pb, p.Cin, p.group_rows, rb[j], rsp[j] + ksp[q], kc[q]);
                 }
                 if (e == 0) mbar_wait(empty(s), (n_use & 1) ^ 1, 1, g_it);
 #pragma unroll
@@ -813,17 +818,25 @@ __global__ void split_f16_kernel(const float* __restrict__ in, __half* __restric
 // Activation [rows, ics] (channels [ico, ico + Cin)) -> split form [rows, 2 Cin] fp16 for the im2col A loads: channel
 // block cb of a row holds hi at [128 cb, 128 cb + 64) and lo at [128 cb + 64, 128 cb + 128), position p from channel
 // 64 cb + f16_k_source(p).  A thread makes one 16-byte chunk of each from the same two float4 loads and the same
-// split_f16x2 calls as a producer thread of conv_tc2_kernel, so the tiles are bit-identical.
+// split_f16x2 calls as a producer thread of conv_tc2_kernel, so the tiles are bit-identical.  With a prologue
+// (G6D_TC_PRENORM) every element is transformed by prologue4 first, as the producers transform every in-bounds
+// element; the padding stays zero, as the im2col map fills it after this pass.  plane = H * W pixels per image.
 __global__ void split_input_f16_kernel(const float* __restrict__ x, int ics, int ico, int Cin, long long rows,
-                                       __half* __restrict__ out) {
+                                       long long plane, int pro, const float* __restrict__ ps, const float* __restrict__ pb,
+                                       long long group_rows, __half* __restrict__ out) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const int chunks = Cin / 8;
     if (i >= rows * chunks) return;
     const long long r = i / chunks;
     const int q = (int)(i - r * chunks), cb = q >> 3, c = q & 7;
     const float* src = x + r * ics + ico + cb * 64 + 4 * c;
-    const float4 a = __ldg(reinterpret_cast<const float4*>(src));
-    const float4 b = __ldg(reinterpret_cast<const float4*>(src + 32));
+    float4 a = __ldg(reinterpret_cast<const float4*>(src));
+    float4 b = __ldg(reinterpret_cast<const float4*>(src + 32));
+    if (pro != G6D_PRO_NONE) {
+        const long long img = r / plane, sp = r - img * plane;
+        a = prologue4(a, pro, ps, pb, Cin, group_rows, img, sp, cb * 64 + 4 * c);
+        b = prologue4(b, pro, ps, pb, Cin, group_rows, img, sp, cb * 64 + 32 + 4 * c);
+    }
     uint4 h, l;
     split_f16x2(a.x, a.y, h.x, l.x);
     split_f16x2(a.z, a.w, h.y, l.y);
@@ -1180,18 +1193,20 @@ struct ConvPlan {
 // convolutions with stride 1 and no prologue: the gather, split and swizzle of 8 producer warps (each input
 // element once per tap, 16 KB in flight per SM) become two bulk copies per K-block.  The split pass reads and
 // writes the input once.  The bounding box of the im2col map is the output plane shifted by the padding.
-static bool split_input_ok(const g6d_conv_desc* d, int kind, bool use_flat) {
-    return !use_flat && kind == G6D_TC_F16 && d->prologue == G6D_PRO_NONE && d->stride == 1 && d->kd == 1 && d->D == 1 &&
-           d->kh * d->kw > 1 && d->kw <= 64 && d->kh <= 64 && d->pw < 64 && d->ph < 64;
+// G6D_TC_PRENORM extends this to layers with a prologue: the split pass applies it (see split_input_f16_kernel).
+static bool split_input_ok(const g6d_conv_desc* d, int kind, int flags, bool use_flat) {
+    return !use_flat && kind == G6D_TC_F16 && (d->prologue == G6D_PRO_NONE || (flags & G6D_TC_PRENORM)) && d->stride == 1 &&
+           d->kd == 1 && d->D == 1 && d->kh * d->kw > 1 && d->kw <= 64 && d->kh <= 64 && d->pw < 64 && d->ph < 64;
 }
 
-static int make_plan(const g6d_conv_desc* d, int kind, ConvPlan& pl) {
+static int make_plan(const g6d_conv_desc* d, int kind, int flags, ConvPlan& pl) {
+    G6D_REQUIRE((flags & ~G6D_TC_PRENORM) == 0, "g6d_conv_tc: bad flags %d", flags);
     const int rc = fill_tc_params(d, kind, pl.tc);
     if (rc != G6D_OK) return rc;
     pl.use_flat = fill_flat_params(d, kind, pl.flat, &pl.flat_smem);
     pl.bn = tc_block_n(d->Cout);
     pl.splits = pl.use_flat ? pl.flat.splits : pl.tc.splits;
-    pl.tc.split_in = split_input_ok(d, kind, pl.use_flat) ? 1 : 0;
+    pl.tc.split_in = split_input_ok(d, kind, flags, pl.use_flat) ? 1 : 0;
     const long long partials = pl.splits > 1 ? (long long)pl.splits * pl.tc.M * pl.tc.Cout * (long long)sizeof(float) : 0;
     pl.split_in_off = (partials + 255) / 256 * 256;
     pl.ws_bytes = pl.tc.split_in ? pl.split_in_off + (long long)d->B * d->H * d->W * d->Cin * 2 * (long long)sizeof(__half)
@@ -1244,24 +1259,28 @@ extern "C" int g6d_conv_tc_debug(int* host_out8) {
 
 extern "C" int g6d_conv_tc_supported(const g6d_conv_desc* d, int kind) {
     ConvPlan pl{};
-    return make_plan(d, kind, pl) == G6D_OK ? 1 : 0;
+    return make_plan(d, kind, 0, pl) == G6D_OK ? 1 : 0;
+}
+
+extern "C" long long g6d_conv_tc_workspace_bytes_ex(const g6d_conv_desc* desc, int kind, int flags) {
+    ConvPlan pl{};
+    if (make_plan(desc, kind, flags, pl) != G6D_OK) return -1;
+    return pl.ws_bytes;
 }
 
 extern "C" long long g6d_conv_tc_workspace_bytes(const g6d_conv_desc* desc, int kind) {
-    ConvPlan pl{};
-    if (make_plan(desc, kind, pl) != G6D_OK) return -1;
-    return pl.ws_bytes;
+    return g6d_conv_tc_workspace_bytes_ex(desc, kind, 0);
 }
 
 extern "C" int g6d_conv_tc_stats_supported(const g6d_conv_desc* desc, int kind, long long stats_rows) {
     ConvPlan pl{};
-    return make_plan(desc, kind, pl) == G6D_OK && stats_ok(pl, stats_rows) ? 1 : 0;
+    return make_plan(desc, kind, 0, pl) == G6D_OK && stats_ok(pl, stats_rows) ? 1 : 0;
 }
 
-extern "C" int g6d_conv_tc_plan(const g6d_conv_desc* desc, int kind, int* out4) {
+extern "C" int g6d_conv_tc_plan_ex(const g6d_conv_desc* desc, int kind, int flags, int* out4) {
     G6D_REQUIRE(out4 != nullptr, "g6d_conv_tc_plan: null output");
     ConvPlan pl{};
-    const int rc = make_plan(desc, kind, pl);
+    const int rc = make_plan(desc, kind, flags, pl);
     if (rc != G6D_OK) return rc;
     out4[0] = pl.use_flat ? 1 : 0;
     out4[1] = pl.bn;
@@ -1270,11 +1289,15 @@ extern "C" int g6d_conv_tc_plan(const g6d_conv_desc* desc, int kind, int* out4) 
     return G6D_OK;
 }
 
-extern "C" int g6d_conv_tc(const g6d_conv_desc* desc, const float* x, const void* w_hi, const void* w_lo, int w_rows,
-                           int kind, const float* bias, const float* pro_scale, const float* pro_shift, float* y,
-                           void* ws, double* stats, long long stats_rows, g6d_stream_t stream) {
+extern "C" int g6d_conv_tc_plan(const g6d_conv_desc* desc, int kind, int* out4) {
+    return g6d_conv_tc_plan_ex(desc, kind, 0, out4);
+}
+
+extern "C" int g6d_conv_tc_ex(const g6d_conv_desc* desc, const float* x, const void* w_hi, const void* w_lo, int w_rows,
+                              int kind, const float* bias, const float* pro_scale, const float* pro_shift, float* y,
+                              void* ws, double* stats, long long stats_rows, int flags, g6d_stream_t stream) {
     ConvPlan pl{};
-    int rc = make_plan(desc, kind, pl);
+    int rc = make_plan(desc, kind, flags, pl);
     if (rc != G6D_OK) return rc;
     const ConvTcP& p = pl.tc;
     if (stats) G6D_REQUIRE(stats_ok(pl, stats_rows), "g6d_conv_tc: fused statistics need groups of whole 32-row slices / planes (stats_rows %lld)", stats_rows);
@@ -1296,8 +1319,9 @@ extern "C" int g6d_conv_tc(const g6d_conv_desc* desc, const float* x, const void
     if (p.split_in) {
         __half* xs = reinterpret_cast<__half*>(static_cast<char*>(ws) + pl.split_in_off);
         if ((rc = make_split_input_map(&ma, xs, desc)) != G6D_OK) return rc;
-        const long long rows = (long long)p.B * p.H * p.W, n = rows * (p.Cin / 8);
-        split_input_f16_kernel<<<ceil_div(n, 256), 256, 0, st>>>(x, p.ics, p.ico, p.Cin, rows, xs);
+        const long long plane = (long long)p.H * p.W, rows = p.B * plane, n = rows * (p.Cin / 8);
+        split_input_f16_kernel<<<ceil_div(n, 256), 256, 0, st>>>(x, p.ics, p.ico, p.Cin, rows, plane, p.pro, pro_scale,
+                                                                  pro_shift, p.group_rows, xs);
         G6D_CHECK_LAUNCH("g6d_conv_tc(split input)");
     }
     rc = kind == G6D_TC_F16 ? dispatch<G6D_TC_F16>(pl, mh, ml, ma, st) : dispatch<G6D_TC_TF32>(pl, mh, ml, ma, st);
@@ -1307,6 +1331,12 @@ extern "C" int g6d_conv_tc(const g6d_conv_desc* desc, const float* x, const void
         G6D_CHECK_LAUNCH("g6d_conv_tc(split reduce)");
     }
     return G6D_OK;
+}
+
+extern "C" int g6d_conv_tc(const g6d_conv_desc* desc, const float* x, const void* w_hi, const void* w_lo, int w_rows,
+                           int kind, const float* bias, const float* pro_scale, const float* pro_shift, float* y,
+                           void* ws, double* stats, long long stats_rows, g6d_stream_t stream) {
+    return g6d_conv_tc_ex(desc, x, w_hi, w_lo, w_rows, kind, bias, pro_scale, pro_shift, y, ws, stats, stats_rows, 0, stream);
 }
 
 extern "C" int g6d_split_operand(const float* in, void* hi, void* lo, long long n, int kind, g6d_stream_t stream) {

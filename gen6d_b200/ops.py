@@ -34,15 +34,17 @@ def _p(t, dtype=torch.float32):
 _PROFILE = None   # when enabled: {name: [(start_event, end_event, work), ...]}
 
 
-def _call(name, *args, work=None, tag=None):
+def _call(name, *args, work=None, tag=None, key=None):
+    """key: the profile entry the call is timed under (default: name)."""
     if _PROFILE is not None and work is not None:
+        key = key or name
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         _lib.check(getattr(_lib.lib(), name)(*args), name)
         e1.record()
-        _PROFILE.setdefault(name, []).append((e0, e1, work))
+        _PROFILE.setdefault(key, []).append((e0, e1, work))
         if tag is not None:
-            _PROFILE.setdefault('#calls', []).append((e0, e1, work, name, tag))
+            _PROFILE.setdefault('#calls', []).append((e0, e1, work, key, tag))
         return
     _lib.check(getattr(_lib.lib(), name)(*args), name)
 
@@ -359,12 +361,14 @@ def transpose_to_packed(x2d):
 
 
 def conv(x, pc, prologue=PRO_NONE, pro_scale=None, pro_shift=None, group_rows=1, act=ACT_NONE,
-         in_coff=0, out=None, out_coff=0, stats_rows=None):
+         in_coff=0, out=None, out_coff=0, stats_rows=None, prenorm=False):
     """x [B, D, H, W, cs] or [B, H, W, cs]; returns [B, Do, Ho, Wo, Cout] (or 4-D for 4-D input).
     stats_rows: also return the InstanceNorm moments of the OUTPUT, (y, ws) with ws float64
     [groups, Cout, 2] = per group of `stats_rows` consecutive output rows (sum y, sum y^2) -- fused into the
     convolution's epilogue on the tensor-core path (no extra pass over y), else by g6d_instnorm_partial;
-    pass ws to instnorm_finalize (after any cross-GPU all-reduce)."""
+    pass ws to instnorm_finalize (after any cross-GPU all-reduce).
+    prenorm: G6D_TC_PRENORM -- a prologue layer the persistent kernel would gather takes its A operand by TMA
+    im2col from a prologue-applied split copy of x instead (same result bit for bit; no-op elsewhere)."""
     four = x.dim() == 4
     if four:
         B, H, W, cs = x.shape
@@ -385,21 +389,23 @@ def conv(x, pc, prologue=PRO_NONE, pro_scale=None, pro_shift=None, group_rows=1,
     M = B * Do * Ho * Wo
     stats = None
     if pc.w_hi is not None and conv_path() == 'tc' and _lib.lib().g6d_conv_tc_supported(C.byref(d), pc.kind):
-        nbytes = _lib.lib().g6d_conv_tc_workspace_bytes(C.byref(d), pc.kind)
+        flags = _lib.TC_PRENORM if prenorm else 0
+        nbytes = _lib.lib().g6d_conv_tc_workspace_bytes_ex(C.byref(d), pc.kind, flags)
         if nbytes < 0:
-            _lib.check(-1, 'g6d_conv_tc_workspace_bytes')
+            _lib.check(-1, 'g6d_conv_tc_workspace_bytes_ex')
         ws = torch.empty(nbytes // 4, device=x.device, dtype=torch.float32) if nbytes > 0 else None
         fuse = stats_rows is not None and _lib.lib().g6d_conv_tc_stats_supported(C.byref(d), pc.kind, stats_rows)
         if fuse:
             stats = torch.empty(M // stats_rows, pc.cout, 2, device=x.device, dtype=torch.float64)
-        def tag(d=d, kind=pc.kind):        # formatted by collect_profile, outside the timed launches
+        def tag(d=d, kind=pc.kind, flags=flags):        # formatted by collect_profile, outside the timed launches
             plan = (C.c_int * 4)()
-            _lib.check(_lib.lib().g6d_conv_tc_plan(C.byref(d), kind, plan), 'g6d_conv_tc_plan')
+            _lib.check(_lib.lib().g6d_conv_tc_plan_ex(C.byref(d), kind, flags, plan), 'g6d_conv_tc_plan_ex')
+            a_op = (' prenorm' if prologue != PRO_NONE else ' im2col') if plan[3] else ''
             return (f'M={M} N={pc.cout} K={kd * kh * kw * pc.cin} k={kd}x{kh}x{kw} s={s} pro={prologue} '
-                    f'{"reuse" if plan[0] else "persist"} BN={plan[1]} splits={plan[2]}{" im2col" if plan[3] else ""}')
-        _call('g6d_conv_tc', C.byref(d), _p(x), _p(pc.w_hi, pc.w_hi.dtype), _p(pc.w_lo, pc.w_lo.dtype), pc.w_hi.shape[0],
+                    f'{"reuse" if plan[0] else "persist"} BN={plan[1]} splits={plan[2]}{a_op}')
+        _call('g6d_conv_tc_ex', C.byref(d), _p(x), _p(pc.w_hi, pc.w_hi.dtype), _p(pc.w_lo, pc.w_lo.dtype), pc.w_hi.shape[0],
               pc.kind, _p(pc.bias), _p(pro_scale), _p(pro_shift), _p(out), _p(ws), _p(stats, torch.float64), stats_rows or 0,
-              _stream(), work=work, tag=tag)
+              flags, _stream(), work=work, tag=tag, key='g6d_conv_tc')
     else:
         if pc.w is None:
             raise _lib.Gen6DLibraryError('this operand was packed for the tensor-core path only and the problem is not supported there')

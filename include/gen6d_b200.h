@@ -255,12 +255,23 @@ long long g6d_conv_tc_workspace_bytes(const g6d_conv_desc* desc, int kind);
 int g6d_conv_tc_stats_supported(const g6d_conv_desc* desc, int kind, long long stats_rows);
 /* What g6d_conv_tc would launch for desc (no launch): out4 = {kernel (0 persistent, 1 A-reuse), BN, K splits,
  * split input (1: the persistent kernel loads A by TMA im2col from an fp16 hi/lo copy of x that the call writes
- * into the workspace -- fp16 kind, stride 1, no prologue, 2-D multi-tap)}.  G6D_EINVAL with g6d_conv_tc's
+ * into the workspace -- fp16 kind, stride 1, no prologue (see G6D_TC_PRENORM), 2-D multi-tap)}.  G6D_EINVAL with g6d_conv_tc's
  * message when the descriptor is rejected. */
 int g6d_conv_tc_plan(const g6d_conv_desc* desc, int kind, int* out4);
 int g6d_conv_tc(const g6d_conv_desc* desc, const float* x, const void* w_hi, const void* w_lo, int w_rows, int kind,
                 const float* bias, const float* pro_scale, const float* pro_shift, float* y, void* ws,
                 double* stats, long long stats_rows, g6d_stream_t stream);
+/* The same three entry points with option flags; flags = 0 is exactly g6d_conv_tc_plan / _workspace_bytes / g6d_conv_tc.
+ * G6D_TC_PRENORM: where the split input would apply if the layer had no prologue (fp16 kind, persistent kernel, 2-D,
+ * stride 1, multi-tap), it applies with the prologue too: the call's split pass writes prologue(x) split into hi/lo,
+ * and the kernel loads A from it by TMA im2col.  Bit-identical to the producer warps (selector towers: their 8x8
+ * and 4x4 InstanceNorm-ed layers).  Elsewhere the flag changes nothing.  Other bits: G6D_EINVAL. */
+#define G6D_TC_PRENORM 1
+int g6d_conv_tc_plan_ex(const g6d_conv_desc* desc, int kind, int flags, int* out4);
+long long g6d_conv_tc_workspace_bytes_ex(const g6d_conv_desc* desc, int kind, int flags);
+int g6d_conv_tc_ex(const g6d_conv_desc* desc, const float* x, const void* w_hi, const void* w_lo, int w_rows, int kind,
+                   const float* bias, const float* pro_scale, const float* pro_shift, float* y, void* ws,
+                   double* stats, long long stats_rows, int flags, g6d_stream_t stream);
 /* [Cout, Cin, taps] (reference layout) -> hi/lo [rows_pad, taps*Cin_pad] of the given kind; optional BN-fold scale */
 int g6d_pack_conv_weight_tc(const float* w, void* out_hi, void* out_lo, int Cout, int Cin, int Cin_pad, int taps,
                             int rows_pad, const float* cout_scale, int kind, g6d_stream_t stream);

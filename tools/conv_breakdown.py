@@ -8,7 +8,9 @@ arguments of every convolution.  Each distinct call is then timed on its own: a 
 it, replayed R times, median per copy (timing the calls inside the eager replay would measure the host
 whenever a kernel is shorter than its launch).  Each line aggregates the calls of one tag; the tag names
 the kernel the planner picked (persist: the persistent kernel, reuse: the A-reuse kernel), the prologue,
-BN and the K splits.  Times are per step of B poses."""
+BN, the K splits and how a persistent call gets its A operand (im2col: by TMA from a split copy of the input,
+prenorm: the same from a copy with the prologue applied; neither: gathered by the producer warps).  Times
+are per step of B poses, split pass included."""
 import argparse
 import collections
 import os
@@ -105,19 +107,27 @@ def no_prologue_3x3_persistent(tag):
     return ' k=1x3x3 s=1 pro=0 persist ' in f' {tag} '
 
 
+def prologue_3x3_persistent(tag):
+    """The layers a prologue-applied split input can feed (the selector towers' 8x8 and 4x4 layers), whichever way
+    they ran: stride-1 3x3 with a prologue on the persistent kernel."""
+    return ' k=1x3x3 s=1 pro=' in f' {tag} ' and ' pro=0 ' not in f' {tag} ' and ' persist ' in f' {tag} '
+
+
 def report(agg, top=40):
     tot_ms, tot_w = sum(a[1] for a in agg.values()), sum(a[2] for a in agg.values())
     print(f'conv_tc calls {sum(a[0] for a in agg.values())} total {tot_ms:.2f} ms, {tot_w / tot_ms / 1e9:.1f} TFLOP/s')
     classes = collections.OrderedDict()
     for tag, (n, ms, w) in agg.items():
-        key = ' '.join(t for t in tag.split() if t.startswith(('pro=', 'persist', 'reuse')))
+        key = ' '.join(t for t in tag.split() if t.startswith(('pro=', 'persist', 'reuse', 'prenorm')))
         c = classes.setdefault(key, [0, 0.0, 0.0]); c[0] += n; c[1] += ms; c[2] += w
     for key, (n, ms, w) in sorted(classes.items(), key=lambda kv: -kv[1][1]):
         print(f'  {ms:7.3f} ms x{n:3d} {w / ms / 1e9:6.1f} TF/s  [{key}]')
-    sel = [a for t, a in agg.items() if no_prologue_3x3_persistent(t)]
-    if sel:
-        ms, w = sum(a[1] for a in sel), sum(a[2] for a in sel)
-        print(f'  {ms:7.3f} ms x{sum(a[0] for a in sel):3d} {w / ms / 1e9:6.1f} TF/s  [3x3 stride 1, no prologue, persistent]')
+    for what, pick in (('3x3 stride 1, no prologue, persistent', no_prologue_3x3_persistent),
+                       ('3x3 stride 1, prologue, persistent', prologue_3x3_persistent)):
+        sel = [a for t, a in agg.items() if pick(t)]
+        if sel:
+            ms, w = sum(a[1] for a in sel), sum(a[2] for a in sel)
+            print(f'  {ms:7.3f} ms x{sum(a[0] for a in sel):3d} {w / ms / 1e9:6.1f} TF/s  [{what}]')
     for tag, (n, ms, w) in sorted(agg.items(), key=lambda kv: -kv[1][1])[:top]:
         print(f'{ms:7.3f} ms x{n:3d} {w / ms / 1e9:6.1f} TF/s  {tag}')
 
