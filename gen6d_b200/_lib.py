@@ -16,7 +16,7 @@ G6D_DET_MAX_SCALES = 8
 PRO_NONE, PRO_AFFINE, PRO_AFFINE_RELU, PRO_CORR = 0, 1, 2, 3
 ACT_NONE, ACT_RELU, ACT_LEAKY01 = 0, 1, 2
 TC_TF32, TC_F16 = 0, 1
-TC_PRENORM = 1          # g6d_conv_tc_ex flags
+TC_PRENORM, TC_REUSE_IM2COL = 1, 4          # g6d_conv_tc_ex flags
 
 
 class ConvDesc(C.Structure):

@@ -33,7 +33,7 @@
 //               epilogue (bias / activation -> global, or split-K partials) straight from the
 //               accumulator registers.  The first consumer thread also streams the pre-split weight
 //               tiles W_hi / W_lo [Cout, K] (K-major) by TMA (cp.async.bulk.tensor.2d, 128B swizzle)
-//               into the stages the consumers free.
+//               into the stages the consumers free (with a split input, the thread that loads A does).
 // A consumer's accumulators alone take 128 registers, the launch bound of 512 threads allows 128 per
 // thread: the producer warpgroups give registers up (setmaxnreg.dec to TC_PRODUCER_REGS) and the
 // consumer warpgroups take them (setmaxnreg.inc to TC_CONSUMER_REGS); ptxas allocates the code after
@@ -94,7 +94,25 @@ struct ConvTcP {
     int M, K, kblocks, splits, kb_per_split;
     double* stats; long long stats_rows;      // fused InstanceNorm statistics of the OUTPUT (see epilogue_stats)
     int split_in;                             // A tiles by TMA im2col from the pre-split input (see split_input_ok)
+    int reuse_order;                          // K-blocks in the A-reuse kernel's order (G6D_TC_REUSE_IM2COL, see kblock_src)
 };
+
+// Filter tap (kz, ky, kx flattened) and 64-channel block of K-block `it` of split `sp` when the input is split
+// (K = tap * Cin + c).  Default: tap-major over the whole K.  reuse_order: the A-reuse kernel's order -- splits
+// over channel blocks, then per channel block kz, then the (ky, kx) tap -- so that every output element sums the
+// same products into the same accumulators in the same order as conv_tcflat_kernel.
+__device__ __forceinline__ void kblock_src(const ConvTcP& p, int sp, int it, int& tap, int& cb) {
+    if (p.reuse_order) {
+        const int taps2 = p.kh * p.kw;
+        const int u = it / taps2, t = it - u * taps2;            // unit (channel block, kz), tap (ky, kx)
+        cb = sp * (p.kb_per_split / (taps2 * p.kd)) + u / p.kd;
+        tap = (u % p.kd) * taps2 + t;
+    } else {
+        const int cblocks = p.Cin / 64, kb = sp * p.kb_per_split + it;
+        tap = kb / cblocks;
+        cb = kb - tap * cblocks;
+    }
+}
 
 // ------------------------------------------------------------------------------------------ operand split
 // fp16 pair (element 0 in the low half, as laid out in memory), saturating instead of overflowing to inf
@@ -149,6 +167,13 @@ __device__ __forceinline__ void tma_im2col_4d(uint32_t dst, const CUtensorMap* m
     asm volatile(
         "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
         ::"r"(dst), "l"(map), "r"(bar), "r"(c), "r"(w), "r"(h), "r"(n), "h"(ox), "h"(oy) : "memory");
+}
+// the same over a 5-D NDHWC tensor: the traversal runs over (w, h, d, n), the tap is (ox, oy, oz)
+__device__ __forceinline__ void tma_im2col_5d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c, int w, int h, int d,
+                                              int n, uint16_t ox, uint16_t oy, uint16_t oz) {
+    asm volatile(
+        "cp.async.bulk.tensor.5d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2], {%8, %9, %10};"
+        ::"r"(dst), "l"(map), "r"(bar), "r"(c), "r"(w), "r"(h), "r"(d), "r"(n), "h"(ox), "h"(oy), "h"(oz) : "memory");
 }
 
 __device__ __forceinline__ float4 affine4(float4 x, const float4 sc, const float4 sh, bool relu) {
@@ -219,6 +244,18 @@ __device__ __forceinline__ void mma_stage(float (&main)[BN / 2], float (&cross)[
     wgmma_commit();
 }
 
+// (sum y, sum y^2) of one column over a warp's 16-row slice, rows r and r + 8 (y0, y1) per lane, r = lane / 4, in every
+// lane of the column.  epilogue_tile and flat_moments_kernel share it, so the same slice gives the same fp32 partials.
+__device__ __forceinline__ float2 slice_moments(float y0, float y1) {
+    float s1 = y0 + y1, s2 = y0 * y0 + y1 * y1;
+#pragma unroll
+    for (int o = 4; o < 32; o <<= 1) {                // the 8 lanes that share this column
+        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+        s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+    }
+    return make_float2(s1, s2);
+}
+
 // Epilogue of one consumer thread: rows r and r + 8 of the tile (dst0 / dst1 point at column n_base of
 // their output row, nullptr for rows outside the output), columns 8 i + 2 (lane & 3) + {0, 1}.  Folds the
 // cross terms (smallest magnitude first, scaled back by the lo pre-scale) and the main chains, adds
@@ -271,16 +308,11 @@ __device__ __forceinline__ void epilogue_tile(float (&acc)[AccCfg<BN>::NMAIN][BN
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
             const float y0 = dst0 ? cross[4 * i + e] : 0.f, y1 = dst1 ? cross[4 * i + 2 + e] : 0.f;
-            float s1 = y0 + y1, s2 = y0 * y0 + y1 * y1;
-#pragma unroll
-            for (int o = 4; o < 32; o <<= 1) {                // the 8 lanes that share this column
-                s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-                s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-            }
+            const float2 s = slice_moments(y0, y1);
             const int n = n_base + 8 * i + cq + e;
             if (lane < 4 && n < Cout) {
-                atomicAdd(stats + (group * Cout + n) * 2, (double)s1);
-                atomicAdd(stats + (group * Cout + n) * 2 + 1, (double)s2);
+                atomicAdd(stats + (group * Cout + n) * 2, (double)s.x);
+                atomicAdd(stats + (group * Cout + n) * 2 + 1, (double)s.y);
             }
         }
     }
@@ -363,8 +395,16 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
             // The input is already split (hi / lo of channel block cb at channels [128 cb, 128 cb + 64) /
             // [128 cb + 64, 128 cb + 128) of each pixel, in f16_k_source order), so a K-block of tap (kx, ky)
             // is two im2col boxes of the 128 output pixels of the tile: byte for byte what the producers
-            // below would store.  One thread issues them; the other producer warps have nothing to do.
+            // below would store.  One thread issues them, and the stage's weight tiles with them (the consumers
+            // then issue no loads); the other producer warps have nothing to do.  Volumes (D > 1 or kd > 1) use
+            // the rank-5 map, see make_split_input_map.
             if (threadIdx.x == 0) {
+                const bool vol = p.D > 1 || p.kd > 1;
+                auto kcoord = [&](int sp, int it) {             // K coordinate of the weight tiles of a K-block
+                    int tap, cb;
+                    kblock_src(p, sp, it, tap, cb);
+                    return tap * p.Cin + cb * BK;
+                };
                 int g = 0;
                 for (int w = blockIdx.x; w < wk.total; w += gridDim.x) {
                     int mt, nt, sp;
@@ -372,19 +412,36 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
                     const int nkb = kblocks_of(sp);
                     int m = mt * TC_BM;
                     const int xo = m % p.Wo; m /= p.Wo;
-                    const int yo = m % p.Ho;
-                    const int b = m / p.Ho;
-                    const int k = sp * p.kb_per_split * BK;
-                    int tap = k / p.Cin, c0 = k - tap * p.Cin;
+                    const int yo = m % p.Ho; m /= p.Ho;
+                    const int zo = m % p.Do;
+                    const int b = m / p.Do;
+                    // L2 prefetch of the weight tiles PF K-blocks ahead, as the consumers' weight stream does
+                    for (int i = 0; i < min(nkb, PF - 1); ++i) {
+                        tma_prefetch_2d(&map_hi, kcoord(sp, i), nt * BN);
+                        tma_prefetch_2d(&map_lo, kcoord(sp, i), nt * BN);
+                    }
                     for (int it = 0; it < nkb; ++it, ++g) {
+                        if (it + PF - 1 < nkb) {
+                            tma_prefetch_2d(&map_hi, kcoord(sp, it + PF - 1), nt * BN);
+                            tma_prefetch_2d(&map_lo, kcoord(sp, it + PF - 1), nt * BN);
+                        }
+                        int tap, cb;
+                        kblock_src(p, sp, it, tap, cb);
+                        const uint16_t ox = (uint16_t)(tap % p.kw), oy = (uint16_t)((tap / p.kw) % p.kh);
+                        const uint16_t oz = (uint16_t)(tap / (p.kw * p.kh));
                         const int s = g % STAGES;
                         mbar_wait(empty(s), ((g / STAGES) & 1) ^ 1, 1, g);
+                        mbar_expect_tx(full_b(s), 2 * Cfg::B_BYTES);
+                        tma_load_2d(b_hi(s), &map_hi, full_b(s), tap * p.Cin + cb * BK, nt * BN);
+                        tma_load_2d(b_lo(s), &map_lo, full_b(s), tap * p.Cin + cb * BK, nt * BN);
                         mbar_expect_tx(full_a(s), 2 * Cfg::A_BYTES);
-                        const uint16_t ox = (uint16_t)(tap % p.kw), oy = (uint16_t)(tap / p.kw);
-                        tma_im2col_4d(a_hi(s), &map_a, full_a(s), 2 * c0, xo - p.pw, yo - p.ph, b, ox, oy);
-                        tma_im2col_4d(a_lo(s), &map_a, full_a(s), 2 * c0 + BK, xo - p.pw, yo - p.ph, b, ox, oy);
-                        c0 += BK;
-                        if (c0 == p.Cin) { c0 = 0; ++tap; }
+                        if (vol) {
+                            tma_im2col_5d(a_hi(s), &map_a, full_a(s), 2 * BK * cb, xo - p.pw, yo - p.ph, zo - p.pd, b, ox, oy, oz);
+                            tma_im2col_5d(a_lo(s), &map_a, full_a(s), 2 * BK * cb + BK, xo - p.pw, yo - p.ph, zo - p.pd, b, ox, oy, oz);
+                        } else {
+                            tma_im2col_4d(a_hi(s), &map_a, full_a(s), 2 * BK * cb, xo - p.pw, yo - p.ph, b, ox, oy);
+                            tma_im2col_4d(a_lo(s), &map_a, full_a(s), 2 * BK * cb + BK, xo - p.pw, yo - p.ph, b, ox, oy);
+                        }
                     }
                 }
             }
@@ -494,7 +551,7 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
         setmaxnreg_inc<TC_CONSUMER_REGS>();
         const int cw = warp - NPW;                     // consumer warp: rows 16 cw .. 16 cw + 15 of the tile
         const uint32_t a_row = (cw >> 2) * 64 * 128;   // this warpgroup's 64 rows of the A tiles
-        const bool issuer = threadIdx.x == TC_ISSUER;
+        const bool issuer = threadIdx.x == TC_ISSUER && !p.split_in;      // with the split input, the A issuer loads B
         // weight-tile stream of the issuer: the next global K-block lg = K-block lit of work item lw
         int lw = blockIdx.x, lit = 0, lg = 0;
         auto load_next = [&]() {
@@ -694,17 +751,22 @@ static EncodeIm2colFn get_encode_im2col_fn() {
 
 // im2col map over the split input [B, H, W, 2 Cin] fp16: 64 channels x 128 pixels per box (one 128-byte swizzle
 // row per pixel); the bounding box of filter origins runs from -pad to dim - 1 + pad - (k - 1), i.e. the output
-// plane of a stride-1 convolution, and taps outside the tensor are filled with zeros (the padding)
+// plane of a stride-1 convolution, and taps outside the tensor are filled with zeros (the padding).  Volumes
+// (D > 1 or kd > 1, the same test as the kernel's) get the rank-5 map over [B, D, H, W, 2 Cin].
+static bool split_input_rank5(const g6d_conv_desc* d) { return d->D > 1 || d->kd > 1; }
+
 static int make_split_input_map(CUtensorMap* map, const void* xs, const g6d_conv_desc* d) {
     EncodeIm2colFn enc = get_encode_im2col_fn();
     if (!enc) { set_error("g6d_conv_tc: cuTensorMapEncodeIm2col unavailable"); return G6D_ECUDA; }
     const cuuint64_t C2 = 2ull * d->Cin;
-    cuuint64_t dims[4] = {C2, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->B};
-    cuuint64_t strides[3] = {C2 * 2, C2 * 2 * d->W, C2 * 2 * d->W * d->H};
-    int lower[2] = {-d->pw, -d->ph};
-    int upper[2] = {d->pw - (d->kw - 1), d->ph - (d->kh - 1)};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(xs), dims, strides, lower, upper, 64, TC_BM, estr,
+    const cuuint32_t rank = split_input_rank5(d) ? 5 : 4;
+    cuuint64_t dims[5] = {C2, (cuuint64_t)d->W, (cuuint64_t)d->H, (cuuint64_t)d->D, (cuuint64_t)d->B};
+    cuuint64_t strides[4] = {C2 * 2, C2 * 2 * d->W, C2 * 2 * d->W * d->H, C2 * 2 * d->W * d->H * d->D};
+    if (rank == 4) dims[3] = d->B;
+    int lower[3] = {-d->pw, -d->ph, -d->pd};
+    int upper[3] = {d->pw - (d->kw - 1), d->ph - (d->kh - 1), d->pd - (d->kd - 1)};
+    cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(xs), dims, strides, lower, upper, 64, TC_BM, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error("g6d_conv_tc: cuTensorMapEncodeIm2col failed (%d)", (int)r); return G6D_ECUDA; }
@@ -820,7 +882,7 @@ __global__ void split_f16_kernel(const float* __restrict__ in, __half* __restric
 // 64 cb + f16_k_source(p).  A thread makes one 16-byte chunk of each from the same two float4 loads and the same
 // split_f16x2 calls as a producer thread of conv_tc2_kernel, so the tiles are bit-identical.  With a prologue
 // (G6D_TC_PRENORM) every element is transformed by prologue4 first, as the producers transform every in-bounds
-// element; the padding stays zero, as the im2col map fills it after this pass.  plane = H * W pixels per image.
+// element; the padding stays zero, as the im2col map fills it after this pass.  plane = D * H * W pixels per image.
 __global__ void split_input_f16_kernel(const float* __restrict__ x, int ics, int ico, int Cin, long long rows,
                                        long long plane, int pro, const float* __restrict__ ps, const float* __restrict__ pb,
                                        long long group_rows, __half* __restrict__ out) {
@@ -1163,6 +1225,47 @@ static bool fill_flat_params(const g6d_conv_desc* d, int kind, ConvFlatP& p, int
     return true;
 }
 
+// The fused moments conv_tcflat_kernel's epilogue adds, from the output of a layer that ran on the persistent kernel
+// in that kernel's K order instead (G6D_TC_REUSE_IM2COL, one K split): the same 16-row slices of each plane's padded
+// enumeration f = yo * Wp + xo (columns xo >= Wo count as zeros) through slice_moments.  So the fp32 partials are the
+// same; the fp64 sums of a plane's slices are added in another order (the A-reuse kernel's atomics have no fixed order
+// either).  The persistent kernel's own slices (16 output rows) would round differently.  A block sums one plane for
+// 8 channels: its 8 warps take every 8th slice, then one atomic pair per channel.
+__global__ void __launch_bounds__(256) flat_moments_kernel(const float* __restrict__ y, int ocs, int oco, int Cout, int Ho, int Wo,
+                                                           int Wp, int slices_per_plane, double* __restrict__ stats,
+                                                           long long stats_rows) {
+    __shared__ double red[8][4][4];                              // [warp][lane < 4][(sum, sum^2) of column e = 0, 1]
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const long long m_plane = (long long)blockIdx.x * Ho * Wo;
+    const int n0 = 8 * blockIdx.y + 2 * (lane & 3);
+    double acc[4] = {0.0, 0.0, 0.0, 0.0};
+    for (int sl = warp; sl < slices_per_plane; sl += 8) {
+        const int f = sl * 16 + (lane >> 2);
+        const float* row[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int yo = (f + 8 * h) / Wp, xo = (f + 8 * h) % Wp;
+            row[h] = yo < Ho && xo < Wo ? y + (m_plane + (long long)yo * Wo + xo) * ocs + oco : nullptr;
+        }
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+            const int n = n0 + e;
+            const float2 s = slice_moments(row[0] && n < Cout ? row[0][n] : 0.f, row[1] && n < Cout ? row[1][n] : 0.f);
+            acc[2 * e] += (double)s.x;
+            acc[2 * e + 1] += (double)s.y;
+        }
+    }
+    if (lane < 4)
+        for (int q = 0; q < 4; ++q) red[warp][lane][q] = acc[q];
+    __syncthreads();
+    if (threadIdx.x < 16) {
+        const int l = threadIdx.x >> 2, q = threadIdx.x & 3, n = 8 * blockIdx.y + 2 * l + (q >> 1);
+        double t = 0.0;
+        for (int w = 0; w < 8; ++w) t += red[w][l][q];
+        if (n < Cout) atomicAdd(stats + ((m_plane / stats_rows) * Cout + n) * 2 + (q & 1), t);
+    }
+}
+
 template <int BN, int KIND>
 static int launch_flat(const ConvFlatP& p, int smem, const CUtensorMap& mh, const CUtensorMap& ml, cudaStream_t st) {
     static bool configured = false;
@@ -1194,31 +1297,47 @@ struct ConvPlan {
 // element once per tap, 16 KB in flight per SM) become two bulk copies per K-block.  The split pass reads and
 // writes the input once.  The bounding box of the im2col map is the output plane shifted by the padding.
 // G6D_TC_PRENORM extends this to layers with a prologue: the split pass applies it (see split_input_f16_kernel).
+// G6D_TC_REUSE_IM2COL extends it to volumes through the rank-5 map, whose box corners the driver only takes in
+// [-16, 15]; a volume outside that range keeps the producer warps.
 static bool split_input_ok(const g6d_conv_desc* d, int kind, int flags, bool use_flat) {
-    return !use_flat && kind == G6D_TC_F16 && (d->prologue == G6D_PRO_NONE || (flags & G6D_TC_PRENORM)) && d->stride == 1 &&
-           d->kd == 1 && d->D == 1 && d->kh * d->kw > 1 && d->kw <= 64 && d->kh <= 64 && d->pw < 64 && d->ph < 64;
+    if (use_flat || kind != G6D_TC_F16 || (d->prologue != G6D_PRO_NONE && !(flags & G6D_TC_PRENORM)) || d->stride != 1 ||
+        d->kd * d->kh * d->kw == 1)
+        return false;
+    if (!split_input_rank5(d)) return d->kw <= 64 && d->kh <= 64 && d->pw < 64 && d->ph < 64;
+    auto corners_ok = [](int k, int pad) { return k <= 16 && pad <= 16 && pad - (k - 1) >= -16 && pad - (k - 1) <= 15; };
+    return (flags & G6D_TC_REUSE_IM2COL) && corners_ok(d->kw, d->pw) && corners_ok(d->kh, d->ph) && corners_ok(d->kd, d->pd);
 }
 
 static int make_plan(const g6d_conv_desc* d, int kind, int flags, ConvPlan& pl) {
-    G6D_REQUIRE((flags & ~G6D_TC_PRENORM) == 0, "g6d_conv_tc: bad flags %d", flags);
+    G6D_REQUIRE((flags & ~(G6D_TC_PRENORM | G6D_TC_REUSE_IM2COL)) == 0, "g6d_conv_tc: bad flags %d", flags);
     const int rc = fill_tc_params(d, kind, pl.tc);
     if (rc != G6D_OK) return rc;
     pl.use_flat = fill_flat_params(d, kind, pl.flat, &pl.flat_smem);
+    pl.tc.reuse_order = 0;
+    if (pl.use_flat && (flags & G6D_TC_REUSE_IM2COL) && split_input_ok(d, kind, flags, false)) {
+        // the persistent kernel with im2col A, in the A-reuse kernel's K order and K splits (bit-identical)
+        pl.use_flat = false;
+        pl.tc.reuse_order = 1;
+        pl.tc.kb_per_split = pl.flat.cb_per_split * d->kd * d->kh * d->kw;
+        pl.tc.splits = pl.flat.splits;
+    }
     pl.bn = tc_block_n(d->Cout);
     pl.splits = pl.use_flat ? pl.flat.splits : pl.tc.splits;
     pl.tc.split_in = split_input_ok(d, kind, flags, pl.use_flat) ? 1 : 0;
     const long long partials = pl.splits > 1 ? (long long)pl.splits * pl.tc.M * pl.tc.Cout * (long long)sizeof(float) : 0;
     pl.split_in_off = (partials + 255) / 256 * 256;
-    pl.ws_bytes = pl.tc.split_in ? pl.split_in_off + (long long)d->B * d->H * d->W * d->Cin * 2 * (long long)sizeof(__half)
-                                 : partials;
+    pl.ws_bytes = pl.tc.split_in
+                      ? pl.split_in_off + (long long)d->B * d->D * d->H * d->W * d->Cin * 2 * (long long)sizeof(__half)
+                      : partials;
     return G6D_OK;
 }
 
 // fused output statistics are possible when every 32-row epilogue slice lies in one group; the A-reuse
-// kernel's tiles never span image planes, so its groups must also be made of whole planes
+// kernel's tiles never span image planes, so its groups (and those of flat_moments_kernel) must also be made of
+// whole planes
 static bool stats_ok(const ConvPlan& pl, long long stats_rows) {
     if (stats_rows <= 0 || stats_rows % 32 != 0 || pl.tc.M % stats_rows != 0) return false;
-    return !pl.use_flat || stats_rows % ((long long)pl.flat.Ho * pl.flat.Wo) == 0;
+    return !(pl.use_flat || pl.tc.reuse_order) || stats_rows % ((long long)pl.flat.Ho * pl.flat.Wo) == 0;
 }
 
 template <class P>
@@ -1310,8 +1429,10 @@ extern "C" int g6d_conv_tc_ex(const g6d_conv_desc* desc, const float* x, const v
         cudaError_t e = cudaMemsetAsync(stats, 0, sizeof(double) * 2 * (p.M / stats_rows) * p.Cout, st);
         if (e != cudaSuccess) { set_error("g6d_conv_tc: memset: %s", cudaGetErrorString(e)); return G6D_ECUDA; }
     }
+    // in the A-reuse kernel's K order without K splits, the moments are those of its epilogue (flat_moments_kernel)
+    const bool flat_moments = stats && p.reuse_order && pl.splits == 1;
     if (pl.use_flat) bind_tensors(pl.flat, x, bias, pro_scale, pro_shift, y, ws, stats, stats_rows);
-    else bind_tensors(pl.tc, x, bias, pro_scale, pro_shift, y, ws, stats, stats_rows);
+    else bind_tensors(pl.tc, x, bias, pro_scale, pro_shift, y, ws, flat_moments ? nullptr : stats, stats_rows);
     CUtensorMap mh, ml, ma;
     if ((rc = make_weight_map(&mh, w_hi, w_rows, p.K, pl.bn, kind)) != G6D_OK) return rc;
     if ((rc = make_weight_map(&ml, w_lo, w_rows, p.K, pl.bn, kind)) != G6D_OK) return rc;
@@ -1319,13 +1440,20 @@ extern "C" int g6d_conv_tc_ex(const g6d_conv_desc* desc, const float* x, const v
     if (p.split_in) {
         __half* xs = reinterpret_cast<__half*>(static_cast<char*>(ws) + pl.split_in_off);
         if ((rc = make_split_input_map(&ma, xs, desc)) != G6D_OK) return rc;
-        const long long plane = (long long)p.H * p.W, rows = p.B * plane, n = rows * (p.Cin / 8);
+        const long long plane = (long long)p.D * p.H * p.W, rows = p.B * plane, n = rows * (p.Cin / 8);
         split_input_f16_kernel<<<ceil_div(n, 256), 256, 0, st>>>(x, p.ics, p.ico, p.Cin, rows, plane, p.pro, pro_scale,
                                                                   pro_shift, p.group_rows, xs);
         G6D_CHECK_LAUNCH("g6d_conv_tc(split input)");
     }
     rc = kind == G6D_TC_F16 ? dispatch<G6D_TC_F16>(pl, mh, ml, ma, st) : dispatch<G6D_TC_TF32>(pl, mh, ml, ma, st);
     if (rc != G6D_OK) return rc;
+    if (flat_moments) {
+        const ConvFlatP& f = pl.flat;
+        dim3 grid((unsigned)((long long)f.B * f.Do), ceil_div(f.Cout, 8));
+        flat_moments_kernel<<<grid, 256, 0, st>>>(y, f.ocs, f.oco, f.Cout, f.Ho, f.Wo, f.Wp, f.tiles_per_plane * TC_CONSUMER_WARPS,
+                                                  stats, stats_rows);
+        G6D_CHECK_LAUNCH("g6d_conv_tc(moments)");
+    }
     if (pl.splits > 1) {
         launch_reduce(static_cast<float*>(ws), bias, y, p.M, p.Cout, pl.splits, p.ocs, p.oco, p.act, stats, stats_rows, st);
         G6D_CHECK_LAUNCH("g6d_conv_tc(split reduce)");

@@ -19,6 +19,9 @@ from .params import RefineFeatureParams, RefineRegressorParams, RefineVolumePara
 
 IN_EPS = 1e-5
 _UPLOAD_LOCK = threading.Lock()
+# The volume net's and the feature branches' stride-1 convolutions load A by TMA im2col from a split copy of
+# their input (prologue applied) on the persistent kernel, in the A-reuse kernel's K order: bit-identical results.
+IM2COL = dict(prenorm=True, reuse_im2col=True)
 
 
 @dataclass
@@ -76,9 +79,10 @@ class VolumeRefiner(PackedModule):
     # ------------------------------------------------------------------ cores (channels-last)
     def _conv_in_conv(self, x, pcs, rows_per_img):
         """conv -> InstanceNorm -> ReLU -> conv -> InstanceNorm (stats returned, not applied)."""
-        y, ws = ops.conv(x, pcs[0], stats_rows=rows_per_img)          # moments fused into the conv epilogue
+        y, ws = ops.conv(x, pcs[0], stats_rows=rows_per_img, **IM2COL)          # moments fused into the conv epilogue
         ps, pb = ops.instnorm_finalize(ws, rows_per_img, IN_EPS)
-        y, ws = ops.conv(y, pcs[1], prologue=ops.PRO_AFFINE_RELU, pro_scale=ps, pro_shift=pb, group_rows=1, stats_rows=rows_per_img)
+        y, ws = ops.conv(y, pcs[1], prologue=ops.PRO_AFFINE_RELU, pro_scale=ps, pro_shift=pb, group_rows=1, stats_rows=rows_per_img,
+                         **IM2COL)
         ps, pb = ops.instnorm_finalize(ws, rows_per_img, IN_EPS)
         return y, ps, pb
 
@@ -115,10 +119,10 @@ class VolumeRefiner(PackedModule):
         br, keep = Branches(2), []
 
         def one_embed(bi, name, x):
-            y, ws = ops.conv(x, p[name][0], stats_rows=sn ** 3)
+            y, ws = ops.conv(x, p[name][0], stats_rows=sn ** 3, **IM2COL)
             ps, pb = ops.instnorm_finalize(ws, sn ** 3, IN_EPS)
             ops.conv(y, p[name][1], prologue=ops.PRO_AFFINE_RELU, pro_scale=ps, pro_shift=pb, group_rows=1,
-                     out=cat, out_coff=64 * bi)
+                     out=cat, out_coff=64 * bi, **IM2COL)
             keep.append((y, ps, pb))
 
         for bi, (name, x) in enumerate((('mean_embed', mean_in), ('var_embed', stdv))):
@@ -127,10 +131,10 @@ class VolumeRefiner(PackedModule):
         x, pro, ps, pb = cat, ops.PRO_NONE, None, None
         for pc in p['trunk']:
             vox = ((x.shape[1] - 1) // pc.stride + 1) ** 3                  # output voxels per pose (k 3, pad 1)
-            y, ws = ops.conv(x, pc, prologue=pro, pro_scale=ps, pro_shift=pb, group_rows=1, stats_rows=vox)
+            y, ws = ops.conv(x, pc, prologue=pro, pro_scale=ps, pro_shift=pb, group_rows=1, stats_rows=vox, **IM2COL)
             ps, pb = ops.instnorm_finalize(ws, vox, IN_EPS)
             x, pro = y, ops.PRO_AFFINE_RELU
-        return ops.conv(x, p['conv5_3'], prologue=pro, pro_scale=ps, pro_shift=pb, group_rows=1)
+        return ops.conv(x, p['conv5_3'], prologue=pro, pro_scale=ps, pro_shift=pb, group_rows=1, **IM2COL)
 
     def _regress(self, x):
         """RefineRegressor.forward (refiner.py:153-166); x [qn, n_vox*512] channels-last flattened."""

@@ -255,7 +255,7 @@ long long g6d_conv_tc_workspace_bytes(const g6d_conv_desc* desc, int kind);
 int g6d_conv_tc_stats_supported(const g6d_conv_desc* desc, int kind, long long stats_rows);
 /* What g6d_conv_tc would launch for desc (no launch): out4 = {kernel (0 persistent, 1 A-reuse), BN, K splits,
  * split input (1: the persistent kernel loads A by TMA im2col from an fp16 hi/lo copy of x that the call writes
- * into the workspace -- fp16 kind, stride 1, no prologue (see G6D_TC_PRENORM), 2-D multi-tap)}.  G6D_EINVAL with g6d_conv_tc's
+ * into the workspace -- fp16 kind, stride 1, no prologue (see G6D_TC_PRENORM), 2-D multi-tap (3-D: G6D_TC_REUSE_IM2COL))}.  G6D_EINVAL with g6d_conv_tc's
  * message when the descriptor is rejected. */
 int g6d_conv_tc_plan(const g6d_conv_desc* desc, int kind, int* out4);
 int g6d_conv_tc(const g6d_conv_desc* desc, const float* x, const void* w_hi, const void* w_lo, int w_rows, int kind,
@@ -265,8 +265,15 @@ int g6d_conv_tc(const g6d_conv_desc* desc, const float* x, const void* w_hi, con
  * G6D_TC_PRENORM: where the split input would apply if the layer had no prologue (fp16 kind, persistent kernel, 2-D,
  * stride 1, multi-tap), it applies with the prologue too: the call's split pass writes prologue(x) split into hi/lo,
  * and the kernel loads A from it by TMA im2col.  Bit-identical to the producer warps (selector towers: their 8x8
- * and 4x4 InstanceNorm-ed layers).  Elsewhere the flag changes nothing.  Other bits: G6D_EINVAL. */
+ * and 4x4 InstanceNorm-ed layers).  Elsewhere the flag changes nothing.
+ * G6D_TC_REUSE_IM2COL: a layer the A-reuse kernel would take that could have the split input (as above, with
+ * G6D_TC_PRENORM where it has a prologue) runs on the persistent kernel with TMA im2col A instead, in the A-reuse
+ * kernel's K order and K splits: bit-identical outputs.  It also lets 3-D layers (and 2-D planes stacked in D)
+ * have the split input on the persistent kernel, through a rank-5 im2col map; a volume whose box corners leave
+ * [-16, 15] (pad > 16 or kernel > 16) keeps the gathering kernels.  Elsewhere (1x1, stride 2, tf32) it changes nothing.
+ * Other bits: G6D_EINVAL. */
 #define G6D_TC_PRENORM 1
+#define G6D_TC_REUSE_IM2COL 4
 int g6d_conv_tc_plan_ex(const g6d_conv_desc* desc, int kind, int flags, int* out4);
 long long g6d_conv_tc_workspace_bytes_ex(const g6d_conv_desc* desc, int kind, int flags);
 int g6d_conv_tc_ex(const g6d_conv_desc* desc, const float* x, const void* w_hi, const void* w_lo, int w_rows, int kind,

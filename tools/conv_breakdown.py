@@ -9,8 +9,9 @@ it, replayed R times, median per copy (timing the calls inside the eager replay 
 whenever a kernel is shorter than its launch).  Each line aggregates the calls of one tag; the tag names
 the kernel the planner picked (persist: the persistent kernel, reuse: the A-reuse kernel), the prologue,
 BN, the K splits and how a persistent call gets its A operand (im2col: by TMA from a split copy of the input,
-prenorm: the same from a copy with the prologue applied; neither: gathered by the producer warps).  Times
-are per step of B poses, split pass included."""
+prenorm: the same from a copy with the prologue applied; neither: gathered by the producer warps; a '-ro' suffix
+marks a layer the A-reuse kernel would take, run in its K order by G6D_TC_REUSE_IM2COL).  Times are per step of B
+poses, split pass included.  A total line sums the refiner's volume net and feature branches."""
 import argparse
 import collections
 import os
@@ -42,20 +43,39 @@ def record_step(batch, refine_iter):
     return est, rec
 
 
+REFINER_METHODS = ('_volume_net', '_conv_in_conv')     # the refiner's 3-D stack and its feature branches
+
+
 def conv_calls(rec):
-    """The arguments of every ops.conv call of one eager replay of the recorded stages (the tensors stay alive)."""
-    calls, orig = [], ops.conv
+    """(args, kwargs, from the refiner) of every ops.conv call of one eager replay of the recorded stages (the tensors
+    stay alive).  A call is the refiner's when it comes from one of REFINER_METHODS."""
+    from gen6d_b200.network.refiner import VolumeRefiner
+    calls, orig, depth = [], ops.conv, [0]
+    saved = {n: getattr(VolumeRefiner, n) for n in REFINER_METHODS}
 
     def wrapped(*a, **k):
-        calls.append((a, k))
+        calls.append((a, k, depth[0] > 0))
         return orig(*a, **k)
+
+    def marking(f):
+        def g(*a, **k):
+            depth[0] += 1
+            try:
+                return f(*a, **k)
+            finally:
+                depth[0] -= 1
+        return g
     ops.conv = wrapped
+    for n, f in saved.items():
+        setattr(VolumeRefiner, n, marking(f))
     try:
         with torch.no_grad():
             for fn, inputs in rec:
                 fn(*inputs)
     finally:
         ops.conv = orig
+        for n, f in saved.items():
+            setattr(VolumeRefiner, n, f)
     torch.cuda.synchronize()
     return calls
 
@@ -85,9 +105,10 @@ def time_call(a, k, reps, repeat):
 
 
 def breakdown(calls, reps=10, repeat=5):
-    """{tag: [calls, ms, flop]} per step.  Calls with the same tag are timed once (the first of them)."""
-    agg, timed = collections.OrderedDict(), {}
-    for a, k in calls:
+    """({tag: [calls, ms, flop]} per step, the same summed over the refiner's calls).  Calls with the same tag are
+    timed once (the first of them)."""
+    agg, timed, refiner = collections.OrderedDict(), {}, [0, 0.0, 0.0]
+    for a, k, in_refiner in calls:
         prof = ops.enable_profiling()
         ops.conv(*a, **k)
         c = ops.collect_profile(prof).get('#calls')
@@ -97,9 +118,9 @@ def breakdown(calls, reps=10, repeat=5):
         if tag not in timed:
             timed[tag] = time_call(a, k, reps, repeat)
         _, work, ms = timed[tag]
-        e = agg.setdefault(tag, [0, 0.0, 0.0])
-        e[0] += 1; e[1] += ms; e[2] += work
-    return agg
+        for e in (agg.setdefault(tag, [0, 0.0, 0.0]),) + ((refiner,) if in_refiner else ()):
+            e[0] += 1; e[1] += ms; e[2] += work
+    return agg, refiner
 
 
 def no_prologue_3x3_persistent(tag):
@@ -113,12 +134,12 @@ def prologue_3x3_persistent(tag):
     return ' k=1x3x3 s=1 pro=' in f' {tag} ' and ' pro=0 ' not in f' {tag} ' and ' persist ' in f' {tag} '
 
 
-def report(agg, top=40):
+def report(agg, refiner, top=40):
     tot_ms, tot_w = sum(a[1] for a in agg.values()), sum(a[2] for a in agg.values())
     print(f'conv_tc calls {sum(a[0] for a in agg.values())} total {tot_ms:.2f} ms, {tot_w / tot_ms / 1e9:.1f} TFLOP/s')
     classes = collections.OrderedDict()
     for tag, (n, ms, w) in agg.items():
-        key = ' '.join(t for t in tag.split() if t.startswith(('pro=', 'persist', 'reuse', 'prenorm')))
+        key = ' '.join(t for t in tag.split() if t.startswith(('pro=', 'persist', 'reuse', 'prenorm', 'im2col')))
         c = classes.setdefault(key, [0, 0.0, 0.0]); c[0] += n; c[1] += ms; c[2] += w
     for key, (n, ms, w) in sorted(classes.items(), key=lambda kv: -kv[1][1]):
         print(f'  {ms:7.3f} ms x{n:3d} {w / ms / 1e9:6.1f} TF/s  [{key}]')
@@ -128,6 +149,10 @@ def report(agg, top=40):
         if sel:
             ms, w = sum(a[1] for a in sel), sum(a[2] for a in sel)
             print(f'  {ms:7.3f} ms x{sum(a[0] for a in sel):3d} {w / ms / 1e9:6.1f} TF/s  [{what}]')
+    n, ms, w = refiner
+    if n:
+        print(f'  {ms:7.3f} ms x{n:3d} {w / ms / 1e9:6.1f} TF/s  [refiner volume net + feature branches, '
+              f'{100 * ms / tot_ms:.1f} % of the total]')
     for tag, (n, ms, w) in sorted(agg.items(), key=lambda kv: -kv[1][1])[:top]:
         print(f'{ms:7.3f} ms x{n:3d} {w / ms / 1e9:6.1f} TF/s  {tag}')
 
@@ -144,7 +169,7 @@ def main():
     _, rec = record_step(a.batch, a.refine_iter)
     print(f'{torch.cuda.get_device_name()}: batch {a.batch}, {a.refine_iter} refinements, '
           f'median of {a.repeat} replays of {a.reps} copies per shape')
-    report(breakdown(conv_calls(rec), a.reps, a.repeat), a.top)
+    report(*breakdown(conv_calls(rec), a.reps, a.repeat), top=a.top)
 
 
 if __name__ == '__main__':
