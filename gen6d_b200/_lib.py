@@ -13,6 +13,7 @@ LIB_PATH = os.path.join(HERE, 'libgen6d_b200.so')
 HEADER_PATH = os.path.join(os.path.dirname(HERE), 'include', 'gen6d_b200.h')
 
 G6D_DET_MAX_SCALES = 8
+G6D_GLUE_MAX_OBJECTS = 16                   # objects per g6d_glue_*_objects launch
 PRO_NONE, PRO_AFFINE, PRO_AFFINE_RELU, PRO_CORR = 0, 1, 2, 3
 ACT_NONE, ACT_RELU, ACT_LEAKY01 = 0, 1, 2
 TC_TF32, TC_F16 = 0, 1
@@ -61,8 +62,14 @@ _SIGNATURES = {
     'g6d_glue_refine_problems_host': [C.POINTER(GlueViews), P, P, I, I, P, I, I, P, P, P, P, P, P, P],
     'g6d_glue_apply_refinements': [C.POINTER(GlueViews), P, P, P, P, I, P, P],
     'g6d_glue_apply_refinements_host': [C.POINTER(GlueViews), P, P, P, P, I, P],
+    'g6d_glue_refine_problems_objects': [C.POINTER(GlueViews), I, I, P, P, I, I, P, I, P, P, P, P, P, P, P, P],
+    'g6d_glue_refine_problems_objects_host': [C.POINTER(GlueViews), I, I, P, P, I, I, P, I, P, P, P, P, P, P, P],
+    'g6d_glue_apply_refinements_objects': [C.POINTER(GlueViews), I, I, P, P, P, P, P, P],
+    'g6d_glue_apply_refinements_objects_host': [C.POINTER(GlueViews), I, I, P, P, P, P, P],
     'g6d_track_smooth': [P, I, P, P, P, P, I, P, I, P, P, P],
     'g6d_track_smooth_host': [P, I, P, P, P, P, I, P, I, P, P],
+    'g6d_track_smooth_objects': [P, I, P, I, I, P, P, P, I, P, P, P, P],
+    'g6d_track_smooth_objects_host': [P, I, P, I, I, P, P, P, I, P, P, P],
     'g6d_nchw_to_nhwc': [P, P, I, I, I, I, I, P],
     'g6d_nhwc_to_nchw': [P, P, I, I, I, I, I, P],
     'g6d_resize_bilinear': [P, P, I, I, I, I, I, I, I, I, P],

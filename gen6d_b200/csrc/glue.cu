@@ -127,6 +127,65 @@ static bool views_ok(const g6d_glue_views* v) {
            v->norm_scale > 0;
 }
 
+// ------------------------------------------------------------------------------------------ several objects
+// Rows are object-major: row i = o * rows_per_obj + s is object o on frame s, so it reads views[o], cams[s] and frame s, and
+// writes row i of every output (the layout of the per-object calls concatenated).  The per-row functions above get the
+// frame's camera and image as row 0 of shifted pointers and the row's outputs at index i, so every row runs the very code
+// of the single-object kernels.
+struct GlueViewsPack {                 // by value: one kernel parameter block for all objects of a launch
+    g6d_glue_views v[G6D_GLUE_MAX_OBJECTS];
+};
+static_assert(sizeof(GlueViewsPack) + 256 <= 4096, "the objects' view structs must fit the 4 KB kernel parameter space");
+
+G6D_HD void do_refine_frame_objects(int i, int s, const g6d_glue_views& v, const g6d_glue_camera* cams, const uint8_t* frames,
+                                    int rows, int cols, const double* poses, int in_f32, g6d_warp_job* jobs, float* que_K,
+                                    float* que_pose, float* rect, FrameProblem& fp, int* chosen) {
+    do_refine_frame(0, v, cams + s, poses + (long long)i * 12, in_f32, fp, chosen);
+    store_frame(0, v, fp, frames + (long long)s * rows * cols * 3, rows, cols, jobs + (long long)i * (v.ref_num + 1), que_K + (long long)i * 9,
+                que_pose + (long long)i * 12, rect + (long long)i * 12);
+}
+
+__global__ void __launch_bounds__(32) glue_refine_problems_objects_kernel(const GlueViewsPack pk, int rows_per_obj,
+                                                                          const g6d_glue_camera* cams, const uint8_t* frames, int rows,
+                                                                          int cols, const double* poses, int in_f32, g6d_warp_job* jobs,
+                                                                          float* que_K, float* que_pose, float* rect, float* ref_Ks,
+                                                                          float* ref_poses, int* ref_rows) {
+    __shared__ double s_Rq[9];
+    __shared__ int s_rows[kGlueMaxViews];
+    const int i = blockIdx.x;
+    const g6d_glue_views v = pk.v[i / rows_per_obj];
+    if (threadIdx.x == 0) {
+        FrameProblem fp;
+        do_refine_frame_objects(i, i % rows_per_obj, v, cams, frames, rows, cols, poses, in_f32, jobs, que_K, que_pose, rect, fp, s_rows);
+        for (int e = 0; e < 9; ++e) s_Rq[e] = fp.Rq[e];
+    }
+    __syncthreads();
+    if ((int)threadIdx.x < v.ref_num) do_refine_view(i, threadIdx.x, s_rows[threadIdx.x], v, s_Rq, jobs, ref_Ks, ref_poses, ref_rows);
+}
+__global__ void glue_apply_objects_kernel(const GlueViewsPack pk, int rows_per_obj, const float* que_pose, const float* que_K,
+                                          const float* rect, const float* net_out, int qn, double* poses) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < qn) do_apply(i, pk.v[i / rows_per_obj], que_pose, que_K, rect, net_out, poses);
+}
+
+// host checks shared by the device and host entry points; also fills the parameter block
+static int objects_ok(const char* name, const g6d_glue_views* views, int n_obj, int rows_per_obj, bool full, GlueViewsPack* pk) {
+    G6D_REQUIRE(views, "%s: null views", name);
+    G6D_REQUIRE(n_obj >= 1 && n_obj <= G6D_GLUE_MAX_OBJECTS, "%s: need 1 <= n_obj <= %d (got n_obj=%d)", name, G6D_GLUE_MAX_OBJECTS, n_obj);
+    G6D_REQUIRE(rows_per_obj >= 1, "%s: need rows_per_obj >= 1 (got %d)", name, rows_per_obj);
+    for (int o = 0; o < n_obj; ++o) {
+        if (full) {
+            G6D_REQUIRE(views_ok(views + o), "%s: incomplete view tables of object %d (2 <= ref_num < %d)", name, o, kGlueMaxViews);
+            G6D_REQUIRE(views[o].ref_num == views[0].ref_num, "%s: object %d has ref_num %d, object 0 has %d; all objects need the same",
+                        name, o, views[o].ref_num, views[0].ref_num);
+        } else {
+            G6D_REQUIRE(views[o].norm_scale > 0, "%s: object %d has no normalisation (norm_scale <= 0)", name, o);
+        }
+        pk->v[o] = views[o];
+    }
+    return G6D_OK;
+}
+
 }  // namespace g6d
 
 using namespace g6d;
@@ -198,5 +257,64 @@ extern "C" int g6d_glue_apply_refinements_host(const g6d_glue_views* views, cons
                                                const float* net_out, int qn, double* poses) {
     G6D_REQUIRE(views && views->norm_scale > 0 && que_pose && que_K && rect && net_out && poses && qn > 0, "g6d_glue_apply_refinements_host: bad args");
     for (int i = 0; i < qn; ++i) do_apply(i, *views, que_pose, que_K, rect, net_out, poses);
+    return G6D_OK;
+}
+
+extern "C" int g6d_glue_refine_problems_objects(const g6d_glue_views* views, int n_obj, int rows_per_obj, const g6d_glue_camera* cams,
+                                                const uint8_t* frames, int rows, int cols, const double* poses, int poses_are_f32,
+                                                g6d_warp_job* jobs, float* que_K, float* que_pose, float* rect, float* ref_Ks,
+                                                float* ref_poses, int* ref_rows, g6d_stream_t stream) {
+    const char* name = "g6d_glue_refine_problems_objects";
+    GlueViewsPack pk;
+    const int rc = objects_ok(name, views, n_obj, rows_per_obj, true, &pk);
+    if (rc != G6D_OK) return rc;
+    G6D_REQUIRE(cams && frames && poses && jobs && que_K && que_pose && rect && ref_Ks && ref_poses && ref_rows && rows > 0 && cols > 0,
+                "%s: bad args", name);
+    glue_refine_problems_objects_kernel<<<n_obj * rows_per_obj, 32, 0, as_stream(stream)>>>(
+        pk, rows_per_obj, cams, frames, rows, cols, poses, poses_are_f32, jobs, que_K, que_pose, rect, ref_Ks, ref_poses, ref_rows);
+    G6D_CHECK_LAUNCH(name);
+    return G6D_OK;
+}
+extern "C" int g6d_glue_refine_problems_objects_host(const g6d_glue_views* views, int n_obj, int rows_per_obj, const g6d_glue_camera* cams,
+                                                     const uint8_t* frames, int rows, int cols, const double* poses, int poses_are_f32,
+                                                     g6d_warp_job* jobs, float* que_K, float* que_pose, float* rect, float* ref_Ks,
+                                                     float* ref_poses, int* ref_rows) {
+    const char* name = "g6d_glue_refine_problems_objects_host";
+    GlueViewsPack pk;
+    const int rc = objects_ok(name, views, n_obj, rows_per_obj, true, &pk);
+    if (rc != G6D_OK) return rc;
+    G6D_REQUIRE(cams && poses && jobs && que_K && que_pose && rect && ref_Ks && ref_poses && ref_rows, "%s: bad args", name);
+    for (int i = 0; i < n_obj * rows_per_obj; ++i) {
+        const g6d_glue_views& v = pk.v[i / rows_per_obj];
+        FrameProblem fp;
+        int chosen[kGlueMaxViews];
+        do_refine_frame_objects(i, i % rows_per_obj, v, cams, frames, rows, cols, poses, poses_are_f32, jobs, que_K, que_pose, rect, fp,
+                                chosen);
+        for (int r = 0; r < v.ref_num; ++r) do_refine_view(i, r, chosen[r], v, fp.Rq, jobs, ref_Ks, ref_poses, ref_rows);
+    }
+    return G6D_OK;
+}
+
+extern "C" int g6d_glue_apply_refinements_objects(const g6d_glue_views* views, int n_obj, int rows_per_obj, const float* que_pose,
+                                                  const float* que_K, const float* rect, const float* net_out, double* poses,
+                                                  g6d_stream_t stream) {
+    const char* name = "g6d_glue_apply_refinements_objects";
+    GlueViewsPack pk;
+    const int rc = objects_ok(name, views, n_obj, rows_per_obj, false, &pk);
+    if (rc != G6D_OK) return rc;
+    G6D_REQUIRE(que_pose && que_K && rect && net_out && poses, "%s: bad args", name);
+    const int qn = n_obj * rows_per_obj;
+    glue_apply_objects_kernel<<<ceil_div(qn, 32), 32, 0, as_stream(stream)>>>(pk, rows_per_obj, que_pose, que_K, rect, net_out, qn, poses);
+    G6D_CHECK_LAUNCH(name);
+    return G6D_OK;
+}
+extern "C" int g6d_glue_apply_refinements_objects_host(const g6d_glue_views* views, int n_obj, int rows_per_obj, const float* que_pose,
+                                                       const float* que_K, const float* rect, const float* net_out, double* poses) {
+    const char* name = "g6d_glue_apply_refinements_objects_host";
+    GlueViewsPack pk;
+    const int rc = objects_ok(name, views, n_obj, rows_per_obj, false, &pk);
+    if (rc != G6D_OK) return rc;
+    G6D_REQUIRE(que_pose && que_K && rect && net_out && poses, "%s: bad args", name);
+    for (int i = 0; i < n_obj * rows_per_obj; ++i) do_apply(i, pk.v[i / rows_per_obj], que_pose, que_K, rect, net_out, poses);
     return G6D_OK;
 }

@@ -137,3 +137,48 @@ def host_apply_refinements(tables, prob, net_out):
                                                           prob['pose_rect'].ctypes.data, net.ctypes.data, len(net), poses.ctypes.data),
                'g6d_glue_apply_refinements_host')
     return poses
+
+
+def _views_array(structs):
+    return (_lib.GlueViews * len(structs))(*structs)
+
+
+def host_refine_problems_objects(tables_list, cams, poses, poses_are_f32, rows, cols, frame_ptr=0, sources=None):
+    """g6d_glue_refine_problems_objects_host: K objects' tables, cams [qn,20], poses [K*qn,3,4] object-major (row o*qn + s
+    is object o on frame s) -> the outputs of host_refine_problems, K*qn rows.  sources: per object (src, img_rows,
+    img_cols) of its views, as host_refine_problems takes them (default zeros)."""
+    K, qn = len(tables_list), len(cams)
+    n, R = len(poses), tables_list[0]['ref_num']
+    if sources is None:
+        sources = [(None, None, None)] * K
+    keep = []
+    for t, (src, img_rows, img_cols) in zip(tables_list, sources):
+        nv = len(t['ids'])
+        keep.append((np.zeros(nv, np.uint64) if src is None else np.ascontiguousarray(src, np.uint64),
+                     np.zeros(nv, np.int32) if img_rows is None else np.ascontiguousarray(img_rows, np.int32),
+                     np.zeros(nv, np.int32) if img_cols is None else np.ascontiguousarray(img_cols, np.int32)))
+    views = _views_array([views_struct(t, t, *k) for t, k in zip(tables_list, keep)])
+    cams, poses = np.ascontiguousarray(cams, np.float64), np.ascontiguousarray(poses, np.float64)
+    out = {'jobs': np.zeros(n * (R + 1), JOB), 'que_K': np.zeros((n, 3, 3), np.float32), 'que_pose': np.zeros((n, 3, 4), np.float32),
+           'pose_rect': np.zeros((n, 3, 4), np.float32), 'ref_Ks': np.zeros((n, R, 3, 3), np.float32),
+           'ref_poses': np.zeros((n, R, 3, 4), np.float32), 'ref_rows': np.zeros((n, R), np.int32)}
+    _lib.check(_lib.lib().g6d_glue_refine_problems_objects_host(views, K, qn, cams.ctypes.data, frame_ptr, rows, cols, poses.ctypes.data,
+                                                                int(poses_are_f32), *[out[k].ctypes.data for k in
+                                                                                      ('jobs', 'que_K', 'que_pose', 'pose_rect', 'ref_Ks',
+                                                                                       'ref_poses', 'ref_rows')]),
+               'g6d_glue_refine_problems_objects_host')
+    return out
+
+
+def host_apply_refinements_objects(tables_list, prob, net_out):
+    """g6d_glue_apply_refinements_objects_host: K objects' tables, the K*qn problems of host_refine_problems_objects and
+    network outputs [K*qn,7] -> refined poses [K*qn,3,4]."""
+    K = len(tables_list)
+    views = _views_array([views_struct(t, t) for t in tables_list])
+    net = np.ascontiguousarray(net_out, np.float32)
+    poses = np.zeros((len(net), 3, 4), np.float64)
+    _lib.check(_lib.lib().g6d_glue_apply_refinements_objects_host(views, K, len(net) // K, prob['que_pose'].ctypes.data,
+                                                                  prob['que_K'].ctypes.data, prob['pose_rect'].ctypes.data,
+                                                                  net.ctypes.data, poses.ctypes.data),
+               'g6d_glue_apply_refinements_objects_host')
+    return poses

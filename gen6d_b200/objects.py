@@ -8,10 +8,12 @@ same frames as ONE captured graph with one synchronising read:
   upload -> ONE detection stage for all objects (the query's VGG pyramid once per scale, one correlation GEMM per level
   over the objects' concatenated kernels, g6d_det_corr_rowsum_objects, then score fusion / heads / argmax on K*qn
   "queries") -> the K*qn selector crops in one warp and one crop VGG, each object's selection against its own reference
-  stack -> refine_iter x (per-object refinement problems, ONE refiner stage over all K*qn poses, per-object update).
+  stack -> refine_iter x (the objects' refinement problems in one launch, ONE refiner stage over all K*qn poses, the
+  objects' updates in one launch; g6d_glue_*_objects).
 
 Rows are object-major (object, frame) everywhere after the correlation, so each object's detections, crops and poses are
-a contiguous slice whose row i is frame i, which is the layout the g6d_glue_* kernels take.
+a contiguous slice whose row i is frame i, which is the layout the g6d_glue_* kernels take.  ObjectSet.tracker() follows
+the set's objects through videos (gen6d_b200/track.py ObjectTracker).
 """
 import numpy as np
 import torch
@@ -46,6 +48,7 @@ class ObjectSet:
         self.est = est
         self._objects = {}
         self._kernels = None            # the objects' detector kernels concatenated (rebuilt when membership changes)
+        self.membership = 0             # counts add / remove: a tracker made before a change is stale
         self.stages = StageCache()      # the set's prediction graph
 
     # -------------------------------------------------------------- membership
@@ -93,6 +96,7 @@ class ObjectSet:
         self._membership_changed()
 
     def _membership_changed(self):
+        self.membership += 1
         self._kernels = None
         self.stages.clear()             # the graph captured the previous objects' state
 
@@ -121,12 +125,15 @@ class ObjectSet:
         out, _ = ops.det_parse(o['score_predict'], o['scale_predict'], o['offset_predict'], det.pool_ratio)
         return out, o
 
-    def _predict_fn(self):
-        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> (packed results f64 as bytes ++ crops u8): every stage, back to back."""
+    def _predict_device_fn(self):
+        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> every stage, back to back, as device tensors: (chain f64
+        [refine_iter+1, K*qn, 12] of object-major poses, det [K*qn,4], [(sel_idx, sel_out, logits)] per object, crops u8
+        [K*qn, res, res, 3])."""
         est = self.est
         objs = list(self._objects.values())
         K, res, iters = len(objs), est.cfg['ref_resolution'], est.cfg['refine_iter']
         R = objs[0].tables['tables']['ref_num']
+        views = [ob.tables['views'] for ob in objs]
         sel, refine = est.selector, est.refiner._refine_warped(128)
 
         def fn(frames, cams):
@@ -148,19 +155,28 @@ class ObjectSet:
                 idx, sel_out = ops.sel_parse(logits, torch.stack(ang, 0))
                 sels.append((idx, sel_out, logits))
                 poses.append(ops.glue_initial_poses(rows(det, o), idx, sel_out, ob.tables['refs'], cams))
-            chains = [[p] for p in poses]
+            poses = cat(poses)                                                       # [K*qn,12], object-major
+            chain = [poses]
             for it in range(iters):
-                probs = [ops.glue_refine_problems(ob.tables['views'], R, cams, frames, poses[o], it > 0) for o, ob in enumerate(objs)]
-                jobs_r, que_K, que_pose, ref_Ks, ref_poses = [cat([p[i] for p in probs]) for i in (0, 1, 2, 4, 5)]
+                jobs_r, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems_objects(views, R, cams, frames, poses,
+                                                                                                       it > 0)
                 out = refine(jobs_r, que_K, que_pose, ref_Ks, ref_poses)              # one refiner stage for all K*qn poses
-                poses = [ops.glue_apply_refinements(ob.tables['views'], probs[o][2], probs[o][1], probs[o][3], rows(out, o))
-                         for o, ob in enumerate(objs)]
-                for o in range(K):
-                    chains[o].append(poses[o])
+                poses = ops.glue_apply_refinements_objects(views, que_pose, que_K, rect, out)
+                chain.append(poses)
+            return torch.stack(chain, 0), det, sels, crop
+        return fn
+
+    def _predict_fn(self):
+        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> (packed results f64 as bytes ++ crops u8): every stage, back to back."""
+        stages, K = self._predict_device_fn(), len(self._objects)
+
+        def fn(frames, cams):
+            qn = frames.shape[0]
+            chain, det, sels, crop = stages(frames, cams)
             parts = []
             for o in range(K):
                 idx, sel_out, logits = sels[o]
-                parts += [torch.stack(chains[o], 0), rows(det, o), idx, sel_out, logits]
+                parts += [chain[:, o * qn:(o + 1) * qn], det[o * qn:(o + 1) * qn], idx, sel_out, logits]
             packed = torch.cat([t.reshape(-1).to(torch.float64) for t in parts])
             return torch.cat([packed.view(torch.uint8), crop.reshape(-1)])
         return fn
@@ -202,6 +218,14 @@ class ObjectSet:
                      'sel_ref_idx': idx, 'refine_poses': [chain[0].copy()] + refined}
             out[name] = (refined[-1] if refined else chain[0].copy(), inter)
         return out
+
+    def tracker(self, num_sequences=1, refine_iter=1, smooth_num=5, smooth_std=2.5, bboxes=None):
+        """An ObjectTracker (gen6d_b200/track.py): every object of the set followed through `num_sequences` videos in
+        lockstep, with Tracker's semantics per object; each step is one captured graph and one synchronising read.
+        bboxes: {name: 8 box corners [8,3]}; a missing name takes the box of the object's database point cloud."""
+        from .track import ObjectTracker
+        return ObjectTracker(self, num_sequences, refine_iter=refine_iter, smooth_num=smooth_num, smooth_std=smooth_std,
+                             bboxes=bboxes)
 
     def raw_correlation(self, que_imgs):
         """The detector's raw correlation maps for inspection: {name: [scale][level] float32 [qn, H, W, rfn]} (the maps

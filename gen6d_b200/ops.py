@@ -144,6 +144,70 @@ def glue_apply_refinements(views_struct, que_pose, que_K, rect, net_out):
     return poses
 
 
+def _object_chunks(n_obj):
+    """Object ranges of the g6d_glue_*_objects launches (their view structs travel as one kernel parameter block)."""
+    step = _lib.G6D_GLUE_MAX_OBJECTS
+    return [(o, min(o + step, n_obj)) for o in range(0, n_obj, step)]
+
+
+def _views_array(views_structs, o0, o1):
+    return (_lib.GlueViews * (o1 - o0))(*views_structs[o0:o1])
+
+
+def glue_refine_problems_objects(views_structs, ref_num, cams, frames, poses, poses_are_f32):
+    """glue_refine_problems for K objects on the same qn frames: poses float64 [K*qn,12], object-major (row o*qn + s is
+    object o on frame s, with views_structs[o]) -> the per-object results concatenated along the rows, in one launch
+    per G6D_GLUE_MAX_OBJECTS objects."""
+    qn, h, w, _ = frames.shape
+    K = len(views_structs)
+    n = K * qn
+    if poses.shape != (n, 12):
+        raise ValueError(f'glue_refine_problems_objects: poses {tuple(poses.shape)} for {K} objects x {qn} frames')
+    dev, f32 = frames.device, torch.float32
+    jobs = torch.empty(n, (ref_num + 1) * WARP_JOB_BYTES, device=dev, dtype=torch.uint8)
+    que_K, que_pose, rect = torch.empty(n, 3, 3, device=dev, dtype=f32), torch.empty(n, 3, 4, device=dev, dtype=f32), \
+        torch.empty(n, 3, 4, device=dev, dtype=f32)
+    ref_Ks, ref_poses = torch.empty(n, ref_num, 3, 3, device=dev, dtype=f32), torch.empty(n, ref_num, 3, 4, device=dev, dtype=f32)
+    rows = torch.empty(n, ref_num, device=dev, dtype=torch.int32)
+    for o0, o1 in _object_chunks(K):
+        r = slice(o0 * qn, o1 * qn)
+        _call('g6d_glue_refine_problems_objects', _views_array(views_structs, o0, o1), o1 - o0, qn, _p(cams, torch.float64),
+              _p(frames, torch.uint8), h, w, _p(poses[r], torch.float64), int(poses_are_f32), _p(jobs[r], torch.uint8), _p(que_K[r]),
+              _p(que_pose[r]), _p(rect[r]), _p(ref_Ks[r]), _p(ref_poses[r]), _p(rows[r], torch.int32), _stream())
+    return jobs.reshape(-1), que_K, que_pose, rect, ref_Ks, ref_poses, rows
+
+
+def glue_apply_refinements_objects(views_structs, que_pose, que_K, rect, net_out):
+    """glue_apply_refinements for K objects, rows object-major (K*qn rows, row o*qn + s with views_structs[o]) ->
+    refined poses float64 [K*qn,12], in one launch per G6D_GLUE_MAX_OBJECTS objects."""
+    K, n = len(views_structs), net_out.shape[0]
+    if n % K:
+        raise ValueError(f'glue_apply_refinements_objects: {n} rows for {K} objects')
+    qn = n // K
+    poses = torch.empty(n, 12, device=net_out.device, dtype=torch.float64)
+    for o0, o1 in _object_chunks(K):
+        r = slice(o0 * qn, o1 * qn)
+        _call('g6d_glue_apply_refinements_objects', _views_array(views_structs, o0, o1), o1 - o0, qn, _p(que_pose[r]), _p(que_K[r]),
+              _p(rect[r]), _p(net_out[r]), _p(poses[r], torch.float64), _stream())
+    return poses
+
+
+def track_smooth_objects(poses, poses_are_f32, bboxes, Ks, ring, count, weights):
+    """track_smooth for K objects through S sequences in one launch, rows object-major: poses float64 [K*S,12] (row o*S + s
+    is object o on sequence s), bboxes float32 [K,8,3], Ks float64 [S,9], ring float32 [K*S,num,8,2] and count int32 [K*S]
+    (updated in place), weights float64 [num] -> (smoothed float64 [K*S,12], averaged corners float64 [K*S,8,2])."""
+    K, S, n, num = bboxes.shape[0], Ks.shape[0], poses.shape[0], ring.shape[1]
+    if (bboxes.shape != (K, 8, 3) or Ks.shape != (S, 9) or n != K * S or ring.shape != (n, num, 8, 2) or count.shape != (n,)
+            or weights.shape != (num,)):
+        raise ValueError(f'track_smooth_objects: inconsistent shapes poses {tuple(poses.shape)}, bboxes {tuple(bboxes.shape)}, '
+                         f'Ks {tuple(Ks.shape)}, ring {tuple(ring.shape)}, count {tuple(count.shape)}, weights {tuple(weights.shape)}')
+    smoothed = torch.empty(n, 12, device=poses.device, dtype=torch.float64)
+    avg = torch.empty(n, 8, 2, device=poses.device, dtype=torch.float64)
+    _call('g6d_track_smooth_objects', _p(poses, torch.float64), int(poses_are_f32), _p(bboxes), K, S, _p(Ks, torch.float64), _p(ring),
+          _p(count, torch.int32), num, _p(weights, torch.float64), _p(smoothed, torch.float64), _p(avg, torch.float64), _stream())
+    return smoothed, avg
+
+
 def track_smooth(poses, poses_are_f32, bbox, Ks, ring, count, weights):
     """One smoothing step for S tracked sequences (g6d_track_smooth): poses float64 [S,12] (raw), bbox float32 [8,3],
     Ks float64 [S,9], ring float32 [S,num,8,2] and count int32 [S] (updated in place), weights float64 [num] ->

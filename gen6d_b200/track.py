@@ -7,6 +7,9 @@ With cfg['device_glue'] a tracking step for S sequences in lockstep is ONE captu
 (csrc/glue.cu + the refiner) followed by the smoothing kernel (csrc/track.cu) -- and one synchronising read; the
 previous poses and the corner histories stay on the device between steps.  Otherwise the host sequences the step
 with predict_batch's host path and runs the smoothing through g6d_track_smooth_host (same code, on the CPU).
+
+ObjectTracker (ObjectSet.tracker()) does the same for every object of an object set at once: one graph per step whose
+glue and smoothing launches (the g6d_*_objects entry points) and refiner stage cover all K objects' K*S rows.
 """
 import numpy as np
 import torch
@@ -80,6 +83,26 @@ def host_smooth(poses, poses_are_f32, bbox, Ks, ring, count, weights):
                                                 w.ctypes.data, S, smoothed.ctypes.data, avg.ctypes.data),
                'g6d_track_smooth_host')
     return smoothed.reshape(S, 3, 4), avg
+
+
+def host_smooth_objects(poses, poses_are_f32, bboxes, Ks, ring, count, weights):
+    """g6d_track_smooth_objects_host on numpy arrays: K objects through S sequences, rows object-major (row o*S + s):
+    poses [K*S,3,4], bboxes [K,8,3], Ks [S,3,3]; ring float32 [K*S,num,8,2] and count int32 [K*S] are updated in place.
+    Returns (smoothed float64 [K*S,3,4], averaged corners float64 [K*S,8,2])."""
+    n, K, S = len(poses), len(bboxes), len(Ks)
+    p = np.ascontiguousarray(np.asarray(poses, np.float64).reshape(n, 12))
+    K9 = np.ascontiguousarray(np.asarray(Ks, np.float64).reshape(S, 9))
+    box = np.ascontiguousarray(bboxes, np.float32)
+    w = np.ascontiguousarray(weights, np.float64)
+    for a, dt in ((ring, np.float32), (count, np.int32)):
+        if a.dtype != dt or not a.flags.c_contiguous:
+            raise ValueError(f'host_smooth_objects: ring / count must be contiguous {dt.__name__} arrays (updated in place)')
+    smoothed, avg = np.zeros((n, 12), np.float64), np.zeros((n, 8, 2), np.float64)
+    _lib.check(_lib.lib().g6d_track_smooth_objects_host(p.ctypes.data, int(poses_are_f32), box.ctypes.data, K, S, K9.ctypes.data,
+                                                        ring.ctypes.data, count.ctypes.data, ring.shape[1] if ring.ndim > 1 else 0,
+                                                        w.ctypes.data, smoothed.ctypes.data, avg.ctypes.data),
+               'g6d_track_smooth_objects_host')
+    return smoothed.reshape(n, 3, 4), avg
 
 
 # ------------------------------------------------------------------------------------------ the tracker
@@ -264,3 +287,183 @@ class Tracker:
         inter['bbox_pts'] = ring_h[np.arange(S), count_h - 1].copy()
         inter['smoothed_pts'] = vals['avg'].reshape(S, 8, 2).copy()
         return (refined[-1] if refined else first), vals['smoothed'].reshape(S, 3, 4).copy(), inter
+
+
+# ------------------------------------------------------------------------------------------ several objects
+class ObjectTracker:
+    """Every object of an ObjectSet tracked through S sequences in lockstep; see ObjectSet.tracker().
+
+    Per object the semantics are Tracker's: the first step (and the first after reset()) is the set's full prediction
+    with cfg['refine_iter'] refinements, every later step `refine_iter` refinements from the previous poses, each followed
+    by predict.py's smoothing.  Rows are object-major (row o*S + s is object o on sequence s), and each step is ONE
+    captured graph: refine_iter x (g6d_glue_refine_problems_objects -> one refiner stage over all K*S poses ->
+    g6d_glue_apply_refinements_objects), then g6d_track_smooth_objects, so the number of launches does not grow with
+    K.  The previous poses [K*S,12], the corner histories and their counts stay on the device between steps."""
+
+    def __init__(self, objs, num_sequences, refine_iter=1, smooth_num=5, smooth_std=2.5, bboxes=None):
+        if int(num_sequences) < 1:
+            raise ValueError(f'num_sequences must be >= 1, got {num_sequences}')
+        if int(refine_iter) < 1:
+            raise ValueError(f'refine_iter must be >= 1, got {refine_iter}')
+        if int(smooth_num) < 1:
+            raise ValueError(f'smooth_num must be >= 1, got {smooth_num}')
+        if not float(smooth_std) > 0:
+            raise ValueError(f'smooth_std must be > 0, got {smooth_std}')
+        objs._check()
+        bboxes = dict(bboxes or {})
+        unknown = sorted(set(bboxes) - set(objs.names))
+        if unknown:
+            raise ValueError(f'bboxes names objects that are not in the set: {unknown} (objects: {objs.names})')
+        boxes = []
+        for name, ob in objs._objects.items():
+            box = bboxes.get(name)
+            if box is None:
+                box = object_bbox(ob.ref.database)
+                if box is None:
+                    raise ValueError(f'object {name!r}: its database has no object point cloud: pass bboxes[{name!r}] (the 8 '
+                                     'corners of the object box)')
+            boxes.append(check_bbox(box))
+        self.objs, self.est = objs, objs.est
+        self.names = objs.names
+        self.K, self.S, self.refine_iter = len(self.names), int(num_sequences), int(refine_iter)
+        self.num, self.std = int(smooth_num), float(smooth_std)
+        self.bboxes = np.ascontiguousarray(np.stack(boxes, 0))
+        self.weights = smoothing_weights(self.num, self.std)
+        self._membership = objs.membership
+        self.stages = StageCache()       # this tracker's step graphs (they capture its device state)
+        dev = self.est.detector.device
+        self._dev = {'bboxes': torch.from_numpy(self.bboxes).to(dev), 'weights': torch.from_numpy(self.weights.copy()).to(dev)}
+        self.reset()
+
+    # -------------------------------------------------------------- state
+    def reset(self):
+        """The next step is a full prediction for every object and sequence, and the smoothing histories restart."""
+        dev, n = self.est.detector.device, self.K * self.S
+        self._prev, self._prev_f32 = None, True
+        self._ring = torch.zeros(n, self.num, 8, 2, device=dev, dtype=torch.float32)
+        self._count = torch.zeros(n, device=dev, dtype=torch.int32)
+
+    def start(self, poses):
+        """Begin (or restart) every object's sequences from known poses {name: [S,3,4]} (every object of the set, one
+        dtype for all): the next step refines from them, and the smoothing histories restart."""
+        missing = [n for n in self.names if n not in poses]
+        extra = sorted(set(poses) - set(self.names))
+        if missing or extra:
+            raise ValueError(f'start: need poses for exactly the set\'s objects {self.names}; missing {missing}, unknown {extra}')
+        arrs = [np.asarray(poses[n]) for n in self.names]
+        for n, a in zip(self.names, arrs):
+            if a.shape != (self.S, 3, 4):
+                raise ValueError(f'start: object {n!r}: expected poses [{self.S},3,4], got {a.shape}')
+        dtypes = {a.dtype for a in arrs}
+        if len(dtypes) != 1:
+            raise ValueError(f'start: the objects\' poses have different dtypes {sorted(str(d) for d in dtypes)}; the refinement '
+                             'reads them all as float32 or all as float64, so pass one dtype')
+        self.reset()
+        prev = np.ascontiguousarray(np.concatenate(arrs, 0).astype(np.float64).reshape(self.K * self.S, 12))
+        self._prev, self._prev_f32 = torch.from_numpy(prev).to(self.est.detector.device), arrs[0].dtype == np.float32
+
+    def _check(self):
+        if self.objs.membership != self._membership:
+            raise RuntimeError('this tracker is stale: objects were added to or removed from the set since it was created; '
+                               'create a new one with objs.tracker()')
+        self.objs._check()
+
+    # -------------------------------------------------------------- one step
+    def _full_fn(self):
+        predict, c, K = self.objs._predict_device_fn(), self._dev, self.K
+
+        def fn(frames, cams, ring, count):
+            S = frames.shape[0]
+            chain, det, sels, crop = predict(frames, cams)
+            poses = chain[-1]
+            smoothed, avg = ops.track_smooth_objects(poses, chain.shape[0] > 1, c['bboxes'], cams[:, :9].contiguous(), ring, count,
+                                                     c['weights'])
+            parts = [chain, smoothed, avg, ring, count]
+            for o in range(K):
+                parts += [det[o * S:(o + 1) * S], *sels[o]]
+            packed = torch.cat([t.reshape(-1).to(torch.float64) for t in parts])
+            return torch.cat([packed.view(torch.uint8), crop.reshape(-1)]), poses, ring, count
+        return fn
+
+    def _refine_fn(self, first_f32):
+        objs, iters, c = list(self.objs._objects.values()), self.refine_iter, self._dev
+        views, R = [ob.tables['views'] for ob in objs], objs[0].tables['tables']['ref_num']
+        refine = self.est.refiner._refine_warped(128)
+
+        def fn(frames, cams, prev, ring, count):
+            poses, chain = prev, [prev]
+            for it in range(iters):
+                jobs, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems_objects(views, R, cams, frames, poses,
+                                                                                                     first_f32 or it > 0)
+                out = refine(jobs, que_K, que_pose, ref_Ks, ref_poses)           # one refiner stage for all K*S poses
+                poses = ops.glue_apply_refinements_objects(views, que_pose, que_K, rect, out)
+                chain.append(poses)
+            smoothed, avg = ops.track_smooth_objects(poses, True, c['bboxes'], cams[:, :9].contiguous(), ring, count, c['weights'])
+            packed = torch.cat([t.reshape(-1).to(torch.float64) for t in (torch.stack(chain, 0), smoothed, avg, ring, count)])
+            return packed.view(torch.uint8), poses, ring, count
+        return fn
+
+    def step(self, frames, Ks):
+        """frames: S uint8 [h,w,3] of one size; Ks: [S,3,3] (shared by all objects).  Returns {name: (raw poses float32
+        [S,3,4], smoothed poses float64 [S,3,4], inter)}: inter has Tracker.step's keys, and a full-prediction step adds
+        those of ObjectSet.predict (det_score included)."""
+        self._check()
+        K, S, num, est = self.K, self.S, self.num, self.est
+        if len(frames) != S or len(Ks) != S:
+            raise ValueError(f'step: this tracker follows {S} sequences, got {len(frames)} frames and {len(Ks)} Ks')
+        Ks = np.stack([np.asarray(k) for k in Ks], 0)
+        if Ks.shape != (S, 3, 3):
+            raise ValueError(f'step: Ks must be [{S},3,3], got {Ks.shape}')
+        full = self._prev is None
+        with torch.no_grad():
+            dev_frames = est.detector.upload_frame([np.asarray(f) for f in frames])
+            cams = est.detector._to_dev(glue.cameras(Ks))
+            if full:
+                outs = self.stages.run('track_full', self._full_fn(), [dev_frames, cams, self._ring, self._count])
+            else:
+                outs = self.stages.run(f'track_refine{int(self._prev_f32)}', self._refine_fn(self._prev_f32),
+                                       [dev_frames, cams, self._prev, self._ring, self._count])
+            buf, poses_dev, ring, count = outs
+            prev_f32 = self._prev_f32
+            self._prev = poses_dev.clone()
+            self._ring.copy_(ring)
+            self._count.copy_(count)
+            host = est.detector._to_host(buf)                        # the step's one synchronising read
+        self._prev_f32 = True
+        n, n_chain = K * S, (est.cfg['refine_iter'] if full else self.refine_iter) + 1
+        if full:
+            res = est.cfg['ref_resolution']
+            crop_bytes = n * res * res * 3
+            f64 = host[:len(host) - crop_bytes].view(np.float64)
+            crops = host[len(host) - crop_bytes:].reshape(K, S, res, res, 3)
+        else:
+            f64 = host.view(np.float64)
+        off = 0
+
+        def take(m):
+            nonlocal off
+            off += m
+            return f64[off - m:off]
+        chain = take(n_chain * n * 12).reshape(n_chain, K, S, 3, 4)
+        smoothed = take(n * 12).reshape(K, S, 3, 4)
+        avg = take(n * 16).reshape(K, S, 8, 2)
+        ring_h = take(n * num * 16).reshape(K, S, num, 8, 2).astype(np.float32)
+        count_h = take(n).reshape(K, S).astype(np.int64)
+        out = {}
+        for o, (name, ob) in enumerate(self.objs._objects.items()):
+            refined = [c.astype(np.float32) for c in chain[1:, o]]
+            first = chain[0, o].astype(np.float32) if (not full and prev_f32) else chain[0, o].copy()
+            inter = {}
+            if full:
+                d = take(S * 4).reshape(S, 4).astype(np.float32)
+                idx = take(S).astype(np.int64)
+                sel_out = take(S * 2).reshape(S, 2).astype(np.float32)
+                logits = take(S * len(ob.ref_info['poses'])).reshape(S, -1).astype(np.float32)
+                inter.update({'det_position': d[:, :2].copy(), 'det_scale_r2q': d[:, 2].copy(), 'det_score': d[:, 3].copy(),
+                              'det_que_img': crops[o].copy(), 'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': logits,
+                              'sel_ref_idx': idx})
+            inter['refine_poses'] = [first] + refined
+            inter['bbox_pts'] = ring_h[o, np.arange(S), count_h[o] - 1].copy()
+            inter['smoothed_pts'] = avg[o].copy()
+            out[name] = (refined[-1] if refined else first), smoothed[o].copy(), inter
+        return out

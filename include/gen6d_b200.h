@@ -122,6 +122,25 @@ int g6d_glue_apply_refinements(const g6d_glue_views* views, const float* que_pos
                                const float* net_out, int qn, double* poses, g6d_stream_t stream);
 int g6d_glue_apply_refinements_host(const g6d_glue_views* views, const float* que_pose, const float* que_K, const float* rect,
                                     const float* net_out, int qn, double* poses);
+/* ---- the same two refinement steps for several objects in one launch each (an object set; gen6d_b200/objects.py).
+ * views [n_obj] (host array, passed to the kernel by value: 1 <= n_obj <= G6D_GLUE_MAX_OBJECTS, every object with the
+ * same ref_num).  Rows are object-major: row i = o*rows_per_obj + s is object o on frame s, reading views[o], cams[s]
+ * and frame s at frames + s*rows*cols*3, and writing row i of every output, i.e. the per-object calls' outputs
+ * concatenated: jobs [n_obj*rows_per_obj*(ref_num+1)], then [n_obj*rows_per_obj, ...].  Every row runs the code of
+ * g6d_glue_refine_problems / g6d_glue_apply_refinements and is bit-identical to that call on the object's slice. */
+#define G6D_GLUE_MAX_OBJECTS 16
+int g6d_glue_refine_problems_objects(const g6d_glue_views* views, int n_obj, int rows_per_obj, const g6d_glue_camera* cams,
+                                     const uint8_t* frames, int rows, int cols, const double* poses, int poses_are_f32,
+                                     g6d_warp_job* jobs, float* que_K, float* que_pose, float* rect, float* ref_Ks, float* ref_poses,
+                                     int* ref_rows, g6d_stream_t stream);
+int g6d_glue_refine_problems_objects_host(const g6d_glue_views* views, int n_obj, int rows_per_obj, const g6d_glue_camera* cams,
+                                          const uint8_t* frames, int rows, int cols, const double* poses, int poses_are_f32,
+                                          g6d_warp_job* jobs, float* que_K, float* que_pose, float* rect, float* ref_Ks,
+                                          float* ref_poses, int* ref_rows);
+int g6d_glue_apply_refinements_objects(const g6d_glue_views* views, int n_obj, int rows_per_obj, const float* que_pose,
+                                       const float* que_K, const float* rect, const float* net_out, double* poses, g6d_stream_t stream);
+int g6d_glue_apply_refinements_objects_host(const g6d_glue_views* views, int n_obj, int rows_per_obj, const float* que_pose,
+                                            const float* que_K, const float* rect, const float* net_out, double* poses);
 /* ---- temporal smoothing of tracked poses (predict.py:18-26,61-70; utils/base_utils.py:256-265 project_points;
  * utils/pose_utils.py:246-279 pnp).  Per sequence s: project the object's bounding box bbox [8,3] (float32) with the raw
  * pose poses[s] [12] (float64 storage; poses_are_f32: float32 values, projected in float32 like numpy does with
@@ -135,6 +154,16 @@ int g6d_track_smooth(const double* poses, int poses_are_f32, const float* bbox, 
                      const double* weights, int S, double* smoothed, double* avg_pts, g6d_stream_t stream);
 int g6d_track_smooth_host(const double* poses, int poses_are_f32, const float* bbox, const double* Ks, float* ring, int* count,
                           int num, const double* weights, int S, double* smoothed, double* avg_pts);
+/* The same smoothing for n_obj objects tracked through rows_per_obj sequences, rows object-major: row i = o*rows_per_obj
+ * + s smooths poses[i] with box bboxes[o] ([n_obj,8,3]) and Ks[s] ([rows_per_obj,9]), into ring[i] ([n_obj*rows_per_obj,
+ * num,8,2]), count[i], smoothed[i] and avg_pts[i].  Each row runs g6d_track_smooth's per-sequence code.  One thread per
+ * row; the *_host variant also rejects a count beyond the ring. */
+int g6d_track_smooth_objects(const double* poses, int poses_are_f32, const float* bboxes, int n_obj, int rows_per_obj, const double* Ks,
+                             float* ring, int* count, int num, const double* weights, double* smoothed, double* avg_pts,
+                             g6d_stream_t stream);
+int g6d_track_smooth_objects_host(const double* poses, int poses_are_f32, const float* bboxes, int n_obj, int rows_per_obj,
+                                  const double* Ks, float* ring, int* count, int num, const double* weights, double* smoothed,
+                                  double* avg_pts);
 /* (x - mean) / std on f32 [n_pixels, in_c] -> [n_pixels, out_c] (in_c, out_c in {3,4})
  * (network/detector.py:189, selector.py:115, refiner.py:65) */
 int g6d_imagenet_norm(const float* in, float* out, long long n_pixels, int in_c, int out_c, g6d_stream_t stream);
