@@ -646,6 +646,47 @@ __global__ void conv_tc_reduce_kernel(const float* __restrict__ ws, const float*
     y[m * ocs + oco + n] = tc_act(v, act);
 }
 
+// The same for Cout % 4 == 0, four columns of one output row per thread: 128-bit partial loads, all `splits` of them
+// issued before the first add, and one divide per four elements.  Each element is summed in the same order (split 0
+// first, then bias), so the output equals conv_tc_reduce_kernel's bit for bit.  vec_out: y + oco and ocs keep 16-byte
+// alignment, so the row is stored as one float4.
+template <int SPLITS>
+__device__ __forceinline__ float4 sum_splits4(const float4* __restrict__ ws4, long long slab4, long long i4, int splits) {
+    float4 p[SPLITS > 0 ? SPLITS : 1];
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if constexpr (SPLITS > 0) {
+#pragma unroll
+        for (int s = 0; s < SPLITS; ++s) p[s] = __ldg(ws4 + s * slab4 + i4);
+#pragma unroll
+        for (int s = 0; s < SPLITS; ++s) { v.x += p[s].x; v.y += p[s].y; v.z += p[s].z; v.w += p[s].w; }
+    } else {
+        for (int s = 0; s < splits; ++s) {
+            const float4 q = __ldg(ws4 + s * slab4 + i4);
+            v.x += q.x; v.y += q.y; v.z += q.z; v.w += q.w;
+        }
+    }
+    return v;
+}
+
+template <int SPLITS>
+__global__ void conv_tc_reduce4_kernel(const float* __restrict__ ws, const float* __restrict__ bias, float* __restrict__ y,
+                                       int M, int Cout, int splits, int ocs, int oco, int act, bool vec_out) {
+    const long long i4 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int c4 = Cout >> 2;
+    if (i4 >= (long long)M * c4) return;
+    const long long m = i4 / c4;
+    const int n = (int)(i4 - m * c4) * 4;
+    float4 v = sum_splits4<SPLITS>(reinterpret_cast<const float4*>(ws), (long long)M * c4, i4, splits);
+    if (bias) { v.x += bias[n]; v.y += bias[n + 1]; v.z += bias[n + 2]; v.w += bias[n + 3]; }
+    v = make_float4(tc_act(v.x, act), tc_act(v.y, act), tc_act(v.z, act), tc_act(v.w, act));
+    float* dst = y + m * ocs + oco + n;
+    if (vec_out) {
+        *reinterpret_cast<float4*>(dst) = v;
+    } else {
+        dst[0] = v.x; dst[1] = v.y; dst[2] = v.z; dst[3] = v.w;
+    }
+}
+
 // The same with the fused InstanceNorm statistics of y: a 256-thread block owns 32 consecutive output
 // rows (one group: stats_rows % 32 == 0) x 64 channels; thread = (channel, 8-row slice); the four slices
 // are combined in shared memory and one (sum, sum^2) pair per (block, channel) goes to the fp64 accumulators.
@@ -687,6 +728,17 @@ static void launch_reduce(const float* ws, const float* bias, float* y, int M, i
     if (stats) {
         dim3 grid(ceil_div(M, 32), ceil_div(Cout, 64));
         conv_tc_reduce_stats_kernel<<<grid, 256, 0, st>>>(ws, bias, y, M, Cout, splits, ocs, oco, act, stats, stats_rows);
+    } else if ((Cout & 3) == 0) {
+        const long long n4 = (long long)M * (Cout / 4);
+        const bool vec_out = (ocs & 3) == 0 && (oco & 3) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0;
+        const unsigned grid = (unsigned)ceil_div(n4, 256);
+        switch (splits) {       // the split counts of the network's layers get their loads unrolled
+            case 2: conv_tc_reduce4_kernel<2><<<grid, 256, 0, st>>>(ws, bias, y, M, Cout, splits, ocs, oco, act, vec_out); break;
+            case 3: conv_tc_reduce4_kernel<3><<<grid, 256, 0, st>>>(ws, bias, y, M, Cout, splits, ocs, oco, act, vec_out); break;
+            case 4: conv_tc_reduce4_kernel<4><<<grid, 256, 0, st>>>(ws, bias, y, M, Cout, splits, ocs, oco, act, vec_out); break;
+            case 8: conv_tc_reduce4_kernel<8><<<grid, 256, 0, st>>>(ws, bias, y, M, Cout, splits, ocs, oco, act, vec_out); break;
+            default: conv_tc_reduce4_kernel<0><<<grid, 256, 0, st>>>(ws, bias, y, M, Cout, splits, ocs, oco, act, vec_out);
+        }
     } else {
         const long long n = (long long)M * Cout;
         conv_tc_reduce_kernel<<<ceil_div(n, 256), 256, 0, st>>>(ws, bias, y, M, Cout, splits, ocs, oco, act);

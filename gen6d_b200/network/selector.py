@@ -186,18 +186,20 @@ class ViewpointSelector(PackedModule):
 
     def _tower(self, level, ref, scale, shift, cat_buf, S, refs):
         """corr_conv_list[level] (selector.py:27-69) on the implicit correlation volume.  Every layer has a
-        prologue; on the 8x8 and 4x4 planes (persistent kernel) prenorm applies it in a split pass over the
-        input, so the A operand arrives by TMA instead of a per-tap gather."""
+        prologue; prenorm applies it in a split pass over the input, so the A operand arrives by TMA instead of a
+        per-tap gather.  The 16x16 level-0 layers, which the A-reuse kernel would take, run on the persistent kernel
+        in that kernel's K order (reuse_im2col), so the result is the same bit for bit."""
         convs = self.packed()['towers'][level]
         x, pro, ps, pb = ref, ops.PRO_CORR, scale, shift
         for i, (pc, post) in enumerate(convs):
             last = i + 1 == len(convs)
             if last:
                 ops.conv(x, pc, prologue=pro, pro_scale=ps, pro_shift=pb, group_rows=S, out=cat_buf, out_coff=256 * level,
-                         prenorm=True)
+                         prenorm=True, reuse_im2col=True)
                 break
             rows = x.shape[0] * x.shape[1] * x.shape[2]                   # stride-1 same-size convolution
-            y, ws = ops.conv(x, pc, prologue=pro, pro_scale=ps, pro_shift=pb, group_rows=S, stats_rows=rows, prenorm=True)
+            y, ws = ops.conv(x, pc, prologue=pro, pro_scale=ps, pro_shift=pb, group_rows=S, stats_rows=rows, prenorm=True,
+                             reuse_im2col=True)
             # InstanceNorm3d statistics over (S, h, w) of the raw conv output; the normalisation
             # itself (and the ReLU) is applied by the next conv's loader.  MaxPool commutes with
             # the positive-slope affine, so pooling the raw tensor first is exact.
@@ -230,11 +232,11 @@ class ViewpointSelector(PackedModule):
                 def step(l=l, st=st, pc=pc, last=last):
                     if last:
                         ops.conv(st['x'], pc, prologue=st['pro'], pro_scale=st['ps'], pro_shift=st['pb'], group_rows=S,
-                                 out=cat_buf, out_coff=256 * l, prenorm=True)
+                                 out=cat_buf, out_coff=256 * l, prenorm=True, reuse_im2col=True)
                         return None
                     rows = st['x'].shape[0] * st['x'].shape[1] * st['x'].shape[2]
                     return ops.conv(st['x'], pc, prologue=st['pro'], pro_scale=st['ps'], pro_shift=st['pb'], group_rows=S,
-                                    stats_rows=rows, prenorm=True) + (rows,)
+                                    stats_rows=rows, prenorm=True, reuse_im2col=True) + (rows,)
                 res = br.run(l, step)
                 st['i'] += 1
                 if res is not None:

@@ -11,7 +11,9 @@ the kernel the planner picked (persist: the persistent kernel, reuse: the A-reus
 BN, the K splits and how a persistent call gets its A operand (im2col: by TMA from a split copy of the input,
 prenorm: the same from a copy with the prologue applied; neither: gathered by the producer warps; a '-ro' suffix
 marks a layer the A-reuse kernel would take, run in its K order by G6D_TC_REUSE_IM2COL).  Times are per step of B
-poses, split pass included.  A total line sums the refiner's volume net and feature branches."""
+poses, split pass included.  Class lines sum the calls of each part of the network (detector correlation, the
+crops' VGG, selector towers, ...; see CLASSES) and list those of its tags that plan the A-reuse kernel or were taken
+from it."""
 import argparse
 import collections
 import os
@@ -43,39 +45,54 @@ def record_step(batch, refine_iter):
     return est, rec
 
 
-REFINER_METHODS = ('_volume_net', '_conv_in_conv')     # the refiner's 3-D stack and its feature branches
+# (class, method name, label): each ops.conv call is labelled by the innermost of these methods it runs under
+CLASSES = (
+    ('Detector', '_detect_maps', 'detector heads'),
+    ('Detector', '_features', 'detector VGG'),
+    ('Detector', '_raw_correlation', 'detector correlation'),
+    ('Detector', '_raw_correlation_objects', 'detector correlation'),
+    ('ViewpointSelector', '_select_one', 'selector 1x1 layers'),
+    ('ViewpointSelector', '_feats', 'selector crop VGG'),
+    ('ViewpointSelector', '_tower', 'selector towers'),
+    ('ViewpointSelector', '_towers_sharded', 'selector towers'),
+    ('VolumeRefiner', '_feature_net', 'refiner crop VGG'),
+    ('VolumeRefiner', '_volume_net', 'refiner volume net + feature branches'),
+    ('VolumeRefiner', '_conv_in_conv', 'refiner volume net + feature branches'),
+)
 
 
 def conv_calls(rec):
-    """(args, kwargs, from the refiner) of every ops.conv call of one eager replay of the recorded stages (the tensors
-    stay alive).  A call is the refiner's when it comes from one of REFINER_METHODS."""
-    from gen6d_b200.network.refiner import VolumeRefiner
-    calls, orig, depth = [], ops.conv, [0]
-    saved = {n: getattr(VolumeRefiner, n) for n in REFINER_METHODS}
+    """(args, kwargs, label) of every ops.conv call of one eager replay of the recorded stages (the tensors stay
+    alive).  The label is that of the innermost method of CLASSES the call runs under ('other' outside them)."""
+    from gen6d_b200.network import detector, refiner, selector
+    owners = {'Detector': detector.Detector, 'ViewpointSelector': selector.ViewpointSelector,
+              'VolumeRefiner': refiner.VolumeRefiner}
+    calls, orig, stack = [], ops.conv, ['other']
+    saved = [(owners[c], n, getattr(owners[c], n), label) for c, n, label in CLASSES]
 
     def wrapped(*a, **k):
-        calls.append((a, k, depth[0] > 0))
+        calls.append((a, k, stack[-1]))
         return orig(*a, **k)
 
-    def marking(f):
+    def marking(f, label):
         def g(*a, **k):
-            depth[0] += 1
+            stack.append(label)
             try:
                 return f(*a, **k)
             finally:
-                depth[0] -= 1
+                stack.pop()
         return g
     ops.conv = wrapped
-    for n, f in saved.items():
-        setattr(VolumeRefiner, n, marking(f))
+    for cls, n, f, label in saved:
+        setattr(cls, n, marking(f, label))
     try:
         with torch.no_grad():
             for fn, inputs in rec:
                 fn(*inputs)
     finally:
         ops.conv = orig
-        for n, f in saved.items():
-            setattr(VolumeRefiner, n, f)
+        for cls, n, f, _ in saved:
+            setattr(cls, n, f)
     torch.cuda.synchronize()
     return calls
 
@@ -105,10 +122,10 @@ def time_call(a, k, reps, repeat):
 
 
 def breakdown(calls, reps=10, repeat=5):
-    """({tag: [calls, ms, flop]} per step, the same summed over the refiner's calls).  Calls with the same tag are
-    timed once (the first of them)."""
-    agg, timed, refiner = collections.OrderedDict(), {}, [0, 0.0, 0.0]
-    for a, k, in_refiner in calls:
+    """({tag: [calls, ms, flop]} per step, {label: {tag: [calls, ms, flop]}}).  Calls with the same tag are timed
+    once (the first of them)."""
+    agg, timed, labels = collections.OrderedDict(), {}, collections.OrderedDict()
+    for a, k, label in calls:
         prof = ops.enable_profiling()
         ops.conv(*a, **k)
         c = ops.collect_profile(prof).get('#calls')
@@ -118,9 +135,9 @@ def breakdown(calls, reps=10, repeat=5):
         if tag not in timed:
             timed[tag] = time_call(a, k, reps, repeat)
         _, work, ms = timed[tag]
-        for e in (agg.setdefault(tag, [0, 0.0, 0.0]),) + ((refiner,) if in_refiner else ()):
+        for e in (agg.setdefault(tag, [0, 0.0, 0.0]), labels.setdefault(label, {}).setdefault(tag, [0, 0.0, 0.0])):
             e[0] += 1; e[1] += ms; e[2] += work
-    return agg, refiner
+    return agg, labels
 
 
 def no_prologue_3x3_persistent(tag):
@@ -134,7 +151,7 @@ def prologue_3x3_persistent(tag):
     return ' k=1x3x3 s=1 pro=' in f' {tag} ' and ' pro=0 ' not in f' {tag} ' and ' persist ' in f' {tag} '
 
 
-def report(agg, refiner, top=40):
+def report(agg, labels, top=40):
     tot_ms, tot_w = sum(a[1] for a in agg.values()), sum(a[2] for a in agg.values())
     print(f'conv_tc calls {sum(a[0] for a in agg.values())} total {tot_ms:.2f} ms, {tot_w / tot_ms / 1e9:.1f} TFLOP/s')
     classes = collections.OrderedDict()
@@ -149,10 +166,12 @@ def report(agg, refiner, top=40):
         if sel:
             ms, w = sum(a[1] for a in sel), sum(a[2] for a in sel)
             print(f'  {ms:7.3f} ms x{sum(a[0] for a in sel):3d} {w / ms / 1e9:6.1f} TF/s  [{what}]')
-    n, ms, w = refiner
-    if n:
-        print(f'  {ms:7.3f} ms x{n:3d} {w / ms / 1e9:6.1f} TF/s  [refiner volume net + feature branches, '
-              f'{100 * ms / tot_ms:.1f} % of the total]')
+    for label, tags in labels.items():
+        n, ms, w = (sum(a[i] for a in tags.values()) for i in range(3))
+        print(f'  {ms:7.3f} ms x{n:3d} {w / ms / 1e9:6.1f} TF/s  [{label}, {100 * ms / tot_ms:.1f} % of the total]')
+        for tag, (n, ms, w) in sorted(tags.items(), key=lambda kv: -kv[1][1]):
+            if ' reuse ' in f' {tag} ' or tag.endswith('-ro'):
+                print(f'      {ms:7.3f} ms x{n:3d} {w / ms / 1e9:6.1f} TF/s  {tag}')
     for tag, (n, ms, w) in sorted(agg.items(), key=lambda kv: -kv[1][1])[:top]:
         print(f'{ms:7.3f} ms x{n:3d} {w / ms / 1e9:6.1f} TF/s  {tag}')
 
