@@ -66,6 +66,10 @@ _SIGNATURES = {
     'g6d_glue_refine_problems_objects_host': [C.POINTER(GlueViews), I, I, P, P, I, I, P, I, P, P, P, P, P, P, P],
     'g6d_glue_apply_refinements_objects': [C.POINTER(GlueViews), I, I, P, P, P, P, P, P],
     'g6d_glue_apply_refinements_objects_host': [C.POINTER(GlueViews), I, I, P, P, P, P, P],
+    'g6d_glue_refine_problems_rows': [C.POINTER(GlueViews), I, I, P, P, I, I, P, P, I, P, P, P, P, P, P, P, P, P],
+    'g6d_glue_refine_problems_rows_host': [C.POINTER(GlueViews), I, I, P, P, I, I, P, P, I, P, P, P, P, P, P, P, P],
+    'g6d_glue_apply_refinements_rows': [C.POINTER(GlueViews), I, I, P, P, P, P, P, I, P, P],
+    'g6d_glue_apply_refinements_rows_host': [C.POINTER(GlueViews), I, I, P, P, P, P, P, I, P],
     'g6d_track_smooth': [P, I, P, P, P, P, I, P, I, P, P, P],
     'g6d_track_smooth_host': [P, I, P, P, P, P, I, P, I, P, P],
     'g6d_track_smooth_objects': [P, I, P, I, I, P, P, P, I, P, P, P, P],

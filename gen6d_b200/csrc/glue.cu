@@ -6,6 +6,8 @@
 #include "common.cuh"
 #include "glue_math.cuh"
 
+#include <vector>
+
 namespace g6d {
 using namespace glue;
 
@@ -137,12 +139,18 @@ struct GlueViewsPack {                 // by value: one kernel parameter block f
 };
 static_assert(sizeof(GlueViewsPack) + 256 <= 4096, "the objects' view structs must fit the 4 KB kernel parameter space");
 
+// the frame part of input row `row` (frame s), written to output row j
+G6D_HD void do_refine_frame_row(int j, int row, int s, const g6d_glue_views& v, const g6d_glue_camera* cams, const uint8_t* frames,
+                                int rows, int cols, const double* poses, int in_f32, g6d_warp_job* jobs, float* que_K,
+                                float* que_pose, float* rect, FrameProblem& fp, int* chosen) {
+    do_refine_frame(0, v, cams + s, poses + (long long)row * 12, in_f32, fp, chosen);
+    store_frame(0, v, fp, frames + (long long)s * rows * cols * 3, rows, cols, jobs + (long long)j * (v.ref_num + 1), que_K + (long long)j * 9,
+                que_pose + (long long)j * 12, rect + (long long)j * 12);
+}
 G6D_HD void do_refine_frame_objects(int i, int s, const g6d_glue_views& v, const g6d_glue_camera* cams, const uint8_t* frames,
                                     int rows, int cols, const double* poses, int in_f32, g6d_warp_job* jobs, float* que_K,
                                     float* que_pose, float* rect, FrameProblem& fp, int* chosen) {
-    do_refine_frame(0, v, cams + s, poses + (long long)i * 12, in_f32, fp, chosen);
-    store_frame(0, v, fp, frames + (long long)s * rows * cols * 3, rows, cols, jobs + (long long)i * (v.ref_num + 1), que_K + (long long)i * 9,
-                que_pose + (long long)i * 12, rect + (long long)i * 12);
+    do_refine_frame_row(i, i, s, v, cams, frames, rows, cols, poses, in_f32, jobs, que_K, que_pose, rect, fp, chosen);
 }
 
 __global__ void __launch_bounds__(32) glue_refine_problems_objects_kernel(const GlueViewsPack pk, int rows_per_obj,
@@ -166,6 +174,47 @@ __global__ void glue_apply_objects_kernel(const GlueViewsPack pk, int rows_per_o
                                           const float* rect, const float* net_out, int qn, double* poses) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < qn) do_apply(i, pk.v[i / rows_per_obj], que_pose, que_K, rect, net_out, poses);
+}
+
+// ------------------------------------------------------------------------------------------ a subset of the rows
+// Output row j is input row row_idx[j] (object-major numbering as above): the problem is built from poses[row_idx[j]] with
+// that row's own dtype flag row_f32[row_idx[j]], and the update of output row j goes back to poses[row_idx[j]].  Rows that
+// are not listed are neither read nor written, so a tracker refines exactly the rows whose chain is still running.
+G6D_HD void do_refine_frame_rows(int j, const GlueViewsPack& pk, int rows_per_obj, const int* row_idx, const uint8_t* row_f32,
+                                 const g6d_glue_camera* cams, const uint8_t* frames, int rows, int cols, const double* poses,
+                                 g6d_warp_job* jobs, float* que_K, float* que_pose, float* rect, FrameProblem& fp, int* chosen) {
+    const int row = row_idx[j];
+    do_refine_frame_row(j, row, row % rows_per_obj, pk.v[row / rows_per_obj], cams, frames, rows, cols, poses, row_f32[row], jobs, que_K,
+                        que_pose, rect, fp, chosen);
+}
+G6D_HD void do_apply_rows(int j, const GlueViewsPack& pk, int rows_per_obj, const int* row_idx, const float* que_pose, const float* que_K,
+                          const float* rect, const float* net_out, double* poses) {
+    const int row = row_idx[j];
+    do_apply(0, pk.v[row / rows_per_obj], que_pose + (long long)j * 12, que_K + (long long)j * 9, rect + (long long)j * 12,
+             net_out + (long long)j * 7, poses + (long long)row * 12);
+}
+
+__global__ void __launch_bounds__(32) glue_refine_problems_rows_kernel(const GlueViewsPack pk, int rows_per_obj, const g6d_glue_camera* cams,
+                                                                       const uint8_t* frames, int rows, int cols, const double* poses,
+                                                                       const int* row_idx, const uint8_t* row_f32, g6d_warp_job* jobs,
+                                                                       float* que_K, float* que_pose, float* rect, float* ref_Ks,
+                                                                       float* ref_poses, int* ref_rows) {
+    __shared__ double s_Rq[9];
+    __shared__ int s_rows[kGlueMaxViews];
+    const int j = blockIdx.x;
+    const g6d_glue_views& v = pk.v[row_idx[j] / rows_per_obj];
+    if (threadIdx.x == 0) {
+        FrameProblem fp;
+        do_refine_frame_rows(j, pk, rows_per_obj, row_idx, row_f32, cams, frames, rows, cols, poses, jobs, que_K, que_pose, rect, fp, s_rows);
+        for (int e = 0; e < 9; ++e) s_Rq[e] = fp.Rq[e];
+    }
+    __syncthreads();
+    if ((int)threadIdx.x < v.ref_num) do_refine_view(j, threadIdx.x, s_rows[threadIdx.x], v, s_Rq, jobs, ref_Ks, ref_poses, ref_rows);
+}
+__global__ void glue_apply_rows_kernel(const GlueViewsPack pk, int rows_per_obj, const float* que_pose, const float* que_K,
+                                       const float* rect, const float* net_out, const int* row_idx, int n_sel, double* poses) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < n_sel) do_apply_rows(j, pk, rows_per_obj, row_idx, que_pose, que_K, rect, net_out, poses);
 }
 
 // host checks shared by the device and host entry points; also fills the parameter block
@@ -316,5 +365,85 @@ extern "C" int g6d_glue_apply_refinements_objects_host(const g6d_glue_views* vie
     if (rc != G6D_OK) return rc;
     G6D_REQUIRE(que_pose && que_K && rect && net_out && poses, "%s: bad args", name);
     for (int i = 0; i < n_obj * rows_per_obj; ++i) do_apply(i, pk.v[i / rows_per_obj], que_pose, que_K, rect, net_out, poses);
+    return G6D_OK;
+}
+
+// check_idx (host twins): every index in range and, for the updates (unique), no row listed twice
+static int rows_ok(const char* name, int n_obj, int rows_per_obj, const int* row_idx, int n_sel, bool check_idx, bool unique) {
+    G6D_REQUIRE(row_idx && n_sel >= 1, "%s: need a row list and n_sel >= 1 (got n_sel=%d)", name, n_sel);
+    if (check_idx) {
+        const long long n = (long long)n_obj * rows_per_obj;
+        std::vector<unsigned char> seen(unique ? n : 0, 0);
+        for (int j = 0; j < n_sel; ++j) {
+            G6D_REQUIRE(row_idx[j] >= 0 && row_idx[j] < n, "%s: row_idx[%d] = %d is outside [0, %lld)", name, j, row_idx[j], n);
+            if (unique) {
+                G6D_REQUIRE(!seen[row_idx[j]], "%s: row %d is listed twice (each row takes one update)", name, row_idx[j]);
+                seen[row_idx[j]] = 1;
+            }
+        }
+    }
+    return G6D_OK;
+}
+
+extern "C" int g6d_glue_refine_problems_rows(const g6d_glue_views* views, int n_obj, int rows_per_obj, const g6d_glue_camera* cams,
+                                             const uint8_t* frames, int rows, int cols, const double* poses, const int* row_idx, int n_sel,
+                                             const uint8_t* row_f32, g6d_warp_job* jobs, float* que_K, float* que_pose, float* rect,
+                                             float* ref_Ks, float* ref_poses, int* ref_rows, g6d_stream_t stream) {
+    const char* name = "g6d_glue_refine_problems_rows";
+    GlueViewsPack pk;
+    int rc = objects_ok(name, views, n_obj, rows_per_obj, true, &pk);
+    if (rc == G6D_OK) rc = rows_ok(name, n_obj, rows_per_obj, row_idx, n_sel, false, false);
+    if (rc != G6D_OK) return rc;
+    G6D_REQUIRE(cams && frames && poses && row_f32 && jobs && que_K && que_pose && rect && ref_Ks && ref_poses && ref_rows && rows > 0 &&
+                    cols > 0, "%s: bad args", name);
+    glue_refine_problems_rows_kernel<<<n_sel, 32, 0, as_stream(stream)>>>(pk, rows_per_obj, cams, frames, rows, cols, poses, row_idx, row_f32,
+                                                                          jobs, que_K, que_pose, rect, ref_Ks, ref_poses, ref_rows);
+    G6D_CHECK_LAUNCH(name);
+    return G6D_OK;
+}
+extern "C" int g6d_glue_refine_problems_rows_host(const g6d_glue_views* views, int n_obj, int rows_per_obj, const g6d_glue_camera* cams,
+                                                  const uint8_t* frames, int rows, int cols, const double* poses, const int* row_idx,
+                                                  int n_sel, const uint8_t* row_f32, g6d_warp_job* jobs, float* que_K, float* que_pose,
+                                                  float* rect, float* ref_Ks, float* ref_poses, int* ref_rows) {
+    const char* name = "g6d_glue_refine_problems_rows_host";
+    GlueViewsPack pk;
+    int rc = objects_ok(name, views, n_obj, rows_per_obj, true, &pk);
+    if (rc == G6D_OK) rc = rows_ok(name, n_obj, rows_per_obj, row_idx, n_sel, true, false);
+    if (rc != G6D_OK) return rc;
+    G6D_REQUIRE(cams && poses && row_f32 && jobs && que_K && que_pose && rect && ref_Ks && ref_poses && ref_rows, "%s: bad args", name);
+    for (int j = 0; j < n_sel; ++j) {
+        const g6d_glue_views& v = pk.v[row_idx[j] / rows_per_obj];
+        FrameProblem fp;
+        int chosen[kGlueMaxViews];
+        do_refine_frame_rows(j, pk, rows_per_obj, row_idx, row_f32, cams, frames, rows, cols, poses, jobs, que_K, que_pose, rect, fp, chosen);
+        for (int r = 0; r < v.ref_num; ++r) do_refine_view(j, r, chosen[r], v, fp.Rq, jobs, ref_Ks, ref_poses, ref_rows);
+    }
+    return G6D_OK;
+}
+
+extern "C" int g6d_glue_apply_refinements_rows(const g6d_glue_views* views, int n_obj, int rows_per_obj, const float* que_pose,
+                                               const float* que_K, const float* rect, const float* net_out, const int* row_idx, int n_sel,
+                                               double* poses, g6d_stream_t stream) {
+    const char* name = "g6d_glue_apply_refinements_rows";
+    GlueViewsPack pk;
+    int rc = objects_ok(name, views, n_obj, rows_per_obj, false, &pk);
+    if (rc == G6D_OK) rc = rows_ok(name, n_obj, rows_per_obj, row_idx, n_sel, false, false);
+    if (rc != G6D_OK) return rc;
+    G6D_REQUIRE(que_pose && que_K && rect && net_out && poses, "%s: bad args", name);
+    glue_apply_rows_kernel<<<ceil_div(n_sel, 32), 32, 0, as_stream(stream)>>>(pk, rows_per_obj, que_pose, que_K, rect, net_out, row_idx,
+                                                                              n_sel, poses);
+    G6D_CHECK_LAUNCH(name);
+    return G6D_OK;
+}
+extern "C" int g6d_glue_apply_refinements_rows_host(const g6d_glue_views* views, int n_obj, int rows_per_obj, const float* que_pose,
+                                                    const float* que_K, const float* rect, const float* net_out, const int* row_idx,
+                                                    int n_sel, double* poses) {
+    const char* name = "g6d_glue_apply_refinements_rows_host";
+    GlueViewsPack pk;
+    int rc = objects_ok(name, views, n_obj, rows_per_obj, false, &pk);
+    if (rc == G6D_OK) rc = rows_ok(name, n_obj, rows_per_obj, row_idx, n_sel, true, true);
+    if (rc != G6D_OK) return rc;
+    G6D_REQUIRE(que_pose && que_K && rect && net_out && poses, "%s: bad args", name);
+    for (int j = 0; j < n_sel; ++j) do_apply_rows(j, pk, rows_per_obj, row_idx, que_pose, que_K, rect, net_out, poses);
     return G6D_OK;
 }

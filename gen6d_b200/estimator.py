@@ -207,15 +207,26 @@ class Gen6DEstimator:
                 'views': glue.views_struct(ptr(views_dev), tables, views_dev['src'].data_ptr(), views_dev['rows'].data_ptr(),
                                            views_dev['cols'].data_ptr())}
 
-    def _predict_device_fn(self, st):
-        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> every stage of predict_batch, enqueued back to back."""
-        res, iters, R = self.cfg['ref_resolution'], self.cfg['refine_iter'], st['tables']['ref_num']
-        select, refine = self.selector._select_warped(res), self.refiner._refine_warped(128)
+    def _initial_poses_device_fn(self, st):
+        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> detection, selection and the initial poses float64 [qn,12]:
+        (poses, det, crop, idx, sel_out, logits), enqueued back to back."""
+        res = self.cfg['ref_resolution']
+        select = self.selector._select_warped(res)
 
         def fn(frames, cams):
             det = self.detector._detect_u8(frames)                                  # [qn,4]: x, y, scale, score
             crop, idx, sel_out, logits = select(ops.glue_detection_jobs(det, frames, res))
             poses = ops.glue_initial_poses(det, idx, sel_out, st['refs'], cams)
+            return poses, det, crop, idx, sel_out, logits
+        return fn
+
+    def _predict_device_fn(self, st):
+        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> every stage of predict_batch, enqueued back to back."""
+        iters, R = self.cfg['refine_iter'], st['tables']['ref_num']
+        initial, refine = self._initial_poses_device_fn(st), self.refiner._refine_warped(128)
+
+        def fn(frames, cams):
+            poses, det, crop, idx, sel_out, logits = initial(frames, cams)
             chain = [poses]
             for it in range(iters):
                 jobs, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems(st['views'], R, cams, frames, poses, it > 0)

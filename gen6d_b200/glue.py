@@ -182,3 +182,47 @@ def host_apply_refinements_objects(tables_list, prob, net_out):
                                                                   net.ctypes.data, poses.ctypes.data),
                'g6d_glue_apply_refinements_objects_host')
     return poses
+
+
+def host_refine_problems_rows(tables_list, cams, poses, row_idx, row_f32, rows, cols, frame_ptr=0, sources=None):
+    """g6d_glue_refine_problems_rows_host: poses [K*qn,3,4] object-major as host_refine_problems_objects takes them, row_idx
+    [n_sel] the listed rows, row_f32 [K*qn] each row's dtype flag -> the outputs of host_refine_problems for the n_sel
+    listed rows, output row j being row row_idx[j]."""
+    K, qn = len(tables_list), len(cams)
+    R = tables_list[0]['ref_num']
+    if sources is None:
+        sources = [(None, None, None)] * K
+    keep = []
+    for t, (src, img_rows, img_cols) in zip(tables_list, sources):
+        nv = len(t['ids'])
+        keep.append((np.zeros(nv, np.uint64) if src is None else np.ascontiguousarray(src, np.uint64),
+                     np.zeros(nv, np.int32) if img_rows is None else np.ascontiguousarray(img_rows, np.int32),
+                     np.zeros(nv, np.int32) if img_cols is None else np.ascontiguousarray(img_cols, np.int32)))
+    views = _views_array([views_struct(t, t, *k) for t, k in zip(tables_list, keep)])
+    cams, poses = np.ascontiguousarray(cams, np.float64), np.ascontiguousarray(poses, np.float64)
+    idx, flags = np.ascontiguousarray(row_idx, np.int32), np.ascontiguousarray(row_f32, np.uint8)
+    n = len(idx)
+    out = {'jobs': np.zeros(n * (R + 1), JOB), 'que_K': np.zeros((n, 3, 3), np.float32), 'que_pose': np.zeros((n, 3, 4), np.float32),
+           'pose_rect': np.zeros((n, 3, 4), np.float32), 'ref_Ks': np.zeros((n, R, 3, 3), np.float32),
+           'ref_poses': np.zeros((n, R, 3, 4), np.float32), 'ref_rows': np.zeros((n, R), np.int32)}
+    _lib.check(_lib.lib().g6d_glue_refine_problems_rows_host(views, K, qn, cams.ctypes.data, frame_ptr, rows, cols, poses.ctypes.data,
+                                                             idx.ctypes.data, n, flags.ctypes.data,
+                                                             *[out[k].ctypes.data for k in ('jobs', 'que_K', 'que_pose', 'pose_rect',
+                                                                                            'ref_Ks', 'ref_poses', 'ref_rows')]),
+               'g6d_glue_refine_problems_rows_host')
+    return out
+
+
+def host_apply_refinements_rows(tables_list, prob, net_out, row_idx, poses):
+    """g6d_glue_apply_refinements_rows_host: the n_sel problems of host_refine_problems_rows and network outputs [n_sel,7]
+    update rows row_idx of poses (float64 [K*qn,3,4], contiguous, in place).  Returns poses."""
+    K = len(tables_list)
+    views = _views_array([views_struct(t, t) for t in tables_list])
+    net, idx = np.ascontiguousarray(net_out, np.float32), np.ascontiguousarray(row_idx, np.int32)
+    if poses.dtype != np.float64 or not poses.flags.c_contiguous or len(poses) % K:
+        raise ValueError('host_apply_refinements_rows: poses must be a contiguous float64 array of K*qn rows (updated in place)')
+    _lib.check(_lib.lib().g6d_glue_apply_refinements_rows_host(views, K, len(poses) // K, prob['que_pose'].ctypes.data,
+                                                               prob['que_K'].ctypes.data, prob['pose_rect'].ctypes.data, net.ctypes.data,
+                                                               idx.ctypes.data, len(idx), poses.ctypes.data),
+               'g6d_glue_apply_refinements_rows_host')
+    return poses

@@ -125,16 +125,13 @@ class ObjectSet:
         out, _ = ops.det_parse(o['score_predict'], o['scale_predict'], o['offset_predict'], det.pool_ratio)
         return out, o
 
-    def _predict_device_fn(self):
-        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> every stage, back to back, as device tensors: (chain f64
-        [refine_iter+1, K*qn, 12] of object-major poses, det [K*qn,4], [(sel_idx, sel_out, logits)] per object, crops u8
-        [K*qn, res, res, 3])."""
+    def _initial_poses_device_fn(self):
+        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> the shared detection, each object's selection and the initial poses:
+        (poses f64 [K*qn,12] object-major, det [K*qn,4], [(sel_idx, sel_out, logits)] per object, crops u8 [K*qn,res,res,3])."""
         est = self.est
         objs = list(self._objects.values())
-        K, res, iters = len(objs), est.cfg['ref_resolution'], est.cfg['refine_iter']
-        R = objs[0].tables['tables']['ref_num']
-        views = [ob.tables['views'] for ob in objs]
-        sel, refine = est.selector, est.refiner._refine_warped(128)
+        K, res = len(objs), est.cfg['ref_resolution']
+        sel = est.selector
 
         def fn(frames, cams):
             qn = frames.shape[0]
@@ -155,7 +152,21 @@ class ObjectSet:
                 idx, sel_out = ops.sel_parse(logits, torch.stack(ang, 0))
                 sels.append((idx, sel_out, logits))
                 poses.append(ops.glue_initial_poses(rows(det, o), idx, sel_out, ob.tables['refs'], cams))
-            poses = cat(poses)                                                       # [K*qn,12], object-major
+            return cat(poses), det, sels, crop                                       # poses [K*qn,12], object-major
+        return fn
+
+    def _predict_device_fn(self):
+        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> every stage, back to back, as device tensors: (chain f64
+        [refine_iter+1, K*qn, 12] of object-major poses, det [K*qn,4], [(sel_idx, sel_out, logits)] per object, crops u8
+        [K*qn, res, res, 3])."""
+        est = self.est
+        objs = list(self._objects.values())
+        iters, R = est.cfg['refine_iter'], objs[0].tables['tables']['ref_num']
+        views = [ob.tables['views'] for ob in objs]
+        initial, refine = self._initial_poses_device_fn(), est.refiner._refine_warped(128)
+
+        def fn(frames, cams):
+            poses, det, sels, crop = initial(frames, cams)
             chain = [poses]
             for it in range(iters):
                 jobs_r, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems_objects(views, R, cams, frames, poses,

@@ -192,6 +192,60 @@ def glue_apply_refinements_objects(views_structs, que_pose, que_K, rect, net_out
     return poses
 
 
+def _row_chunks(views_structs, rows_per_obj, row_idx):
+    """(o0, o1, list slice, row indices relative to object o0) per G6D_GLUE_MAX_OBJECTS objects: the list is object-major
+    with the same number of entries per object, so it splits at static offsets."""
+    K, n_sel = len(views_structs), row_idx.shape[0]
+    if n_sel < 1 or n_sel % K:
+        raise ValueError(f'glue rows: {n_sel} listed rows for {K} objects; every object lists the same number of rows')
+    per = n_sel // K
+    out = []
+    for o0, o1 in _object_chunks(K):
+        r = slice(o0 * per, o1 * per)
+        idx = row_idx[r] if o0 == 0 else (row_idx[r] - o0 * rows_per_obj).contiguous()
+        out.append((o0, o1, r, idx))
+    return out
+
+
+def glue_refine_problems_rows(views_structs, ref_num, rows_per_obj, cams, frames, poses, row_idx, row_f32):
+    """glue_refine_problems_objects on the listed rows only: poses float64 [K*rows_per_obj,12] (object-major, row o*rows_per_obj
+    + s is object o on frame s), row_idx int32 [n_sel] (object-major, the same count per object), row_f32 uint8
+    [K*rows_per_obj] (each row's dtype flag) -> the problems of the listed rows, output row j being row row_idx[j]."""
+    qn, h, w, _ = frames.shape
+    K, n_sel = len(views_structs), row_idx.shape[0]
+    n = K * rows_per_obj
+    if poses.shape != (n, 12) or row_f32.shape != (n,) or qn != rows_per_obj or cams.shape[0] != rows_per_obj:
+        raise ValueError(f'glue_refine_problems_rows: poses {tuple(poses.shape)}, row_f32 {tuple(row_f32.shape)}, frames {qn}, '
+                         f'cams {cams.shape[0]} for {K} objects x {rows_per_obj} rows')
+    dev, f32 = frames.device, torch.float32
+    jobs = torch.empty(n_sel, (ref_num + 1) * WARP_JOB_BYTES, device=dev, dtype=torch.uint8)
+    que_K, que_pose, rect = torch.empty(n_sel, 3, 3, device=dev, dtype=f32), torch.empty(n_sel, 3, 4, device=dev, dtype=f32), \
+        torch.empty(n_sel, 3, 4, device=dev, dtype=f32)
+    ref_Ks, ref_poses = torch.empty(n_sel, ref_num, 3, 3, device=dev, dtype=f32), torch.empty(n_sel, ref_num, 3, 4, device=dev, dtype=f32)
+    rows = torch.empty(n_sel, ref_num, device=dev, dtype=torch.int32)
+    for o0, o1, r, idx in _row_chunks(views_structs, rows_per_obj, row_idx):
+        p = slice(o0 * rows_per_obj, o1 * rows_per_obj)
+        _call('g6d_glue_refine_problems_rows', _views_array(views_structs, o0, o1), o1 - o0, rows_per_obj, _p(cams, torch.float64),
+              _p(frames, torch.uint8), h, w, _p(poses[p], torch.float64), _p(idx, torch.int32), idx.shape[0], _p(row_f32[p], torch.uint8),
+              _p(jobs[r], torch.uint8), _p(que_K[r]), _p(que_pose[r]), _p(rect[r]), _p(ref_Ks[r]), _p(ref_poses[r]),
+              _p(rows[r], torch.int32), _stream())
+    return jobs.reshape(-1), que_K, que_pose, rect, ref_Ks, ref_poses, rows
+
+
+def glue_apply_refinements_rows(views_structs, rows_per_obj, que_pose, que_K, rect, net_out, row_idx, poses):
+    """glue_apply_refinements_objects for the rows of glue_refine_problems_rows: network output row j updates
+    poses[row_idx[j]] (float64 [K*rows_per_obj,12]) in place; the other rows are untouched.  Returns poses."""
+    K = len(views_structs)
+    if poses.shape != (K * rows_per_obj, 12) or net_out.shape[0] != row_idx.shape[0]:
+        raise ValueError(f'glue_apply_refinements_rows: poses {tuple(poses.shape)}, {net_out.shape[0]} outputs for {row_idx.shape[0]} '
+                         f'rows, {K} objects x {rows_per_obj} rows')
+    for o0, o1, r, idx in _row_chunks(views_structs, rows_per_obj, row_idx):
+        p = slice(o0 * rows_per_obj, o1 * rows_per_obj)
+        _call('g6d_glue_apply_refinements_rows', _views_array(views_structs, o0, o1), o1 - o0, rows_per_obj, _p(que_pose[r]), _p(que_K[r]),
+              _p(rect[r]), _p(net_out[r]), _p(idx, torch.int32), idx.shape[0], _p(poses[p], torch.float64), _stream())
+    return poses
+
+
 def track_smooth_objects(poses, poses_are_f32, bboxes, Ks, ring, count, weights):
     """track_smooth for K objects through S sequences in one launch, rows object-major: poses float64 [K*S,12] (row o*S + s
     is object o on sequence s), bboxes float32 [K,8,3], Ks float64 [S,9], ring float32 [K*S,num,8,2] and count int32 [K*S]

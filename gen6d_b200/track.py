@@ -10,6 +10,9 @@ with predict_batch's host path and runs the smoothing through g6d_track_smooth_h
 
 ObjectTracker (ObjectSet.tracker()) does the same for every object of an object set at once: one graph per step whose
 glue and smoothing launches (the g6d_*_objects entry points) and refiner stage cover all K objects' K*S rows.
+
+reset(sequences) / start(poses, sequences) re-initialise or restart single sequences while the others keep tracking;
+the step after them is the mixed step below, also one graph and one read.
 """
 import numpy as np
 import torch
@@ -105,6 +108,98 @@ def host_smooth_objects(poses, poses_are_f32, bboxes, Ks, ring, count, weights):
     return smoothed.reshape(n, 3, 4), avg
 
 
+# ------------------------------------------------------------------------------------------ the mixed step
+# A step in which some sequences are re-initialised (a full prediction) and the others refine from their previous pose,
+# or in which the rows' previous poses have different dtypes.  It is one captured graph: the re-initialised sequences'
+# frames are gathered and run through detection, selection and the initial poses as a batch padded to a power of two
+# (the bucket b, capped at S: the padding repeats a re-initialised sequence), the initial poses are scattered into a
+# working array [K*(S+b),12] that holds the other rows' previous poses (per object S real rows, then b scratch rows), and
+# max(cfg['refine_iter'], refine_iter) iterations refine the rows whose chain is still running, in ascending row order,
+# through the row-indexed glue and ONE refiner stage per iteration.  Every shape depends on the bucket only, so every
+# subset of a bucket replays one graph: an iteration in which every real row refines lists exactly the S real rows (the
+# refiner stage of a plain refine step), and a shorter list is padded with scratch rows to a length fixed by the bucket;
+# scratch rows hold copies of the bucket's initial poses and their results are dropped.
+def _bucket(m, S):
+    return 0 if m == 0 else min(S, 1 << (m - 1).bit_length())
+
+
+def _iter_lengths(S, b, F, r):
+    """Rows per object of each refinement iteration (F: the re-initialised rows' chain length, r: the others')."""
+    return [S if (it < F and it < r) or it >= F else b for it in range(max(F, r))]
+
+
+def _mixed_inputs(S, K, pending, f32, F, r, device):
+    """Host side of a mixed step -> (re-initialised sequences [m], bucket, graph inputs: gathered sequences int64 [b], scatter
+    rows int64 [K*b], first-iteration dtype flags uint8 [K*(S+b)], the iterations' row lists int32, object-major)."""
+    reinit, others = np.flatnonzero(pending), np.flatnonzero(~pending)
+    m = len(reinit)
+    b = _bucket(m, S)
+    n = S + b
+    seq = np.concatenate([reinit, np.full(b - m, reinit[-1] if m else 0)])
+    tgt = np.concatenate([reinit, S + np.arange(m, b)])
+    flags = np.zeros(n, np.uint8)
+    flags[others] = f32[others]
+    lists = []
+    for it, L in enumerate(_iter_lengths(S, b, F, r)):
+        if it < F and it < r:
+            rows = np.arange(S)
+        elif it < F:
+            rows = np.concatenate([reinit, S + np.arange(b - m)])        # re-initialised rows only, padded to b
+        else:
+            rows = np.concatenate([others, S + np.arange(m)])            # the other rows only, padded to S
+        assert len(rows) == L
+        lists += [o * n + rows for o in range(K)]
+    up = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dt)).to(device)
+    tgt_k = np.concatenate([o * n + tgt for o in range(K)])
+    inputs = [up(seq, np.int64), up(tgt_k, np.int64), up(np.tile(flags, K), np.uint8),
+              up(np.concatenate(lists) if lists else np.zeros(0), np.int32)]
+    return reinit, b, inputs
+
+
+def _mixed_fn(K, S, b, F, r, initial, views, R, refine, smooth):
+    """The mixed step's graph body.  initial(frames, cams) -> (poses [K*b,12], crops, [tensors packed after the smoothing]);
+    smooth(poses [K*S,12], Ks [S,9], ring, count) -> (smoothed, averaged corners)."""
+    n, lens = S + b, _iter_lengths(S, b, F, r)
+
+    def fn(frames, cams, prev, ring, count, seq, tgt, flags0, lists):
+        if b:
+            gf, gc = frames.index_select(0, seq), cams.index_select(0, seq)
+            init, crop, extras = initial(gf, gc)
+            frames_x, cams_x = torch.cat([frames, gf], 0), torch.cat([cams, gc], 0)
+            work = torch.cat([prev.view(K, S, 12), init.view(K, b, 12)], 1).reshape(K * n, 12)
+            work.index_copy_(0, tgt, init)
+        else:
+            frames_x, cams_x, work, extras = frames, cams, prev.clone(), []
+        real = lambda: work.view(K, n, 12)[:, :S].reshape(K * S, 12).clone()
+        ones = torch.ones_like(flags0)
+        chain, off = [real()], 0
+        for it, L in enumerate(lens):
+            if L:
+                idx = lists[off:off + K * L]
+                off += K * L
+                jobs, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems_rows(views, R, n, cams_x, frames_x, work, idx,
+                                                                                                  flags0 if it == 0 else ones)
+                out = refine(jobs, que_K, que_pose, ref_Ks, ref_poses)            # one refiner stage over the listed rows
+                ops.glue_apply_refinements_rows(views, n, que_pose, que_K, rect, out, idx, work)
+            chain.append(real())
+        poses = chain[-1]
+        smoothed, avg = smooth(poses, cams[:, :9].contiguous(), ring, count)
+        packed = torch.cat([t.reshape(-1).to(torch.float64) for t in [torch.stack(chain, 0), smoothed, avg, ring, count] + extras])
+        return (torch.cat([packed.view(torch.uint8), crop.reshape(-1)]) if b else packed.view(torch.uint8)), poses, ring, count
+    return fn
+
+
+def _sequences(S, sequences):
+    """Validated sequence indices, in the caller's order (start() pairs poses[i] with sequences[i])."""
+    seqs = [int(s) for s in sequences]
+    if len(set(seqs)) != len(seqs):
+        raise ValueError(f'sequences {seqs} lists a sequence twice')
+    bad = [s for s in seqs if not 0 <= s < S]
+    if bad:
+        raise ValueError(f'sequences {bad} are outside [0, {S})')
+    return np.asarray(seqs, np.int64)
+
+
 # ------------------------------------------------------------------------------------------ the tracker
 class Tracker:
     """S sequences tracked in lockstep (one frame each per step); see Gen6DEstimator.tracker()."""
@@ -135,21 +230,53 @@ class Tracker:
         self.reset()
 
     # -------------------------------------------------------------- state
-    def reset(self):
+    def reset(self, sequences=None):
         """The next step is a full prediction (detect -> select -> cfg['refine_iter'] refinements) for every sequence,
-        and the smoothing histories restart."""
-        self._prev, self._prev_f32 = None, True
-        self._ring = np.zeros((self.S, self.num, 8, 2), np.float32)
-        self._count = np.zeros(self.S, np.int32)
+        and the smoothing histories restart.  sequences: only those sequences are re-initialised at the next step and
+        restart their histories; the others keep tracking (that step is the mixed step)."""
+        if sequences is None:
+            self._prev = None                        # float64 previous poses ([S,12] on the device, [S,3,4] on the host)
+            self._pending = np.ones(self.S, bool)    # a full prediction at the next step
+            self._f32 = np.ones(self.S, bool)        # each row's previous pose holds float32 values
+            self._ring = np.zeros((self.S, self.num, 8, 2), np.float32)
+            self._count = np.zeros(self.S, np.int32)
+            return
+        seqs = _sequences(self.S, sequences)
+        self._pending[seqs] = True
+        self._restart(seqs)
 
-    def start(self, poses):
+    def _restart(self, seqs):
+        """Restart the smoothing of `seqs`: count 0 and a zero ring, the bytes of a fresh tracker's history."""
+        if len(seqs):
+            idx = seqs if isinstance(self._ring, np.ndarray) else torch.from_numpy(seqs).to(self._ring.device)
+            self._ring[idx] = 0
+            self._count[idx] = 0
+
+    def start(self, poses, sequences=None):
         """Begin (or restart) every sequence from known poses [S,3,4]: the next step refines from them, and the
-        smoothing histories restart."""
+        smoothing histories restart.  sequences: poses [len(sequences),3,4] for those sequences only; the others are
+        unaffected.  A float32 array marks its poses as float32 values (as after a refinement), any other dtype float64."""
         poses = np.asarray(poses)
-        if poses.shape != (self.S, 3, 4):
-            raise ValueError(f'start: expected poses [{self.S},3,4], got {poses.shape}')
-        self.reset()
-        self._prev, self._prev_f32 = poses.copy(), poses.dtype == np.float32
+        if sequences is None:
+            if poses.shape != (self.S, 3, 4):
+                raise ValueError(f'start: expected poses [{self.S},3,4], got {poses.shape}')
+            self.reset()
+            seqs = np.arange(self.S)
+        else:
+            seqs = _sequences(self.S, sequences)
+            if poses.shape != (len(seqs), 3, 4):
+                raise ValueError(f'start: expected poses [{len(seqs)},3,4] for sequences {seqs.tolist()}, got {poses.shape}')
+            self._restart(seqs)
+        p64 = np.asarray(poses, np.float64).reshape(len(seqs), 12)
+        if self._prev is None:
+            self._prev = np.zeros((self.S, 3, 4)) if isinstance(self._ring, np.ndarray) else \
+                torch.zeros(self.S, 12, dtype=torch.float64, device=self._ring.device)
+        if isinstance(self._prev, np.ndarray):
+            self._prev[seqs] = p64.reshape(-1, 3, 4)
+        else:
+            self._prev[torch.from_numpy(seqs).to(self._prev.device)] = torch.from_numpy(p64).to(self._prev.device)
+        self._pending[seqs] = False
+        self._f32[seqs] = poses.dtype == np.float32
 
     def _check(self):
         if self.est._generation() != self._gen:
@@ -170,38 +297,81 @@ class Tracker:
         elif isinstance(self._ring, torch.Tensor):
             self._ring, self._count = self._ring.cpu().numpy(), self._count.cpu().numpy()
             if self._prev is not None:
-                p = self._prev.cpu().numpy().reshape(self.S, 3, 4)
-                self._prev = p.astype(np.float32) if self._prev_f32 else p
+                self._prev = self._prev.cpu().numpy().reshape(self.S, 3, 4)
+
+    def _kind(self):
+        """'full', 'refine' or 'mixed': the graph the next step replays."""
+        if self._pending.all():
+            return 'full'
+        if not self._pending.any() and (self._f32.all() or not self._f32.any()):
+            return 'refine'
+        if self._pending.any() and self.est.cfg['refine_iter'] < 1:
+            raise ValueError("re-initialising some sequences while others track needs cfg['refine_iter'] >= 1 (the step "
+                             'smooths float32 poses)')
+        return 'mixed'
 
     # -------------------------------------------------------------- one step
     def step(self, frames, Ks):
         """frames: S uint8 [h,w,3] of one size; Ks: [S,3,3].  Returns (raw poses float32 [S,3,4], smoothed poses float64
         [S,3,4], inter): inter['refine_poses'] is this step's chain, inter['bbox_pts'] the projected box corners
         [S,8,2], inter['smoothed_pts'] their weighted average [S,8,2]; a full-prediction step adds the detection and
-        selection entries of predict_batch."""
+        selection entries of predict_batch.  A mixed step (some sequences re-initialised by reset(sequences), or previous
+        poses of different dtypes) adds inter['reinit'] (the re-initialised sequences, ascending) with the detection and
+        selection entries of those sequences in that order, and its chain has 1 + max(cfg['refine_iter'], refine_iter)
+        entries [S,3,4]: entry 0 the starting poses (float64), a row whose chain is shorter repeating its final pose."""
         self._check()
         if len(frames) != self.S or len(Ks) != self.S:
             raise ValueError(f'step: this tracker follows {self.S} sequences, got {len(frames)} frames and {len(Ks)} Ks')
         Ks = np.stack([np.asarray(K) for K in Ks], 0)
-        if self._device_path():
-            return self._step_device(frames, Ks)
-        return self._step_host(frames, Ks)
+        kind = self._kind()
+        out = self._step_device(frames, Ks, kind) if self._device_path() else self._step_host(frames, Ks, kind)
+        self._pending[:] = False
+        return out
 
-    def _step_host(self, frames, Ks):
-        est = self.est
+    def _step_host(self, frames, Ks, kind):
+        est, S = self.est, self.S
         self._to(False)
-        if self._prev is None:
+        if kind == 'full':
             poses, inter = est.predict_batch(frames, list(Ks))
-        else:
+        elif kind == 'refine':
             dev_frames = est.detector.upload_frame([np.asarray(f) for f in frames])
-            poses, chain = est._refine_batch_host(dev_frames, list(Ks), np.stack(list(self._prev), 0), self.refine_iter)
+            prev = self._prev.astype(np.float32) if self._f32[0] else self._prev
+            poses, chain = est._refine_batch_host(dev_frames, list(Ks), prev, self.refine_iter)
             inter = {'refine_poses': chain}
+        else:
+            poses, inter = self._mixed_host(frames, Ks)
         poses = np.asarray(poses)
         smoothed, avg = host_smooth(poses, poses.dtype == np.float32, self.bbox, Ks, self._ring, self._count, self.weights)
-        self._prev, self._prev_f32 = poses, poses.dtype == np.float32
-        inter['bbox_pts'] = self._ring[np.arange(self.S), self._count - 1].copy()
+        self._prev = np.asarray(poses, np.float64).reshape(S, 3, 4).copy()
+        self._f32[:] = poses.dtype == np.float32
+        inter['bbox_pts'] = self._ring[np.arange(S), self._count - 1].copy()
         inter['smoothed_pts'] = avg
         return poses, smoothed, inter
+
+    def _mixed_host(self, frames, Ks):
+        """The mixed step on the host: predict_batch on the re-initialised frames, _refine_batch_host on the others (one
+        call per dtype of their previous poses)."""
+        est, S, F, r = self.est, self.S, self.est.cfg['refine_iter'], self.refine_iter
+        reinit, others = np.flatnonzero(self._pending), np.flatnonzero(~self._pending)
+        n_it = max(F, r)
+        chain = np.zeros((n_it + 1, S, 3, 4))
+        inter = {}
+        if len(reinit):
+            _, pb = est.predict_batch([frames[i] for i in reinit], list(Ks[reinit]))
+            for k in range(n_it + 1):
+                chain[k, reinit] = pb['refine_poses'][min(k, F)]
+            inter.update({k: v for k, v in pb.items() if k != 'refine_poses'})
+        for f32 in (True, False):
+            rows = others[self._f32[others] == f32]
+            if len(rows):
+                dev_frames = est.detector.upload_frame([np.asarray(frames[i]) for i in rows])
+                prev = self._prev[rows].astype(np.float32) if f32 else self._prev[rows]
+                _, ch = est._refine_batch_host(dev_frames, list(Ks[rows]), prev, r)
+                for k in range(n_it + 1):
+                    chain[k, rows] = ch[min(k, r)]
+        inter['reinit'] = reinit.astype(np.int64)
+        inter['refine_poses'] = [chain[0]] + [c.astype(np.float32) for c in chain[1:]]
+        return inter['refine_poses'][-1], inter
 
     def _device_consts(self):
         if self._dev is None:
@@ -237,26 +407,46 @@ class Tracker:
             return packed.view(torch.uint8), poses, ring, count
         return fn
 
-    def _step_device(self, frames, Ks):
+    def _mixed_fn(self, st, b):
+        est, c = self.est, self._device_consts()
+        initial = est._initial_poses_device_fn(st)
+
+        def init(frames, cams):
+            poses, det, crop, idx, sel_out, logits = initial(frames, cams)
+            return poses, crop, [det, idx, sel_out, logits]
+
+        smooth = lambda poses, Ks, ring, count: ops.track_smooth(poses, True, c['bbox'], Ks, ring, count, c['weights'])
+        return _mixed_fn(1, self.S, b, est.cfg['refine_iter'], self.refine_iter, init, [st['views']], st['tables']['ref_num'],
+                         est.refiner._refine_warped(128), smooth)
+
+    def _step_device(self, frames, Ks, kind):
         est, S, num = self.est, self.S, self.num
         st = est._glue_state()
         self._to(True)
-        full = self._prev is None
+        full = kind == 'full'
         with torch.no_grad():
             dev_frames = est.detector.upload_frame([np.asarray(f) for f in frames])
             cams = est.detector._to_dev(glue.cameras(Ks))
             if full:
                 outs = self.stages.run('track_full', self._full_fn(st), [dev_frames, cams, self._ring, self._count])
-            else:
-                outs = self.stages.run(f'track_refine{int(self._prev_f32)}', self._refine_fn(st, self._prev_f32),
+            elif kind == 'refine':
+                prev_f32 = bool(self._f32[0])
+                outs = self.stages.run(f'track_refine{int(prev_f32)}', self._refine_fn(st, prev_f32),
                                        [dev_frames, cams, self._prev, self._ring, self._count])
+            else:
+                F = est.cfg['refine_iter']
+                reinit, b, extra = _mixed_inputs(S, 1, self._pending, self._f32, F, self.refine_iter, dev_frames.device)
+                prev = self._prev if self._prev is not None else torch.zeros(S, 12, dtype=torch.float64, device=dev_frames.device)
+                outs = self.stages.run(f'track_mixed{b}', self._mixed_fn(st, b), [dev_frames, cams, prev, self._ring, self._count] + extra)
             buf, poses_dev, ring, count = outs
-            prev_f32 = self._prev_f32
             self._prev = poses_dev.clone()
             self._ring.copy_(ring)
             self._count.copy_(count)
             host = est.detector._to_host(buf)                        # the step's one synchronising read
-        self._prev_f32 = True
+        prev_f32 = bool(self._f32[0])
+        self._f32[:] = True
+        if kind == 'mixed':
+            return self._decode_mixed(host, reinit, b)
         n_chain = (est.cfg['refine_iter'] if full else self.refine_iter) + 1
         sizes = [('chain', n_chain * S * 12), ('smoothed', S * 12), ('avg', S * 16), ('ring', S * num * 16), ('count', S)]
         if full:
@@ -287,6 +477,37 @@ class Tracker:
         inter['bbox_pts'] = ring_h[np.arange(S), count_h - 1].copy()
         inter['smoothed_pts'] = vals['avg'].reshape(S, 8, 2).copy()
         return (refined[-1] if refined else first), vals['smoothed'].reshape(S, 3, 4).copy(), inter
+
+    def _decode_mixed(self, host, reinit, b):
+        est, S, num, m = self.est, self.S, self.num, len(reinit)
+        n_chain = max(est.cfg['refine_iter'], self.refine_iter) + 1
+        res = est.cfg['ref_resolution']
+        crop_bytes = b * res * res * 3
+        f64 = host[:len(host) - crop_bytes].view(np.float64)
+        off = 0
+
+        def take(n):
+            nonlocal off
+            off += n
+            return f64[off - n:off]
+        chain = take(n_chain * S * 12).reshape(n_chain, S, 3, 4)
+        smoothed = take(S * 12).reshape(S, 3, 4).copy()
+        avg = take(S * 16).reshape(S, 8, 2).copy()
+        ring_h = take(S * num * 16).reshape(S, num, 8, 2).astype(np.float32)
+        count_h = take(S).astype(np.int64)
+        inter = {'reinit': reinit.astype(np.int64)}
+        if b:
+            det = take(b * 4).reshape(b, 4)[:m].astype(np.float32)
+            idx = take(b)[:m].astype(np.int64)
+            sel_out = take(b * 2).reshape(b, 2)[:m].astype(np.float32)
+            logits = f64[off:].reshape(b, -1)[:m].astype(np.float32)
+            crop = host[len(host) - crop_bytes:].reshape(b, res, res, 3)[:m].copy()
+            inter.update({'det_position': det[:, :2].copy(), 'det_scale_r2q': det[:, 2].copy(), 'det_que_img': crop,
+                          'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': logits, 'sel_ref_idx': idx})
+        inter['refine_poses'] = [chain[0].copy()] + [c.astype(np.float32) for c in chain[1:]]
+        inter['bbox_pts'] = ring_h[np.arange(S), count_h - 1].copy()
+        inter['smoothed_pts'] = avg
+        return inter['refine_poses'][-1], smoothed, inter
 
 
 # ------------------------------------------------------------------------------------------ several objects
@@ -336,31 +557,61 @@ class ObjectTracker:
         self.reset()
 
     # -------------------------------------------------------------- state
-    def reset(self):
-        """The next step is a full prediction for every object and sequence, and the smoothing histories restart."""
+    def reset(self, sequences=None):
+        """The next step is a full prediction for every object and sequence, and the smoothing histories restart.
+        sequences: only those sequences are re-initialised (for every object) and restart their histories."""
         dev, n = self.est.detector.device, self.K * self.S
-        self._prev, self._prev_f32 = None, True
-        self._ring = torch.zeros(n, self.num, 8, 2, device=dev, dtype=torch.float32)
-        self._count = torch.zeros(n, device=dev, dtype=torch.int32)
+        if sequences is None:
+            self._prev = None
+            self._pending, self._f32 = np.ones(self.S, bool), np.ones(self.S, bool)
+            self._ring = torch.zeros(n, self.num, 8, 2, device=dev, dtype=torch.float32)
+            self._count = torch.zeros(n, device=dev, dtype=torch.int32)
+            return
+        seqs = _sequences(self.S, sequences)
+        self._pending[seqs] = True
+        self._restart(seqs)
 
-    def start(self, poses):
+    def _rows(self, seqs):
+        """Object-major rows of sequences `seqs` for every object, on the device."""
+        rows = np.concatenate([o * self.S + seqs for o in range(self.K)])
+        return torch.from_numpy(rows).to(self.est.detector.device)
+
+    def _restart(self, seqs):
+        if len(seqs):
+            rows = self._rows(seqs)
+            self._ring[rows] = 0
+            self._count[rows] = 0
+
+    def start(self, poses, sequences=None):
         """Begin (or restart) every object's sequences from known poses {name: [S,3,4]} (every object of the set, one
-        dtype for all): the next step refines from them, and the smoothing histories restart."""
+        dtype for all): the next step refines from them, and the smoothing histories restart.  sequences: poses
+        {name: [len(sequences),3,4]} for those sequences only; the other sequences are unaffected."""
         missing = [n for n in self.names if n not in poses]
         extra = sorted(set(poses) - set(self.names))
         if missing or extra:
             raise ValueError(f'start: need poses for exactly the set\'s objects {self.names}; missing {missing}, unknown {extra}')
+        seqs = np.arange(self.S) if sequences is None else _sequences(self.S, sequences)
         arrs = [np.asarray(poses[n]) for n in self.names]
         for n, a in zip(self.names, arrs):
-            if a.shape != (self.S, 3, 4):
-                raise ValueError(f'start: object {n!r}: expected poses [{self.S},3,4], got {a.shape}')
+            if a.shape != (len(seqs), 3, 4):
+                raise ValueError(f'start: object {n!r}: expected poses [{len(seqs)},3,4], got {a.shape}')
         dtypes = {a.dtype for a in arrs}
         if len(dtypes) != 1:
             raise ValueError(f'start: the objects\' poses have different dtypes {sorted(str(d) for d in dtypes)}; the refinement '
                              'reads them all as float32 or all as float64, so pass one dtype')
-        self.reset()
-        prev = np.ascontiguousarray(np.concatenate(arrs, 0).astype(np.float64).reshape(self.K * self.S, 12))
-        self._prev, self._prev_f32 = torch.from_numpy(prev).to(self.est.detector.device), arrs[0].dtype == np.float32
+        if sequences is None:
+            self.reset()
+        else:
+            self._restart(seqs)
+        dev = self.est.detector.device
+        prev = torch.from_numpy(np.ascontiguousarray(np.concatenate(arrs, 0).astype(np.float64).reshape(-1, 12))).to(dev)
+        if self._prev is None:
+            self._prev = torch.zeros(self.K * self.S, 12, dtype=torch.float64, device=dev)
+        self._prev[self._rows(seqs)] = prev
+        self._pending[seqs] = False
+        self._f32[seqs] = arrs[0].dtype == np.float32
+
+    _kind = Tracker._kind
 
     def _check(self):
         if self.objs.membership != self._membership:
@@ -403,10 +654,26 @@ class ObjectTracker:
             return packed.view(torch.uint8), poses, ring, count
         return fn
 
+    def _mixed_fn(self, b):
+        objs, c, K = list(self.objs._objects.values()), self._dev, self.K
+        initial = self.objs._initial_poses_device_fn()
+
+        def init(frames, cams):
+            poses, det, sels, crop = initial(frames, cams)          # the set's shared detection on the gathered frames
+            extras = []
+            for o in range(K):
+                extras += [det[o * b:(o + 1) * b], *sels[o]]
+            return poses, crop, extras
+
+        smooth = lambda poses, Ks, ring, count: ops.track_smooth_objects(poses, True, c['bboxes'], Ks, ring, count, c['weights'])
+        return _mixed_fn(K, self.S, b, self.est.cfg['refine_iter'], self.refine_iter, init, [ob.tables['views'] for ob in objs],
+                         objs[0].tables['tables']['ref_num'], self.est.refiner._refine_warped(128), smooth)
+
     def step(self, frames, Ks):
         """frames: S uint8 [h,w,3] of one size; Ks: [S,3,3] (shared by all objects).  Returns {name: (raw poses float32
         [S,3,4], smoothed poses float64 [S,3,4], inter)}: inter has Tracker.step's keys, and a full-prediction step adds
-        those of ObjectSet.predict (det_score included)."""
+        those of ObjectSet.predict (det_score included); a mixed step adds 'reinit' and those entries for the
+        re-initialised sequences, as Tracker.step does."""
         self._check()
         K, S, num, est = self.K, self.S, self.num, self.est
         if len(frames) != S or len(Ks) != S:
@@ -414,28 +681,40 @@ class ObjectTracker:
         Ks = np.stack([np.asarray(k) for k in Ks], 0)
         if Ks.shape != (S, 3, 3):
             raise ValueError(f'step: Ks must be [{S},3,3], got {Ks.shape}')
-        full = self._prev is None
+        kind = self._kind()
+        full, mixed = kind == 'full', kind == 'mixed'
         with torch.no_grad():
             dev_frames = est.detector.upload_frame([np.asarray(f) for f in frames])
             cams = est.detector._to_dev(glue.cameras(Ks))
             if full:
                 outs = self.stages.run('track_full', self._full_fn(), [dev_frames, cams, self._ring, self._count])
-            else:
-                outs = self.stages.run(f'track_refine{int(self._prev_f32)}', self._refine_fn(self._prev_f32),
+            elif not mixed:
+                prev_f32 = bool(self._f32[0])
+                outs = self.stages.run(f'track_refine{int(prev_f32)}', self._refine_fn(prev_f32),
                                        [dev_frames, cams, self._prev, self._ring, self._count])
+            else:
+                reinit, b, extra = _mixed_inputs(S, K, self._pending, self._f32, est.cfg['refine_iter'], self.refine_iter,
+                                                 dev_frames.device)
+                prev = self._prev if self._prev is not None else torch.zeros(K * S, 12, dtype=torch.float64, device=dev_frames.device)
+                outs = self.stages.run(f'track_mixed{b}', self._mixed_fn(b), [dev_frames, cams, prev, self._ring, self._count] + extra)
             buf, poses_dev, ring, count = outs
-            prev_f32 = self._prev_f32
+            prev_f32 = bool(self._f32[0])
             self._prev = poses_dev.clone()
             self._ring.copy_(ring)
             self._count.copy_(count)
             host = est.detector._to_host(buf)                        # the step's one synchronising read
-        self._prev_f32 = True
-        n, n_chain = K * S, (est.cfg['refine_iter'] if full else self.refine_iter) + 1
-        if full:
+        self._pending[:] = False
+        self._f32[:] = True
+        n = K * S
+        if mixed:
+            n_chain, qn, m = max(est.cfg['refine_iter'], self.refine_iter) + 1, b, len(reinit)
+        else:
+            n_chain, qn, m = (est.cfg['refine_iter'] if full else self.refine_iter) + 1, S, S
+        if full or (mixed and qn):
             res = est.cfg['ref_resolution']
-            crop_bytes = n * res * res * 3
+            crop_bytes = K * qn * res * res * 3
             f64 = host[:len(host) - crop_bytes].view(np.float64)
-            crops = host[len(host) - crop_bytes:].reshape(K, S, res, res, 3)
+            crops = host[len(host) - crop_bytes:].reshape(K, qn, res, res, 3)
         else:
             f64 = host.view(np.float64)
         off = 0
@@ -452,15 +731,15 @@ class ObjectTracker:
         out = {}
         for o, (name, ob) in enumerate(self.objs._objects.items()):
             refined = [c.astype(np.float32) for c in chain[1:, o]]
-            first = chain[0, o].astype(np.float32) if (not full and prev_f32) else chain[0, o].copy()
-            inter = {}
-            if full:
-                d = take(S * 4).reshape(S, 4).astype(np.float32)
-                idx = take(S).astype(np.int64)
-                sel_out = take(S * 2).reshape(S, 2).astype(np.float32)
-                logits = take(S * len(ob.ref_info['poses'])).reshape(S, -1).astype(np.float32)
+            first = chain[0, o].astype(np.float32) if (kind == 'refine' and prev_f32) else chain[0, o].copy()
+            inter = {'reinit': reinit.astype(np.int64)} if mixed else {}
+            if full or (mixed and qn):
+                d = take(qn * 4).reshape(qn, 4)[:m].astype(np.float32)
+                idx = take(qn)[:m].astype(np.int64)
+                sel_out = take(qn * 2).reshape(qn, 2)[:m].astype(np.float32)
+                logits = take(qn * len(ob.ref_info['poses'])).reshape(qn, -1)[:m].astype(np.float32)
                 inter.update({'det_position': d[:, :2].copy(), 'det_scale_r2q': d[:, 2].copy(), 'det_score': d[:, 3].copy(),
-                              'det_que_img': crops[o].copy(), 'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': logits,
+                              'det_que_img': crops[o, :m].copy(), 'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': logits,
                               'sel_ref_idx': idx})
             inter['refine_poses'] = [first] + refined
             inter['bbox_pts'] = ring_h[o, np.arange(S), count_h[o] - 1].copy()

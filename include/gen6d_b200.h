@@ -141,6 +141,29 @@ int g6d_glue_apply_refinements_objects(const g6d_glue_views* views, int n_obj, i
                                        const float* que_K, const float* rect, const float* net_out, double* poses, g6d_stream_t stream);
 int g6d_glue_apply_refinements_objects_host(const g6d_glue_views* views, int n_obj, int rows_per_obj, const float* que_pose,
                                             const float* que_K, const float* rect, const float* net_out, double* poses);
+/* ---- the same two steps on a subset of those rows (a tracker whose sequences are at different points of their chains).
+ * views, n_obj, rows_per_obj, cams, frames and the object-major row numbering are those of the *_objects calls; row_idx
+ * [n_sel] (int32, device memory for the device calls) lists the rows, in any order, n_sel >= 1.
+ * refine_problems_rows: output row j is the problem of poses[row_idx[j]], read with that row's own dtype flag
+ * row_f32[row_idx[j]] (uint8 [n_obj*rows_per_obj]; 1: float32 values), into row j of jobs [n_sel*(ref_num+1)], que_K
+ * [n_sel,9], ... ref_rows [n_sel,ref_num]; bit-identical to that row of g6d_glue_refine_problems_objects with that flag.
+ * apply_refinements_rows: network output row j [7] updates poses[row_idx[j]] in place; unlisted rows are untouched.  Its
+ * list must name each row at most once (on the device a row listed twice is a race: undefined result).  The *_host
+ * variants reject an index outside [0, n_obj*rows_per_obj), and apply_refinements_rows_host a row listed twice. */
+int g6d_glue_refine_problems_rows(const g6d_glue_views* views, int n_obj, int rows_per_obj, const g6d_glue_camera* cams,
+                                  const uint8_t* frames, int rows, int cols, const double* poses, const int* row_idx, int n_sel,
+                                  const uint8_t* row_f32, g6d_warp_job* jobs, float* que_K, float* que_pose, float* rect, float* ref_Ks,
+                                  float* ref_poses, int* ref_rows, g6d_stream_t stream);
+int g6d_glue_refine_problems_rows_host(const g6d_glue_views* views, int n_obj, int rows_per_obj, const g6d_glue_camera* cams,
+                                       const uint8_t* frames, int rows, int cols, const double* poses, const int* row_idx, int n_sel,
+                                       const uint8_t* row_f32, g6d_warp_job* jobs, float* que_K, float* que_pose, float* rect,
+                                       float* ref_Ks, float* ref_poses, int* ref_rows);
+int g6d_glue_apply_refinements_rows(const g6d_glue_views* views, int n_obj, int rows_per_obj, const float* que_pose, const float* que_K,
+                                    const float* rect, const float* net_out, const int* row_idx, int n_sel, double* poses,
+                                    g6d_stream_t stream);
+int g6d_glue_apply_refinements_rows_host(const g6d_glue_views* views, int n_obj, int rows_per_obj, const float* que_pose,
+                                         const float* que_K, const float* rect, const float* net_out, const int* row_idx, int n_sel,
+                                         double* poses);
 /* ---- temporal smoothing of tracked poses (predict.py:18-26,61-70; utils/base_utils.py:256-265 project_points;
  * utils/pose_utils.py:246-279 pnp).  Per sequence s: project the object's bounding box bbox [8,3] (float32) with the raw
  * pose poses[s] [12] (float64 storage; poses_are_f32: float32 values, projected in float32 like numpy does with
