@@ -17,7 +17,7 @@ G6D_GLUE_MAX_OBJECTS = 16                   # objects per g6d_glue_*_objects lau
 PRO_NONE, PRO_AFFINE, PRO_AFFINE_RELU, PRO_CORR = 0, 1, 2, 3
 ACT_NONE, ACT_RELU, ACT_LEAKY01 = 0, 1, 2
 TC_TF32, TC_F16 = 0, 1
-TC_PRENORM, TC_REUSE_IM2COL = 1, 4          # g6d_conv_tc_ex flags
+TC_PRENORM, TC_REUSE_IM2COL, TC_FOLD_SPLITS = 1, 4, 32     # g6d_conv_tc_ex flags
 
 
 class ConvDesc(C.Structure):
@@ -98,6 +98,7 @@ _SIGNATURES = {
     'g6d_conv_tc_stats_supported': [C.POINTER(ConvDesc), I, L],
     'g6d_conv_tc_plan': [C.POINTER(ConvDesc), I, C.POINTER(C.c_int)],
     'g6d_conv_tc_plan_ex': [C.POINTER(ConvDesc), I, I, C.POINTER(C.c_int)],
+    'g6d_conv_tc_plan_v2': [C.POINTER(ConvDesc), I, I, C.POINTER(C.c_int), I],
     'g6d_conv_tc_workspace_bytes_ex': [C.POINTER(ConvDesc), I, I],
     'g6d_conv_tc_ex': [C.POINTER(ConvDesc), P, P, P, I, I, P, P, P, P, P, P, L, I, P],
     'g6d_pack_conv_weight_tc': [P, P, P, I, I, I, I, I, P, I, P],

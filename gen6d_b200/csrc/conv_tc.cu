@@ -54,6 +54,10 @@ constexpr int TC_THREADS = (TC_PRODUCER_WARPS + TC_CONSUMER_WARPS) * 32;
 constexpr int TC_ISSUER = TC_PRODUCER_WARPS * 32;          // consumer thread that also issues the weight TMA
 constexpr int TC_PRODUCER_REGS = 96, TC_CONSUMER_REGS = 160;
 static_assert(TC_PRODUCER_WARPS * TC_PRODUCER_REGS + TC_CONSUMER_WARPS * TC_CONSUMER_REGS <= 65536 / 32, "register file of one SM");
+// Folded K splits (G6D_TC_FOLD_SPLITS, split input only): one producer thread issues every load, so the producer warps
+// give up most of their registers and each consumer thread keeps the tile's running sum (BN / 2 more) in registers.
+constexpr int TC_FOLD_PRODUCER_REGS = 40, TC_FOLD_CONSUMER_REGS = 216;
+static_assert(TC_PRODUCER_WARPS * TC_FOLD_PRODUCER_REGS + TC_CONSUMER_WARPS * TC_FOLD_CONSUMER_REGS <= 65536 / 32, "register file of one SM");
 static_assert(TC_BM == 64 * (TC_CONSUMER_WARPS / 4), "one 64-row wgmma tile per consumer warpgroup");
 constexpr int TC_MAX_K_PER_CHAIN = 2048;                   // longest accumulate chain per CTA (see fill_tc_params)
 
@@ -95,6 +99,7 @@ struct ConvTcP {
     double* stats; long long stats_rows;      // fused InstanceNorm statistics of the OUTPUT (see epilogue_stats)
     int split_in;                             // A tiles by TMA im2col from the pre-split input (see split_input_ok)
     int reuse_order;                          // K-blocks in the A-reuse kernel's order (G6D_TC_REUSE_IM2COL, see kblock_src)
+    int fold;                                 // a work item is a tile whose K splits one CTA sums (G6D_TC_FOLD_SPLITS)
 };
 
 // Filter tap (kz, ky, kx flattened) and 64-channel block of K-block `it` of split `sp` when the input is split
@@ -256,20 +261,11 @@ __device__ __forceinline__ float2 slice_moments(float y0, float y1) {
     return make_float2(s1, s2);
 }
 
-// Epilogue of one consumer thread: rows r and r + 8 of the tile (dst0 / dst1 point at column n_base of
-// their output row, nullptr for rows outside the output), columns 8 i + 2 (lane & 3) + {0, 1}.  Folds the
-// cross terms (smallest magnitude first, scaled back by the lo pre-scale) and the main chains, adds
-// bias + activation unless the output is a split-K partial, stores, and -- when stats is given --
-// adds the InstanceNorm moments of the stored values to the per (group, channel) fp64 accumulators
-// (the reference normalises the raw conv result and the next layer's loader applies it).  All 16 rows
-// of a warp belong to one group (the host only enables this for groups of whole 32-row slices / planes).
+// Folds the cross terms (smallest magnitude first, scaled back by the lo pre-scale) and the main chains of a consumer
+// thread's accumulators into `cross`: the sum of the tile's K-blocks (of one K split).
 template <int BN, int KIND>
-__device__ __forceinline__ void epilogue_tile(float (&acc)[AccCfg<BN>::NMAIN][BN / 2], float (&cross)[BN / 2], int n_acc,
-                                              float* dst0, float* dst1, int n_base, int Cout, const float* __restrict__ bias,
-                                              int act, bool partial, bool vec2, double* __restrict__ stats, long long group,
-                                              int lane) {
+__device__ __forceinline__ void sum_chains(float (&acc)[AccCfg<BN>::NMAIN][BN / 2], float (&cross)[BN / 2], int n_acc) {
     constexpr int NMAIN = AccCfg<BN>::NMAIN;
-    const int cq = 2 * (lane & 3);
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) {
         float v = cross[j] * KindCfg<KIND>::CROSS;
@@ -278,6 +274,19 @@ __device__ __forceinline__ void epilogue_tile(float (&acc)[AccCfg<BN>::NMAIN][BN
             if (a < n_acc) v += acc[a][j];
         cross[j] = v;
     }
+}
+
+// Epilogue of one consumer thread: rows r and r + 8 of the tile (dst0 / dst1 point at column n_base of
+// their output row, nullptr for rows outside the output), columns 8 i + 2 (lane & 3) + {0, 1}.  Takes the
+// summed tile (sum_chains), adds bias + activation unless the output is a split-K partial, stores, and -- when
+// stats is given -- adds the InstanceNorm moments of the stored values to the per (group, channel) fp64 accumulators
+// (the reference normalises the raw conv result and the next layer's loader applies it).  All 16 rows
+// of a warp belong to one group (the host only enables this for groups of whole 32-row slices / planes).
+template <int BN>
+__device__ __forceinline__ void store_tile(float (&cross)[BN / 2], float* dst0, float* dst1, int n_base, int Cout,
+                                           const float* __restrict__ bias, int act, bool partial, bool vec2,
+                                           double* __restrict__ stats, long long group, int lane) {
+    const int cq = 2 * (lane & 3);
 #pragma unroll
     for (int i = 0; i < BN / 8; ++i) {
         const int c = 8 * i + cq, n = n_base + c;
@@ -318,6 +327,15 @@ __device__ __forceinline__ void epilogue_tile(float (&acc)[AccCfg<BN>::NMAIN][BN
     }
 }
 
+template <int BN, int KIND>
+__device__ __forceinline__ void epilogue_tile(float (&acc)[AccCfg<BN>::NMAIN][BN / 2], float (&cross)[BN / 2], int n_acc,
+                                              float* dst0, float* dst1, int n_base, int Cout, const float* __restrict__ bias,
+                                              int act, bool partial, bool vec2, double* __restrict__ stats, long long group,
+                                              int lane) {
+    sum_chains<BN, KIND>(acc, cross, n_acc);
+    store_tile<BN>(cross, dst0, dst1, n_base, Cout, bias, act, partial, vec2, stats, group, lane);
+}
+
 // ==========================================================================================
 // conv_tc2_kernel: persistent implicit-GEMM convolution.
 //   * one CTA per SM loops over (M tile, N tile, K split) work items, so there is no wave tail and
@@ -341,7 +359,7 @@ template <int BN> struct Tc2Cfg {
 
 struct Tc2Work { int m_tiles, n_tiles, total; };
 
-template <int BN, int KIND>
+template <int BN, int KIND, bool FOLD>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUtensorMap map_hi,
                 const __grid_constant__ CUtensorMap map_lo, const __grid_constant__ CUtensorMap map_a) {
@@ -387,10 +405,22 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
         sp = w / wk.m_tiles;
     };
     auto kblocks_of = [&](int sp) { return min(p.kblocks, sp * p.kb_per_split + p.kb_per_split) - sp * p.kb_per_split; };
+    // The CTA's j-th chain: work item blockIdx.x + (j / chains) gridDim.x.  Folded (FOLD), an item is a tile and its K
+    // splits are consecutive chains; otherwise an item is one (tile, split) chain.  The A/B TMA thread and the consumers
+    // walk the same sequence.  Folding is only planned with the split input, so the producer warps and the consumers'
+    // weight stream (gathered A) keep their per-item loops.  False past the last item.
+    const int chains = FOLD ? p.splits : 1;
+    auto chain_of = [&](int j, int& mt, int& nt, int& sp) {
+        const int w = blockIdx.x + (j / chains) * gridDim.x;
+        if (w >= wk.total) return false;
+        decode(w, mt, nt, sp);
+        sp += j % chains;
+        return true;
+    };
 
     if (warp < NPW) {
-        setmaxnreg_dec<TC_PRODUCER_REGS>();
-        if (p.split_in) {
+        setmaxnreg_dec<FOLD ? TC_FOLD_PRODUCER_REGS : TC_PRODUCER_REGS>();
+        if (FOLD || p.split_in) {
             // =========================== A by TMA im2col ===========================
             // The input is already split (hi / lo of channel block cb at channels [128 cb, 128 cb + 64) /
             // [128 cb + 64, 128 cb + 128) of each pixel, in f16_k_source order), so a K-block of tap (kx, ky)
@@ -406,9 +436,8 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
                     return tap * p.Cin + cb * BK;
                 };
                 int g = 0;
-                for (int w = blockIdx.x; w < wk.total; w += gridDim.x) {
-                    int mt, nt, sp;
-                    decode(w, mt, nt, sp);
+                int mt, nt, sp;
+                for (int j = 0; chain_of(j, mt, nt, sp); ++j) {
                     const int nkb = kblocks_of(sp);
                     int m = mt * TC_BM;
                     const int xo = m % p.Wo; m /= p.Wo;
@@ -548,10 +577,10 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
         }
     } else {
         // =============================== consumer warpgroups ===============================
-        setmaxnreg_inc<TC_CONSUMER_REGS>();
+        setmaxnreg_inc<FOLD ? TC_FOLD_CONSUMER_REGS : TC_CONSUMER_REGS>();
         const int cw = warp - NPW;                     // consumer warp: rows 16 cw .. 16 cw + 15 of the tile
         const uint32_t a_row = (cw >> 2) * 64 * 128;   // this warpgroup's 64 rows of the A tiles
-        const bool issuer = threadIdx.x == TC_ISSUER && !p.split_in;      // with the split input, the A issuer loads B
+        const bool issuer = !FOLD && threadIdx.x == TC_ISSUER && !p.split_in;      // with the split input, the A issuer loads B
         // weight-tile stream of the issuer: the next global K-block lg = K-block lit of work item lw
         int lw = blockIdx.x, lit = 0, lg = 0;
         auto load_next = [&]() {
@@ -593,10 +622,10 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
 
         float acc[NMAIN][BN / 2];
         float cross[BN / 2];
+        float run[FOLD ? BN / 2 : 1];                  // FOLD: the tile's sum of its splits so far
         int g = 0;
-        for (int w = blockIdx.x; w < wk.total; w += gridDim.x) {
-            int mt, nt, sp;
-            decode(w, mt, nt, sp);
+        int mt, nt, sp;
+        for (int j = 0; chain_of(j, mt, nt, sp); ++j) {
             const int nkb = kblocks_of(sp);
             zero_acc<BN, NMAIN>(acc, cross);
             for (int it0 = 0; it0 < nkb; it0 += NMAIN) {
@@ -617,7 +646,17 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
             wgmma_wait<0>();
             if (nkb > 0) release(g - 1);
 
-            const bool partial = p.splits > 1;
+            sum_chains<BN, KIND>(acc, cross, nkb < NMAIN ? nkb : NMAIN);
+            if constexpr (FOLD) {
+                // the running sum in conv_tc_reduce4_kernel's order: 0.f + split 0, then each further split; the last
+                // split stores it with bias + activation
+#pragma unroll
+                for (int jj = 0; jj < BN / 2; ++jj) run[jj] = (sp == 0 ? 0.f : run[jj]) + cross[jj];
+                if (sp < p.splits - 1) continue;
+#pragma unroll
+                for (int jj = 0; jj < BN / 2; ++jj) cross[jj] = run[jj];
+            }
+            const bool partial = p.splits > 1 && !FOLD;
             const int n_base = nt * BN;
             const int m0 = mt * TC_BM + 16 * cw + (lane >> 2), m1 = m0 + 8;
             float* out = partial ? p.ws + (long long)sp * p.M * p.Cout + n_base : p.y + p.oco + n_base;
@@ -625,9 +664,8 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
             // 64-bit stores need 8-byte aligned column pairs
             const bool vec2 = partial ? (p.Cout & 1) == 0
                                       : ((p.ocs & 1) == 0 && (p.oco & 1) == 0 && (reinterpret_cast<uintptr_t>(p.y) & 7) == 0);
-            epilogue_tile<BN, KIND>(acc, cross, nkb < NMAIN ? nkb : NMAIN, m0 < p.M ? out + m0 * ld : nullptr,
-                                    m1 < p.M ? out + m1 * ld : nullptr, n_base, p.Cout, p.bias, p.act, partial, vec2,
-                                    p.stats, (long long)(mt * TC_BM + 16 * cw) / p.stats_rows, lane);
+            store_tile<BN>(cross, m0 < p.M ? out + m0 * ld : nullptr, m1 < p.M ? out + m1 * ld : nullptr, n_base, p.Cout, p.bias,
+                           p.act, partial, vec2, p.stats, (long long)(mt * TC_BM + 16 * cw) / p.stats_rows, lane);
         }
     }
 }
@@ -690,26 +728,22 @@ __global__ void conv_tc_reduce4_kernel(const float* __restrict__ ws, const float
 // The same with the fused InstanceNorm statistics of y: a 256-thread block owns 32 consecutive output
 // rows (one group: stats_rows % 32 == 0) x 64 channels; thread = (channel, 8-row slice); the four slices
 // are combined in shared memory and one (sum, sum^2) pair per (block, channel) goes to the fp64 accumulators.
-__global__ void __launch_bounds__(256) conv_tc_reduce_stats_kernel(const float* __restrict__ ws, const float* __restrict__ bias,
-                                                                   float* __restrict__ y, int M, int Cout, int splits, int ocs,
-                                                                   int oco, int act, double* __restrict__ stats, long long stats_rows) {
+// value(m, n) is output element (m, n) (n < Cout, m < M).  conv_tc_reduce_stats_kernel and fold_moments_kernel
+// share this, so a folded layer's moments have the same fp32 partials as the split-K reduce's.
+template <class Value>
+__device__ __forceinline__ void block_moments_32x64(Value value, int M, int Cout, double* __restrict__ stats,
+                                                    long long stats_rows) {
     __shared__ float red[2][4][64];
     const int c = threadIdx.x & 63, rg = threadIdx.x >> 6;
     const int n = blockIdx.y * 64 + c;
     const int m0 = blockIdx.x * 32 + rg * 8;
-    const long long slab = (long long)M * Cout;
     float s1 = 0.f, s2 = 0.f;
     if (n < Cout) {
-        const float b = bias ? bias[n] : 0.f;
 #pragma unroll
         for (int r = 0; r < 8; ++r) {
             const int m = m0 + r;
             if (m < M) {
-                const long long i = (long long)m * Cout + n;
-                float v = 0.f;
-                for (int s = 0; s < splits; ++s) v += ws[(long long)s * slab + i];
-                v = tc_act(v + b, act);
-                y[(long long)m * ocs + oco + n] = v;
+                const float v = value(m, n);
                 s1 += v; s2 = fmaf(v, v, s2);
             }
         }
@@ -721,6 +755,27 @@ __global__ void __launch_bounds__(256) conv_tc_reduce_stats_kernel(const float* 
         const float t = red[q][0][c] + red[q][1][c] + red[q][2][c] + red[q][3][c];
         if (n < Cout) atomicAdd(stats + ((long long)((blockIdx.x * 32) / stats_rows) * Cout + n) * 2 + q, (double)t);
     }
+}
+
+__global__ void __launch_bounds__(256) conv_tc_reduce_stats_kernel(const float* __restrict__ ws, const float* __restrict__ bias,
+                                                                   float* __restrict__ y, int M, int Cout, int splits, int ocs,
+                                                                   int oco, int act, double* __restrict__ stats, long long stats_rows) {
+    const long long slab = (long long)M * Cout;
+    block_moments_32x64([&](int m, int n) {
+        const long long i = (long long)m * Cout + n;
+        float v = 0.f;
+        for (int s = 0; s < splits; ++s) v += ws[(long long)s * slab + i];
+        v = tc_act(v + (bias ? bias[n] : 0.f), act);
+        y[(long long)m * ocs + oco + n] = v;
+        return v;
+    }, M, Cout, stats, stats_rows);
+}
+
+// The moments of a folded layer (G6D_TC_FOLD_SPLITS with stats): the conv wrote the final y, which is what
+// conv_tc_reduce_stats_kernel would have written, and this pass takes that kernel's moments of it.
+__global__ void __launch_bounds__(256) fold_moments_kernel(const float* __restrict__ y, int M, int Cout, int ocs, int oco,
+                                                           double* __restrict__ stats, long long stats_rows) {
+    block_moments_32x64([&](int m, int n) { return y[(long long)m * ocs + oco + n]; }, M, Cout, stats, stats_rows);
 }
 
 static void launch_reduce(const float* ws, const float* bias, float* y, int M, int Cout, int splits, int ocs, int oco, int act,
@@ -888,21 +943,21 @@ static int fill_tc_params(const g6d_conv_desc* d, int kind, ConvTcP& p) {
     return G6D_OK;
 }
 
-template <int BN, int KIND>
+template <int BN, int KIND, bool FOLD>
 static int launch_tc2(const ConvTcP& p, const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& ma, cudaStream_t st) {
     using Cfg = Tc2Cfg<BN>;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+        cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN, KIND, FOLD>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
         if (e != cudaSuccess) { set_error("g6d_conv_tc: cannot opt in to %d B of shared memory: %s", Cfg::SMEM_BYTES, cudaGetErrorString(e)); return G6D_ECUDA; }
         configured = true;
     }
     Tc2Work wk;
     wk.m_tiles = ceil_div(p.M, TC_BM); wk.n_tiles = ceil_div(p.Cout, BN);
-    const long long total = (long long)wk.m_tiles * wk.n_tiles * p.splits;
+    const long long total = (long long)wk.m_tiles * wk.n_tiles * (FOLD ? 1 : p.splits);
     wk.total = (int)total;
     const int grid = total < kNumSMs ? (int)total : kNumSMs;
-    conv_tc2_kernel<BN, KIND><<<grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(p, wk, mh, ml, ma);
+    conv_tc2_kernel<BN, KIND, FOLD><<<grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(p, wk, mh, ml, ma);
     G6D_CHECK_LAUNCH("g6d_conv_tc");
     return G6D_OK;
 }
@@ -1341,8 +1396,22 @@ struct ConvPlan {
     bool use_flat;
     int bn, splits, flat_smem;
     long long split_in_off;    // byte offset of the split input in the workspace (tc.split_in)
-    long long ws_bytes;        // workspace: split-K partials, then the split input
+    long long ws_bytes;        // workspace: split-K partials (none when folded), then the split input
 };
+
+// G6D_TC_FOLD_SPLITS: the K splits of a persistent split-input plan run back to back in the CTA of their tile, which
+// keeps their running sum in registers and stores the total in the split-K reduce's order (no partials, no reduce pass,
+// same bits).  A tile's splits then take one CTA, so the grid loses the splits' parallelism: fold only when the waves of
+// S-chain tiles, ceil(T / P) S, are within TC_FOLD_SLACK of the waves of single chains, ceil(T S / P).  The slack is what
+// the saved partial traffic and reduce pass pay for, measured per layer on an H100 (DESIGN.md section 5): folding was
+// faster at every ratio up to 1.143 and 0-4 % slower from 1.154.
+constexpr double TC_FOLD_SLACK = 0.15;
+
+static bool fold_ok(const ConvPlan& pl) {
+    if (pl.use_flat || !pl.tc.split_in || pl.splits < 2) return false;
+    const long long T = (long long)ceil_div(pl.tc.M, TC_BM) * ceil_div(pl.tc.Cout, pl.bn), S = pl.splits;
+    return (double)(ceil_div(T, kNumSMs) * S) <= (1.0 + TC_FOLD_SLACK) * (double)ceil_div(T * S, kNumSMs);
+}
 
 // The persistent kernel loads A by TMA im2col from a pre-split copy of the input for fp16 multi-tap 2-D
 // convolutions with stride 1 and no prologue: the gather, split and swizzle of 8 producer warps (each input
@@ -1361,7 +1430,7 @@ static bool split_input_ok(const g6d_conv_desc* d, int kind, int flags, bool use
 }
 
 static int make_plan(const g6d_conv_desc* d, int kind, int flags, ConvPlan& pl) {
-    G6D_REQUIRE((flags & ~(G6D_TC_PRENORM | G6D_TC_REUSE_IM2COL)) == 0, "g6d_conv_tc: bad flags %d", flags);
+    G6D_REQUIRE((flags & ~(G6D_TC_PRENORM | G6D_TC_REUSE_IM2COL | G6D_TC_FOLD_SPLITS)) == 0, "g6d_conv_tc: bad flags %d", flags);
     const int rc = fill_tc_params(d, kind, pl.tc);
     if (rc != G6D_OK) return rc;
     pl.use_flat = fill_flat_params(d, kind, pl.flat, &pl.flat_smem);
@@ -1376,7 +1445,9 @@ static int make_plan(const g6d_conv_desc* d, int kind, int flags, ConvPlan& pl) 
     pl.bn = tc_block_n(d->Cout);
     pl.splits = pl.use_flat ? pl.flat.splits : pl.tc.splits;
     pl.tc.split_in = split_input_ok(d, kind, flags, pl.use_flat) ? 1 : 0;
-    const long long partials = pl.splits > 1 ? (long long)pl.splits * pl.tc.M * pl.tc.Cout * (long long)sizeof(float) : 0;
+    pl.tc.fold = (flags & G6D_TC_FOLD_SPLITS) && fold_ok(pl) ? 1 : 0;
+    const long long partials =
+        pl.splits > 1 && !pl.tc.fold ? (long long)pl.splits * pl.tc.M * pl.tc.Cout * (long long)sizeof(float) : 0;
     pl.split_in_off = (partials + 255) / 256 * 256;
     pl.ws_bytes = pl.tc.split_in
                       ? pl.split_in_off + (long long)d->B * d->D * d->H * d->W * d->Cin * 2 * (long long)sizeof(__half)
@@ -1401,7 +1472,10 @@ static void bind_tensors(P& p, const float* x, const float* bias, const float* p
 
 template <int BN, int KIND>
 static int launch_plan(const ConvPlan& pl, const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& ma, cudaStream_t st) {
-    return pl.use_flat ? launch_flat<BN, KIND>(pl.flat, pl.flat_smem, mh, ml, st) : launch_tc2<BN, KIND>(pl.tc, mh, ml, ma, st);
+    if (pl.use_flat) return launch_flat<BN, KIND>(pl.flat, pl.flat_smem, mh, ml, st);
+    if constexpr (KIND == G6D_TC_F16)                      // the split input, hence folding, is fp16 only
+        if (pl.tc.fold) return launch_tc2<BN, KIND, true>(pl.tc, mh, ml, ma, st);
+    return launch_tc2<BN, KIND, false>(pl.tc, mh, ml, ma, st);
 }
 template <int KIND>
 static int dispatch(const ConvPlan& pl, const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& ma, cudaStream_t st) {
@@ -1460,6 +1534,16 @@ extern "C" int g6d_conv_tc_plan_ex(const g6d_conv_desc* desc, int kind, int flag
     return G6D_OK;
 }
 
+extern "C" int g6d_conv_tc_plan_v2(const g6d_conv_desc* desc, int kind, int flags, int* out, int n) {
+    G6D_REQUIRE(out != nullptr && n > 0, "g6d_conv_tc_plan_v2: null output");
+    ConvPlan pl{};
+    const int rc = make_plan(desc, kind, flags, pl);
+    if (rc != G6D_OK) return rc;
+    const int v[5] = {pl.use_flat ? 1 : 0, pl.bn, pl.splits, pl.tc.split_in, pl.tc.fold};
+    for (int i = 0; i < n && i < 5; ++i) out[i] = v[i];
+    return G6D_OK;
+}
+
 extern "C" int g6d_conv_tc_plan(const g6d_conv_desc* desc, int kind, int* out4) {
     return g6d_conv_tc_plan_ex(desc, kind, 0, out4);
 }
@@ -1483,8 +1567,10 @@ extern "C" int g6d_conv_tc_ex(const g6d_conv_desc* desc, const float* x, const v
     }
     // in the A-reuse kernel's K order without K splits, the moments are those of its epilogue (flat_moments_kernel)
     const bool flat_moments = stats && p.reuse_order && pl.splits == 1;
+    // folded, the split-K reduce's moments, taken from the final y by fold_moments_kernel
+    const bool fold_moments = stats && p.fold;
     if (pl.use_flat) bind_tensors(pl.flat, x, bias, pro_scale, pro_shift, y, ws, stats, stats_rows);
-    else bind_tensors(pl.tc, x, bias, pro_scale, pro_shift, y, ws, flat_moments ? nullptr : stats, stats_rows);
+    else bind_tensors(pl.tc, x, bias, pro_scale, pro_shift, y, ws, flat_moments || fold_moments ? nullptr : stats, stats_rows);
     CUtensorMap mh, ml, ma;
     if ((rc = make_weight_map(&mh, w_hi, w_rows, p.K, pl.bn, kind)) != G6D_OK) return rc;
     if ((rc = make_weight_map(&ml, w_lo, w_rows, p.K, pl.bn, kind)) != G6D_OK) return rc;
@@ -1506,7 +1592,12 @@ extern "C" int g6d_conv_tc_ex(const g6d_conv_desc* desc, const float* x, const v
                                                   stats, stats_rows);
         G6D_CHECK_LAUNCH("g6d_conv_tc(moments)");
     }
-    if (pl.splits > 1) {
+    if (fold_moments) {
+        fold_moments_kernel<<<dim3(ceil_div(p.M, 32), ceil_div(p.Cout, 64)), 256, 0, st>>>(y, p.M, p.Cout, p.ocs, p.oco, stats,
+                                                                                          stats_rows);
+        G6D_CHECK_LAUNCH("g6d_conv_tc(fold moments)");
+    }
+    if (pl.splits > 1 && !p.fold) {
         launch_reduce(static_cast<float*>(ws), bias, y, p.M, p.Cout, pl.splits, p.ocs, p.oco, p.act, stats, stats_rows, st);
         G6D_CHECK_LAUNCH("g6d_conv_tc(split reduce)");
     }

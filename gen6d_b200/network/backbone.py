@@ -45,7 +45,8 @@ def vgg_pyramid(packed, x, full_res=False):
         for slot in block:
             # reuse_im2col: the small maps the A-reuse kernel would take run on the persistent kernel with TMA
             # im2col A instead, in its K order (bit-identical); the larger maps are planned as without it
-            x = ops.conv(x, packed[slot], act=ops.ACT_NONE if slot == 25 else ops.ACT_RELU, reuse_im2col=True)
+            x = ops.conv(x, packed[slot], act=ops.ACT_NONE if slot == 25 else ops.ACT_RELU, reuse_im2col=True,
+                         fold_splits=True)
         outs.append(x)
     outs.append(ops.maxpool2x2(x))
     return outs

@@ -118,7 +118,7 @@ class Detector(PackedModule):
         feats = self._features(que01)
         out = []
         for f, pc in zip(feats, self.ref_kernels):
-            y = ops.conv(f, pc, reuse_im2col=True)      # persistent kernel, TMA im2col A, the A-reuse kernel's K order
+            y = ops.conv(f, pc, reuse_im2col=True, fold_splits=True)      # persistent kernel, TMA im2col A, the A-reuse kernel's K order
             rows = getattr(pc, 'rows', None)
             out.append(ops.det_corr_rowsum(y, *rows) if rows is not None else y)
         return out
@@ -129,7 +129,7 @@ class Detector(PackedModule):
         feats = self._features(que01)
         out = []
         for f, pc in zip(feats, kernels):
-            y = ops.conv(f, pc, reuse_im2col=True)
+            y = ops.conv(f, pc, reuse_im2col=True, fold_splits=True)
             k = pc.rows[0] if pc.rows is not None else 1
             m = ops.det_corr_rowsum_objects(y, n_obj, k, rfn)
             out.append(m.reshape(n_obj * m.shape[1], *m.shape[2:]))
@@ -170,7 +170,7 @@ class Detector(PackedModule):
         def one_head(head):
             x = feats
             for i, pc in enumerate(p[head]):
-                x = ops.conv(x, pc, act=ops.ACT_RELU if i < 2 else ops.ACT_NONE, reuse_im2col=True)
+                x = ops.conv(x, pc, act=ops.ACT_RELU if i < 2 else ops.ACT_NONE, reuse_im2col=True, fold_splits=True)
             return x
 
         for i, head in enumerate(heads):

@@ -21,7 +21,7 @@ IN_EPS = 1e-5
 _UPLOAD_LOCK = threading.Lock()
 # The volume net's and the feature branches' stride-1 convolutions load A by TMA im2col from a split copy of
 # their input (prologue applied) on the persistent kernel, in the A-reuse kernel's K order: bit-identical results.
-IM2COL = dict(prenorm=True, reuse_im2col=True)
+IM2COL = dict(prenorm=True, reuse_im2col=True, fold_splits=True)
 
 
 @dataclass

@@ -195,11 +195,11 @@ class ViewpointSelector(PackedModule):
             last = i + 1 == len(convs)
             if last:
                 ops.conv(x, pc, prologue=pro, pro_scale=ps, pro_shift=pb, group_rows=S, out=cat_buf, out_coff=256 * level,
-                         prenorm=True, reuse_im2col=True)
+                         prenorm=True, reuse_im2col=True, fold_splits=True)
                 break
             rows = x.shape[0] * x.shape[1] * x.shape[2]                   # stride-1 same-size convolution
             y, ws = ops.conv(x, pc, prologue=pro, pro_scale=ps, pro_shift=pb, group_rows=S, stats_rows=rows, prenorm=True,
-                             reuse_im2col=True)
+                             reuse_im2col=True, fold_splits=True)
             # InstanceNorm3d statistics over (S, h, w) of the raw conv output; the normalisation
             # itself (and the ReLU) is applied by the next conv's loader.  MaxPool commutes with
             # the positive-slope affine, so pooling the raw tensor first is exact.
@@ -232,11 +232,12 @@ class ViewpointSelector(PackedModule):
                 def step(l=l, st=st, pc=pc, last=last):
                     if last:
                         ops.conv(st['x'], pc, prologue=st['pro'], pro_scale=st['ps'], pro_shift=st['pb'], group_rows=S,
-                                 out=cat_buf, out_coff=256 * l, prenorm=True, reuse_im2col=True)
+                                 out=cat_buf, out_coff=256 * l, prenorm=True, reuse_im2col=True,
+                                 fold_splits=True)
                         return None
                     rows = st['x'].shape[0] * st['x'].shape[1] * st['x'].shape[2]
                     return ops.conv(st['x'], pc, prologue=st['pro'], pro_scale=st['ps'], pro_shift=st['pb'], group_rows=S,
-                                    stats_rows=rows, prenorm=True, reuse_im2col=True) + (rows,)
+                                    stats_rows=rows, prenorm=True, reuse_im2col=True, fold_splits=True) + (rows,)
                 res = br.run(l, step)
                 st['i'] += 1
                 if res is not None:

@@ -479,7 +479,7 @@ def transpose_to_packed(x2d):
 
 
 def conv(x, pc, prologue=PRO_NONE, pro_scale=None, pro_shift=None, group_rows=1, act=ACT_NONE,
-         in_coff=0, out=None, out_coff=0, stats_rows=None, prenorm=False, reuse_im2col=False):
+         in_coff=0, out=None, out_coff=0, stats_rows=None, prenorm=False, reuse_im2col=False, fold_splits=False):
     """x [B, D, H, W, cs] or [B, H, W, cs]; returns [B, Do, Ho, Wo, Cout] (or 4-D for 4-D input).
     stats_rows: also return the InstanceNorm moments of the OUTPUT, (y, ws) with ws float64
     [groups, Cout, 2] = per group of `stats_rows` consecutive output rows (sum y, sum y^2) -- fused into the
@@ -488,7 +488,10 @@ def conv(x, pc, prologue=PRO_NONE, pro_scale=None, pro_shift=None, group_rows=1,
     prenorm: G6D_TC_PRENORM -- a prologue layer the persistent kernel would gather takes its A operand by TMA
     im2col from a prologue-applied split copy of x instead (same result bit for bit; no-op elsewhere).
     reuse_im2col: G6D_TC_REUSE_IM2COL -- a layer the A-reuse kernel would take (and 3-D layers on the persistent
-    kernel) get the split input on the persistent kernel, in the A-reuse kernel's K order (same result bit for bit)."""
+    kernel) get the split input on the persistent kernel, in the A-reuse kernel's K order (same result bit for bit).
+    fold_splits: G6D_TC_FOLD_SPLITS -- a split-input layer whose tiles keep the GPU about as busy without the K splits'
+    parallelism sums its splits inside the convolution instead of through fp32 partials and a reduce pass (same result
+    bit for bit, smaller workspace)."""
     four = x.dim() == 4
     if four:
         B, H, W, cs = x.shape
@@ -509,7 +512,8 @@ def conv(x, pc, prologue=PRO_NONE, pro_scale=None, pro_shift=None, group_rows=1,
     M = B * Do * Ho * Wo
     stats = None
     if pc.w_hi is not None and conv_path() == 'tc' and _lib.lib().g6d_conv_tc_supported(C.byref(d), pc.kind):
-        flags = (_lib.TC_PRENORM if prenorm else 0) | (_lib.TC_REUSE_IM2COL if reuse_im2col else 0)
+        flags = ((_lib.TC_PRENORM if prenorm else 0) | (_lib.TC_REUSE_IM2COL if reuse_im2col else 0)
+                 | (_lib.TC_FOLD_SPLITS if fold_splits else 0))
         nbytes = _lib.lib().g6d_conv_tc_workspace_bytes_ex(C.byref(d), pc.kind, flags)
         if nbytes < 0:
             _lib.check(-1, 'g6d_conv_tc_workspace_bytes_ex')
@@ -518,8 +522,8 @@ def conv(x, pc, prologue=PRO_NONE, pro_scale=None, pro_shift=None, group_rows=1,
         if fuse:
             stats = torch.empty(M // stats_rows, pc.cout, 2, device=x.device, dtype=torch.float64)
         def tag(d=d, kind=pc.kind, flags=flags):        # formatted by collect_profile, outside the timed launches
-            plan = (C.c_int * 4)()
-            _lib.check(_lib.lib().g6d_conv_tc_plan_ex(C.byref(d), kind, flags, plan), 'g6d_conv_tc_plan_ex')
+            plan = (C.c_int * 5)()
+            _lib.check(_lib.lib().g6d_conv_tc_plan_v2(C.byref(d), kind, flags, plan, 5), 'g6d_conv_tc_plan_v2')
             a_op = (' prenorm' if prologue != PRO_NONE else ' im2col') if plan[3] else ''
             if flags & _lib.TC_REUSE_IM2COL and plan[3]:       # '-ro': taken from the A-reuse kernel, in its K order
                 plain = (C.c_int * 4)()
@@ -527,7 +531,7 @@ def conv(x, pc, prologue=PRO_NONE, pro_scale=None, pro_shift=None, group_rows=1,
                            'g6d_conv_tc_plan_ex')
                 a_op += '-ro' if plain[0] else ''
             return (f'M={M} N={pc.cout} K={kd * kh * kw * pc.cin} k={kd}x{kh}x{kw} s={s} pro={prologue} '
-                    f'{"reuse" if plan[0] else "persist"} BN={plan[1]} splits={plan[2]}{a_op}')
+                    f'{"reuse" if plan[0] else "persist"} BN={plan[1]} splits={plan[2]}{" fold" if plan[4] else ""}{a_op}')
         _call('g6d_conv_tc_ex', C.byref(d), _p(x), _p(pc.w_hi, pc.w_hi.dtype), _p(pc.w_lo, pc.w_lo.dtype), pc.w_hi.shape[0],
               pc.kind, _p(pc.bias), _p(pro_scale), _p(pro_shift), _p(out), _p(ws), _p(stats, torch.float64), stats_rows or 0,
               flags, _stream(), work=work, tag=tag, key='g6d_conv_tc')

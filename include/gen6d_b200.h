@@ -323,10 +323,19 @@ int g6d_conv_tc(const g6d_conv_desc* desc, const float* x, const void* w_hi, con
  * kernel's K order and K splits: bit-identical outputs.  It also lets 3-D layers (and 2-D planes stacked in D)
  * have the split input on the persistent kernel, through a rank-5 im2col map; a volume whose box corners leave
  * [-16, 15] (pad > 16 or kernel > 16) keeps the gathering kernels.  Elsewhere (1x1, stride 2, tf32) it changes nothing.
+ * G6D_TC_FOLD_SPLITS: a persistent-kernel plan with the split input and K splits whose tiles keep the GPU about as busy
+ * without the splits' parallelism (the wave count grows by at most 15 %) runs each tile's splits back to back in one CTA,
+ * which keeps their running sum in registers and stores it in the split-K reduce's order: bit-identical outputs, no fp32
+ * partials in the workspace and no reduce pass.  The splits and their
+ * K-blocks are unchanged.  With stats the moments are taken from y afterwards in the reduce's grouping (only the order
+ * of the fp64 additions differs).  Elsewhere the flag changes nothing.
  * Other bits: G6D_EINVAL. */
 #define G6D_TC_PRENORM 1
 #define G6D_TC_REUSE_IM2COL 4
+#define G6D_TC_FOLD_SPLITS 32
 int g6d_conv_tc_plan_ex(const g6d_conv_desc* desc, int kind, int flags, int* out4);
+/* g6d_conv_tc_plan_ex's four values, then folded (1: G6D_TC_FOLD_SPLITS applies); the first min(n, 5) are written. */
+int g6d_conv_tc_plan_v2(const g6d_conv_desc* desc, int kind, int flags, int* out, int n);
 long long g6d_conv_tc_workspace_bytes_ex(const g6d_conv_desc* desc, int kind, int flags);
 int g6d_conv_tc_ex(const g6d_conv_desc* desc, const float* x, const void* w_hi, const void* w_lo, int w_rows, int kind,
                    const float* bias, const float* pro_scale, const float* pro_shift, float* y, void* ws,

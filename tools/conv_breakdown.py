@@ -10,7 +10,8 @@ whenever a kernel is shorter than its launch).  Each line aggregates the calls o
 the kernel the planner picked (persist: the persistent kernel, reuse: the A-reuse kernel), the prologue,
 BN, the K splits and how a persistent call gets its A operand (im2col: by TMA from a split copy of the input,
 prenorm: the same from a copy with the prologue applied; neither: gathered by the producer warps; a '-ro' suffix
-marks a layer the A-reuse kernel would take, run in its K order by G6D_TC_REUSE_IM2COL).  Times are per step of B
+marks a layer the A-reuse kernel would take, run in its K order by G6D_TC_REUSE_IM2COL; 'fold' marks K splits summed in
+the output by G6D_TC_FOLD_SPLITS instead of through fp32 partials and a reduce pass).  Times are per step of B
 poses, split pass included.  Class lines sum the calls of each part of the network (detector correlation, the
 crops' VGG, selector towers, ...; see CLASSES) and list those of its tags that plan the A-reuse kernel or were taken
 from it."""
@@ -151,12 +152,20 @@ def prologue_3x3_persistent(tag):
     return ' k=1x3x3 s=1 pro=' in f' {tag} ' and ' pro=0 ' not in f' {tag} ' and ' persist ' in f' {tag} '
 
 
+def folded_partial_bytes(tag):
+    """The fp32 split-K partials (splits x M x N) a call tagged 'fold' no longer writes; 0 for other calls."""
+    if ' fold' not in tag:
+        return 0
+    f = dict(t.split('=', 1) for t in tag.split() if t.startswith(('M=', 'N=', 'splits=')))
+    return 4 * int(f['splits']) * int(f['M']) * int(f['N'])
+
+
 def report(agg, labels, top=40):
     tot_ms, tot_w = sum(a[1] for a in agg.values()), sum(a[2] for a in agg.values())
     print(f'conv_tc calls {sum(a[0] for a in agg.values())} total {tot_ms:.2f} ms, {tot_w / tot_ms / 1e9:.1f} TFLOP/s')
     classes = collections.OrderedDict()
     for tag, (n, ms, w) in agg.items():
-        key = ' '.join(t for t in tag.split() if t.startswith(('pro=', 'persist', 'reuse', 'prenorm', 'im2col')))
+        key = ' '.join(t for t in tag.split() if t.startswith(('pro=', 'persist', 'reuse', 'fold', 'prenorm', 'im2col')))
         c = classes.setdefault(key, [0, 0.0, 0.0]); c[0] += n; c[1] += ms; c[2] += w
     for key, (n, ms, w) in sorted(classes.items(), key=lambda kv: -kv[1][1]):
         print(f'  {ms:7.3f} ms x{n:3d} {w / ms / 1e9:6.1f} TF/s  [{key}]')
@@ -169,6 +178,9 @@ def report(agg, labels, top=40):
     for label, tags in labels.items():
         n, ms, w = (sum(a[i] for a in tags.values()) for i in range(3))
         print(f'  {ms:7.3f} ms x{n:3d} {w / ms / 1e9:6.1f} TF/s  [{label}, {100 * ms / tot_ms:.1f} % of the total]')
+        saved = sum(a[0] * folded_partial_bytes(t) for t, a in tags.items())
+        if saved:
+            print(f'      fold: {saved / 1e9:.2f} GB of fp32 partials not written (nor read back by a reduce pass)')
         for tag, (n, ms, w) in sorted(tags.items(), key=lambda kv: -kv[1][1]):
             if ' reuse ' in f' {tag} ' or tag.endswith('-ro'):
                 print(f'      {ms:7.3f} ms x{n:3d} {w / ms / 1e9:6.1f} TF/s  {tag}')
