@@ -14,6 +14,8 @@ HEADER_PATH = os.path.join(os.path.dirname(HERE), 'include', 'gen6d_b200.h')
 
 G6D_DET_MAX_SCALES = 8
 G6D_GLUE_MAX_OBJECTS = 16                   # objects per g6d_glue_*_objects launch
+G6D_DET_MAX_INSTANCES = 16                  # instances per map of g6d_det_parse_peaks
+G6D_DET_MAX_PEAK_RADIUS = 3
 PRO_NONE, PRO_AFFINE, PRO_AFFINE_RELU, PRO_CORR = 0, 1, 2, 3
 ACT_NONE, ACT_RELU, ACT_LEAKY01 = 0, 1, 2
 TC_TF32, TC_F16 = 0, 1
@@ -107,6 +109,8 @@ _SIGNATURES = {
     'g6d_linear_smallm': [P, P, P, P, I, I, I, I, P],
     'g6d_det_score_fuse': [C.POINTER(DetMaps), I, P, P, P, P, P, P],
     'g6d_det_parse': [P, P, P, I, I, I, I, P, P, P],
+    'g6d_det_parse_peaks': [P, P, P, I, I, I, I, I, I, F, F, F, P, P, P, P, P],
+    'g6d_det_parse_peaks_host': [P, P, P, I, I, I, I, I, I, F, F, F, P, P, P, P],
     'g6d_det_corr_rowsum': [P, P, I, I, I, I, I, P],
     'g6d_det_corr_rowsum_objects': [P, P, I, I, I, I, I, I, P],
     'g6d_sel_ref_sums': [P, I, I, I, P, P, P],

@@ -1,5 +1,7 @@
 // Detector-specific kernels: fused normalise/clip/upsample/resize/stack/score_conv/max-over-refs
 // (D2 epilogue + D3 head) and the argmax decode (D4).
+#include <cmath>
+
 #include "common.cuh"
 
 namespace g6d {
@@ -145,6 +147,258 @@ __global__ void det_parse_kernel(const float* __restrict__ scores, const float* 
     }
 }
 
+// ---- multi-peak detection with greedy non-maximum suppression (g6d_det_parse_peaks) ----------------------------------
+// The selection code is shared by the kernel and the host twin; only the decode differs (see det_peak_decode).
+// first-max order of det_parse_kernel: NaN counts as the maximum, ties go to the lower flat index
+__host__ __device__ __forceinline__ bool peak_beats(float v, int i, float bv, int bi) {
+    const bool vn = v != v, bn = bv != bv;
+    if (vn || bn) return vn && (!bn || i < bi);
+    return v > bv || (v == bv && i < bi);
+}
+
+// fp32 arithmetic that is never contracted into an FMA (the IoU's operation order is part of the contract)
+__host__ __device__ __forceinline__ float pk_add(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+__host__ __device__ __forceinline__ float pk_sub(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fsub_rn(a, b);
+#else
+    return a - b;
+#endif
+}
+__host__ __device__ __forceinline__ float pk_mul(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+__host__ __device__ __forceinline__ float pk_div(float a, float b) {
+#ifdef __CUDA_ARCH__
+    return __fdiv_rn(a, b);
+#else
+    return a / b;
+#endif
+}
+
+struct PeakBox { float x0, y0, x1, y1, area; };
+
+// the square of side box_size * scale centred at (x, y)
+__host__ __device__ __forceinline__ PeakBox peak_box(float x, float y, float scale, float box_size) {
+    const float side = pk_mul(box_size, scale), half = pk_mul(side, 0.5f);
+    return {pk_sub(x, half), pk_sub(y, half), pk_add(x, half), pk_add(y, half), pk_mul(side, side)};
+}
+
+__host__ __device__ __forceinline__ float peak_iou(const PeakBox& a, const PeakBox& b) {
+    const float iw = fmaxf(pk_sub(fminf(a.x1, b.x1), fmaxf(a.x0, b.x0)), 0.f);
+    const float ih = fmaxf(pk_sub(fminf(a.y1, b.y1), fmaxf(a.y0, b.y0)), 0.f);
+    const float inter = pk_mul(iw, ih);
+    return pk_div(inter, pk_sub(pk_add(a.area, b.area), inter));
+}
+
+// det_parse_kernel's decode of cell idx: out = (x, y, scale, score).  On the device its compiled form is an fma.rn for the
+// position and ex2.approx for the scale; the host twin uses std::fma and libm's exp2f (a few ulp apart in the scale).
+__host__ __device__ __forceinline__ void det_peak_decode(const float* sc, const float* scl, const float* off, int idx, int ws,
+                                                         int pool, float* out) {
+    const int y = idx / ws, x = idx % ws;
+    const float ox = off[(long long)idx * 2 + 0], oy = off[(long long)idx * 2 + 1];
+#ifdef __CUDA_ARCH__
+    out[0] = fmaf((float)x + ox + 0.5f, (float)pool, -0.5f);
+    out[1] = fmaf((float)y + oy + 0.5f, (float)pool, -0.5f);
+#else
+    out[0] = std::fma((float)x + ox + 0.5f, (float)pool, -0.5f);
+    out[1] = std::fma((float)y + oy + 0.5f, (float)pool, -0.5f);
+#endif
+    out[2] = exp2f(scl[idx]);
+    out[3] = sc[idx];
+}
+
+// no cell within Chebyshev distance `radius` (window clipped at the border) beats cell i
+__host__ __device__ __forceinline__ bool det_is_peak(const float* sc, int i, float v, int hs, int ws, int radius) {
+    const int y = i / ws, x = i % ws;
+    const int y0 = max(y - radius, 0), y1 = min(y + radius, hs - 1), x0 = max(x - radius, 0), x1 = min(x + radius, ws - 1);
+    for (int yy = y0; yy <= y1; ++yy)
+        for (int xx = x0; xx <= x1; ++xx) {
+            const int j = yy * ws + xx;
+            if (j != i && peak_beats(sc[j], j, v, i)) return false;
+        }
+    return true;
+}
+
+struct PeakArgs {
+    int n_maps, hs, ws, pool, max_inst, radius;
+    float nms_iou, box_size, min_score;
+};
+
+// Cell i can be the next instance after the last kept cell (last_v, last_i): it comes after it in the order (the greedy
+// picks are strictly decreasing, so this also excludes every kept cell), clears min_score, is a peak and no kept box
+// suppresses it.  `best` prunes: a cell that cannot beat the caller's running best skips the peak and IoU tests.
+__host__ __device__ __forceinline__ bool peak_candidate(const float* sc, const float* scl, const float* off, int i, float v,
+                                                        float last_v, int last_i, float bv, int bi, const PeakBox* kept, int n_kept,
+                                                        const PeakArgs& a) {
+    if (!(v >= a.min_score) || !peak_beats(last_v, last_i, v, i) || !peak_beats(v, i, bv, bi)) return false;
+    if (!det_is_peak(sc, i, v, a.hs, a.ws, a.radius)) return false;
+    float d[4];
+    det_peak_decode(sc, scl, off, i, a.ws, a.pool, d);
+    const PeakBox b = peak_box(d[0], d[1], d[2], a.box_size);
+    for (int k = 0; k < n_kept; ++k)
+        if (peak_iou(kept[k], b) > a.nms_iou) return false;
+    return true;
+}
+
+// the outputs of map j: rows m*n_maps + j; rows after the kept ones repeat instance 0 with valid = 0
+__host__ __device__ __forceinline__ void peak_write(const PeakArgs& a, int j, int m, const float* d, int idx, int valid, float* det_out,
+                                                   long long* idx_out, int* valid_out) {
+    const long long r = (long long)m * a.n_maps + j;
+    for (int c = 0; c < 4; ++c) det_out[r * 4 + c] = d[c];
+    idx_out[r] = idx;
+    valid_out[r] = valid;
+}
+
+constexpr int kPeakThreads = 512;
+
+// One CTA per map: the instance-0 argmax, then max_inst - 1 rounds of a block-wide argmax over the remaining candidates.
+__global__ void __launch_bounds__(kPeakThreads) det_parse_peaks_kernel(const float* __restrict__ scores, const float* __restrict__ scales,
+                                                                       const float* __restrict__ offsets, const PeakArgs a,
+                                                                       float* __restrict__ det_out, long long* __restrict__ idx_out,
+                                                                       int* __restrict__ valid_out, int* __restrict__ count_out) {
+    const int j = blockIdx.x;
+    const int n = a.hs * a.ws;
+    const float* sc = scores + (long long)j * n;
+    const float* scl = scales + (long long)j * n;
+    const float* off = offsets + (long long)j * n * 2;
+    __shared__ float sv[kPeakThreads / 32];
+    __shared__ int si[kPeakThreads / 32];
+    __shared__ PeakBox kept[G6D_DET_MAX_INSTANCES];
+    __shared__ float first[4], last_v;
+    __shared__ int first_i, last_i, n_kept, done;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+
+    // block argmax of (bv, bi) under peak_beats; the result lands in sv[0], si[0]
+    auto block_best = [&](float bv, int bi) {
+        for (int o = 16; o > 0; o >>= 1) {
+            const float v = __shfl_down_sync(0xffffffffu, bv, o);
+            const int i = __shfl_down_sync(0xffffffffu, bi, o);
+            if (peak_beats(v, i, bv, bi)) { bv = v; bi = i; }
+        }
+        if (lane == 0) { sv[warp] = bv; si[warp] = bi; }
+        __syncthreads();
+        if (warp == 0) {
+            bv = lane < kPeakThreads / 32 ? sv[lane] : -INFINITY;
+            bi = lane < kPeakThreads / 32 ? si[lane] : 0x7fffffff;
+            for (int o = 16; o > 0; o >>= 1) {
+                const float v = __shfl_down_sync(0xffffffffu, bv, o);
+                const int i = __shfl_down_sync(0xffffffffu, bi, o);
+                if (peak_beats(v, i, bv, bi)) { bv = v; bi = i; }
+            }
+            if (lane == 0) { sv[0] = bv; si[0] = bi; }
+        }
+        __syncthreads();
+    };
+
+    float bv = -INFINITY; int bi = 0x7fffffff;       // sentinel: loses to every real element (even -inf) on the index
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const float v = sc[i];
+        if (peak_beats(v, i, bv, bi)) { bv = v; bi = i; }
+    }
+    block_best(bv, bi);
+    if (threadIdx.x == 0) {
+        const int idx = min(max(si[0], 0), n - 1);
+        det_peak_decode(sc, scl, off, idx, a.ws, a.pool, first);
+        const int valid = first[3] >= a.min_score;
+        peak_write(a, j, 0, first, idx, valid, det_out, idx_out, valid_out);
+        kept[0] = peak_box(first[0], first[1], first[2], a.box_size);
+        first_i = idx; last_v = first[3]; last_i = idx;
+        n_kept = 1;
+        done = !valid;                               // an invalid instance 0 ends the map: valid instances form a prefix
+    }
+    __syncthreads();
+    for (int m = 1; m < a.max_inst; ++m) {
+        if (!done) {
+            const float lv = last_v; const int li = last_i, nk = n_kept;
+            bv = -INFINITY; bi = 0x7fffffff;
+            for (int i = threadIdx.x; i < n; i += blockDim.x) {
+                const float v = sc[i];
+                if (peak_candidate(sc, scl, off, i, v, lv, li, bv, bi, kept, nk, a)) { bv = v; bi = i; }
+            }
+            block_best(bv, bi);
+        }
+        if (threadIdx.x == 0) {
+            if (!done && si[0] != 0x7fffffff) {
+                float d[4];
+                det_peak_decode(sc, scl, off, si[0], a.ws, a.pool, d);
+                peak_write(a, j, m, d, si[0], 1, det_out, idx_out, valid_out);
+                kept[n_kept++] = peak_box(d[0], d[1], d[2], a.box_size);
+                last_v = d[3]; last_i = si[0];
+            } else {
+                done = 1;
+                peak_write(a, j, m, first, first_i, 0, det_out, idx_out, valid_out);
+            }
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) count_out[j] = first[3] >= a.min_score ? n_kept : 0;
+}
+
+// the kernel's selection for map j, serially on host memory
+static void det_parse_peaks_map_host(const float* scores, const float* scales, const float* offsets, const PeakArgs& a, int j,
+                                     float* det_out, long long* idx_out, int* valid_out, int* count_out) {
+    const int n = a.hs * a.ws;
+    const float* sc = scores + (long long)j * n;
+    const float* scl = scales + (long long)j * n;
+    const float* off = offsets + (long long)j * n * 2;
+    float bv = -INFINITY; int bi = 0x7fffffff;
+    for (int i = 0; i < n; ++i)
+        if (peak_beats(sc[i], i, bv, bi)) { bv = sc[i]; bi = i; }
+    float first[4];
+    det_peak_decode(sc, scl, off, bi, a.ws, a.pool, first);
+    const int valid0 = first[3] >= a.min_score;
+    peak_write(a, j, 0, first, bi, valid0, det_out, idx_out, valid_out);
+    PeakBox kept[G6D_DET_MAX_INSTANCES];
+    kept[0] = peak_box(first[0], first[1], first[2], a.box_size);
+    int n_kept = 1, last_i = bi;
+    float last_v = first[3];
+    bool done = !valid0;
+    for (int m = 1; m < a.max_inst; ++m) {
+        bv = -INFINITY; bi = 0x7fffffff;
+        if (!done)
+            for (int i = 0; i < n; ++i)
+                if (peak_candidate(sc, scl, off, i, sc[i], last_v, last_i, bv, bi, kept, n_kept, a)) { bv = sc[i]; bi = i; }
+        if (!done && bi != 0x7fffffff) {
+            float d[4];
+            det_peak_decode(sc, scl, off, bi, a.ws, a.pool, d);
+            peak_write(a, j, m, d, bi, 1, det_out, idx_out, valid_out);
+            kept[n_kept++] = peak_box(d[0], d[1], d[2], a.box_size);
+            last_v = d[3]; last_i = bi;
+        } else {
+            done = true;
+            peak_write(a, j, m, first, (int)idx_out[j], 0, det_out, idx_out, valid_out);
+        }
+    }
+    count_out[j] = valid0 ? n_kept : 0;
+}
+
+static int det_parse_peaks_args(const char* name, const void* scores, const void* scales, const void* offsets, int n_maps, int hs, int ws,
+                                int pool_ratio, int max_inst, int radius, float nms_iou, float box_size, float min_score,
+                                const void* det_out, const void* idx_out, const void* valid_out, const void* count_out, PeakArgs* a) {
+    G6D_REQUIRE(scores && scales && offsets && det_out && idx_out && valid_out && count_out, "%s: null pointer", name);
+    G6D_REQUIRE(n_maps > 0 && hs > 0 && ws > 0 && (long long)hs * ws <= 0x7fffffffLL && pool_ratio > 0,
+                "%s: bad map shape (n_maps=%d hs=%d ws=%d pool_ratio=%d)", name, n_maps, hs, ws, pool_ratio);
+    G6D_REQUIRE(max_inst >= 1 && max_inst <= G6D_DET_MAX_INSTANCES, "%s: max_inst=%d outside [1, %d]", name, max_inst,
+                G6D_DET_MAX_INSTANCES);
+    G6D_REQUIRE(radius >= 0 && radius <= G6D_DET_MAX_PEAK_RADIUS, "%s: radius=%d outside [0, %d]", name, radius, G6D_DET_MAX_PEAK_RADIUS);
+    G6D_REQUIRE(nms_iou >= 0.f && nms_iou <= 1.f, "%s: nms_iou=%g outside [0, 1]", name, (double)nms_iou);
+    G6D_REQUIRE(box_size > 0.f && box_size <= 3.0e38f, "%s: box_size=%g must be positive and finite", name, (double)box_size);
+    G6D_REQUIRE(min_score == min_score, "%s: min_score is NaN (use -inf for no threshold)", name);
+    *a = PeakArgs{n_maps, hs, ws, pool_ratio, max_inst, radius, nms_iou, box_size, min_score};
+    return G6D_OK;
+}
+
 // Second half of the row-decomposed sliding inner product (detector.py:222-224 F.conv2d(que, ref) with
 // the reference features as k x k kernels):  out[y,x,r] = sum_ky partial[y + ky, x, ky*rfn + r], where
 // partial = (1 x k convolution with k*rfn output channels (ky-major), zero padding k/2 in BOTH axes) holds,
@@ -250,5 +504,29 @@ extern "C" int g6d_det_parse(const float* scores, const float* scales, const flo
     G6D_REQUIRE(scores && scales && offsets && out && out_idx && qn > 0 && hs > 0 && ws > 0, "g6d_det_parse: bad args");
     det_parse_kernel<<<qn, 256, 0, as_stream(stream)>>>(scores, scales, offsets, hs, ws, pool_ratio, out, out_idx);
     G6D_CHECK_LAUNCH("g6d_det_parse");
+    return G6D_OK;
+}
+
+extern "C" int g6d_det_parse_peaks(const float* scores, const float* scales, const float* offsets, int n_maps, int hs, int ws,
+                                   int pool_ratio, int max_inst, int radius, float nms_iou, float box_size, float min_score,
+                                   float* det_out, long long* idx_out, int* valid_out, int* count_out, g6d_stream_t stream) {
+    PeakArgs a;
+    const int rc = det_parse_peaks_args("g6d_det_parse_peaks", scores, scales, offsets, n_maps, hs, ws, pool_ratio, max_inst, radius,
+                                        nms_iou, box_size, min_score, det_out, idx_out, valid_out, count_out, &a);
+    if (rc != G6D_OK) return rc;
+    det_parse_peaks_kernel<<<n_maps, kPeakThreads, 0, as_stream(stream)>>>(scores, scales, offsets, a, det_out, idx_out, valid_out,
+                                                                            count_out);
+    G6D_CHECK_LAUNCH("g6d_det_parse_peaks");
+    return G6D_OK;
+}
+
+extern "C" int g6d_det_parse_peaks_host(const float* scores, const float* scales, const float* offsets, int n_maps, int hs, int ws,
+                                        int pool_ratio, int max_inst, int radius, float nms_iou, float box_size, float min_score,
+                                        float* det_out, long long* idx_out, int* valid_out, int* count_out) {
+    PeakArgs a;
+    const int rc = det_parse_peaks_args("g6d_det_parse_peaks_host", scores, scales, offsets, n_maps, hs, ws, pool_ratio, max_inst, radius,
+                                        nms_iou, box_size, min_score, det_out, idx_out, valid_out, count_out, &a);
+    if (rc != G6D_OK) return rc;
+    for (int j = 0; j < n_maps; ++j) det_parse_peaks_map_host(scores, scales, offsets, a, j, det_out, idx_out, valid_out, count_out);
     return G6D_OK;
 }

@@ -14,6 +14,7 @@ import yaml
 
 from . import geometry as G
 from . import glue
+from . import instances
 from . import ops
 from .graphs import StageCache
 from .network import name2network
@@ -207,18 +208,39 @@ class Gen6DEstimator:
                 'views': glue.views_struct(ptr(views_dev), tables, views_dev['src'].data_ptr(), views_dev['rows'].data_ptr(),
                                            views_dev['cols'].data_ptr())}
 
-    def _initial_poses_device_fn(self, st):
-        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> detection, selection and the initial poses float64 [qn,12]:
-        (poses, det, crop, idx, sel_out, logits), enqueued back to back."""
+    def _initial_poses_device_fn(self, st, detect=None):
+        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> detection, selection and the initial poses float64 [M*qn,12]:
+        (poses, det, crop, idx, sel_out, logits), enqueued back to back.  detect(frames) -> det [M*qn,4] (x, y, scale,
+        score; row m*qn + f is instance m on frame f) is the detection step: the score-map argmax (M = 1) by default,
+        _peaks_detect_fn's instances for predict_instances.  Every instance slice gets its own crop jobs and initial
+        poses; the M*qn crops go through one warp and one selection."""
         res = self.cfg['ref_resolution']
         select = self.selector._select_warped(res)
+        detect = detect or self.detector._detect_u8
 
         def fn(frames, cams):
-            det = self.detector._detect_u8(frames)                                  # [qn,4]: x, y, scale, score
-            crop, idx, sel_out, logits = select(ops.glue_detection_jobs(det, frames, res))
-            poses = ops.glue_initial_poses(det, idx, sel_out, st['refs'], cams)
-            return poses, det, crop, idx, sel_out, logits
+            qn = frames.shape[0]
+            det = detect(frames)
+            sl = [slice(m * qn, (m + 1) * qn) for m in range(det.shape[0] // qn)]
+            jobs = [ops.glue_detection_jobs(det[s], frames, res) for s in sl]
+            crop, idx, sel_out, logits = select(jobs[0] if len(sl) == 1 else torch.cat(jobs))
+            poses = [ops.glue_initial_poses(det[s], idx[s], sel_out[s], st['refs'], cams) for s in sl]
+            return (poses[0] if len(sl) == 1 else torch.cat(poses)), det, crop, idx, sel_out, logits
         return fn
+
+    def _peaks_detect_fn(self, max_instances, peak_radius, nms_iou, min_score):
+        """frames u8 [qn,h,w,3] -> (det [M*qn,4] instance-major, valid int32 [M*qn], count int32 [qn]): the detector's maps
+        and g6d_det_parse_peaks.  `extra` receives valid and count when the returned function runs."""
+        det_mod, box = self.detector, float(self.cfg['ref_resolution'])
+        extra = []
+
+        def detect(frames):
+            o = det_mod._detect_nhwc(ops.preprocess_u8(frames, out_c=3, imagenet_norm=False))
+            det, _, valid, count = ops.det_parse_peaks(o['score_predict'], o['scale_predict'], o['offset_predict'], max_instances,
+                                                       peak_radius, nms_iou, box, min_score, det_mod.pool_ratio)
+            extra[:] = [valid.reshape(-1), count]
+            return det.reshape(-1, 4)
+        return detect, extra
 
     def _predict_device_fn(self, st):
         """frames u8 [qn,h,w,3], cams f64 [qn,20] -> every stage of predict_batch, enqueued back to back."""
@@ -250,6 +272,56 @@ class Gen6DEstimator:
                  'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': logits, 'sel_ref_idx': idx,
                  'refine_poses': [poses0] + refined}
         return (refined[-1] if refined else poses0), inter
+
+    # ------------------------------------------------------------------ several instances per frame (instances.py)
+    def _instances_fn(self, st, M, radius, nms_iou, min_score):
+        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> packed results of predict_instances: the detector's maps, the peaks,
+        M*qn crops and selections, and refine_iter x (glue over M slots, ONE refiner stage over M*qn poses, glue)."""
+        iters, R = self.cfg['refine_iter'], st['tables']['ref_num']
+        detect, extra = self._peaks_detect_fn(M, radius, nms_iou, min_score)
+        initial, refine = self._initial_poses_device_fn(st, detect), self.refiner._refine_warped(128)
+        views = [st['views']] * M
+
+        def fn(frames, cams):
+            poses, det, crop, idx, sel_out, logits = initial(frames, cams)
+            chain = [poses]
+            for it in range(iters):
+                jobs, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems_objects(views, R, cams, frames, poses, it > 0)
+                out = refine(jobs, que_K, que_pose, ref_Ks, ref_poses)
+                poses = ops.glue_apply_refinements_objects(views, que_pose, que_K, rect, out)
+                chain.append(poses)
+            return instances.pack([torch.stack(chain, 0), det, idx, sel_out, logits] + extra, crop)
+        return fn
+
+    def predict_instances(self, que_imgs, que_Ks, max_instances=4, min_score=None, nms_iou=0.3, peak_radius=1):
+        """Every instance of the object on qn frames of one size: up to `max_instances` detections per frame, the peaks of
+        the detector's score map (within `peak_radius` cells) kept by greedy non-maximum suppression of their
+        ref_resolution * scale boxes at IoU > `nms_iou` (g6d_det_parse_peaks), each selected and refined as predict_batch
+        does.  min_score: a raw score-head threshold (its meaning depends on the checkpoint); None: no threshold.
+        Returns (poses float32 [qn,M,3,4], inter): predict_batch's device-glue keys led by [qn, M], 'det_score' [qn,M],
+        'refine_poses' a list of [qn,M,3,4], 'instance_valid' bool [qn,M] and 'instance_count' [qn].  Instance 0 is
+        predict_batch's detection.  Rows of instances that were not found are computed too (on a repeat of instance 0's
+        detection, so the graph keeps its shapes) and returned, masked by instance_valid: use only the valid rows.
+        One captured graph per (qn, frame shape, max_instances, peak_radius, nms_iou, min_score), one read per call."""
+        from .objects import require_device_pipeline
+        require_device_pipeline(self, 'predict_instances')
+        key = instances.check_args(max_instances, nms_iou, peak_radius, min_score)
+        M = key[0]
+        qn, res = len(que_imgs), self.cfg['ref_resolution']
+        if qn == 0 or len(que_Ks) != qn:
+            raise ValueError(f'predict_instances: {qn} frames and {len(que_Ks)} intrinsics; need one K per frame and at least one frame')
+        st = self._glue_state()
+        det = self.detector
+        with torch.no_grad():
+            frames = det.upload_frame([np.asarray(f) for f in que_imgs])
+            cams = det._to_dev(glue.cameras(np.stack([np.asarray(K) for K in que_Ks], 0)))
+            buf = self.stages.run(('instances',) + key, self._instances_fn(st, *key), [frames, cams])
+            host = det._to_host(buf)                                       # the call's one synchronising read
+        n, n_sel = M * qn, len(self.ref_info['poses'])
+        rd = instances.Unpacker(host, n * res * res * 3)
+        chain = rd.take((self.cfg['refine_iter'] + 1) * n * 12).reshape(-1, n, 12)
+        parts = [rd.take(n * 4), rd.take(n), rd.take(n * 2), rd.take(n * n_sel), rd.take(n), rd.take(qn)]
+        return instances.inter_of(chain, *parts, rd.crops.reshape(n, res, res, 3), M, qn)
 
     # ------------------------------------------------------------------ video tracking (predict.py)
     def tracker(self, num_sequences=1, refine_iter=1, smooth_num=5, smooth_std=2.5, bbox_3d=None):

@@ -19,8 +19,19 @@ import numpy as np
 import torch
 
 from . import glue
+from . import instances
 from . import ops
 from .graphs import StageCache
+
+
+def require_device_pipeline(est, what):
+    """The estimator features an object set and predict_instances need: a refiner, an unsharded selector, device warps."""
+    if est.refiner is None:
+        raise ValueError(f'{what} refines every pose: the estimator needs a refiner')
+    if getattr(est.selector.comm, 'world', 1) > 1:
+        raise ValueError(f'{what} does not shard the selector: the estimator\'s selector is sharded over GPUs')
+    if est.cfg['host_warps']:
+        raise ValueError(f"{what} cuts its crops on the device: cfg['host_warps'] must be False")
 
 
 class _Object:
@@ -39,12 +50,7 @@ class ObjectSet:
     kernels (tens of MB) and the object's database images (66 MB for a 72-view 480x640 object)."""
 
     def __init__(self, est):
-        if est.refiner is None:
-            raise ValueError('an object set refines every pose: the estimator needs a refiner')
-        if getattr(est.selector.comm, 'world', 1) > 1:
-            raise ValueError('an object set does not shard the selector: the estimator\'s selector is sharded over GPUs')
-        if est.cfg['host_warps']:
-            raise ValueError("an object set cuts its crops on the device: cfg['host_warps'] must be False")
+        require_device_pipeline(est, 'an object set')
         self.est = est
         self._objects = {}
         self._kernels = None            # the objects' detector kernels concatenated (rebuilt when membership changes)
@@ -125,9 +131,11 @@ class ObjectSet:
         out, _ = ops.det_parse(o['score_predict'], o['scale_predict'], o['offset_predict'], det.pool_ratio)
         return out, o
 
-    def _initial_poses_device_fn(self):
-        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> the shared detection, each object's selection and the initial poses:
-        (poses f64 [K*qn,12] object-major, det [K*qn,4], [(sel_idx, sel_out, logits)] per object, crops u8 [K*qn,res,res,3])."""
+    def _initial_poses_device_fn(self, detect=None):
+        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> the shared detection, each slot's selection and the initial poses:
+        (poses f64 [S*qn,12] slot-major, det [S*qn,4], [(sel_idx, sel_out, logits)] per slot, crops u8 [S*qn,res,res,3]).
+        detect(frames) -> det [S*qn,4] is the detection step, slot s being object s % K: the argmax of each object's map
+        (S = K) by default, _peaks_detect_fn's instances (S = M*K) for predict_instances."""
         est = self.est
         objs = list(self._objects.values())
         K, res = len(objs), est.cfg['ref_resolution']
@@ -137,33 +145,53 @@ class ObjectSet:
             qn = frames.shape[0]
             rows = lambda t, o: t[o * qn:(o + 1) * qn]
             cat = lambda ts: ts[0] if len(ts) == 1 else torch.cat(ts, 0)
-            det, _ = self._detect(frames)                                            # [K*qn,4]: x, y, scale, score
-            jobs = cat([ops.glue_detection_jobs(rows(det, o), frames, res) for o in range(K)])
-            crop = ops.warp_affine_u8(jobs, K * qn, res, res)
-            feats = sel._feats(ops.preprocess_u8(crop, out_c=4, imagenet_norm=True))  # the crop VGG once for all objects
+            det = self._detect(frames)[0] if detect is None else detect(frames)      # [S*qn,4]: x, y, scale, score
+            S = det.shape[0] // qn
+            jobs = cat([ops.glue_detection_jobs(rows(det, s), frames, res) for s in range(S)])
+            crop = ops.warp_affine_u8(jobs, S * qn, res, res)
+            feats = sel._feats(ops.preprocess_u8(crop, out_c=4, imagenet_norm=True))  # the crop VGG once for all slots
             poses, sels = [], []
-            for o, ob in enumerate(objs):
+            for s in range(S):
+                ob = objs[s % K]
                 lg, ang = [], []
                 for qi in range(qn):
-                    l, a, _ = sel._select_one([f[o * qn + qi] for f in feats], ob.sel, ob.counters)
+                    l, a, _ = sel._select_one([f[s * qn + qi] for f in feats], ob.sel, ob.counters)
                     lg.append(l)
                     ang.append(a)
                 logits = torch.stack(lg, 0)
                 idx, sel_out = ops.sel_parse(logits, torch.stack(ang, 0))
                 sels.append((idx, sel_out, logits))
-                poses.append(ops.glue_initial_poses(rows(det, o), idx, sel_out, ob.tables['refs'], cams))
-            return cat(poses), det, sels, crop                                       # poses [K*qn,12], object-major
+                poses.append(ops.glue_initial_poses(rows(det, s), idx, sel_out, ob.tables['refs'], cams))
+            return cat(poses), det, sels, crop                                       # poses [S*qn,12], slot-major
         return fn
 
-    def _predict_device_fn(self):
+    def _peaks_detect_fn(self, M, radius, nms_iou, min_score):
+        """The detection step of predict_instances: the shared pyramid and correlation of _detect, then g6d_det_parse_peaks
+        on the K*qn maps -> det [M*K*qn,4] (slot m*K + o is instance m of object o).  `extra` receives valid int32 [M*K*qn]
+        and count int32 [K*qn] when the returned function runs."""
+        est = self.est
+        det_mod, box = est.detector, float(est.cfg['ref_resolution'])
+        objs = list(self._objects.values())
+        extra = []
+
+        def detect(frames):
+            o = det_mod._detect_objects_nhwc(ops.preprocess_u8(frames, out_c=3, imagenet_norm=False), self._detector_kernels(),
+                                             len(objs), objs[0].det.rfn)
+            det, _, valid, count = ops.det_parse_peaks(o['score_predict'], o['scale_predict'], o['offset_predict'], M, radius,
+                                                       nms_iou, box, min_score, det_mod.pool_ratio)
+            extra[:] = [valid.reshape(-1), count]
+            return det.reshape(-1, 4)
+        return detect, extra
+
+    def _predict_device_fn(self, detect=None, instances=1):
         """frames u8 [qn,h,w,3], cams f64 [qn,20] -> every stage, back to back, as device tensors: (chain f64
-        [refine_iter+1, K*qn, 12] of object-major poses, det [K*qn,4], [(sel_idx, sel_out, logits)] per object, crops u8
-        [K*qn, res, res, 3])."""
+        [refine_iter+1, S*qn, 12] of slot-major poses, det [S*qn,4], [(sel_idx, sel_out, logits)] per slot, crops u8
+        [S*qn, res, res, 3]) with S = instances*K slots, slot s being object s % K (detect: see _initial_poses_device_fn)."""
         est = self.est
         objs = list(self._objects.values())
         iters, R = est.cfg['refine_iter'], objs[0].tables['tables']['ref_num']
-        views = [ob.tables['views'] for ob in objs]
-        initial, refine = self._initial_poses_device_fn(), est.refiner._refine_warped(128)
+        views = [ob.tables['views'] for ob in objs] * instances
+        initial, refine = self._initial_poses_device_fn(detect), est.refiner._refine_warped(128)
 
         def fn(frames, cams):
             poses, det, sels, crop = initial(frames, cams)
@@ -171,7 +199,7 @@ class ObjectSet:
             for it in range(iters):
                 jobs_r, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems_objects(views, R, cams, frames, poses,
                                                                                                        it > 0)
-                out = refine(jobs_r, que_K, que_pose, ref_Ks, ref_poses)              # one refiner stage for all K*qn poses
+                out = refine(jobs_r, que_K, que_pose, ref_Ks, ref_poses)              # one refiner stage for all S*qn poses
                 poses = ops.glue_apply_refinements_objects(views, que_pose, que_K, rect, out)
                 chain.append(poses)
             return torch.stack(chain, 0), det, sels, crop
@@ -228,6 +256,53 @@ class ObjectSet:
                      'det_que_img': crops[o].copy(), 'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': logits,
                      'sel_ref_idx': idx, 'refine_poses': [chain[0].copy()] + refined}
             out[name] = (refined[-1] if refined else chain[0].copy(), inter)
+        return out
+
+    def _instances_fn(self, M, radius, nms_iou, min_score):
+        """frames u8 [qn,h,w,3], cams f64 [qn,20] -> packed results of predict_instances (the M*K slots' chain, detections,
+        per-slot selections, the peak masks and counts, then the crops)."""
+        detect, extra = self._peaks_detect_fn(M, radius, nms_iou, min_score)
+        stages = self._predict_device_fn(detect, M)
+
+        def fn(frames, cams):
+            chain, det, sels, crop = stages(frames, cams)
+            return instances.pack([chain, det] + [t for sel in sels for t in sel] + extra, crop)
+        return fn
+
+    def predict_instances(self, que_imgs, que_Ks, max_instances=4, min_score=None, nms_iou=0.3, peak_radius=1):
+        """Every instance of every object on the same qn frames: Gen6DEstimator.predict_instances for each object of the set,
+        with the shared query pyramid and correlation of predict().  Slot (m, o) -- instance m of object o -- goes through
+        its own crop and object o's selection; a refinement step over the K*M*qn rows is one refiner stage.  Returns
+        {name: (poses [qn,M,3,4], inter)} with predict_instances' keys.  Rows of instances that were not found are computed
+        and returned, masked by inter['instance_valid'].  One captured graph per argument set and frame shape, one read."""
+        self._check()
+        key = instances.check_args(max_instances, nms_iou, peak_radius, min_score)
+        est = self.est
+        M, K = key[0], len(self._objects)
+        qn, res, iters = len(que_imgs), est.cfg['ref_resolution'], est.cfg['refine_iter']
+        if qn == 0 or len(que_Ks) != qn:
+            raise ValueError(f'predict_instances: {qn} frames and {len(que_Ks)} intrinsics; need one K per frame and at least one frame')
+        det = est.detector
+        with torch.no_grad():
+            frames = det.upload_frame([np.asarray(f) for f in que_imgs])
+            cams = det._to_dev(glue.cameras(np.stack([np.asarray(K_) for K_ in que_Ks], 0)))
+            buf = self.stages.run(('instances',) + key, self._instances_fn(*key), [frames, cams])
+            host = det._to_host(buf)                                       # the call's one synchronising read
+        S = M * K
+        rd = instances.Unpacker(host, S * qn * res * res * 3)
+        chain = rd.take((iters + 1) * S * qn * 12).reshape(iters + 1, M, K, qn, 12)
+        dets = rd.take(S * qn * 4).reshape(M, K, qn, 4)
+        objs = list(self._objects.values())
+        sels = [(rd.take(qn), rd.take(qn * 2), rd.take(qn * len(objs[s % K].ref_info['poses']))) for s in range(S)]
+        valid = rd.take(S * qn).reshape(M, K, qn)
+        count = rd.take(K * qn).reshape(K, qn)
+        crops = rd.crops.reshape(M, K, qn, res, res, 3)
+        out = {}
+        for o, name in enumerate(self._objects):
+            mine = [sels[m * K + o] for m in range(M)]
+            cat = lambda i: np.concatenate([s[i] for s in mine])
+            out[name] = instances.inter_of(chain[:, :, o].reshape(iters + 1, M * qn, 12), dets[:, o], cat(0), cat(1), cat(2),
+                                           valid[:, o], count[o], crops[:, o].reshape(M * qn, res, res, 3), M, qn)
         return out
 
     def tracker(self, num_sequences=1, refine_iter=1, smooth_num=5, smooth_std=2.5, bboxes=None):

@@ -617,6 +617,23 @@ def det_parse(scores, scales, offsets, pool_ratio=8):
     return out, idx
 
 
+def det_parse_peaks(scores, scales, offsets, max_inst, radius=1, nms_iou=0.3, box_size=128.0, min_score=None, pool_ratio=8):
+    """Up to max_inst instances per map by greedy NMS over the score-map peaks (g6d_det_parse_peaks).
+    scores/scales [n,hs,ws,1], offsets [n,hs,ws,2] -> instance-major (det [max_inst,n,4] = x,y,scale,score;
+    idx int64 [max_inst,n]; valid int32 [max_inst,n]; count int32 [n]).  Row 0 is det_parse's output.
+    min_score None: no threshold (a raw score-head value: its meaning depends on the checkpoint)."""
+    n, hs, ws, _ = scores.shape
+    dev = scores.device
+    det = torch.empty(max_inst, n, 4, device=dev, dtype=torch.float32)
+    idx = torch.empty(max_inst, n, device=dev, dtype=torch.int64)
+    valid = torch.empty(max_inst, n, device=dev, dtype=torch.int32)
+    count = torch.empty(n, device=dev, dtype=torch.int32)
+    _call('g6d_det_parse_peaks', _p(scores), _p(scales), _p(offsets), n, hs, ws, pool_ratio, max_inst, radius, float(nms_iou),
+          float(box_size), float('-inf') if min_score is None else float(min_score), _p(det), _p(idx, torch.int64),
+          _p(valid, torch.int32), _p(count, torch.int32), _stream())
+    return det, idx, valid, count
+
+
 # ------------------------------------------------------------------------------- selector
 def sel_ref_sums(ref):
     """ref [S, P, C] -> (sum, sum of squares) over S, float64 [P, C]."""

@@ -388,6 +388,31 @@ int g6d_det_corr_rowsum_objects(const float* partial, float* out, int n_obj, int
  * out [qn, 4] = (x, y, scale, score); out_idx [qn] (int64 flat index y*ws + x). */
 int g6d_det_parse(const float* scores, const float* scales, const float* offsets, int qn, int hs, int ws,
                   int pool_ratio, float* out, long long* out_idx, g6d_stream_t stream);
+/* Every instance of the object in a frame: up to max_inst peaks of each of n_maps score maps (the maps of g6d_det_parse,
+ * qn -> n_maps), chosen by greedy non-maximum suppression.  Order: g6d_det_parse's (NaN is the maximum, ties go to the
+ * lower flat index).  Cell i is a peak when no other cell within Chebyshev distance `radius` (window clipped at the
+ * border) beats it; radius 0 makes every cell a peak.  A cell decodes as g6d_det_parse decodes its argmax (x, y, scale,
+ * score), and its box is the square of side box_size*scale centred at (x, y).  IoU is fp32 in a fixed order
+ *   iw = max(min(x1a,x1b) - max(x0a,x0b), 0), ih likewise, inter = iw*ih, iou = inter / ((area_a + area_b) - inter),
+ * never contracted; a box is suppressed when its IoU with a kept box is strictly greater than nms_iou.
+ * Instance 0 is the argmax, always kept, bit-identical to g6d_det_parse's row.  Instance m > 0 is the best remaining peak
+ * with score >= min_score that no kept box suppresses; the rounds stop after max_inst kept peaks or when none is left.
+ * valid = kept and score >= min_score.  An invalid instance 0 (below min_score, or NaN) ends its map, so the valid
+ * instances always form a prefix and count[j] is their number.  Rows past the kept ones repeat instance 0 with valid 0.
+ * Outputs are instance-major: row m*n_maps + j is instance m of map j: det_out [max_inst, n_maps, 4] (x, y, scale,
+ * score), idx_out [max_inst, n_maps] (flat index y*ws + x), valid_out [max_inst, n_maps], count_out [n_maps].
+ * 1 <= max_inst <= G6D_DET_MAX_INSTANCES, 0 <= radius <= G6D_DET_MAX_PEAK_RADIUS, 0 <= nms_iou <= 1, box_size > 0, finite,
+ * min_score not NaN (-inf: no threshold), pool_ratio > 0.  No workspace, no synchronisation.
+ * The *_host variant runs the same selection on host memory; its decode uses std::fma and libm exp2f, so its scale can
+ * differ by a few ulp from the device's ex2.approx (and with it an IoU, near the threshold). */
+#define G6D_DET_MAX_INSTANCES 16
+#define G6D_DET_MAX_PEAK_RADIUS 3
+int g6d_det_parse_peaks(const float* scores, const float* scales, const float* offsets, int n_maps, int hs, int ws,
+                        int pool_ratio, int max_inst, int radius, float nms_iou, float box_size, float min_score,
+                        float* det_out, long long* idx_out, int* valid_out, int* count_out, g6d_stream_t stream);
+int g6d_det_parse_peaks_host(const float* scores, const float* scales, const float* offsets, int n_maps, int hs, int ws,
+                             int pool_ratio, int max_inst, int radius, float nms_iou, float box_size, float min_score,
+                             float* det_out, long long* idx_out, int* valid_out, int* count_out);
 
 /* ------------------------------------------------------------------ selector ---------------- */
 /* Load-time sums over the reference stack ref [S, P, C]: sum_s ref and sum_s ref^2, as doubles
