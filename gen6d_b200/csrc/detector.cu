@@ -6,6 +6,8 @@
 
 namespace g6d {
 
+constexpr int kDetFuseMaxScales = 6;   // det_score_fuse_kernel is instantiated for 1..6 scales (NIN = 3..18)
+
 struct DetFuseParams {
     g6d_det_maps maps;
     const float* w1; const float* b1; const float* w2; const float* b2;
@@ -477,8 +479,23 @@ extern "C" int g6d_det_corr_rowsum_objects(const float* partial, float* out, int
 extern "C" int g6d_det_score_fuse(const g6d_det_maps* host_maps, int qn, const float* w1, const float* b1,
                                   const float* w2, const float* b2, float* out, g6d_stream_t stream) {
     G6D_REQUIRE(host_maps && w1 && b1 && w2 && b2 && out && qn > 0, "g6d_det_score_fuse: bad args");
-    G6D_REQUIRE(host_maps->n_scales >= 1 && host_maps->n_scales <= G6D_DET_MAX_SCALES && host_maps->rfn > 0,
-                "g6d_det_score_fuse: bad map table");
+    const g6d_det_maps& M = *host_maps;
+    G6D_REQUIRE(M.n_scales >= 1 && M.n_scales <= kDetFuseMaxScales, "g6d_det_score_fuse: n_scales=%d outside [1, %d]",
+                M.n_scales, kDetFuseMaxScales);
+    G6D_REQUIRE(M.rfn > 0 && M.hs > 0 && M.ws > 0, "g6d_det_score_fuse: bad map table (rfn=%d hs=%d ws=%d must be positive)",
+                M.rfn, M.hs, M.ws);
+    // the kernel reads level l at (y >> l, x >> l) for y < H[s][0], x < W[s][0]: exact sizes keep it in bounds
+    for (int s = 0; s < M.n_scales; ++s) {
+        G6D_REQUIRE(M.H[s][0] > 0 && M.W[s][0] > 0, "g6d_det_score_fuse: scale %d has level-0 size %dx%d", s, M.H[s][0],
+                    M.W[s][0]);
+        for (int l = 0; l < 3; ++l) {
+            G6D_REQUIRE(M.map[s][l], "g6d_det_score_fuse: map[%d][%d] is null", s, l);
+            G6D_REQUIRE(M.H[s][l] > 0 && M.W[s][l] > 0 && ((long long)M.H[s][l] << l) == M.H[s][0] &&
+                            ((long long)M.W[s][l] << l) == M.W[s][0],
+                        "g6d_det_score_fuse: scale %d level %d is %dx%d; it must be the level-0 size %dx%d divided by %d exactly",
+                        s, l, M.H[s][l], M.W[s][l], M.H[s][0], M.W[s][0], 1 << l);
+        }
+    }
     DetFuseParams p;
     p.maps = *host_maps; p.w1 = w1; p.b1 = b1; p.w2 = w2; p.b2 = b2; p.out = out; p.qn = qn;
     const long long npix = (long long)qn * host_maps->hs * host_maps->ws;

@@ -103,7 +103,11 @@ __global__ void __launch_bounds__(256, 3) ref_volume_fill_kernel(const VolParams
             const int k = k0 + vq;
             if (k >= sn) break;                                        // warp-uniform
             const long long orow = (long long)qi * nvox + ((long long)i * sn + j) * sn + k;
-            for (int c = lane * 4; c < p.C; c += 128) {
+            // every lane runs ceil(C/128) trips so the full-warp shuffles below see all 32 lanes;
+            // when C % 128 != 0 the lanes past the last channel skip their loads and stores
+            for (int c0 = 0; c0 < p.C; c0 += 128) {
+                const int c = c0 + lane * 4;
+                const bool on = c < p.C;
                 float4 s[kViewsMax];
                 float4 mean = make_float4(0.f, 0.f, 0.f, 0.f), qs = mean;
 #pragma unroll
@@ -116,7 +120,7 @@ __global__ void __launch_bounds__(256, 3) ref_volume_fill_kernel(const VolParams
                         for (int t = 0; t < 4; ++t) {
                             const int idx = __shfl_sync(0xffffffffu, tidx[t], v * 4 + vq);
                             w[t] = __shfl_sync(0xffffffffu, tw[t], v * 4 + vq);
-                            f[t] = __ldg(reinterpret_cast<const float4*>(fmap + idx));
+                            f[t] = on ? __ldg(reinterpret_cast<const float4*>(fmap + idx)) : make_float4(0.f, 0.f, 0.f, 0.f);
                         }
                         float4 acc;
                         acc.x = f[0].x * w[0]; acc.y = f[0].y * w[0]; acc.z = f[0].z * w[0]; acc.w = f[0].w * w[0];
@@ -149,6 +153,7 @@ __global__ void __launch_bounds__(256, 3) ref_volume_fill_kernel(const VolParams
                 const float inv_u = 1.f / (float)(R - 1);      // unbiased (torch.std default, refiner.py:237)
                 float4 sd;
                 sd.x = sqrtf(var.x * inv_u); sd.y = sqrtf(var.y * inv_u); sd.z = sqrtf(var.z * inv_u); sd.w = sqrtf(var.w * inv_u);
+                if (!on) continue;
                 float* mrow = p.mean_in + orow * (2 * p.C);
                 __stcs(reinterpret_cast<float4*>(mrow + c), mean);
                 __stcs(reinterpret_cast<float4*>(mrow + p.C + c), qs);
@@ -327,12 +332,13 @@ extern "C" int g6d_ref_volume_fill(const float* ref_feats, const float* que_feat
                                    g6d_stream_t stream) {
     G6D_REQUIRE(ref_feats && que_feats && ref_Ks && ref_poses && que_Ks && que_poses && mean_in && stdv,
                 "g6d_ref_volume_fill: null pointer");
-    G6D_REQUIRE(Q > 0 && R >= 2 && R <= kMaxRefViews && fh > 0 && fw > 0 && C > 0 && (C & 3) == 0 && sn >= 2 &&
+    // at most 7 references: they and the query fill the 8 projection lanes x 4 voxels of a warp
+    G6D_REQUIRE(Q > 0 && R >= 2 && R <= kMaxRefViews - 1 && fh > 0 && fw > 0 && C > 0 && (C & 3) == 0 && sn >= 2 &&
                     img_h > 0 && img_w > 0,
-                "g6d_ref_volume_fill: bad dims (2 <= R <= %d, C%%4 == 0, sn >= 2)", kMaxRefViews);
+                "g6d_ref_volume_fill: bad dims (Q=%d R=%d fh=%d fw=%d C=%d sn=%d img %dx%d; need 2 <= R <= %d, C > 0, "
+                "C%%4 == 0, sn >= 2)", Q, R, fh, fw, C, sn, img_h, img_w, kMaxRefViews - 1);
     VolParams p{ref_feats, que_feats, ref_Ks, ref_poses, que_Ks, que_poses, mean_in, stdv,
                 Q, R, fh, fw, C, sn, img_h, img_w};
-    G6D_REQUIRE(R <= 7, "g6d_ref_volume_fill: at most 7 reference views (7 + query fill the 8 projection lanes x 4 voxels)");
     const long long bricks = (long long)((sn + 1) / 2) * ((sn + 3) / 4) * ((sn + 7) / 8);
     if (R == 6 && C == 128) ref_volume_fill_c128_kernel<6><<<(unsigned)(Q * bricks), 256, 0, as_stream(stream)>>>(p);
     else if (R == 6) ref_volume_fill_kernel<6><<<(unsigned)(Q * bricks), 256, 0, as_stream(stream)>>>(p);

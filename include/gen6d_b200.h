@@ -367,7 +367,11 @@ typedef struct g6d_det_maps {
 } g6d_det_maps;
 /* Fuses detector.py:225-226 (nearest x2/x4), :207-216 (normalise + clip), :243 (bilinear resize
  * to (hs,ws)), :245 (stack), :246 score_conv (1x1x1 Conv3d 3S->64, ReLU, 64->64) and :247 (max
- * over references).  w1 [64, 3S] (channel = scale*3 + level), w2 [64, 64].  out [qn, hs, ws, 64]. */
+ * over references).  w1 [64, 3S] (channel = scale*3 + level), w2 [64, 64].  out [qn, hs, ws, 64].
+ * 1 <= n_scales <= 6; rfn, hs, ws > 0; every map non-null.  Level l of scale s must have exactly
+ * H[s][0] >> l rows and W[s][0] >> l columns, i.e. H[s][l] << l == H[s][0] and W[s][l] << l == W[s][0]
+ * (the nearest x2^l upsampling of detector.py:225-226 must land on the level-0 grid); otherwise
+ * G6D_EINVAL. */
 int g6d_det_score_fuse(const g6d_det_maps* host_maps, int qn, const float* w1, const float* b1,
                        const float* w2, const float* b2, float* out, g6d_stream_t stream);
 /* Row-decomposed form of the sliding inner product of detector.py:222-224: with the reference features

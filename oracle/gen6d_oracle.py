@@ -103,16 +103,25 @@ def det_raw_correlation(que_feats, ref_feats):
     return out  # level 0, 1, 2: [qn, rfn, H/8.., W/8..]
 
 
-def det_scores_one_scale(sd, cfg, que_imgs, ref_feats):
-    """Detector.get_scores + normalize_scores (detector.py:207-230)."""
-    s0, s1, s2 = det_raw_correlation(det_extract(sd, que_imgs), ref_feats)
-    s2 = F.interpolate(s2, scale_factor=4)
-    s1 = F.interpolate(s1, scale_factor=2)
+def det_fuse_scores(sd, cfg, raw_scales, hs, ws):
+    """The post-correlation part of Detector.detect_impl (detector.py:207-216,225-226,243-247).
+    raw_scales[s] = the three raw correlation maps [qn, rfn, H/2^l, W/2^l] of scale s: level l is
+    nearest-upsampled by 2^l, normalised and clipped, resized bilinearly to (hs, ws); the scales are
+    stacked, run through score_conv and maxed over the references.
+    -> (feats [qn, 64, hs, ws], stacked [qn, 3*scales, rfn, hs, ws])."""
     stats, mx = cfg['vgg_score_stats'], cfg['vgg_score_max']
-    lv = []
-    for s, (mu, sigma) in zip((s0, s1, s2), stats):
-        lv.append(torch.clip((s - mu) / sigma, min=-mx, max=mx))
-    return torch.stack(lv, 1)  # qn,3,rfn,h,w
+    per_scale = []
+    for s0, s1, s2 in raw_scales:
+        s2 = F.interpolate(s2, scale_factor=4)
+        s1 = F.interpolate(s1, scale_factor=2)
+        lv = [torch.clip((s - mu) / sigma, min=-mx, max=mx) for s, (mu, sigma) in zip((s0, s1, s2), stats)]
+        sc = torch.stack(lv, 1)  # qn,3,rfn,h,w
+        qn, _, rfn, hc, wc = sc.shape
+        per_scale.append(F.interpolate(sc.reshape(qn, 3 * rfn, hc, wc), size=(hs, ws), mode='bilinear')
+                         .reshape(qn, 3, rfn, hs, ws))
+    stacked = torch.cat(per_scale, 1)  # qn, 3*scales, rfn, hs, ws
+    x = _seq_conv(sd, 'score_conv', (0, 2), stacked, F.conv3d)
+    return torch.max(x, 2)[0], stacked
 
 
 def det_scale_sizes(hq, wq, scales):
@@ -141,16 +150,9 @@ def det_detect(sd, cfg, que_imgs, ref_feats, return_taps=False):
     cfg = {**DET_DEFAULT_CFG, **cfg}
     qn, _, hq, wq = que_imgs.shape
     hs, ws = hq // 8, wq // 8
-    per_scale = []
-    for ht, wt in det_scale_sizes(hq, wq, cfg['detection_scales']):
-        cur = F.interpolate(que_imgs, size=(ht, wt), mode='bilinear')
-        sc = det_scores_one_scale(sd, cfg, cur, ref_feats)
-        qn, _, rfn, hc, wc = sc.shape
-        per_scale.append(F.interpolate(sc.reshape(qn, 3 * rfn, hc, wc), size=(hs, ws), mode='bilinear')
-                         .reshape(qn, 3, rfn, hs, ws))
-    stacked = torch.cat(per_scale, 1)  # qn, 3*scales, rfn, hs, ws
-    x = _seq_conv(sd, 'score_conv', (0, 2), stacked, F.conv3d)
-    feats = torch.max(x, 2)[0]
+    raw = [det_raw_correlation(det_extract(sd, F.interpolate(que_imgs, size=(ht, wt), mode='bilinear')), ref_feats)
+           for ht, wt in det_scale_sizes(hq, wq, cfg['detection_scales'])]
+    feats, stacked = det_fuse_scores(sd, cfg, raw, hs, ws)
     scores = _seq_conv(sd, 'score_predict', (0, 2, 4), feats, F.conv2d, padding=1)
     offset = _seq_conv(sd, 'offset_predict', (0, 2, 4), feats, F.conv2d, padding=1)
     scale = _seq_conv(sd, 'scale_predict', (0, 2, 4), feats, F.conv2d, padding=1)
@@ -343,7 +345,7 @@ def ref_sample_volume(feats, verts, projs, h_in, w_in):
 
 def ref_volume_coords(poses_in, sn):
     """Unit-cube grid rotated by the input pose (refiner.py:211-222): row vectors @ R_in."""
-    c = torch.linspace(-1, 1, sn, dtype=torch.float32, device=poses_in.device)
+    c = torch.linspace(-1, 1, sn, dtype=torch.float32, device=poses_in.device).to(poses_in.dtype)   # fp32 grid, as the reference
     g = torch.stack(torch.meshgrid(c, c, c, indexing='ij'), -1).reshape(1, sn ** 3, 3)
     return g @ poses_in[:, :3, :3]  # qn, sn^3, 3
 

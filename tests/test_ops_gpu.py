@@ -200,10 +200,27 @@ def test_attention_head_major_tiled(ops, n):
     close(got, ops.attention(q.cuda(), k.cuda(), v.cuda(), heads)[:, hm.cuda()], atol=1e-5)
 
 
+_SMALLM_ACTS = {0: lambda y: y, 1: F.relu, 2: lambda y: F.leaky_relu(y, 0.1)}      # ACT_NONE, ACT_RELU, ACT_LEAKY01
+
+
 def test_linear_smallm(ops):
-    x = torch.randn(3, 4096, generator=g(25)); w = torch.randn(64, 4096, generator=g(26)) * 0.02
-    b = torch.randn(64, generator=g(27))
-    close(ops.linear_smallm(x.cuda(), w.cuda(), b.cuda(), act=ops.ACT_LEAKY01), F.leaky_relu(F.linear(x, w, b), 0.1))
+    """linear_smallm against float64 at the refiner's regressor shapes: M in {1, 7, 8} poses (the kernel's limit is 8),
+    K in {4, 512, 32768} (32768 is the flattened volume encoding), N in {1, 512}, every activation, plus the original
+    M = 3, K = 4096, N = 64 leaky case.  Weights ~ 1/sqrt(K) keep the outputs O(1), where the fp32 dot of K terms is
+    well inside the 1e-4 tolerance.  Every case runs; the failing ones are listed together."""
+    cases = [(3, 4096, 64, ops.ACT_LEAKY01, 0.02)] + [(M, K, N, act, K ** -.5) for M in (1, 7, 8) for K in (4, 512, 32768)
+                                                       for N in (1, 512) for act in (ops.ACT_NONE, ops.ACT_RELU, ops.ACT_LEAKY01)]
+    failed = []
+    for M, K, N, act, wscale in cases:
+        x = torch.randn(M, K, generator=g(25)); w = torch.randn(N, K, generator=g(26)) * wscale
+        b = torch.randn(N, generator=g(27))
+        want = _SMALLM_ACTS[act](F.linear(x.double(), w.double(), b.double()))
+        got = ops.linear_smallm(x.cuda(), w.cuda(), b.cuda(), act=act)
+        try:
+            close(got, want)
+        except AssertionError as e:
+            failed.append(f'M={M} K={K} N={N} act={act}: {str(e).strip().splitlines()[-1]}')
+    assert not failed, f'{len(failed)} of {len(cases)} cases out of tolerance:\n' + '\n'.join(failed)
 
 
 @pytest.mark.parametrize('B,H,W', [(1, 64, 96), (3, 18, 22), (2, 128, 128)])
