@@ -50,7 +50,7 @@ class GlueViews(C.Structure):         # g6d_glue_views
                 ('norm_scale', C.c_double), ('norm_offset', C.c_float * 3), ('size_scale', C.c_float)]
 
 
-P, I, L, F = C.c_void_p, C.c_int, C.c_longlong, C.c_float
+P, I, L, F, D = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_double
 _SIGNATURES = {
     'g6d_preprocess_u8': [P, P, L, I, I, P],
     'g6d_imagenet_norm': [P, P, L, I, I, P],
@@ -76,6 +76,8 @@ _SIGNATURES = {
     'g6d_track_smooth_host': [P, I, P, P, P, P, I, P, I, P, P],
     'g6d_track_smooth_objects': [P, I, P, I, I, P, P, P, I, P, P, P, P],
     'g6d_track_smooth_objects_host': [P, I, P, I, I, P, P, P, I, P, P, P],
+    'g6d_instances_associate': [I, I, I, I, P, P, P, P, D, D, D, D, D, I, P, P, P, P, P, P, P, P, I, P, P, P, P, P, P, P],
+    'g6d_instances_associate_host': [I, I, I, I, P, P, P, P, D, D, D, D, D, I, P, P, P, P, P, P, P, P, I, P, P, P, P, P, P],
     'g6d_nchw_to_nhwc': [P, P, I, I, I, I, I, P],
     'g6d_nhwc_to_nchw': [P, P, I, I, I, I, I, P],
     'g6d_resize_bilinear': [P, P, I, I, I, I, I, I, I, I, P],

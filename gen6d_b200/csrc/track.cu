@@ -1,9 +1,11 @@
 // Temporal smoothing of tracked poses on the device (see track_math.cuh): one thread per sequence projects the box
 // with the new raw pose, updates the sequence's corner history, averages it and solves the PnP, so a tracking step's
 // graph runs from the uploaded frames to the smoothed poses without the host.  The *_host entry point runs the same
-// code on host memory (CPU tests against numpy and cv2.solvePnP, no GPU needed).
+// code on host memory (CPU tests against numpy and cv2.solvePnP, no GPU needed).  The multi-instance tracker's
+// association (instance_track_math.cuh) lives here too: it needs the same no-contraction fp64.
 #include "common.cuh"
 #include "track_math.cuh"
+#include "instance_track_math.cuh"
 
 namespace g6d {
 
@@ -30,9 +32,94 @@ __global__ void __launch_bounds__(32) track_smooth_objects_kernel(const double* 
     if (i < n_rows) smooth_row_objects(i, rows_per_obj, poses, in_f32, bboxes, Ks, ring, count, num, weights, smoothed, avg_pts);
 }
 
+// Association of the multi-instance tracker (instance_track_math.cuh): ONE CTA.  Phase 1 runs one thread per sequence;
+// phase 2 numbers the spawned tracks in ascending (sequence, slot) order -- which is (sequence, detection) order, since a
+// sequence's unmatched detections take its empty slots in ascending order -- by an exclusive block scan of the
+// sequences' spawn counts, chunk by chunk; thread 0 then advances the counter.
+constexpr int kAssocThreads = 256;
+
+__global__ void __launch_bounds__(kAssocThreads) instances_associate_kernel(assoc::Args a, long long* next_id) {
+    __shared__ int s_warp[kAssocThreads / 32];
+    __shared__ long long s_base;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    for (int s = tid; s < a.S; s += kAssocThreads) assoc::associate_sequence(s, a);
+    if (tid == 0) s_base = *next_id;
+    __syncthreads();
+    for (int s0 = 0; s0 < a.S; s0 += kAssocThreads) {
+        const int s = s0 + tid;
+        int n = 0;
+        if (s < a.S)
+            for (int m = 0; m < a.M; ++m) n += a.spawned[(long long)m * a.S + s];
+        int incl = n;
+        for (int o = 1; o < 32; o <<= 1) {
+            const int x = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += x;
+        }
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        int before = 0, total = 0;
+        for (int w = 0; w < kAssocThreads / 32; ++w) {
+            before += w < warp ? s_warp[w] : 0;
+            total += s_warp[w];
+        }
+        long long id = s_base + before + incl - n;
+        if (s < a.S)
+            for (int m = 0; m < a.M; ++m) {
+                const long long i = (long long)m * a.S + s;
+                if (a.spawned[i]) a.ids[i] = id++;
+            }
+        __syncthreads();
+        if (tid == 0) s_base += total;
+        __syncthreads();
+    }
+    if (tid == 0) *next_id = s_base;
+}
+
+static int associate_ok(const char* name, const assoc::Args& a, const long long* next_id) {
+    G6D_REQUIRE(a.S >= 1 && a.M >= 1 && a.M <= assoc::kMaxSlots, "%s: need S >= 1 and 1 <= M <= %d (got S=%d, M=%d)", name,
+                assoc::kMaxSlots, a.S, a.M);
+    G6D_REQUIRE(a.F >= 0 && a.r >= 0 && (a.F > 0 || a.r > 0) && a.num >= 1 && a.max_misses >= 0,
+                "%s: need F, r >= 0 with max(F, r) >= 1, num >= 1 and max_misses >= 0 (got F=%d, r=%d, num=%d, max_misses=%d)", name,
+                a.F, a.r, a.num, a.max_misses);
+    G6D_REQUIRE(a.gate > 0. && a.gate < INFINITY && a.ref_resolution > 0., "%s: need a finite gate > 0 and ref_resolution > 0", name);
+    G6D_REQUIRE(a.det && a.valid && a.init && a.cams && a.prev && a.live && a.ids && a.misses && a.park && a.ring && a.count && a.work &&
+                a.flags0 && a.lists && a.det_slot && a.spawned && a.dropped && next_id, "%s: null pointer", name);
+    return G6D_OK;
+}
+
 }  // namespace g6d
 
 using namespace g6d;
+
+extern "C" int g6d_instances_associate(int S, int M, int F, int r, const float* det, const int* valid, const double* init,
+                                       const g6d_glue_camera* cams, double cx, double cy, double cz, double ref_resolution, double gate,
+                                       int max_misses, const double* prev, int* live, long long* ids, int* misses, long long* next_id,
+                                       double* park, float* ring, int* count, int num, double* work, uint8_t* flags0, int* lists,
+                                       int* det_slot, int* spawned, long long* dropped, g6d_stream_t stream) {
+    const assoc::Args a{S, M, F, r, num, max_misses, det, valid, init, reinterpret_cast<const double*>(cams), cx, cy, cz, ref_resolution,
+                        gate, prev, live, ids, misses, park, ring, count, work, flags0, lists, det_slot, spawned, dropped};
+    const int rc = associate_ok("g6d_instances_associate", a, next_id);
+    if (rc != G6D_OK) return rc;
+    instances_associate_kernel<<<1, kAssocThreads, 0, as_stream(stream)>>>(a, next_id);
+    G6D_CHECK_LAUNCH("g6d_instances_associate");
+    return G6D_OK;
+}
+
+extern "C" int g6d_instances_associate_host(int S, int M, int F, int r, const float* det, const int* valid, const double* init,
+                                            const g6d_glue_camera* cams, double cx, double cy, double cz, double ref_resolution,
+                                            double gate, int max_misses, const double* prev, int* live, long long* ids, int* misses,
+                                            long long* next_id, double* park, float* ring, int* count, int num, double* work,
+                                            uint8_t* flags0, int* lists, int* det_slot, int* spawned, long long* dropped) {
+    const assoc::Args a{S, M, F, r, num, max_misses, det, valid, init, reinterpret_cast<const double*>(cams), cx, cy, cz, ref_resolution,
+                        gate, prev, live, ids, misses, park, ring, count, work, flags0, lists, det_slot, spawned, dropped};
+    const int rc = associate_ok("g6d_instances_associate_host", a, next_id);
+    if (rc != G6D_OK) return rc;
+    for (int s = 0; s < S; ++s) assoc::associate_sequence(s, a);
+    for (int s = 0; s < S; ++s)
+        for (int m = 0; m < M; ++m)
+            if (spawned[(long long)m * S + s]) ids[(long long)m * S + s] = (*next_id)++;
+    return G6D_OK;
+}
 
 extern "C" int g6d_track_smooth(const double* poses, int poses_are_f32, const float* bbox, const double* Ks, float* ring, int* count,
                                 int num, const double* weights, int S, double* smoothed, double* avg_pts, g6d_stream_t stream) {

@@ -334,6 +334,20 @@ class Gen6DEstimator:
         return Tracker(self, num_sequences, refine_iter=refine_iter, smooth_num=smooth_num, smooth_std=smooth_std,
                        bbox_3d=bbox_3d)
 
+    def instance_tracker(self, num_sequences=1, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
+                         min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bbox_3d=None):
+        """An InstanceTracker (gen6d_b200/instance_track.py): every instance of the object, up to `max_instances` per frame,
+        followed through `num_sequences` videos in lockstep.  The first step (and the one after reset() / redetect(), and
+        every `redetect_every`-th step after the last re-detection) detects predict_instances' instances (min_score,
+        nms_iou, peak_radius) and associates them with the live tracks: the greedy matching of the smallest
+        |projected object centre - detected position| / (ref_resolution * detected scale) below `gate`; a track unmatched
+        more than `max_misses` re-detections in a row is dropped, and unmatched detections start new tracks.  Every other
+        step refines each track `refine_iter` times from its previous pose.  Both smooth as tracker() does."""
+        from .instance_track import InstanceTracker
+        return InstanceTracker(self, num_sequences, max_instances=max_instances, refine_iter=refine_iter,
+                               redetect_every=redetect_every, gate=gate, max_misses=max_misses, min_score=min_score, nms_iou=nms_iou,
+                               peak_radius=peak_radius, smooth_num=smooth_num, smooth_std=smooth_std, bbox_3d=bbox_3d)
+
     def track(self, que_imgs, que_K, **tracker_kwargs):
         """predict.py's loop over one video: que_imgs uint8 [h,w,3] frames of one size, que_K [3,3] (or one per frame).
         Returns [(pose, smoothed_pose, inter)] per frame: the raw pose [3,4], the smoothed pose [3,4] (float64, as

@@ -1,0 +1,270 @@
+"""Multi-instance tracking (Gen6DEstimator.instance_tracker()): every instance of an object followed through S videos in
+lockstep, with identities kept across periodic re-detection.
+
+Each sequence has M slots (instances.py's instance-major layout: row m*S + s is slot m of sequence s).  A slot holds a live
+track (an id, its previous pose, a miss count, its smoothing ring) or nothing.  Two kinds of step, each ONE captured graph
+and one read (instances.pack):
+
+- a re-detection step (the first, the one after reset() / redetect(), and every `redetect_every`-th after the last one)
+  runs predict_instances' detection half (the detector's maps, g6d_det_parse_peaks, the M*S crops and selections, the
+  initial poses), then g6d_instances_associate: the live tracks are matched greedily to the detections by the distance of
+  their projected object centre to the detected position, in units of the detection box; unmatched tracks take a miss
+  and are dropped past max_misses, unmatched detections start tracks in the lowest empty slots, and every slot still
+  empty parks on detection row m of its frame.  Continuing tracks run `refine_iter` refinements, new tracks and parked
+  slots cfg['refine_iter'], through the row-indexed glue (csrc/glue.cu) with scratch rows for finished chains, so every
+  iteration is one refiner stage over exactly M*S poses;
+- every other step refines every slot `refine_iter` times from its previous pose (an empty slot from its parking pose),
+  as Tracker's refine step does for one instance.
+
+Both finish with predict.py's smoothing, slots standing in for the objects of g6d_track_smooth_objects.  Shapes are
+fixed, so empty slots are computed too; their results come back as NaN.  The slot state stays on the device.
+"""
+import numpy as np
+import torch
+
+from . import _lib
+from . import glue
+from . import instances
+from . import ops
+from .graphs import StageCache
+from .track import _sequences, check_bbox, object_bbox, smoothing_weights
+
+
+def host_associate(det, valid, init, cams, center, ref_resolution, gate, max_misses, F, r, prev, live, ids, misses, next_id,
+                   park, ring, count):
+    """g6d_instances_associate_host on numpy arrays (the shapes and dtypes of ops.instances_associate; cams float64 [S,20]).
+    live, ids, misses, next_id, park, ring and count are updated in place.  Returns (work, flags0, lists, det_slot, spawned,
+    dropped) as numpy arrays."""
+    n, S = len(live), len(cams)
+    M, num = n // S, ring.shape[1]
+    for a, dt in ((live, np.int32), (ids, np.int64), (misses, np.int32), (next_id, np.int64), (park, np.float64),
+                  (ring, np.float32), (count, np.int32)):
+        if a.dtype != dt or not a.flags.c_contiguous:
+            raise ValueError(f'host_associate: the state arrays must be contiguous {dt.__name__} arrays (updated in place)')
+    c = lambda a, dt: np.ascontiguousarray(a, dt)
+    det, valid, init, cams, prev = c(det, np.float32), c(valid, np.int32), c(init, np.float64), c(cams, np.float64), c(prev, np.float64)
+    work, flags0 = np.zeros((2 * n, 12)), np.zeros(2 * n, np.uint8)
+    lists = np.zeros(max(F, r) * n, np.int32)
+    det_slot, spawned, dropped = np.zeros(n, np.int32), np.zeros(n, np.int32), np.zeros(n, np.int64)
+    cx, cy, cz = (float(v) for v in center)
+    _lib.check(_lib.lib().g6d_instances_associate_host(
+        S, M, int(F), int(r), det.ctypes.data, valid.ctypes.data, init.ctypes.data, cams.ctypes.data, cx, cy, cz,
+        float(ref_resolution), float(gate), int(max_misses), prev.ctypes.data, live.ctypes.data, ids.ctypes.data,
+        misses.ctypes.data, next_id.ctypes.data, park.ctypes.data, ring.ctypes.data, count.ctypes.data, num,
+        work.ctypes.data, flags0.ctypes.data, lists.ctypes.data, det_slot.ctypes.data, spawned.ctypes.data,
+        dropped.ctypes.data), 'g6d_instances_associate_host')
+    return work, flags0, lists, det_slot, spawned, dropped
+
+
+def check_args(num_sequences, max_instances, refine_iter, redetect_every, gate, max_misses, min_score, nms_iou, peak_radius,
+               smooth_num, smooth_std):
+    """-> the detection key of instances.check_args; ValueError for a bad argument."""
+    key = instances.check_args(max_instances, nms_iou, peak_radius, min_score)
+    if int(num_sequences) < 1:
+        raise ValueError(f'num_sequences must be >= 1, got {num_sequences}')
+    if int(refine_iter) < 1:
+        raise ValueError(f'refine_iter must be >= 1, got {refine_iter}')
+    if redetect_every is not None and int(redetect_every) < 1:
+        raise ValueError(f'redetect_every must be None or >= 1, got {redetect_every}')
+    if not (np.isfinite(float(gate)) and float(gate) > 0):
+        raise ValueError(f'gate must be finite and > 0, got {gate}')
+    if int(max_misses) < 0:
+        raise ValueError(f'max_misses must be >= 0, got {max_misses}')
+    if int(smooth_num) < 1:
+        raise ValueError(f'smooth_num must be >= 1, got {smooth_num}')
+    if not float(smooth_std) > 0:
+        raise ValueError(f'smooth_std must be > 0, got {smooth_std}')
+    return key
+
+
+class InstanceTracker:
+    """Every instance of the estimator's object tracked through S sequences in lockstep; see Gen6DEstimator.instance_tracker()."""
+
+    def __init__(self, est, num_sequences, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
+                 min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bbox_3d=None):
+        from .objects import require_device_pipeline
+        require_device_pipeline(est, 'instance tracking')
+        self.key = check_args(num_sequences, max_instances, refine_iter, redetect_every, gate, max_misses, min_score, nms_iou,
+                              peak_radius, smooth_num, smooth_std)
+        if bbox_3d is None:
+            bbox_3d = object_bbox(est.refiner.ref_database)
+            if bbox_3d is None:
+                raise ValueError('the database has no object point cloud: pass bbox_3d (the 8 corners of the object box)')
+        self.est = est
+        self.S, self.M, self.refine_iter = int(num_sequences), self.key[0], int(refine_iter)
+        self.redetect_every = None if redetect_every is None else int(redetect_every)
+        self.gate, self.max_misses = float(gate), int(max_misses)
+        self.num, self.std = int(smooth_num), float(smooth_std)
+        self.bbox = check_bbox(bbox_3d)
+        self.weights = smoothing_weights(self.num, self.std)
+        self._gen = est._generation()
+        self.stages = StageCache()       # the detect and refine graphs (they capture this tracker's device state)
+        dev = est.detector.device
+        self._dev = {'bboxes': torch.from_numpy(np.ascontiguousarray(np.repeat(self.bbox[None], self.M, 0))).to(dev),
+                     'weights': torch.from_numpy(self.weights.copy()).to(dev)}
+        n = self.M * self.S
+        self._next_id = torch.zeros(1, dtype=torch.int64, device=dev)     # ids are unique over the tracker's life
+        self._state = {'prev': torch.zeros(n, 12, dtype=torch.float64, device=dev),
+                       'park': torch.zeros(n, 12, dtype=torch.float64, device=dev),
+                       'live': torch.zeros(n, dtype=torch.int32, device=dev),
+                       'ids': torch.full((n,), -1, dtype=torch.int64, device=dev),
+                       'misses': torch.zeros(n, dtype=torch.int32, device=dev),
+                       'ring': torch.zeros(n, self.num, 8, 2, dtype=torch.float32, device=dev),
+                       'count': torch.zeros(n, dtype=torch.int32, device=dev)}
+        self._pending, self._since = True, 0
+
+    # -------------------------------------------------------------- state
+    def reset(self, sequences=None):
+        """Drop the tracks of `sequences` (None: every sequence); the next step re-detects.  Ids are never reused."""
+        st = self._state
+        if sequences is None:
+            rows = slice(None)
+        else:
+            seqs = _sequences(self.S, sequences)
+            rows = torch.from_numpy(np.concatenate([m * self.S + seqs for m in range(self.M)])).to(st['live'].device)
+        st['live'][rows] = 0
+        st['ids'][rows] = -1
+        st['misses'][rows] = 0
+        st['ring'][rows] = 0
+        st['count'][rows] = 0
+        self._pending = True
+
+    def redetect(self):
+        """The next step re-detects: the live tracks are kept and associated with the new detections."""
+        self._pending = True
+
+    def _check(self):
+        if self.est._generation() != self._gen:
+            raise RuntimeError('this instance tracker is stale: the estimator was rebuilt (build() on another object) or its '
+                               'weights changed since the tracker was created; create a new one with est.instance_tracker()')
+
+    def _detecting(self):
+        return self._pending or (self.redetect_every is not None and self._since >= self.redetect_every)
+
+    # -------------------------------------------------------------- the graphs
+    def _detect_fn(self, st):
+        est, M, S, r = self.est, self.M, self.S, self.refine_iter
+        F, R, c = est.cfg['refine_iter'], st['tables']['ref_num'], self._dev
+        detect, extra = est._peaks_detect_fn(*self.key)
+        initial, refine = est._initial_poses_device_fn(st, detect), est.refiner._refine_warped(128)
+        views, center = [st['views']] * M, [float(v) for v in np.asarray(est.ref_info['center']).reshape(3)]
+        res = float(est.cfg['ref_resolution'])
+
+        def fn(frames, cams, prev, park, live, ids, misses, next_id, ring, count):
+            init, det, crop, idx, sel_out, logits = initial(frames, cams)
+            valid, inst_count = extra
+            work, flags0, lists, det_slot, spawned, dropped = ops.instances_associate(
+                det, valid, init, cams, center, res, self.gate, self.max_misses, F, r, prev, live, ids, misses, next_id, park,
+                ring, count)
+            frames_x, cams_x = torch.cat([frames, frames], 0), torch.cat([cams, cams], 0)
+            real = lambda: work.view(M, 2 * S, 12)[:, :S].reshape(M * S, 12).clone()
+            ones, chain = torch.ones_like(flags0), [real()]
+            for it in range(max(F, r)):
+                rows = lists[it * M * S:(it + 1) * M * S]
+                jobs, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems_rows(
+                    views, R, 2 * S, cams_x, frames_x, work, rows, flags0 if it == 0 else ones)
+                out = refine(jobs, que_K, que_pose, ref_Ks, ref_poses)            # one refiner stage over M*S poses
+                ops.glue_apply_refinements_rows(views, 2 * S, que_pose, que_K, rect, out, rows, work)
+                chain.append(real())
+            poses = chain[-1]
+            smoothed, avg = ops.track_smooth_objects(poses, True, c['bboxes'], cams[:, :9].contiguous(), ring, count, c['weights'])
+            buf = instances.pack([torch.stack(chain, 0), smoothed, avg, ring, count, ids, det, idx, sel_out, logits, valid,
+                                  inst_count, det_slot, spawned, dropped], crop)
+            return buf, poses, park, live, ids, misses, next_id, ring, count
+        return fn
+
+    def _refine_fn(self, st):
+        est, M, S, r, c = self.est, self.M, self.S, self.refine_iter, self._dev
+        R, refine = st['tables']['ref_num'], est.refiner._refine_warped(128)
+        views = [st['views']] * M
+
+        def fn(frames, cams, prev, park, live, ids, ring, count):
+            work = torch.where((live != 0)[:, None], prev, park)                 # empty slots restart from their parking pose
+            flags0 = live.to(torch.uint8)                                        # tracks hold float32 values, parking poses not
+            rows = torch.arange(M * S, device=live.device, dtype=torch.int32)
+            ones, chain = torch.ones_like(flags0), [work.clone()]
+            for it in range(r):
+                jobs, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems_rows(
+                    views, R, S, cams, frames, work, rows, flags0 if it == 0 else ones)
+                out = refine(jobs, que_K, que_pose, ref_Ks, ref_poses)
+                ops.glue_apply_refinements_rows(views, S, que_pose, que_K, rect, out, rows, work)
+                chain.append(work.clone())
+            poses = chain[-1]
+            smoothed, avg = ops.track_smooth_objects(poses, True, c['bboxes'], cams[:, :9].contiguous(), ring, count, c['weights'])
+            buf = instances.pack([torch.stack(chain, 0), smoothed, avg, ring, count, ids], torch.empty(0, dtype=torch.uint8,
+                                                                                                     device=live.device))
+            return buf, poses, ring, count
+        return fn
+
+    # -------------------------------------------------------------- one step
+    def step(self, frames, Ks):
+        """frames: S uint8 [h,w,3] of one size; Ks: [S,3,3].  Returns (poses float32 [S,M,3,4], smoothed float64 [S,M,3,4],
+        track_ids int64 [S,M] (-1: empty slot), inter): inter['refine_poses'] a list of [S,M,3,4] (entry 0 the starting
+        poses, float64 on a re-detection step; a row whose chain is shorter repeats its final pose), 'bbox_pts' and
+        'smoothed_pts' [S,M,8,2].  Empty slots' poses and points are NaN.  A re-detection step adds predict_instances'
+        keys led by [S,M], 'det_slot' int64 [S,M] (the slot detection m went to, -1: discarded), 'spawned' bool [S,M]
+        (the slots that started a track) and 'dropped' (the ids removed this step, ascending)."""
+        self._check()
+        est, S, M, num = self.est, self.S, self.M, self.num
+        if len(frames) != S or len(Ks) != S:
+            raise ValueError(f'step: this tracker follows {S} sequences, got {len(frames)} frames and {len(Ks)} Ks')
+        Ks = np.stack([np.asarray(k) for k in Ks], 0)
+        if Ks.shape != (S, 3, 3):
+            raise ValueError(f'step: Ks must be [{S},3,3], got {Ks.shape}')
+        detecting = self._detecting()
+        F = est.cfg['refine_iter']
+        if detecting and F < 1:
+            raise ValueError("instance tracking needs cfg['refine_iter'] >= 1 (a re-detection step smooths float32 poses)")
+        stt, x = est._glue_state(), self._state
+        with torch.no_grad():
+            dev_frames = est.detector.upload_frame([np.asarray(f) for f in frames])
+            cams = est.detector._to_dev(glue.cameras(Ks))
+            if detecting:
+                outs = self.stages.run('detect', self._detect_fn(stt), [dev_frames, cams, x['prev'], x['park'], x['live'], x['ids'],
+                                                                        x['misses'], self._next_id, x['ring'], x['count']])
+                buf, poses, park, live, ids, misses, next_id, ring, count = outs
+                for k, v in (('park', park), ('live', live), ('ids', ids), ('misses', misses)):
+                    x[k].copy_(v)
+                self._next_id.copy_(next_id)
+            else:
+                outs = self.stages.run('refine', self._refine_fn(stt), [dev_frames, cams, x['prev'], x['park'], x['live'], x['ids'],
+                                                                        x['ring'], x['count']])
+                buf, poses, ring, count = outs
+            x['prev'].copy_(poses)
+            x['ring'].copy_(ring)
+            x['count'].copy_(count)
+            host = est.detector._to_host(buf)                        # the step's one synchronising read
+        self._pending = False
+        self._since = 1 if detecting else self._since + 1
+        return self._decode(host, detecting)
+
+    def _decode(self, host, detecting):
+        est, S, M, num, n = self.est, self.S, self.M, self.num, self.M * self.S
+        n_chain = (max(est.cfg['refine_iter'], self.refine_iter) if detecting else self.refine_iter) + 1
+        res = est.cfg['ref_resolution']
+        rd = instances.Unpacker(host, n * res * res * 3 if detecting else 0)
+        chain = rd.take(n_chain * n * 12).reshape(n_chain, n, 12)
+        smoothed, avg = rd.take(n * 12), rd.take(n * 16)
+        ring_h, count_h = rd.take(n * num * 16).reshape(n, num, 8, 2).astype(np.float32), rd.take(n).astype(np.int64)
+        ids = instances.frame_major(rd.take(n).astype(np.int64), M, S)
+        empty = ids < 0
+        fm = lambda a: instances.frame_major(a, M, S)
+
+        def nan(a):
+            a[empty] = np.nan
+            return a
+        first = fm(chain[0].reshape(n, 3, 4))
+        inter = {'refine_poses': [nan(first if detecting else first.astype(np.float32))] +
+                                 [nan(fm(c.reshape(n, 3, 4)).astype(np.float32)) for c in chain[1:]],
+                 'bbox_pts': nan(fm(ring_h[np.arange(n), count_h - 1])), 'smoothed_pts': nan(fm(avg.reshape(n, 8, 2)))}
+        if detecting:
+            n_sel = len(est.ref_info['poses'])
+            parts = [rd.take(n * 4), rd.take(n), rd.take(n * 2), rd.take(n * n_sel), rd.take(n), rd.take(S)]
+            _, det_inter = instances.inter_of(chain[:1], *parts, rd.crops.reshape(n, res, res, 3), M, S)
+            det_inter.pop('refine_poses')
+            inter.update(det_inter)
+            inter['det_slot'] = fm(rd.take(n).astype(np.int64))
+            inter['spawned'] = fm(rd.take(n).astype(bool))
+            dropped = rd.take(n)
+            inter['dropped'] = sorted(int(i) for i in dropped if i >= 0)
+        return inter['refine_poses'][-1], nan(fm(smoothed.reshape(n, 3, 4))), ids, inter

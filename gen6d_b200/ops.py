@@ -277,6 +277,34 @@ def track_smooth(poses, poses_are_f32, bbox, Ks, ring, count, weights):
     return smoothed, avg
 
 
+def instances_associate(det, valid, init, cams, center, ref_resolution, gate, max_misses, F, r, prev, live, ids, misses, next_id,
+                        park, ring, count):
+    """The multi-instance tracker's association for S sequences x M slots (g6d_instances_associate), rows instance-major
+    (row m*S + s): det float32 [M*S,4], valid int32 [M*S], init float64 [M*S,12] (the detections' initial poses), cams
+    float64 [S,20], center (3 floats).  The slot state prev float64 [M*S,12], live int32, ids int64, misses int32 [M*S],
+    next_id int64 [1], park float64 [M*S,12], ring float32 [M*S,num,8,2] and count int32 [M*S] is updated in place.
+    Returns (work float64 [M*2S,12], flags0 uint8 [M*2S], lists int32 [max(F,r)*M*S], det_slot int32 [M*S], spawned int32
+    [M*S], dropped int64 [M*S])."""
+    n, S = live.shape[0], cams.shape[0]
+    M, num, dev = n // S, ring.shape[1], live.device
+    if (n != M * S or det.shape != (n, 4) or valid.shape != (n,) or init.shape != (n, 12) or prev.shape != (n, 12)
+            or park.shape != (n, 12) or ids.shape != (n,) or misses.shape != (n,) or next_id.shape != (1,)
+            or ring.shape != (n, num, 8, 2) or count.shape != (n,)):
+        raise ValueError(f'instances_associate: inconsistent shapes for {n} rows over {S} sequences')
+    work = torch.empty(2 * n, 12, device=dev, dtype=torch.float64)
+    flags0 = torch.empty(2 * n, device=dev, dtype=torch.uint8)
+    lists = torch.empty(max(F, r) * n, device=dev, dtype=torch.int32)
+    det_slot, spawned = torch.empty(n, device=dev, dtype=torch.int32), torch.empty(n, device=dev, dtype=torch.int32)
+    dropped = torch.empty(n, device=dev, dtype=torch.int64)
+    cx, cy, cz = (float(c) for c in center)
+    _call('g6d_instances_associate', S, M, int(F), int(r), _p(det), _p(valid, torch.int32), _p(init, torch.float64),
+          _p(cams, torch.float64), cx, cy, cz, float(ref_resolution), float(gate), int(max_misses), _p(prev, torch.float64),
+          _p(live, torch.int32), _p(ids, torch.int64), _p(misses, torch.int32), _p(next_id, torch.int64), _p(park, torch.float64),
+          _p(ring), _p(count, torch.int32), num, _p(work, torch.float64), _p(flags0, torch.uint8), _p(lists, torch.int32),
+          _p(det_slot, torch.int32), _p(spawned, torch.int32), _p(dropped, torch.int64), _stream())
+    return work, flags0, lists, det_slot, spawned, dropped
+
+
 def imagenet_norm(x, out_c=4):
     out = torch.empty(*x.shape[:-1], out_c, device=x.device, dtype=torch.float32)
     _call('g6d_imagenet_norm', _p(x), _p(out), x.numel() // x.shape[-1], x.shape[-1], out_c, _stream())

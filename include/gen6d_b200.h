@@ -187,6 +187,38 @@ int g6d_track_smooth_objects(const double* poses, int poses_are_f32, const float
 int g6d_track_smooth_objects_host(const double* poses, int poses_are_f32, const float* bboxes, int n_obj, int rows_per_obj,
                                   const double* Ks, float* ring, int* count, int num, const double* weights, double* smoothed,
                                   double* avg_pts);
+/* ---- the re-detection step of the multi-instance tracker (gen6d_b200/instance_track.py): M slots per sequence, rows
+ * instance-major (row m*S + s is slot m of sequence s; 1 <= M <= G6D_DET_MAX_INSTANCES).  Per sequence s:
+ *  1. the track point of each live slot: the object centre (cx, cy, cz) projected with prev[row] [12] and cams[s].K in
+ *     fp64, p_i = ((P[i,0]*cx + P[i,1]*cy) + P[i,2]*cz) + P[i,3], q_j = (K[j,0]*p_0 + K[j,1]*p_1) + K[j,2]*p_2,
+ *     u = (q_0/q_2, q_1/q_2); cost(t, d) = sqrt(dx*dx + dy*dy) / (ref_resolution * scale_d), (dx, dy) = u - (x_d, y_d)
+ *     from det [M*S,4] (x, y, scale, score), for valid detections (valid [M*S]) only; a track with q_2 <= 0 has no pair.
+ *  2. greedy matching: repeatedly the pair with cost < gate of smallest cost, ties to the lower slot, then the lower
+ *     detection; both leave the pool.
+ *  3. a matched track keeps its id and pose, misses = 0; an unmatched one takes a miss and is dropped (live 0, id -1,
+ *     dropped[row] = its id) when misses > max_misses.  Unmatched valid detections, in index order, take the lowest
+ *     empty slots (det_slot [M*S]: the slot detection d went to, -1 if matched to none and discarded, or invalid);
+ *     spawned [M*S] marks them, their ring rows ([M*S,num,8,2]) and count are zeroed, and they get the ids *next_id,
+ *     *next_id + 1, ... in ascending (sequence, detection) order (the counter [1] is advanced).
+ *  4. every empty slot parks on detection row m of its frame: park[row] = init[row] ([M*S,12], the detections' initial
+ *     poses).
+ *  5. the chain: work [M*2S,12] holds per slot m the S real rows m*2S + s, then S scratch copies m*2S + S + s; a
+ *     continuing track starts from prev (flags0 = 1: float32 values), a spawned one from its detection's initial pose
+ *     and an empty slot from its parking pose (flags0 = 0).  Continuing tracks run r refinements, the others F; lists
+ *     [max(F,r)*M*S] int32 hold each iteration's M*S rows (entry it*M*S + m*S + s), a row whose chain is complete
+ *     replaced by its scratch row.
+ * live, ids, misses and park are updated in place.  The device call is one CTA (one thread per sequence, a block scan for
+ * the ids): no workspace, no synchronisation, deterministic.  The *_host variant runs the same per-sequence code. */
+int g6d_instances_associate(int S, int M, int F, int r, const float* det, const int* valid, const double* init,
+                            const g6d_glue_camera* cams, double cx, double cy, double cz, double ref_resolution, double gate,
+                            int max_misses, const double* prev, int* live, long long* ids, int* misses, long long* next_id,
+                            double* park, float* ring, int* count, int num, double* work, uint8_t* flags0, int* lists,
+                            int* det_slot, int* spawned, long long* dropped, g6d_stream_t stream);
+int g6d_instances_associate_host(int S, int M, int F, int r, const float* det, const int* valid, const double* init,
+                                 const g6d_glue_camera* cams, double cx, double cy, double cz, double ref_resolution, double gate,
+                                 int max_misses, const double* prev, int* live, long long* ids, int* misses, long long* next_id,
+                                 double* park, float* ring, int* count, int num, double* work, uint8_t* flags0, int* lists,
+                                 int* det_slot, int* spawned, long long* dropped);
 /* (x - mean) / std on f32 [n_pixels, in_c] -> [n_pixels, out_c] (in_c, out_c in {3,4})
  * (network/detector.py:189, selector.py:115, refiner.py:65) */
 int g6d_imagenet_norm(const float* in, float* out, long long n_pixels, int in_c, int out_c, g6d_stream_t stream);
