@@ -1,9 +1,14 @@
-// Track/detection association of the multi-instance tracker (gen6d_b200/instance_track.py) as __host__ __device__ code:
-// per sequence, greedy matching of the live tracks to the re-detected instances, the update of the slot state and the
-// set-up of the step's refinement chain (working poses, first-iteration dtype flags, per-iteration row lists).  track.cu
-// runs it inside the re-detection step's graph, one thread per sequence of one CTA followed by a block scan that numbers
-// the new tracks; its *_host entry point runs the very same per-sequence code on host memory, so the CPU tests pin it
-// against a numpy restatement.  The translation unit is compiled with -fmad=false: products and sums round separately.
+// Track/detection association of the multi-instance trackers (gen6d_b200/instance_track.py) as __host__ __device__ code:
+// per (sequence, object) pair, greedy matching of the pair's live tracks to its re-detected instances, the update of the
+// slot state and the set-up of the step's refinement chain (working poses, first-iteration dtype flags, per-iteration row
+// lists).  track.cu runs it inside the re-detection step's graph, one thread per pair of one CTA followed by a block scan
+// that numbers the new tracks; its *_host entry points run the very same per-pair code on host memory, so the CPU tests
+// pin it against a numpy restatement.  The translation unit is compiled with -fmad=false: products and sums round
+// separately.
+//
+// Layout: K objects with M instance slots each over S sequences; slot group g = m*K + o is instance slot m of object o,
+// and row g*S + s is that slot on sequence s.  A single object (g6d_instances_associate) is K = 1, where g = m and every
+// row index, work row and id is the one of the single-object layout.
 #pragma once
 #include <math.h>
 #include <stdint.h>
@@ -16,26 +21,27 @@ namespace assoc {
 constexpr int kMaxSlots = 16;      // G6D_DET_MAX_INSTANCES
 
 struct Args {
-    int S, M, F, r, num, max_misses;
-    const float* det;              // [M*S,4] x, y, scale, score (instance-major: row m*S + s)
-    const int* valid;              // [M*S]
-    const double* init;            // [M*S,12] initial poses of the detections
+    int S, K, M, F, r, num, max_misses;
+    const float* det;              // [M*K*S,4] x, y, scale, score (row g*S + s, g = m*K + o)
+    const int* valid;              // [M*K*S]
+    const double* init;            // [M*K*S,12] initial poses of the detections
     const double* cams;            // [S,20] g6d_glue_camera (K first)
-    double cx, cy, cz;             // object centre
+    const double* centers;         // [K,3] the objects' centres, or null: center1 for the single object
+    double center1[3];
     double ref_resolution, gate;
-    const double* prev;            // [M*S,12] the slots' previous poses
-    int* live;                     // [M*S] in place
-    long long* ids;                // [M*S] in place (-1: empty)
-    int* misses;                   // [M*S] in place
-    double* park;                  // [M*S,12] in place
-    float* ring;                   // [M*S,num,8,2]: zeroed for spawned slots
-    int* count;                    // [M*S]
-    double* work;                  // [M*2S,12] out: per slot m, S real rows then S scratch rows
-    uint8_t* flags0;               // [M*2S] out
-    int* lists;                    // [max(F,r)*M*S] out
-    int* det_slot;                 // [M*S] out
-    int* spawned;                  // [M*S] out
-    long long* dropped;            // [M*S] out
+    const double* prev;            // [M*K*S,12] the slots' previous poses
+    int* live;                     // [M*K*S] in place
+    long long* ids;                // [M*K*S] in place (-1: empty)
+    int* misses;                   // [M*K*S] in place
+    double* park;                  // [M*K*S,12] in place
+    float* ring;                   // [M*K*S,num,8,2]: zeroed for spawned slots
+    int* count;                    // [M*K*S]
+    double* work;                  // [M*K*2S,12] out: per slot group g, S real rows g*2S + s then S scratch rows
+    uint8_t* flags0;               // [M*K*2S] out
+    int* lists;                    // [max(F,r)*M*K*S] out: entry (it*M*K + g)*S + s
+    int* det_slot;                 // [M*K*S] out
+    int* spawned;                  // [M*K*S] out
+    long long* dropped;            // [M*K*S] out
 };
 
 // The object centre projected with a track's previous pose and the frame's K, in fp64 and in this order:
@@ -61,15 +67,20 @@ G6D_HD void copy12(double* dst, const double* src) {
     for (int k = 0; k < 12; ++k) dst[k] = src[k];
 }
 
-// Everything of sequence s except the new tracks' ids; returns the number of tracks it spawns.
-G6D_HD int associate_sequence(int s, const Args& a) {
+// Everything of sequence s and object o except the new tracks' ids; returns the number of tracks it spawns.  The pair's
+// slot t is row base + t*stride (base = o*S + s, stride = K*S: slot group g = t*K + o) and matches only its object's
+// detection rows, with its object's centre.
+G6D_HD int associate_sequence(int s, int o, const Args& a) {
     const int S = a.S, M = a.M;
+    const long long base = (long long)o * S + s, stride = (long long)a.K * S;
     const double* K = a.cams + (long long)s * 20;
+    const double* c = a.centers ? a.centers + (long long)o * 3 : a.center1;
+    const double cx = c[0], cy = c[1], cz = c[2];
     double u[kMaxSlots], v[kMaxSlots];
     bool ok[kMaxSlots];
     for (int t = 0; t < M; ++t) {
-        const long long i = (long long)t * S + s;
-        ok[t] = a.live[i] && track_point(a.prev + i * 12, K, a.cx, a.cy, a.cz, &u[t], &v[t]);
+        const long long i = base + t * stride;
+        ok[t] = a.live[i] && track_point(a.prev + i * 12, K, cx, cy, cz, &u[t], &v[t]);
     }
     // greedy matching: repeatedly the admissible pair (cost < gate) of smallest cost, ties to the lower slot, then the
     // lower detection (the scan order with a strict comparison)
@@ -81,10 +92,10 @@ G6D_HD int associate_sequence(int s, const Args& a) {
         for (int t = 0; t < M; ++t) {
             if (!ok[t] || match[t] >= 0) continue;
             for (int d = 0; d < M; ++d) {
-                const long long j = (long long)d * S + s;
+                const long long j = base + d * stride;
                 if (!a.valid[j] || det_of[d] >= 0) continue;
-                const double c = pair_cost(u[t], v[t], a.det + j * 4, a.ref_resolution);
-                if (c < a.gate && (bt < 0 || c < bc)) { bt = t; bd = d; bc = c; }
+                const double cost = pair_cost(u[t], v[t], a.det + j * 4, a.ref_resolution);
+                if (cost < a.gate && (bt < 0 || cost < bc)) { bt = t; bd = d; bc = cost; }
             }
         }
         if (bt < 0) break;
@@ -95,7 +106,7 @@ G6D_HD int associate_sequence(int s, const Args& a) {
     int chain[kMaxSlots];
     bool is_new[kMaxSlots];
     for (int t = 0; t < M; ++t) {
-        const long long i = (long long)t * S + s;
+        const long long i = base + t * stride;
         a.dropped[i] = -1;
         is_new[t] = false;
         if (!a.live[i]) continue;
@@ -108,28 +119,30 @@ G6D_HD int associate_sequence(int s, const Args& a) {
             a.misses[i] = 0;
         }
     }
+    // work row of slot t: its group's S real rows, then S scratch rows
+    auto real_row = [&](int t) { return (long long)(t * a.K + o) * 2 * S + s; };
     // unmatched valid detections, in peak order, take the lowest empty slots
     int n_new = 0, t_free = 0;
     for (int d = 0; d < M; ++d) {
-        const long long j = (long long)d * S + s;
+        const long long j = base + d * stride;
         if (!a.valid[j]) { a.det_slot[j] = -1; continue; }
         if (det_of[d] >= 0) { a.det_slot[j] = det_of[d]; continue; }
-        while (t_free < M && a.live[(long long)t_free * S + s]) ++t_free;
+        while (t_free < M && a.live[base + t_free * stride]) ++t_free;
         if (t_free == M) { a.det_slot[j] = -1; continue; }
-        const long long i = (long long)t_free * S + s;
+        const long long i = base + t_free * stride;
         a.det_slot[j] = t_free;
         a.live[i] = 1;
         a.misses[i] = 0;
         is_new[t_free] = true;
         det_of[d] = t_free;
-        copy12(a.work + ((long long)t_free * 2 * S + s) * 12, a.init + j * 12);    // the track's start: its detection's pose
+        copy12(a.work + real_row(t_free) * 12, a.init + j * 12);           // the track's start: its detection's pose
         for (long long k = 0; k < (long long)a.num * 16; ++k) a.ring[i * a.num * 16 + k] = 0.f;
         a.count[i] = 0;
         ++n_new;
     }
     // every slot's start, first-iteration flag and chain length; empty slots park on detection row t of the frame
     for (int t = 0; t < M; ++t) {
-        const long long i = (long long)t * S + s, real = (long long)t * 2 * S + s;
+        const long long i = base + t * stride, real = real_row(t);
         a.spawned[i] = is_new[t];
         if (!a.live[i]) {
             copy12(a.park + i * 12, a.init + i * 12);
@@ -145,7 +158,7 @@ G6D_HD int associate_sequence(int s, const Args& a) {
     const int n_it = a.F > a.r ? a.F : a.r;
     for (int it = 0; it < n_it; ++it)
         for (int t = 0; t < M; ++t)
-            a.lists[((long long)it * M + t) * S + s] = t * 2 * S + s + (it < chain[t] ? 0 : S);
+            a.lists[(long long)it * M * stride + base + t * stride] = (int)real_row(t) + (it < chain[t] ? 0 : S);
     return n_new;
 }
 

@@ -32,24 +32,27 @@ __global__ void __launch_bounds__(32) track_smooth_objects_kernel(const double* 
     if (i < n_rows) smooth_row_objects(i, rows_per_obj, poses, in_f32, bboxes, Ks, ring, count, num, weights, smoothed, avg_pts);
 }
 
-// Association of the multi-instance tracker (instance_track_math.cuh): ONE CTA.  Phase 1 runs one thread per sequence;
-// phase 2 numbers the spawned tracks in ascending (sequence, slot) order -- which is (sequence, detection) order, since a
-// sequence's unmatched detections take its empty slots in ascending order -- by an exclusive block scan of the
-// sequences' spawn counts, chunk by chunk; thread 0 then advances the counter.
+// Association of the multi-instance trackers (instance_track_math.cuh): ONE CTA.  Phase 1 runs one thread per
+// (sequence, object) pair, pairs object-major (pair p = o*S + s); phase 2 numbers the spawned tracks in ascending
+// (object, sequence, slot) order -- which is (object, sequence, detection) order, since a pair's unmatched detections take
+// its empty slots in ascending order -- by an exclusive block scan of the pairs' spawn counts, chunk by chunk; thread 0
+// then advances the counter.  Pair p's slot t is row p + t*K*S.
 constexpr int kAssocThreads = 256;
 
 __global__ void __launch_bounds__(kAssocThreads) instances_associate_kernel(assoc::Args a, long long* next_id) {
     __shared__ int s_warp[kAssocThreads / 32];
     __shared__ long long s_base;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    for (int s = tid; s < a.S; s += kAssocThreads) assoc::associate_sequence(s, a);
+    const int P = a.K * a.S;
+    const long long stride = (long long)a.K * a.S;
+    for (int p = tid; p < P; p += kAssocThreads) assoc::associate_sequence(p % a.S, p / a.S, a);
     if (tid == 0) s_base = *next_id;
     __syncthreads();
-    for (int s0 = 0; s0 < a.S; s0 += kAssocThreads) {
-        const int s = s0 + tid;
+    for (int p0 = 0; p0 < P; p0 += kAssocThreads) {
+        const int p = p0 + tid;
         int n = 0;
-        if (s < a.S)
-            for (int m = 0; m < a.M; ++m) n += a.spawned[(long long)m * a.S + s];
+        if (p < P)
+            for (int m = 0; m < a.M; ++m) n += a.spawned[p + m * stride];
         int incl = n;
         for (int o = 1; o < 32; o <<= 1) {
             const int x = __shfl_up_sync(0xffffffffu, incl, o);
@@ -63,9 +66,9 @@ __global__ void __launch_bounds__(kAssocThreads) instances_associate_kernel(asso
             total += s_warp[w];
         }
         long long id = s_base + before + incl - n;
-        if (s < a.S)
+        if (p < P)
             for (int m = 0; m < a.M; ++m) {
-                const long long i = (long long)m * a.S + s;
+                const long long i = p + m * stride;
                 if (a.spawned[i]) a.ids[i] = id++;
             }
         __syncthreads();
@@ -78,12 +81,30 @@ __global__ void __launch_bounds__(kAssocThreads) instances_associate_kernel(asso
 static int associate_ok(const char* name, const assoc::Args& a, const long long* next_id) {
     G6D_REQUIRE(a.S >= 1 && a.M >= 1 && a.M <= assoc::kMaxSlots, "%s: need S >= 1 and 1 <= M <= %d (got S=%d, M=%d)", name,
                 assoc::kMaxSlots, a.S, a.M);
+    G6D_REQUIRE(a.K >= 1 && (long long)a.K * a.S * a.M * 2 <= 0x7fffffffLL, "%s: need K >= 1 and 2*M*K*S rows within int (got K=%d)",
+                name, a.K);
     G6D_REQUIRE(a.F >= 0 && a.r >= 0 && (a.F > 0 || a.r > 0) && a.num >= 1 && a.max_misses >= 0,
                 "%s: need F, r >= 0 with max(F, r) >= 1, num >= 1 and max_misses >= 0 (got F=%d, r=%d, num=%d, max_misses=%d)", name,
                 a.F, a.r, a.num, a.max_misses);
     G6D_REQUIRE(a.gate > 0. && a.gate < INFINITY && a.ref_resolution > 0., "%s: need a finite gate > 0 and ref_resolution > 0", name);
     G6D_REQUIRE(a.det && a.valid && a.init && a.cams && a.prev && a.live && a.ids && a.misses && a.park && a.ring && a.count && a.work &&
                 a.flags0 && a.lists && a.det_slot && a.spawned && a.dropped && next_id, "%s: null pointer", name);
+    return G6D_OK;
+}
+
+static void associate_host(const assoc::Args& a, long long* next_id) {
+    const long long stride = (long long)a.K * a.S;
+    for (int p = 0; p < a.K * a.S; ++p) assoc::associate_sequence(p % a.S, p / a.S, a);
+    for (int p = 0; p < a.K * a.S; ++p)
+        for (int m = 0; m < a.M; ++m)
+            if (a.spawned[p + m * stride]) a.ids[p + m * stride] = (*next_id)++;
+}
+
+static int associate_launch(const char* name, const assoc::Args& a, long long* next_id, g6d_stream_t stream) {
+    const int rc = associate_ok(name, a, next_id);
+    if (rc != G6D_OK) return rc;
+    instances_associate_kernel<<<1, kAssocThreads, 0, as_stream(stream)>>>(a, next_id);
+    G6D_CHECK_LAUNCH(name);
     return G6D_OK;
 }
 
@@ -96,13 +117,9 @@ extern "C" int g6d_instances_associate(int S, int M, int F, int r, const float* 
                                        int max_misses, const double* prev, int* live, long long* ids, int* misses, long long* next_id,
                                        double* park, float* ring, int* count, int num, double* work, uint8_t* flags0, int* lists,
                                        int* det_slot, int* spawned, long long* dropped, g6d_stream_t stream) {
-    const assoc::Args a{S, M, F, r, num, max_misses, det, valid, init, reinterpret_cast<const double*>(cams), cx, cy, cz, ref_resolution,
-                        gate, prev, live, ids, misses, park, ring, count, work, flags0, lists, det_slot, spawned, dropped};
-    const int rc = associate_ok("g6d_instances_associate", a, next_id);
-    if (rc != G6D_OK) return rc;
-    instances_associate_kernel<<<1, kAssocThreads, 0, as_stream(stream)>>>(a, next_id);
-    G6D_CHECK_LAUNCH("g6d_instances_associate");
-    return G6D_OK;
+    const assoc::Args a{S, 1, M, F, r, num, max_misses, det, valid, init, reinterpret_cast<const double*>(cams), nullptr, {cx, cy, cz},
+                        ref_resolution, gate, prev, live, ids, misses, park, ring, count, work, flags0, lists, det_slot, spawned, dropped};
+    return associate_launch("g6d_instances_associate", a, next_id, stream);
 }
 
 extern "C" int g6d_instances_associate_host(int S, int M, int F, int r, const float* det, const int* valid, const double* init,
@@ -110,14 +127,38 @@ extern "C" int g6d_instances_associate_host(int S, int M, int F, int r, const fl
                                             double gate, int max_misses, const double* prev, int* live, long long* ids, int* misses,
                                             long long* next_id, double* park, float* ring, int* count, int num, double* work,
                                             uint8_t* flags0, int* lists, int* det_slot, int* spawned, long long* dropped) {
-    const assoc::Args a{S, M, F, r, num, max_misses, det, valid, init, reinterpret_cast<const double*>(cams), cx, cy, cz, ref_resolution,
-                        gate, prev, live, ids, misses, park, ring, count, work, flags0, lists, det_slot, spawned, dropped};
+    const assoc::Args a{S, 1, M, F, r, num, max_misses, det, valid, init, reinterpret_cast<const double*>(cams), nullptr, {cx, cy, cz},
+                        ref_resolution, gate, prev, live, ids, misses, park, ring, count, work, flags0, lists, det_slot, spawned, dropped};
     const int rc = associate_ok("g6d_instances_associate_host", a, next_id);
     if (rc != G6D_OK) return rc;
-    for (int s = 0; s < S; ++s) assoc::associate_sequence(s, a);
-    for (int s = 0; s < S; ++s)
-        for (int m = 0; m < M; ++m)
-            if (spawned[(long long)m * S + s]) ids[(long long)m * S + s] = (*next_id)++;
+    associate_host(a, next_id);
+    return G6D_OK;
+}
+
+extern "C" int g6d_instances_associate_objects(int S, int K, int M, int F, int r, const float* det, const int* valid, const double* init,
+                                               const g6d_glue_camera* cams, const double* centers, double ref_resolution, double gate,
+                                               int max_misses, const double* prev, int* live, long long* ids, int* misses,
+                                               long long* next_id, double* park, float* ring, int* count, int num, double* work,
+                                               uint8_t* flags0, int* lists, int* det_slot, int* spawned, long long* dropped,
+                                               g6d_stream_t stream) {
+    G6D_REQUIRE(centers, "g6d_instances_associate_objects: null pointer (centers)");
+    const assoc::Args a{S, K, M, F, r, num, max_misses, det, valid, init, reinterpret_cast<const double*>(cams), centers, {0., 0., 0.},
+                        ref_resolution, gate, prev, live, ids, misses, park, ring, count, work, flags0, lists, det_slot, spawned, dropped};
+    return associate_launch("g6d_instances_associate_objects", a, next_id, stream);
+}
+
+extern "C" int g6d_instances_associate_objects_host(int S, int K, int M, int F, int r, const float* det, const int* valid,
+                                                    const double* init, const g6d_glue_camera* cams, const double* centers,
+                                                    double ref_resolution, double gate, int max_misses, const double* prev, int* live,
+                                                    long long* ids, int* misses, long long* next_id, double* park, float* ring, int* count,
+                                                    int num, double* work, uint8_t* flags0, int* lists, int* det_slot, int* spawned,
+                                                    long long* dropped) {
+    G6D_REQUIRE(centers, "g6d_instances_associate_objects_host: null pointer (centers)");
+    const assoc::Args a{S, K, M, F, r, num, max_misses, det, valid, init, reinterpret_cast<const double*>(cams), centers, {0., 0., 0.},
+                        ref_resolution, gate, prev, live, ids, misses, park, ring, count, work, flags0, lists, det_slot, spawned, dropped};
+    const int rc = associate_ok("g6d_instances_associate_objects_host", a, next_id);
+    if (rc != G6D_OK) return rc;
+    associate_host(a, next_id);
     return G6D_OK;
 }
 

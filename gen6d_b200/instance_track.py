@@ -18,6 +18,12 @@ and one read (instances.pack):
 
 Both finish with predict.py's smoothing, slots standing in for the objects of g6d_track_smooth_objects.  Shapes are
 fixed, so empty slots are computed too; their results come back as NaN.  The slot state stays on the device.
+
+ObjectInstanceTracker (ObjectSet.instance_tracker()) does the same for every object of an object set at once: slot group
+g = m*K + o is instance slot m of object o (row g*S + s, the layout of ObjectSet.predict_instances' slots), the
+re-detection step runs the set's shared pyramid and correlation and g6d_instances_associate_objects (each object's
+tracks matched against its own peaks, one id counter), and every refinement iteration is still ONE refiner stage over
+all M*K*S poses.  Both trackers are the class below, parameterised by the per-group tables and the detection.
 """
 import numpy as np
 import torch
@@ -27,7 +33,7 @@ from . import glue
 from . import instances
 from . import ops
 from .graphs import StageCache
-from .track import _sequences, check_bbox, object_bbox, smoothing_weights
+from .track import _sequences, check_bbox, object_bbox, object_bboxes, smoothing_weights
 
 
 def host_associate(det, valid, init, cams, center, ref_resolution, gate, max_misses, F, r, prev, live, ids, misses, next_id,
@@ -56,6 +62,32 @@ def host_associate(det, valid, init, cams, center, ref_resolution, gate, max_mis
     return work, flags0, lists, det_slot, spawned, dropped
 
 
+def host_associate_objects(det, valid, init, cams, centers, ref_resolution, gate, max_misses, F, r, prev, live, ids, misses,
+                           next_id, park, ring, count):
+    """g6d_instances_associate_objects_host on numpy arrays (the shapes and dtypes of ops.instances_associate_objects;
+    centers float64 [K,3], cams float64 [S,20]).  live, ids, misses, next_id, park, ring and count are updated in place.
+    Returns (work, flags0, lists, det_slot, spawned, dropped) as numpy arrays."""
+    c = lambda a, dt: np.ascontiguousarray(a, dt)
+    centers = c(centers, np.float64).reshape(-1, 3)
+    n, S, K = len(live), len(cams), len(centers)
+    M, num = n // max(K * S, 1), ring.shape[1]
+    for a, dt in ((live, np.int32), (ids, np.int64), (misses, np.int32), (next_id, np.int64), (park, np.float64),
+                  (ring, np.float32), (count, np.int32)):
+        if a.dtype != dt or not a.flags.c_contiguous:
+            raise ValueError(f'host_associate_objects: the state arrays must be contiguous {dt.__name__} arrays (updated in place)')
+    det, valid, init, cams, prev = c(det, np.float32), c(valid, np.int32), c(init, np.float64), c(cams, np.float64), c(prev, np.float64)
+    work, flags0 = np.zeros((2 * n, 12)), np.zeros(2 * n, np.uint8)
+    lists = np.zeros(max(F, r) * n, np.int32)
+    det_slot, spawned, dropped = np.zeros(n, np.int32), np.zeros(n, np.int32), np.zeros(n, np.int64)
+    _lib.check(_lib.lib().g6d_instances_associate_objects_host(
+        S, K, M, int(F), int(r), det.ctypes.data, valid.ctypes.data, init.ctypes.data, cams.ctypes.data, centers.ctypes.data,
+        float(ref_resolution), float(gate), int(max_misses), prev.ctypes.data, live.ctypes.data, ids.ctypes.data,
+        misses.ctypes.data, next_id.ctypes.data, park.ctypes.data, ring.ctypes.data, count.ctypes.data, num,
+        work.ctypes.data, flags0.ctypes.data, lists.ctypes.data, det_slot.ctypes.data, spawned.ctypes.data,
+        dropped.ctypes.data), 'g6d_instances_associate_objects_host')
+    return work, flags0, lists, det_slot, spawned, dropped
+
+
 def check_args(num_sequences, max_instances, refine_iter, redetect_every, gate, max_misses, min_score, nms_iou, peak_radius,
                smooth_num, smooth_std):
     """-> the detection key of instances.check_args; ValueError for a bad argument."""
@@ -78,31 +110,39 @@ def check_args(num_sequences, max_instances, refine_iter, redetect_every, gate, 
 
 
 class InstanceTracker:
-    """Every instance of the estimator's object tracked through S sequences in lockstep; see Gen6DEstimator.instance_tracker()."""
+    """Every instance of the estimator's object tracked through S sequences in lockstep; see Gen6DEstimator.instance_tracker().
+
+    The state, the two graph bodies, reset and the decode are written for K objects with M slots each (K = 1 here); a
+    subclass supplies the per-group tables (_groups), the detection (_detection), the id association (_associate) and the
+    readback of the selections (_take_selections)."""
 
     def __init__(self, est, num_sequences, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
                  min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bbox_3d=None):
         from .objects import require_device_pipeline
         require_device_pipeline(est, 'instance tracking')
-        self.key = check_args(num_sequences, max_instances, refine_iter, redetect_every, gate, max_misses, min_score, nms_iou,
-                              peak_radius, smooth_num, smooth_std)
+        key = check_args(num_sequences, max_instances, refine_iter, redetect_every, gate, max_misses, min_score, nms_iou,
+                         peak_radius, smooth_num, smooth_std)
         if bbox_3d is None:
             bbox_3d = object_bbox(est.refiner.ref_database)
             if bbox_3d is None:
                 raise ValueError('the database has no object point cloud: pass bbox_3d (the 8 corners of the object box)')
-        self.est = est
-        self.S, self.M, self.refine_iter = int(num_sequences), self.key[0], int(refine_iter)
+        self.bbox = check_bbox(bbox_3d)
+        self._gen = est._generation()
+        self._setup(est, key, [self.bbox], num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std)
+
+    def _setup(self, est, key, boxes, num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std):
+        """The tracker's constants and device state for K = len(boxes) objects with M = key[0] slots each."""
+        self.est, self.key = est, key
+        self.K, self.S, self.M, self.refine_iter = len(boxes), int(num_sequences), key[0], int(refine_iter)
         self.redetect_every = None if redetect_every is None else int(redetect_every)
         self.gate, self.max_misses = float(gate), int(max_misses)
         self.num, self.std = int(smooth_num), float(smooth_std)
-        self.bbox = check_bbox(bbox_3d)
         self.weights = smoothing_weights(self.num, self.std)
-        self._gen = est._generation()
         self.stages = StageCache()       # the detect and refine graphs (they capture this tracker's device state)
         dev = est.detector.device
-        self._dev = {'bboxes': torch.from_numpy(np.ascontiguousarray(np.repeat(self.bbox[None], self.M, 0))).to(dev),
-                     'weights': torch.from_numpy(self.weights.copy()).to(dev)}
-        n = self.M * self.S
+        groups = np.ascontiguousarray(np.tile(np.stack(boxes, 0), (self.M, 1, 1)))       # group m*K + o smooths with box o
+        self._dev = {'bboxes': torch.from_numpy(groups).to(dev), 'weights': torch.from_numpy(self.weights.copy()).to(dev)}
+        n = self.M * self.K * self.S
         self._next_id = torch.zeros(1, dtype=torch.int64, device=dev)     # ids are unique over the tracker's life
         self._state = {'prev': torch.zeros(n, 12, dtype=torch.float64, device=dev),
                        'park': torch.zeros(n, 12, dtype=torch.float64, device=dev),
@@ -121,7 +161,7 @@ class InstanceTracker:
             rows = slice(None)
         else:
             seqs = _sequences(self.S, sequences)
-            rows = torch.from_numpy(np.concatenate([m * self.S + seqs for m in range(self.M)])).to(st['live'].device)
+            rows = torch.from_numpy(np.concatenate([g * self.S + seqs for g in range(self.M * self.K)])).to(st['live'].device)
         st['live'][rows] = 0
         st['ids'][rows] = -1
         st['misses'][rows] = 0
@@ -141,47 +181,73 @@ class InstanceTracker:
     def _detecting(self):
         return self._pending or (self.redetect_every is not None and self._since >= self.redetect_every)
 
+    # -------------------------------------------------------------- what differs between the estimator and an object set
+    def _tables(self):
+        return self.est._glue_state()
+
+    def _groups(self, st):
+        """-> (the refiner's view table of every slot group, the reference views per table)."""
+        return [st['views']] * self.M, st['tables']['ref_num']
+
+    def _detection(self, st):
+        """-> fn(frames, cams) -> (initial poses [n,12], det [n,4], crops, the selections' tensors in packing order, valid
+        int32 [n], instance count int32 [K*S]): predict_instances' detection half on the S frames."""
+        detect, extra = self.est._peaks_detect_fn(*self.key)
+        initial = self.est._initial_poses_device_fn(st, detect)
+
+        def fn(frames, cams):
+            init, det, crop, idx, sel_out, logits = initial(frames, cams)
+            return (init, det, crop, [idx, sel_out, logits], *extra)
+        return fn
+
+    def _associate(self):
+        center = [float(v) for v in np.asarray(self.est.ref_info['center']).reshape(3)]
+        return lambda det, valid, init, cams, *state: ops.instances_associate(
+            det, valid, init, cams, center, float(self.est.cfg['ref_resolution']), self.gate, self.max_misses,
+            self.est.cfg['refine_iter'], self.refine_iter, *state)
+
+    def _take_selections(self, rd):
+        """-> per object (sel_idx [M*S], sel_out [M*S*2], logits [M*S*n_sel]) instance-major, read in packing order."""
+        n = self.M * self.S
+        return [(rd.take(n), rd.take(n * 2), rd.take(n * len(self.est.ref_info['poses'])))]
+
     # -------------------------------------------------------------- the graphs
     def _detect_fn(self, st):
-        est, M, S, r = self.est, self.M, self.S, self.refine_iter
-        F, R, c = est.cfg['refine_iter'], st['tables']['ref_num'], self._dev
-        detect, extra = est._peaks_detect_fn(*self.key)
-        initial, refine = est._initial_poses_device_fn(st, detect), est.refiner._refine_warped(128)
-        views, center = [st['views']] * M, [float(v) for v in np.asarray(est.ref_info['center']).reshape(3)]
-        res = float(est.cfg['ref_resolution'])
+        est, G, S, r = self.est, self.M * self.K, self.S, self.refine_iter
+        F, c, n = est.cfg['refine_iter'], self._dev, self.M * self.K * self.S
+        views, R = self._groups(st)
+        initial, associate, refine = self._detection(st), self._associate(), est.refiner._refine_warped(128)
 
         def fn(frames, cams, prev, park, live, ids, misses, next_id, ring, count):
-            init, det, crop, idx, sel_out, logits = initial(frames, cams)
-            valid, inst_count = extra
-            work, flags0, lists, det_slot, spawned, dropped = ops.instances_associate(
-                det, valid, init, cams, center, res, self.gate, self.max_misses, F, r, prev, live, ids, misses, next_id, park,
-                ring, count)
+            init, det, crop, sels, valid, inst_count = initial(frames, cams)
+            work, flags0, lists, det_slot, spawned, dropped = associate(det, valid, init, cams, prev, live, ids, misses, next_id,
+                                                                        park, ring, count)
             frames_x, cams_x = torch.cat([frames, frames], 0), torch.cat([cams, cams], 0)
-            real = lambda: work.view(M, 2 * S, 12)[:, :S].reshape(M * S, 12).clone()
+            real = lambda: work.view(G, 2 * S, 12)[:, :S].reshape(n, 12).clone()
             ones, chain = torch.ones_like(flags0), [real()]
             for it in range(max(F, r)):
-                rows = lists[it * M * S:(it + 1) * M * S]
+                rows = lists[it * n:(it + 1) * n]
                 jobs, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems_rows(
                     views, R, 2 * S, cams_x, frames_x, work, rows, flags0 if it == 0 else ones)
-                out = refine(jobs, que_K, que_pose, ref_Ks, ref_poses)            # one refiner stage over M*S poses
+                out = refine(jobs, que_K, que_pose, ref_Ks, ref_poses)            # one refiner stage over all n poses
                 ops.glue_apply_refinements_rows(views, 2 * S, que_pose, que_K, rect, out, rows, work)
                 chain.append(real())
             poses = chain[-1]
             smoothed, avg = ops.track_smooth_objects(poses, True, c['bboxes'], cams[:, :9].contiguous(), ring, count, c['weights'])
-            buf = instances.pack([torch.stack(chain, 0), smoothed, avg, ring, count, ids, det, idx, sel_out, logits, valid,
-                                  inst_count, det_slot, spawned, dropped], crop)
+            buf = instances.pack([torch.stack(chain, 0), smoothed, avg, ring, count, ids, det, *sels, valid, inst_count, det_slot,
+                                  spawned, dropped], crop)
             return buf, poses, park, live, ids, misses, next_id, ring, count
         return fn
 
     def _refine_fn(self, st):
-        est, M, S, r, c = self.est, self.M, self.S, self.refine_iter, self._dev
-        R, refine = st['tables']['ref_num'], est.refiner._refine_warped(128)
-        views = [st['views']] * M
+        est, S, r, c, n = self.est, self.S, self.refine_iter, self._dev, self.M * self.K * self.S
+        views, R = self._groups(st)
+        refine = est.refiner._refine_warped(128)
 
         def fn(frames, cams, prev, park, live, ids, ring, count):
             work = torch.where((live != 0)[:, None], prev, park)                 # empty slots restart from their parking pose
             flags0 = live.to(torch.uint8)                                        # tracks hold float32 values, parking poses not
-            rows = torch.arange(M * S, device=live.device, dtype=torch.int32)
+            rows = torch.arange(n, device=live.device, dtype=torch.int32)
             ones, chain = torch.ones_like(flags0), [work.clone()]
             for it in range(r):
                 jobs, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems_rows(
@@ -204,8 +270,12 @@ class InstanceTracker:
         'smoothed_pts' [S,M,8,2].  Empty slots' poses and points are NaN.  A re-detection step adds predict_instances'
         keys led by [S,M], 'det_slot' int64 [S,M] (the slot detection m went to, -1: discarded), 'spawned' bool [S,M]
         (the slots that started a track) and 'dropped' (the ids removed this step, ascending)."""
+        return self._step(frames, Ks)[0]
+
+    def _step(self, frames, Ks):
+        """One step -> the decoded results of every object, in object order."""
         self._check()
-        est, S, M, num = self.est, self.S, self.M, self.num
+        est, S = self.est, self.S
         if len(frames) != S or len(Ks) != S:
             raise ValueError(f'step: this tracker follows {S} sequences, got {len(frames)} frames and {len(Ks)} Ks')
         Ks = np.stack([np.asarray(k) for k in Ks], 0)
@@ -215,7 +285,7 @@ class InstanceTracker:
         F = est.cfg['refine_iter']
         if detecting and F < 1:
             raise ValueError("instance tracking needs cfg['refine_iter'] >= 1 (a re-detection step smooths float32 poses)")
-        stt, x = est._glue_state(), self._state
+        stt, x = self._tables(), self._state
         with torch.no_grad():
             dev_frames = est.detector.upload_frame([np.asarray(f) for f in frames])
             cams = est.detector._to_dev(glue.cameras(Ks))
@@ -239,14 +309,38 @@ class InstanceTracker:
         return self._decode(host, detecting)
 
     def _decode(self, host, detecting):
-        est, S, M, num, n = self.est, self.S, self.M, self.num, self.M * self.S
+        est, S, M, K, num = self.est, self.S, self.M, self.K, self.num
+        n = M * K * S
         n_chain = (max(est.cfg['refine_iter'], self.refine_iter) if detecting else self.refine_iter) + 1
         res = est.cfg['ref_resolution']
         rd = instances.Unpacker(host, n * res * res * 3 if detecting else 0)
         chain = rd.take(n_chain * n * 12).reshape(n_chain, n, 12)
-        smoothed, avg = rd.take(n * 12), rd.take(n * 16)
+        smoothed, avg = rd.take(n * 12).reshape(n, 12), rd.take(n * 16).reshape(n, 16)
         ring_h, count_h = rd.take(n * num * 16).reshape(n, num, 8, 2).astype(np.float32), rd.take(n).astype(np.int64)
-        ids = instances.frame_major(rd.take(n).astype(np.int64), M, S)
+        ids = rd.take(n)
+        if detecting:
+            det, sels = rd.take(n * 4).reshape(n, 4), self._take_selections(rd)
+            valid, inst_count = rd.take(n), rd.take(K * S).reshape(K, S)
+            det_slot, spawned, dropped = rd.take(n), rd.take(n), rd.take(n)
+            crops = rd.crops.reshape(n, res, res, 3)
+
+        obj = lambda a, o: a.reshape(M, K, S, *a.shape[1:])[:, o].reshape(M * S, *a.shape[1:])      # object o, instance-major
+        out = []
+        for o in range(K):
+            c = chain.reshape(n_chain, M, K, S, 12)[:, :, o].reshape(n_chain, M * S, 12)
+            one = [obj(a, o) for a in (smoothed, avg, ring_h, count_h, ids)]
+            det_parts = None
+            if detecting:
+                det_parts = [obj(det, o), *sels[o], obj(valid, o), inst_count[o], obj(crops, o),
+                             *(obj(a, o) for a in (det_slot, spawned, dropped))]
+            out.append(self._decode_object(c, *one, det_parts, o))
+        return out
+
+    def _decode_object(self, chain, smoothed, avg, ring_h, count_h, ids, det_parts, o):
+        """One object's instance-major rows (row m*S + s) -> (poses, smoothed, track_ids, inter) as step() returns them."""
+        S, M = self.S, self.M
+        n = M * S
+        ids = instances.frame_major(ids.astype(np.int64), M, S)
         empty = ids < 0
         fm = lambda a: instances.frame_major(a, M, S)
 
@@ -254,17 +348,75 @@ class InstanceTracker:
             a[empty] = np.nan
             return a
         first = fm(chain[0].reshape(n, 3, 4))
+        detecting = det_parts is not None
         inter = {'refine_poses': [nan(first if detecting else first.astype(np.float32))] +
                                  [nan(fm(c.reshape(n, 3, 4)).astype(np.float32)) for c in chain[1:]],
                  'bbox_pts': nan(fm(ring_h[np.arange(n), count_h - 1])), 'smoothed_pts': nan(fm(avg.reshape(n, 8, 2)))}
         if detecting:
-            n_sel = len(est.ref_info['poses'])
-            parts = [rd.take(n * 4), rd.take(n), rd.take(n * 2), rd.take(n * n_sel), rd.take(n), rd.take(S)]
-            _, det_inter = instances.inter_of(chain[:1], *parts, rd.crops.reshape(n, res, res, 3), M, S)
+            det, idx, sel_out, logits, valid, inst_count, crops, det_slot, spawned, dropped = det_parts
+            _, det_inter = instances.inter_of(chain[:1], det, idx, sel_out, logits, valid, inst_count, crops, M, S)
             det_inter.pop('refine_poses')
             inter.update(det_inter)
-            inter['det_slot'] = fm(rd.take(n).astype(np.int64))
-            inter['spawned'] = fm(rd.take(n).astype(bool))
-            dropped = rd.take(n)
+            inter['det_slot'] = fm(det_slot.astype(np.int64))
+            inter['spawned'] = fm(spawned.astype(bool))
             inter['dropped'] = sorted(int(i) for i in dropped if i >= 0)
         return inter['refine_poses'][-1], nan(fm(smoothed.reshape(n, 3, 4))), ids, inter
+
+
+class ObjectInstanceTracker(InstanceTracker):
+    """Every instance of every object of an ObjectSet tracked through S sequences in lockstep; see
+    ObjectSet.instance_tracker().  Slot group g = m*K + o is instance slot m of object o; row g*S + s is that slot on
+    sequence s.  reset(sequences) drops those sequences' tracks for every object."""
+
+    def __init__(self, objs, num_sequences, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
+                 min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bboxes=None):
+        key = check_args(num_sequences, max_instances, refine_iter, redetect_every, gate, max_misses, min_score, nms_iou,
+                         peak_radius, smooth_num, smooth_std)
+        objs._check()
+        boxes = object_bboxes(objs, bboxes)
+        self.objs, self.names, self.bboxes = objs, objs.names, np.ascontiguousarray(np.stack(boxes, 0))
+        self._membership = objs.membership
+        self._setup(objs.est, key, boxes, num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std)
+        centers = np.stack([np.asarray(ob.ref_info['center'], np.float64).reshape(3) for ob in objs._objects.values()], 0)
+        self._dev['centers'] = torch.from_numpy(np.ascontiguousarray(centers)).to(self.est.detector.device)
+
+    def _check(self):
+        if self.objs.membership != self._membership:
+            raise RuntimeError('this instance tracker is stale: objects were added to or removed from the set since it was '
+                               'created; create a new one with objs.instance_tracker()')
+        self.objs._check()
+
+    def _tables(self):
+        return None
+
+    def _groups(self, st):
+        objs = list(self.objs._objects.values())
+        return [ob.tables['views'] for ob in objs] * self.M, objs[0].tables['tables']['ref_num']
+
+    def _detection(self, st):
+        detect, extra = self.objs._peaks_detect_fn(*self.key)
+        initial = self.objs._initial_poses_device_fn(detect)
+
+        def fn(frames, cams):
+            init, det, sels, crop = initial(frames, cams)
+            return (init, det, crop, [t for sel in sels for t in sel], *extra)
+        return fn
+
+    def _associate(self):
+        centers, est = self._dev['centers'], self.est
+        return lambda det, valid, init, cams, *state: ops.instances_associate_objects(
+            det, valid, init, cams, centers, float(est.cfg['ref_resolution']), self.gate, self.max_misses, est.cfg['refine_iter'],
+            self.refine_iter, *state)
+
+    def _take_selections(self, rd):
+        S, M, K = self.S, self.M, self.K
+        n_sel = [len(ob.ref_info['poses']) for ob in self.objs._objects.values()]
+        slots = [(rd.take(S), rd.take(S * 2), rd.take(S * n_sel[g % K])) for g in range(M * K)]
+        return [tuple(np.concatenate([slots[m * K + o][i] for m in range(M)]) for i in range(3)) for o in range(K)]
+
+    def step(self, frames, Ks):
+        """frames: S uint8 [h,w,3] of one size; Ks: [S,3,3] (shared by all objects).  Returns {name: (poses float32
+        [S,M,3,4], smoothed float64 [S,M,3,4], track_ids int64 [S,M], inter)}: per object what InstanceTracker.step returns,
+        'det_score' included on a re-detection step; 'dropped' lists that object's ids only.  Ids are unique over every
+        object of the tracker."""
+        return dict(zip(self.names, self._step(frames, Ks)))

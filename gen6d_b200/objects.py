@@ -13,7 +13,8 @@ same frames as ONE captured graph with one synchronising read:
 
 Rows are object-major (object, frame) everywhere after the correlation, so each object's detections, crops and poses are
 a contiguous slice whose row i is frame i, which is the layout the g6d_glue_* kernels take.  ObjectSet.tracker() follows
-the set's objects through videos (gen6d_b200/track.py ObjectTracker).
+the set's objects through videos (gen6d_b200/track.py ObjectTracker), ObjectSet.instance_tracker() every instance of
+each (gen6d_b200/instance_track.py ObjectInstanceTracker).
 """
 import numpy as np
 import torch
@@ -312,6 +313,19 @@ class ObjectSet:
         from .track import ObjectTracker
         return ObjectTracker(self, num_sequences, refine_iter=refine_iter, smooth_num=smooth_num, smooth_std=smooth_std,
                              bboxes=bboxes)
+
+    def instance_tracker(self, num_sequences=1, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
+                         min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bboxes=None):
+        """An ObjectInstanceTracker (gen6d_b200/instance_track.py): every instance of every object of the set, up to
+        `max_instances` per object and frame, followed through `num_sequences` videos in lockstep, with
+        Gen6DEstimator.instance_tracker()'s semantics per object (each object's tracks are matched only to its own
+        detections) and track ids unique over the whole tracker.  Re-detection steps share the set's query pyramid and
+        correlation; each step is one captured graph and one synchronising read.  bboxes: as for tracker()."""
+        from .instance_track import ObjectInstanceTracker
+        return ObjectInstanceTracker(self, num_sequences, max_instances=max_instances, refine_iter=refine_iter,
+                                     redetect_every=redetect_every, gate=gate, max_misses=max_misses, min_score=min_score,
+                                     nms_iou=nms_iou, peak_radius=peak_radius, smooth_num=smooth_num, smooth_std=smooth_std,
+                                     bboxes=bboxes)
 
     def raw_correlation(self, que_imgs):
         """The detector's raw correlation maps for inspection: {name: [scale][level] float32 [qn, H, W, rfn]} (the maps

@@ -305,6 +305,33 @@ def instances_associate(det, valid, init, cams, center, ref_resolution, gate, ma
     return work, flags0, lists, det_slot, spawned, dropped
 
 
+def instances_associate_objects(det, valid, init, cams, centers, ref_resolution, gate, max_misses, F, r, prev, live, ids, misses,
+                                next_id, park, ring, count):
+    """instances_associate for the K objects of an object set with M slots each (g6d_instances_associate_objects): slot
+    group g = m*K + o is instance slot m of object o, and row g*S + s is that slot on sequence s.  det float32 [M*K*S,4],
+    valid int32 [M*K*S], init float64 [M*K*S,12], cams float64 [S,20], centers float64 [K,3] (device); the slot state
+    (prev, live, ids, misses, park, ring, count over M*K*S rows, next_id [1]) is updated in place.  Returns (work float64
+    [M*K*2S,12], flags0 uint8 [M*K*2S], lists int32 [max(F,r)*M*K*S], det_slot int32, spawned int32, dropped int64
+    [M*K*S])."""
+    n, S, K = live.shape[0], cams.shape[0], centers.shape[0]
+    M, num, dev = n // max(K * S, 1), ring.shape[1], live.device
+    if (K < 1 or centers.shape != (K, 3) or n != M * K * S or det.shape != (n, 4) or valid.shape != (n,) or init.shape != (n, 12)
+            or prev.shape != (n, 12) or park.shape != (n, 12) or ids.shape != (n,) or misses.shape != (n,) or next_id.shape != (1,)
+            or ring.shape != (n, num, 8, 2) or count.shape != (n,)):
+        raise ValueError(f'instances_associate_objects: inconsistent shapes for {n} rows over {K} objects and {S} sequences')
+    work = torch.empty(2 * n, 12, device=dev, dtype=torch.float64)
+    flags0 = torch.empty(2 * n, device=dev, dtype=torch.uint8)
+    lists = torch.empty(max(F, r) * n, device=dev, dtype=torch.int32)
+    det_slot, spawned = torch.empty(n, device=dev, dtype=torch.int32), torch.empty(n, device=dev, dtype=torch.int32)
+    dropped = torch.empty(n, device=dev, dtype=torch.int64)
+    _call('g6d_instances_associate_objects', S, K, M, int(F), int(r), _p(det), _p(valid, torch.int32), _p(init, torch.float64),
+          _p(cams, torch.float64), _p(centers, torch.float64), float(ref_resolution), float(gate), int(max_misses),
+          _p(prev, torch.float64), _p(live, torch.int32), _p(ids, torch.int64), _p(misses, torch.int32), _p(next_id, torch.int64),
+          _p(park, torch.float64), _p(ring), _p(count, torch.int32), num, _p(work, torch.float64), _p(flags0, torch.uint8),
+          _p(lists, torch.int32), _p(det_slot, torch.int32), _p(spawned, torch.int32), _p(dropped, torch.int64), _stream())
+    return work, flags0, lists, det_slot, spawned, dropped
+
+
 def imagenet_norm(x, out_c=4):
     out = torch.empty(*x.shape[:-1], out_c, device=x.device, dtype=torch.float32)
     _call('g6d_imagenet_norm', _p(x), _p(out), x.numel() // x.shape[-1], x.shape[-1], out_c, _stream())

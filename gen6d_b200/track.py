@@ -69,6 +69,25 @@ def object_bbox(database):
     return None if pc is None else bbox_from_points(pc)
 
 
+def object_bboxes(objs, bboxes):
+    """The box of every object of an ObjectSet, in set order: bboxes[name] (8 corners [8,3]) where given, else the box of
+    the object's database point cloud."""
+    bboxes = dict(bboxes or {})
+    unknown = sorted(set(bboxes) - set(objs.names))
+    if unknown:
+        raise ValueError(f'bboxes names objects that are not in the set: {unknown} (objects: {objs.names})')
+    boxes = []
+    for name, ob in objs._objects.items():
+        box = bboxes.get(name)
+        if box is None:
+            box = object_bbox(ob.ref.database)
+            if box is None:
+                raise ValueError(f'object {name!r}: its database has no object point cloud: pass bboxes[{name!r}] (the 8 '
+                                 'corners of the object box)')
+        boxes.append(check_bbox(box))
+    return boxes
+
+
 def host_smooth(poses, poses_are_f32, bbox, Ks, ring, count, weights):
     """g6d_track_smooth_host on numpy arrays: poses [S,3,4] / [S,12], Ks [S,3,3]; ring float32 [S,num,8,2] and count
     int32 [S] are updated in place.  Returns (smoothed float64 [S,3,4], averaged corners float64 [S,8,2])."""
@@ -531,19 +550,7 @@ class ObjectTracker:
         if not float(smooth_std) > 0:
             raise ValueError(f'smooth_std must be > 0, got {smooth_std}')
         objs._check()
-        bboxes = dict(bboxes or {})
-        unknown = sorted(set(bboxes) - set(objs.names))
-        if unknown:
-            raise ValueError(f'bboxes names objects that are not in the set: {unknown} (objects: {objs.names})')
-        boxes = []
-        for name, ob in objs._objects.items():
-            box = bboxes.get(name)
-            if box is None:
-                box = object_bbox(ob.ref.database)
-                if box is None:
-                    raise ValueError(f'object {name!r}: its database has no object point cloud: pass bboxes[{name!r}] (the 8 '
-                                     'corners of the object box)')
-            boxes.append(check_bbox(box))
+        boxes = object_bboxes(objs, bboxes)
         self.objs, self.est = objs, objs.est
         self.names = objs.names
         self.K, self.S, self.refine_iter = len(self.names), int(num_sequences), int(refine_iter)

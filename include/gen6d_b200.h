@@ -219,6 +219,27 @@ int g6d_instances_associate_host(int S, int M, int F, int r, const float* det, c
                                  int max_misses, const double* prev, int* live, long long* ids, int* misses, long long* next_id,
                                  double* park, float* ring, int* count, int num, double* work, uint8_t* flags0, int* lists,
                                  int* det_slot, int* spawned, long long* dropped);
+/* The same association for K objects of an object set with M instance slots each (gen6d_b200/instance_track.py,
+ * ObjectSet.instance_tracker()).  Slot group g = m*K + o is instance slot m of object o; det, valid, init, prev, live,
+ * ids, misses, park, ring, count, det_slot, spawned and dropped have M*K*S rows, row g*S + s (the layout of
+ * ObjectSet.predict_instances' slots on S frames).  work [M*K*2S,12] holds group g's S real rows g*2S + s, then its S
+ * scratch copies g*2S + S + s; flags0 has one entry per work row; lists [max(F,r)*M*K*S] has entry (it*M*K + g)*S + s.
+ * centers [K,3] float64 are the objects' centres (device memory for the device call, host memory for the *_host one).
+ * Each (sequence s, object o) pair is associated as above over object o's M slots, with cams[s] and centers[o], against
+ * object o's detections only.  The id counter is shared: the spawned tracks are numbered in ascending (object, sequence,
+ * detection) order, so the call equals K calls of g6d_instances_associate on the objects' slices in object order, each
+ * continuing the counter.  K = 1 is g6d_instances_associate itself, bit for bit.  One CTA, one thread per (sequence,
+ * object) pair; no workspace, no synchronisation.  Needs K >= 1, 1 <= M <= G6D_DET_MAX_INSTANCES and centers. */
+int g6d_instances_associate_objects(int S, int K, int M, int F, int r, const float* det, const int* valid, const double* init,
+                                    const g6d_glue_camera* cams, const double* centers, double ref_resolution, double gate,
+                                    int max_misses, const double* prev, int* live, long long* ids, int* misses, long long* next_id,
+                                    double* park, float* ring, int* count, int num, double* work, uint8_t* flags0, int* lists,
+                                    int* det_slot, int* spawned, long long* dropped, g6d_stream_t stream);
+int g6d_instances_associate_objects_host(int S, int K, int M, int F, int r, const float* det, const int* valid, const double* init,
+                                         const g6d_glue_camera* cams, const double* centers, double ref_resolution, double gate,
+                                         int max_misses, const double* prev, int* live, long long* ids, int* misses,
+                                         long long* next_id, double* park, float* ring, int* count, int num, double* work,
+                                         uint8_t* flags0, int* lists, int* det_slot, int* spawned, long long* dropped);
 /* (x - mean) / std on f32 [n_pixels, in_c] -> [n_pixels, out_c] (in_c, out_c in {3,4})
  * (network/detector.py:189, selector.py:115, refiner.py:65) */
 int g6d_imagenet_norm(const float* in, float* out, long long n_pixels, int in_c, int out_c, g6d_stream_t stream);
