@@ -16,6 +16,7 @@ G6D_DET_MAX_SCALES = 8
 G6D_GLUE_MAX_OBJECTS = 16                   # objects per g6d_glue_*_objects launch
 G6D_DET_MAX_INSTANCES = 16                  # instances per map of g6d_det_parse_peaks
 G6D_DET_MAX_PEAK_RADIUS = 3
+G6D_ATTENTION_MAX_SMEM_FLOATS = 12288 - 32  # n + C/heads of a g6d_attention call
 PRO_NONE, PRO_AFFINE, PRO_AFFINE_RELU, PRO_CORR = 0, 1, 2, 3
 ACT_NONE, ACT_RELU, ACT_LEAKY01 = 0, 1, 2
 TC_TF32, TC_F16 = 0, 1

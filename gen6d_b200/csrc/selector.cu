@@ -542,6 +542,9 @@ extern "C" int g6d_sel_max_angle_add(const float* x, const float* embed, float* 
 extern "C" int g6d_attention(const float* q, const float* k, const float* v, float* out, int n, int C, int heads,
                              g6d_stream_t stream) {
     G6D_REQUIRE(q && k && v && out && n > 0 && n <= 8192 && heads > 0 && C % heads == 0, "g6d_attention: bad args");
+    G6D_REQUIRE((long long)n + C / heads <= G6D_ATTENTION_MAX_SMEM_FLOATS,
+                "g6d_attention: n + C/heads = %lld exceeds the %d floats of shared memory", (long long)n + C / heads,
+                G6D_ATTENTION_MAX_SMEM_FLOATS);
     const size_t smem = sizeof(float) * (n + C / heads);
     attention_kernel<<<dim3(n, heads), 64, smem, as_stream(stream)>>>(q, k, v, out, n, C, heads);
     G6D_CHECK_LAUNCH("g6d_attention");

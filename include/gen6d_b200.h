@@ -501,7 +501,10 @@ int g6d_sel_vp_norm(const float* score, int L, int n, float eps, float* feats, i
 /* selector.py:203-204: out[r,c] = max_a x[r,a,c] + embed[r,c] */
 int g6d_sel_max_angle_add(const float* x, const float* embed, float* out, int rfn, int an, int C, g6d_stream_t stream);
 /* attention.py:4-17 with the reference's channel->(d, head) mapping c = d*heads + head:
- * q,k,v [n, C] -> out [n, C]; softmax(q_h^T k_h / sqrt(C/heads)) over keys. n <= 1024. */
+ * q,k,v [n, C] -> out [n, C]; softmax(q_h^T k_h / sqrt(C/heads)) over keys.  n <= 8192, and a block keeps
+ * its n probabilities and its C/heads query values in shared memory next to a 32-float reduction buffer, all
+ * within the 48 KB a kernel gets without opting in: n + C/heads <= G6D_ATTENTION_MAX_SMEM_FLOATS. */
+#define G6D_ATTENTION_MAX_SMEM_FLOATS (12288 - 32)
 int g6d_attention(const float* q, const float* k, const float* v, float* out, int n, int C, int heads,
                   g6d_stream_t stream);
 /* The same attention over HEAD-MAJOR channels (c = head*64 + d): the layout a caller gets for free by
