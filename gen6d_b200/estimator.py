@@ -12,6 +12,7 @@ import numpy as np
 import torch
 import yaml
 
+from . import frames as F
 from . import geometry as G
 from . import glue
 from . import instances
@@ -143,15 +144,22 @@ class Gen6DEstimator:
 
 
     def predict_batch(self, que_imgs, que_Ks, pose_inits=None):
-        """predict() for a batch of independent frames of one size (row f3): qn frames go through ONE
+        """predict() for a batch of independent frames (row f3): qn frames go through ONE
         detect stage, ONE select stage and ONE refine stage per iteration -- 2 + refine_iter graph launches
         and device->host reads for the whole batch instead of per frame -- with the small per-frame camera
-        algebra on the host in between.  Same results as predict() frame by frame.
+        algebra on the host in between.  Same results as predict() frame by frame.  Frames of different sizes take the
+        device-glue path only (row f13: detection per size, the crops cut from one zero-padded canvas).
         que_imgs: list / array of uint8 [h,w,3]; que_Ks: [qn,3,3].  Returns (poses [qn,3,4], inter dict of lists)."""
         qn, res = len(que_imgs), self.cfg['ref_resolution']
         que_Ks = [np.asarray(K) for K in que_Ks]
-        frames = self.detector.upload_frame([np.asarray(f) for f in que_imgs])  # [qn,h,w,3] once, for all stages
-        if self.cfg['device_glue'] and pose_inits is None and self._glue_possible():
+        device = self.cfg['device_glue'] and pose_inits is None and self._glue_possible()
+        imgs = [np.asarray(f) for f in que_imgs]
+        if F.is_mixed(imgs):                         # frames of different sizes: the device glue path only (row f13)
+            if not device:
+                F.require_one_size(imgs, "predict_batch with pose_inits, cfg['device_glue'] off or cfg['host_warps'] on")
+            return self._predict_batch_device(None, que_Ks, F.check_frames(imgs, que_Ks, 'predict_batch'))
+        frames = self.detector.upload_frame(imgs)  # [qn,h,w,3] once, for all stages
+        if device:
             return self._predict_batch_device(frames, que_Ks)
         inter = {}
         if pose_inits is None:
@@ -216,7 +224,7 @@ class Gen6DEstimator:
         poses; the M*qn crops go through one warp and one selection."""
         res = self.cfg['ref_resolution']
         select = self.selector._select_warped(res)
-        detect = detect or self.detector._detect_u8
+        detect = detect or (lambda u8: F.per_size(self.detector._detect_u8, u8))      # once per frame size (row f13)
 
         def fn(frames, cams):
             qn = frames.shape[0]
@@ -234,12 +242,16 @@ class Gen6DEstimator:
         det_mod, box = self.detector, float(self.cfg['ref_resolution'])
         extra = []
 
-        def detect(frames):
-            o = det_mod._detect_nhwc(ops.preprocess_u8(frames, out_c=3, imagenet_norm=False))
+        def one_size(u8):
+            o = det_mod._detect_nhwc(ops.preprocess_u8(u8, out_c=3, imagenet_norm=False))
             det, _, valid, count = ops.det_parse_peaks(o['score_predict'], o['scale_predict'], o['offset_predict'], max_instances,
                                                        peak_radius, nms_iou, box, min_score, det_mod.pool_ratio)
-            extra[:] = [valid.reshape(-1), count]
-            return det.reshape(-1, 4)
+            return det.reshape(-1, 4), valid.reshape(-1), count
+
+        def detect(frames):
+            det, valid, count = F.per_size(one_size, frames)                       # once per frame size (row f13)
+            extra[:] = [valid, count]
+            return det
         return detect, extra
 
     def _predict_device_fn(self, st):
@@ -258,13 +270,18 @@ class Gen6DEstimator:
             return torch.stack(chain, 0), det, crop, idx, sel_out, logits
         return fn
 
-    def _predict_batch_device(self, frames, que_Ks):
-        """predict_batch with cfg['device_glue']: one graph launch, one synchronising read at the end."""
+    def _predict_batch_device(self, frames, que_Ks, imgs=None):
+        """predict_batch with cfg['device_glue']: one graph launch, one synchronising read at the end.  imgs: frames of
+        different sizes (numpy, not uploaded; frames is None), packed and put on a canvas in the graph."""
         st = self._glue_state()
-        qn = frames.shape[0]
+        qn = len(que_Ks)
         with torch.no_grad():
+            if imgs is None:
+                name, fn, fin = 'predict', self._predict_device_fn(st), [frames]
+            else:
+                name, fn, fin = F.stage(self.detector, 'predict', self._predict_device_fn(st), imgs)
             cams = self.detector._to_dev(glue.cameras(np.stack(que_Ks, 0)))
-            outs = self.stages.run('predict', self._predict_device_fn(st), [frames, cams])
+            outs = self.stages.run(name, fn, fin + [cams])
             chain, det, crop, idx, sel_out, logits = [self.detector._to_host(t) for t in outs]
         chain = chain.reshape(len(chain), qn, 3, 4)
         poses0, refined = chain[0], [c.astype(np.float32) for c in chain[1:]]
@@ -294,7 +311,7 @@ class Gen6DEstimator:
         return fn
 
     def predict_instances(self, que_imgs, que_Ks, max_instances=4, min_score=None, nms_iou=0.3, peak_radius=1):
-        """Every instance of the object on qn frames of one size: up to `max_instances` detections per frame, the peaks of
+        """Every instance of the object on qn frames (of one size or several, row f13): up to `max_instances` detections per frame, the peaks of
         the detector's score map (within `peak_radius` cells) kept by greedy non-maximum suppression of their
         ref_resolution * scale boxes at IoU > `nms_iou` (g6d_det_parse_peaks), each selected and refined as predict_batch
         does.  min_score: a raw score-head threshold (its meaning depends on the checkpoint); None: no threshold.
@@ -310,12 +327,15 @@ class Gen6DEstimator:
         qn, res = len(que_imgs), self.cfg['ref_resolution']
         if qn == 0 or len(que_Ks) != qn:
             raise ValueError(f'predict_instances: {qn} frames and {len(que_Ks)} intrinsics; need one K per frame and at least one frame')
+        imgs = [np.asarray(f) for f in que_imgs]
+        if F.is_mixed(imgs):
+            F.check_frames(imgs, que_Ks, 'predict_instances')
         st = self._glue_state()
         det = self.detector
         with torch.no_grad():
-            frames = det.upload_frame([np.asarray(f) for f in que_imgs])
+            name, fn, fin = F.stage(det, ('instances',) + key, self._instances_fn(st, *key), imgs)
             cams = det._to_dev(glue.cameras(np.stack([np.asarray(K) for K in que_Ks], 0)))
-            buf = self.stages.run(('instances',) + key, self._instances_fn(st, *key), [frames, cams])
+            buf = self.stages.run(name, fn, fin + [cams])
             host = det._to_host(buf)                                       # the call's one synchronising read
         n, n_sel = M * qn, len(self.ref_info['poses'])
         rd = instances.Unpacker(host, n * res * res * 3)
@@ -399,7 +419,8 @@ class Gen6DEstimator:
         weights / reference features, private CUDA graphs) and a CUDA stream, each pushing `batch` frames
         at a time through predict_batch (batch = 1: plain predict), so one batch's host geometry overlaps
         another batch's kernels.  Same results as predict(); returns [(pose, inter)] (inter of a batched
-        frame holds that frame's slices)."""
+        frame holds that frame's slices).  With batch > 1 the frames are grouped by size (in order of first
+        appearance) before they are cut into batches, so every batch has frames of one size."""
         from concurrent.futures import ThreadPoolExecutor
         if len(que_imgs) == 0:
             return []
@@ -413,20 +434,27 @@ class Gen6DEstimator:
             self._warm = set()
         n = len(que_imgs)
         batch = max(1, min(batch, n))
-        warm_key = (batch, bool(self.cfg['device_glue']))
-        if warm_key not in self._warm:               # capture every worker's graphs for this batch size / path, one at a time
-            for est, stream in self._workers:
+        # batches are cut per frame size (groups in order of first appearance, input order inside a group), so every
+        # batch is one predict_batch graph of one size
+        sizes = F.size_pattern(que_imgs) if batch > 1 else [None] * n
+        groups = [[i for i in range(n) if sizes[i] == z] for z in dict.fromkeys(sizes)]
+        for g in groups:
+            warm_key = (batch, bool(self.cfg['device_glue'])) + ((sizes[g[0]],) if len(groups) > 1 else ())
+            if warm_key in self._warm:
+                continue
+            for est, stream in self._workers:        # capture every worker's graphs for this batch size / path, one at a time
                 stream.wait_stream(torch.cuda.current_stream())
                 with torch.cuda.stream(stream):
                     if batch == 1:
                         est.predict(que_imgs[0], que_Ks[0])
                     else:
-                        est.predict_batch([que_imgs[i % n] for i in range(batch)], [que_Ks[i % n] for i in range(batch)])
+                        m = len(g)
+                        est.predict_batch([que_imgs[g[i % m]] for i in range(batch)], [que_Ks[g[i % m]] for i in range(batch)])
                     stream.synchronize()
             self._warm.add(warm_key)
         results = [None] * n
         caller = torch.cuda.current_stream()
-        chunks = [list(range(b, min(b + batch, n))) for b in range(0, n, batch)]
+        chunks = [g[b:b + batch] for g in groups for b in range(0, len(g), batch)]
 
         def run(w):
             est, stream = self._workers[w]

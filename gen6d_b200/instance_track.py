@@ -29,6 +29,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from . import frames as fr
 from . import glue
 from . import instances
 from . import ops
@@ -264,7 +265,7 @@ class InstanceTracker:
 
     # -------------------------------------------------------------- one step
     def step(self, frames, Ks):
-        """frames: S uint8 [h,w,3] of one size; Ks: [S,3,3].  Returns (poses float32 [S,M,3,4], smoothed float64 [S,M,3,4],
+        """frames: S uint8 [h,w,3] (of one size or several, row f13); Ks: [S,3,3].  Returns (poses float32 [S,M,3,4], smoothed float64 [S,M,3,4],
         track_ids int64 [S,M] (-1: empty slot), inter): inter['refine_poses'] a list of [S,M,3,4] (entry 0 the starting
         poses, float64 on a re-detection step; a row whose chain is shorter repeats its final pose), 'bbox_pts' and
         'smoothed_pts' [S,M,8,2].  Empty slots' poses and points are NaN.  A re-detection step adds predict_instances'
@@ -285,20 +286,25 @@ class InstanceTracker:
         F = est.cfg['refine_iter']
         if detecting and F < 1:
             raise ValueError("instance tracking needs cfg['refine_iter'] >= 1 (a re-detection step smooths float32 poses)")
+        imgs = [np.asarray(f) for f in frames]
+        plan = fr.FramePlan(fr.size_pattern(imgs))
+        if plan.mixed:
+            fr.check_frames(imgs, Ks, 'step')
         stt, x = self._tables(), self._state
         with torch.no_grad():
-            dev_frames = est.detector.upload_frame([np.asarray(f) for f in frames])
-            cams = est.detector._to_dev(glue.cameras(Ks))
             if detecting:
-                outs = self.stages.run('detect', self._detect_fn(stt), [dev_frames, cams, x['prev'], x['park'], x['live'], x['ids'],
-                                                                        x['misses'], self._next_id, x['ring'], x['count']])
+                name, fn, fin = fr.stage(est.detector, 'detect', self._detect_fn(stt), imgs, plan)
+                cams = est.detector._to_dev(glue.cameras(Ks))
+                outs = self.stages.run(name, fn, fin + [cams, x['prev'], x['park'], x['live'], x['ids'], x['misses'], self._next_id,
+                                                        x['ring'], x['count']])
                 buf, poses, park, live, ids, misses, next_id, ring, count = outs
                 for k, v in (('park', park), ('live', live), ('ids', ids), ('misses', misses)):
                     x[k].copy_(v)
                 self._next_id.copy_(next_id)
             else:
-                outs = self.stages.run('refine', self._refine_fn(stt), [dev_frames, cams, x['prev'], x['park'], x['live'], x['ids'],
-                                                                        x['ring'], x['count']])
+                name, fn, fin = fr.stage(est.detector, 'refine', self._refine_fn(stt), imgs, plan)
+                cams = est.detector._to_dev(glue.cameras(Ks))
+                outs = self.stages.run(name, fn, fin + [cams, x['prev'], x['park'], x['live'], x['ids'], x['ring'], x['count']])
                 buf, poses, ring, count = outs
             x['prev'].copy_(poses)
             x['ring'].copy_(ring)
@@ -415,7 +421,7 @@ class ObjectInstanceTracker(InstanceTracker):
         return [tuple(np.concatenate([slots[m * K + o][i] for m in range(M)]) for i in range(3)) for o in range(K)]
 
     def step(self, frames, Ks):
-        """frames: S uint8 [h,w,3] of one size; Ks: [S,3,3] (shared by all objects).  Returns {name: (poses float32
+        """frames: S uint8 [h,w,3] (of one size or several, row f13); Ks: [S,3,3] (shared by all objects).  Returns {name: (poses float32
         [S,M,3,4], smoothed float64 [S,M,3,4], track_ids int64 [S,M], inter)}: per object what InstanceTracker.step returns,
         'det_score' included on a re-detection step; 'dropped' lists that object's ids only.  Ids are unique over every
         object of the tracker."""

@@ -85,12 +85,7 @@ class PackedModule(nn.Module):
             if dtype is not None:
                 arr = arr.astype(torch.empty(0, dtype=dtype).numpy().dtype, copy=False)
             shape, dt = arr.shape, arr.dtype
-        key = (shape, dt.str)
-        ring = self._pinned.setdefault(key, [])
-        if len(ring) < 4:
-            ring.append(torch.from_numpy(np.empty(shape, dt)).pin_memory())
-        slot = ring[self._pinned_next.get(key, 0) % len(ring)]
-        self._pinned_next[key] = self._pinned_next.get(key, 0) + 1
+        slot = self._pinned_slot(shape, dt)
         if parts is not None:
             dst = slot.numpy()
             for i, a in enumerate(parts):
@@ -98,6 +93,31 @@ class PackedModule(nn.Module):
         else:
             np.copyto(slot.numpy(), arr)
         IO_BYTES['h2d'] += slot.numel() * slot.element_size()
+        return slot.to(self.device, non_blocking=True)
+
+    def _pinned_slot(self, shape, dt):
+        """The next of (up to) four pinned staging buffers of this shape and dtype, used round robin."""
+        key = (shape, dt.str)
+        ring = self._pinned.setdefault(key, [])
+        if len(ring) < 4:
+            ring.append(torch.from_numpy(np.empty(shape, dt)).pin_memory())
+        slot = ring[self._pinned_next.get(key, 0) % len(ring)]
+        self._pinned_next[key] = self._pinned_next.get(key, 0) + 1
+        return slot
+
+    def upload_packed(self, arrays, offsets, nbytes):
+        """uint8 arrays -> one device uint8 buffer [nbytes] holding array i's bytes at offsets[i], through the pinned
+        staging of _to_dev (one H2D copy).  Bytes no array covers are zero."""
+        slot = self._pinned_slot((int(nbytes),), np.dtype(np.uint8))
+        dst = slot.numpy()
+        end = 0
+        for a, off in zip(arrays, offsets):
+            if off > end:
+                dst[end:off] = 0
+            end = off + a.nbytes
+            np.copyto(dst[off:end].reshape(a.shape), a)
+        dst[end:] = 0
+        IO_BYTES['h2d'] += slot.numel()
         return slot.to(self.device, non_blocking=True)
 
     def upload_frame(self, que_img):

@@ -19,6 +19,7 @@ each (gen6d_b200/instance_track.py ObjectInstanceTracker).
 import numpy as np
 import torch
 
+from . import frames as F
 from . import glue
 from . import instances
 from . import ops
@@ -146,7 +147,7 @@ class ObjectSet:
             qn = frames.shape[0]
             rows = lambda t, o: t[o * qn:(o + 1) * qn]
             cat = lambda ts: ts[0] if len(ts) == 1 else torch.cat(ts, 0)
-            det = self._detect(frames)[0] if detect is None else detect(frames)      # [S*qn,4]: x, y, scale, score
+            det = F.per_size(lambda u8: self._detect(u8)[0], frames) if detect is None else detect(frames)   # [S*qn,4]: x, y, scale, score
             S = det.shape[0] // qn
             jobs = cat([ops.glue_detection_jobs(rows(det, s), frames, res) for s in range(S)])
             crop = ops.warp_affine_u8(jobs, S * qn, res, res)
@@ -175,13 +176,17 @@ class ObjectSet:
         objs = list(self._objects.values())
         extra = []
 
-        def detect(frames):
-            o = det_mod._detect_objects_nhwc(ops.preprocess_u8(frames, out_c=3, imagenet_norm=False), self._detector_kernels(),
+        def one_size(u8):
+            o = det_mod._detect_objects_nhwc(ops.preprocess_u8(u8, out_c=3, imagenet_norm=False), self._detector_kernels(),
                                              len(objs), objs[0].det.rfn)
             det, _, valid, count = ops.det_parse_peaks(o['score_predict'], o['scale_predict'], o['offset_predict'], M, radius,
                                                        nms_iou, box, min_score, det_mod.pool_ratio)
-            extra[:] = [valid.reshape(-1), count]
-            return det.reshape(-1, 4)
+            return det.reshape(-1, 4), valid.reshape(-1), count
+
+        def detect(frames):
+            det, valid, count = F.per_size(one_size, frames)                       # once per frame size (row f13)
+            extra[:] = [valid, count]
+            return det
         return detect, extra
 
     def _predict_device_fn(self, detect=None, instances=1):
@@ -222,7 +227,7 @@ class ObjectSet:
         return fn
 
     def predict(self, que_imgs, que_Ks):
-        """Every object's pose on the same qn frames (uint8 [h,w,3] of one size; que_Ks [qn,3,3]).
+        """Every object's pose on the same qn frames (uint8 [h,w,3], of one size or several: row f13; que_Ks [qn,3,3]).
         Returns {name: (poses [qn,3,4], inter)}: inter has the keys and shapes of predict_batch's device-glue inter, plus
         'det_score' [qn], the maximum of that object's detection score map (is the object in the frame at all)."""
         self._check()
@@ -230,11 +235,14 @@ class ObjectSet:
         qn, res, iters = len(que_imgs), est.cfg['ref_resolution'], est.cfg['refine_iter']
         if qn == 0 or len(que_Ks) != qn:
             raise ValueError(f'predict: {qn} frames and {len(que_Ks)} intrinsics; need one K per frame and at least one frame')
+        imgs = [np.asarray(f) for f in que_imgs]
+        if F.is_mixed(imgs):
+            F.check_frames(imgs, que_Ks, 'predict')
         det = est.detector
         with torch.no_grad():
-            frames = det.upload_frame([np.asarray(f) for f in que_imgs])
+            name, fn, fin = F.stage(det, 'predict', self._predict_fn(), imgs)
             cams = det._to_dev(glue.cameras(np.stack([np.asarray(K) for K in que_Ks], 0)))
-            buf = self.stages.run('predict', self._predict_fn(), [frames, cams])
+            buf = self.stages.run(name, fn, fin + [cams])
             host = det._to_host(buf)                                       # the call's one synchronising read
         crop_bytes = len(self._objects) * qn * res * res * 3
         f64 = host[:len(host) - crop_bytes].view(np.float64)
@@ -283,11 +291,14 @@ class ObjectSet:
         qn, res, iters = len(que_imgs), est.cfg['ref_resolution'], est.cfg['refine_iter']
         if qn == 0 or len(que_Ks) != qn:
             raise ValueError(f'predict_instances: {qn} frames and {len(que_Ks)} intrinsics; need one K per frame and at least one frame')
+        imgs = [np.asarray(f) for f in que_imgs]
+        if F.is_mixed(imgs):
+            F.check_frames(imgs, que_Ks, 'predict_instances')
         det = est.detector
         with torch.no_grad():
-            frames = det.upload_frame([np.asarray(f) for f in que_imgs])
+            name, fn, fin = F.stage(det, ('instances',) + key, self._instances_fn(*key), imgs)
             cams = det._to_dev(glue.cameras(np.stack([np.asarray(K_) for K_ in que_Ks], 0)))
-            buf = self.stages.run(('instances',) + key, self._instances_fn(*key), [frames, cams])
+            buf = self.stages.run(name, fn, fin + [cams])
             host = det._to_host(buf)                                       # the call's one synchronising read
         S = M * K
         rd = instances.Unpacker(host, S * qn * res * res * 3)

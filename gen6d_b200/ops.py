@@ -101,6 +101,23 @@ def warp_affine_u8(jobs, n_jobs, h, w):
     return _warp('g6d_warp_affine_u8', jobs, n_jobs, h, w)
 
 
+class FrameEntry(C.Structure):        # g6d_frame_entry
+    _fields_ = [('offset', C.c_longlong), ('rows', C.c_int), ('cols', C.c_int)]
+
+
+def frames_canvas(packed, table, H, W):
+    """packed u8 (frames back to back) + table [(byte offset, rows, cols)] per frame (host) -> canvas u8 [n,H,W,3]: every
+    frame in the top-left corner, zeros elsewhere (g6d_frames_canvas)."""
+    n = len(table)
+    if packed.dtype != torch.uint8 or packed.dim() != 1:
+        raise ValueError('frames_canvas: packed must be a 1-D uint8 tensor')
+    host = (FrameEntry * max(n, 1))(*[FrameEntry(int(o), int(r), int(c)) for o, r, c in table])
+    out = torch.empty(n, H, W, 3, device=packed.device, dtype=torch.uint8)
+    _call('g6d_frames_canvas', _p(packed, torch.uint8), packed.numel(), host, n, _p(out, torch.uint8) if n else None, H, W,
+          _stream())
+    return out
+
+
 # ------------------------------------------------------------------------------- camera algebra between the stages
 def glue_detection_jobs(det_out, frames, size):
     """det_out [qn,4] (g6d_det_parse) + frames u8 [qn,h,w,3] -> packed g6d_warp_job records [qn*88] of the selector crops."""

@@ -18,6 +18,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from . import frames as fr
 from . import glue
 from . import ops
 from .graphs import StageCache
@@ -147,15 +148,37 @@ def _iter_lengths(S, b, F, r):
     return [S if (it < F and it < r) or it >= F else b for it in range(max(F, r))]
 
 
-def _mixed_inputs(S, K, pending, f32, F, r, device):
+def _size_buckets(reinit, plan):
+    """The re-initialised sequences of a step over frames of different sizes, bucketed per size (row f13) -> (gathered
+    sequences [b], rows per size group [b_z], each re-initialised sequence's position in the gather [m]).  Per size group
+    of g sequences with m_z of them re-initialised, b_z = _bucket(m_z, g): its re-initialised sequences in ascending order,
+    padded by repeating the last; the blocks follow the groups' order."""
+    seq, blocks, pick = [], [], np.zeros(len(reinit), np.int64)
+    for _, _, idx, _ in plan.groups:
+        mine = reinit[np.isin(reinit, idx)]
+        bz = _bucket(len(mine), len(idx))
+        pick[np.searchsorted(reinit, mine)] = len(seq) + np.arange(len(mine))
+        seq += list(mine) + [mine[-1]] * (bz - len(mine)) if bz else []
+        blocks.append(bz)
+    return np.asarray(seq, np.int64), blocks, pick
+
+
+def _mixed_inputs(S, K, pending, f32, F, r, device, plan=None):
     """Host side of a mixed step -> (re-initialised sequences [m], bucket, graph inputs: gathered sequences int64 [b], scatter
-    rows int64 [K*b], first-iteration dtype flags uint8 [K*(S+b)], the iterations' row lists int32, object-major)."""
+    rows int64 [K*b], first-iteration dtype flags uint8 [K*(S+b)], the iterations' row lists int32, object-major).
+    plan: the FramePlan of frames of different sizes, whose buckets are per size (_size_buckets)."""
     reinit, others = np.flatnonzero(pending), np.flatnonzero(~pending)
     m = len(reinit)
-    b = _bucket(m, S)
+    if plan is None or not plan.mixed:
+        b = _bucket(m, S)
+        seq = np.concatenate([reinit, np.full(b - m, reinit[-1] if m else 0)])
+        tgt = np.concatenate([reinit, S + np.arange(m, b)])
+    else:
+        seq, _, pick = _size_buckets(reinit, plan)
+        b = len(seq)
+        tgt = S + np.arange(b)                                            # padding rows go to their scratch rows
+        tgt[pick] = reinit
     n = S + b
-    seq = np.concatenate([reinit, np.full(b - m, reinit[-1] if m else 0)])
-    tgt = np.concatenate([reinit, S + np.arange(m, b)])
     flags = np.zeros(n, np.uint8)
     flags[others] = f32[others]
     lists = []
@@ -175,15 +198,20 @@ def _mixed_inputs(S, K, pending, f32, F, r, device):
     return reinit, b, inputs
 
 
-def _mixed_fn(K, S, b, F, r, initial, views, R, refine, smooth):
+def _mixed_fn(K, S, b, F, r, initial, views, R, refine, smooth, blocks=None):
     """The mixed step's graph body.  initial(frames, cams) -> (poses [K*b,12], crops, [tensors packed after the smoothing]);
-    smooth(poses [K*S,12], Ks [S,9], ring, count) -> (smoothed, averaged corners)."""
+    smooth(poses [K*S,12], Ks [S,9], ring, count) -> (smoothed, averaged corners).  blocks: the gathered rows per size
+    group of frames of different sizes (_size_buckets), detected per size."""
     n, lens = S + b, _iter_lengths(S, b, F, r)
 
     def fn(frames, cams, prev, ring, count, seq, tgt, flags0, lists):
         if b:
             gf, gc = frames.index_select(0, seq), cams.index_select(0, seq)
-            init, crop, extras = initial(gf, gc)
+            if blocks is None:
+                init, crop, extras = initial(gf, gc)
+            else:
+                with fr.gathered(frames, gf, seq, blocks):
+                    init, crop, extras = initial(gf, gc)
             frames_x, cams_x = torch.cat([frames, gf], 0), torch.cat([cams, gc], 0)
             work = torch.cat([prev.view(K, S, 12), init.view(K, b, 12)], 1).reshape(K * n, 12)
             work.index_copy_(0, tgt, init)
@@ -331,7 +359,7 @@ class Tracker:
 
     # -------------------------------------------------------------- one step
     def step(self, frames, Ks):
-        """frames: S uint8 [h,w,3] of one size; Ks: [S,3,3].  Returns (raw poses float32 [S,3,4], smoothed poses float64
+        """frames: S uint8 [h,w,3] (of different sizes on the device path, row f13); Ks: [S,3,3].  Returns (raw poses float32 [S,3,4], smoothed poses float64
         [S,3,4], inter): inter['refine_poses'] is this step's chain, inter['bbox_pts'] the projected box corners
         [S,8,2], inter['smoothed_pts'] their weighted average [S,8,2]; a full-prediction step adds the detection and
         selection entries of predict_batch.  A mixed step (some sequences re-initialised by reset(sequences), or previous
@@ -343,7 +371,12 @@ class Tracker:
             raise ValueError(f'step: this tracker follows {self.S} sequences, got {len(frames)} frames and {len(Ks)} Ks')
         Ks = np.stack([np.asarray(K) for K in Ks], 0)
         kind = self._kind()
-        out = self._step_device(frames, Ks, kind) if self._device_path() else self._step_host(frames, Ks, kind)
+        device = self._device_path()
+        if not device:
+            fr.require_one_size(frames, "tracking with cfg['device_glue'] off or cfg['host_warps'] on")
+        elif fr.is_mixed(frames):
+            fr.check_frames(frames, Ks, 'step')
+        out = self._step_device(frames, Ks, kind) if device else self._step_host(frames, Ks, kind)
         self._pending[:] = False
         return out
 
@@ -426,7 +459,7 @@ class Tracker:
             return packed.view(torch.uint8), poses, ring, count
         return fn
 
-    def _mixed_fn(self, st, b):
+    def _mixed_fn(self, st, b, blocks=None):
         est, c = self.est, self._device_consts()
         initial = est._initial_poses_device_fn(st)
 
@@ -436,27 +469,37 @@ class Tracker:
 
         smooth = lambda poses, Ks, ring, count: ops.track_smooth(poses, True, c['bbox'], Ks, ring, count, c['weights'])
         return _mixed_fn(1, self.S, b, est.cfg['refine_iter'], self.refine_iter, init, [st['views']], st['tables']['ref_num'],
-                         est.refiner._refine_warped(128), smooth)
+                         est.refiner._refine_warped(128), smooth, blocks)
 
     def _step_device(self, frames, Ks, kind):
         est, S, num = self.est, self.S, self.num
         st = est._glue_state()
         self._to(True)
         full = kind == 'full'
+        imgs = [np.asarray(f) for f in frames]
+        plan, pick = fr.FramePlan(fr.size_pattern(imgs)), None
         with torch.no_grad():
-            dev_frames = est.detector.upload_frame([np.asarray(f) for f in frames])
-            cams = est.detector._to_dev(glue.cameras(Ks))
             if full:
-                outs = self.stages.run('track_full', self._full_fn(st), [dev_frames, cams, self._ring, self._count])
+                name, fn, fin = fr.stage(est.detector, 'track_full', self._full_fn(st), imgs, plan)
+                cams = est.detector._to_dev(glue.cameras(Ks))
+                outs = self.stages.run(name, fn, fin + [cams, self._ring, self._count])
             elif kind == 'refine':
                 prev_f32 = bool(self._f32[0])
-                outs = self.stages.run(f'track_refine{int(prev_f32)}', self._refine_fn(st, prev_f32),
-                                       [dev_frames, cams, self._prev, self._ring, self._count])
+                name, fn, fin = fr.stage(est.detector, f'track_refine{int(prev_f32)}', self._refine_fn(st, prev_f32), imgs, plan)
+                cams = est.detector._to_dev(glue.cameras(Ks))
+                outs = self.stages.run(name, fn, fin + [cams, self._prev, self._ring, self._count])
             else:
-                F = est.cfg['refine_iter']
-                reinit, b, extra = _mixed_inputs(S, 1, self._pending, self._f32, F, self.refine_iter, dev_frames.device)
-                prev = self._prev if self._prev is not None else torch.zeros(S, 12, dtype=torch.float64, device=dev_frames.device)
-                outs = self.stages.run(f'track_mixed{b}', self._mixed_fn(st, b), [dev_frames, cams, prev, self._ring, self._count] + extra)
+                F, dev = est.cfg['refine_iter'], est.detector.device
+                fin = plan.upload(est.detector, imgs) if plan.mixed else [est.detector.upload_frame(imgs)]
+                cams = est.detector._to_dev(glue.cameras(Ks))
+                reinit, b, extra = _mixed_inputs(S, 1, self._pending, self._f32, F, self.refine_iter, dev, plan)
+                prev = self._prev if self._prev is not None else torch.zeros(S, 12, dtype=torch.float64, device=dev)
+                if plan.mixed:                   # one graph per size pattern and per-size buckets (row f13)
+                    _, blocks, pick = _size_buckets(reinit, plan)
+                    name, fn = (plan.key('track_mixed'), tuple(blocks)), fr.on_canvas(self._mixed_fn(st, b, blocks), plan)
+                else:
+                    name, fn = f'track_mixed{b}', self._mixed_fn(st, b)
+                outs = self.stages.run(name, fn, fin + [cams, prev, self._ring, self._count] + extra)
             buf, poses_dev, ring, count = outs
             self._prev = poses_dev.clone()
             self._ring.copy_(ring)
@@ -465,7 +508,7 @@ class Tracker:
         prev_f32 = bool(self._f32[0])
         self._f32[:] = True
         if kind == 'mixed':
-            return self._decode_mixed(host, reinit, b)
+            return self._decode_mixed(host, reinit, b, pick)
         n_chain = (est.cfg['refine_iter'] if full else self.refine_iter) + 1
         sizes = [('chain', n_chain * S * 12), ('smoothed', S * 12), ('avg', S * 16), ('ring', S * num * 16), ('count', S)]
         if full:
@@ -497,8 +540,10 @@ class Tracker:
         inter['smoothed_pts'] = vals['avg'].reshape(S, 8, 2).copy()
         return (refined[-1] if refined else first), vals['smoothed'].reshape(S, 3, 4).copy(), inter
 
-    def _decode_mixed(self, host, reinit, b):
+    def _decode_mixed(self, host, reinit, b, pick=None):
+        """pick: the gathered row of each re-initialised sequence (per-size buckets); None: the first m rows."""
         est, S, num, m = self.est, self.S, self.num, len(reinit)
+        pick = slice(0, m) if pick is None else pick
         n_chain = max(est.cfg['refine_iter'], self.refine_iter) + 1
         res = est.cfg['ref_resolution']
         crop_bytes = b * res * res * 3
@@ -516,11 +561,11 @@ class Tracker:
         count_h = take(S).astype(np.int64)
         inter = {'reinit': reinit.astype(np.int64)}
         if b:
-            det = take(b * 4).reshape(b, 4)[:m].astype(np.float32)
-            idx = take(b)[:m].astype(np.int64)
-            sel_out = take(b * 2).reshape(b, 2)[:m].astype(np.float32)
-            logits = f64[off:].reshape(b, -1)[:m].astype(np.float32)
-            crop = host[len(host) - crop_bytes:].reshape(b, res, res, 3)[:m].copy()
+            det = take(b * 4).reshape(b, 4)[pick].astype(np.float32)
+            idx = take(b)[pick].astype(np.int64)
+            sel_out = take(b * 2).reshape(b, 2)[pick].astype(np.float32)
+            logits = f64[off:].reshape(b, -1)[pick].astype(np.float32)
+            crop = host[len(host) - crop_bytes:].reshape(b, res, res, 3)[pick].copy()
             inter.update({'det_position': det[:, :2].copy(), 'det_scale_r2q': det[:, 2].copy(), 'det_que_img': crop,
                           'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': logits, 'sel_ref_idx': idx})
         inter['refine_poses'] = [chain[0].copy()] + [c.astype(np.float32) for c in chain[1:]]
@@ -661,7 +706,7 @@ class ObjectTracker:
             return packed.view(torch.uint8), poses, ring, count
         return fn
 
-    def _mixed_fn(self, b):
+    def _mixed_fn(self, b, blocks=None):
         objs, c, K = list(self.objs._objects.values()), self._dev, self.K
         initial = self.objs._initial_poses_device_fn()
 
@@ -674,10 +719,10 @@ class ObjectTracker:
 
         smooth = lambda poses, Ks, ring, count: ops.track_smooth_objects(poses, True, c['bboxes'], Ks, ring, count, c['weights'])
         return _mixed_fn(K, self.S, b, self.est.cfg['refine_iter'], self.refine_iter, init, [ob.tables['views'] for ob in objs],
-                         objs[0].tables['tables']['ref_num'], self.est.refiner._refine_warped(128), smooth)
+                         objs[0].tables['tables']['ref_num'], self.est.refiner._refine_warped(128), smooth, blocks)
 
     def step(self, frames, Ks):
-        """frames: S uint8 [h,w,3] of one size; Ks: [S,3,3] (shared by all objects).  Returns {name: (raw poses float32
+        """frames: S uint8 [h,w,3] (of one size or several, row f13); Ks: [S,3,3] (shared by all objects).  Returns {name: (raw poses float32
         [S,3,4], smoothed poses float64 [S,3,4], inter)}: inter has Tracker.step's keys, and a full-prediction step adds
         those of ObjectSet.predict (det_score included); a mixed step adds 'reinit' and those entries for the
         re-initialised sequences, as Tracker.step does."""
@@ -690,20 +735,32 @@ class ObjectTracker:
             raise ValueError(f'step: Ks must be [{S},3,3], got {Ks.shape}')
         kind = self._kind()
         full, mixed = kind == 'full', kind == 'mixed'
+        imgs = [np.asarray(f) for f in frames]
+        plan, pick = fr.FramePlan(fr.size_pattern(imgs)), None
+        if plan.mixed:
+            fr.check_frames(imgs, Ks, 'step')
         with torch.no_grad():
-            dev_frames = est.detector.upload_frame([np.asarray(f) for f in frames])
-            cams = est.detector._to_dev(glue.cameras(Ks))
             if full:
-                outs = self.stages.run('track_full', self._full_fn(), [dev_frames, cams, self._ring, self._count])
+                name, fn, fin = fr.stage(est.detector, 'track_full', self._full_fn(), imgs, plan)
+                cams = est.detector._to_dev(glue.cameras(Ks))
+                outs = self.stages.run(name, fn, fin + [cams, self._ring, self._count])
             elif not mixed:
                 prev_f32 = bool(self._f32[0])
-                outs = self.stages.run(f'track_refine{int(prev_f32)}', self._refine_fn(prev_f32),
-                                       [dev_frames, cams, self._prev, self._ring, self._count])
+                name, fn, fin = fr.stage(est.detector, f'track_refine{int(prev_f32)}', self._refine_fn(prev_f32), imgs, plan)
+                cams = est.detector._to_dev(glue.cameras(Ks))
+                outs = self.stages.run(name, fn, fin + [cams, self._prev, self._ring, self._count])
             else:
-                reinit, b, extra = _mixed_inputs(S, K, self._pending, self._f32, est.cfg['refine_iter'], self.refine_iter,
-                                                 dev_frames.device)
-                prev = self._prev if self._prev is not None else torch.zeros(K * S, 12, dtype=torch.float64, device=dev_frames.device)
-                outs = self.stages.run(f'track_mixed{b}', self._mixed_fn(b), [dev_frames, cams, prev, self._ring, self._count] + extra)
+                dev = est.detector.device
+                fin = plan.upload(est.detector, imgs) if plan.mixed else [est.detector.upload_frame(imgs)]
+                cams = est.detector._to_dev(glue.cameras(Ks))
+                reinit, b, extra = _mixed_inputs(S, K, self._pending, self._f32, est.cfg['refine_iter'], self.refine_iter, dev, plan)
+                prev = self._prev if self._prev is not None else torch.zeros(K * S, 12, dtype=torch.float64, device=dev)
+                if plan.mixed:                   # one graph per size pattern and per-size buckets (row f13)
+                    _, blocks, pick = _size_buckets(reinit, plan)
+                    name, fn = (plan.key('track_mixed'), tuple(blocks)), fr.on_canvas(self._mixed_fn(b, blocks), plan)
+                else:
+                    name, fn = f'track_mixed{b}', self._mixed_fn(b)
+                outs = self.stages.run(name, fn, fin + [cams, prev, self._ring, self._count] + extra)
             buf, poses_dev, ring, count = outs
             prev_f32 = bool(self._f32[0])
             self._prev = poses_dev.clone()
@@ -717,6 +774,7 @@ class ObjectTracker:
             n_chain, qn, m = max(est.cfg['refine_iter'], self.refine_iter) + 1, b, len(reinit)
         else:
             n_chain, qn, m = (est.cfg['refine_iter'] if full else self.refine_iter) + 1, S, S
+        pick = slice(0, m) if pick is None else pick             # the gathered row of each re-initialised sequence
         if full or (mixed and qn):
             res = est.cfg['ref_resolution']
             crop_bytes = K * qn * res * res * 3
@@ -741,12 +799,12 @@ class ObjectTracker:
             first = chain[0, o].astype(np.float32) if (kind == 'refine' and prev_f32) else chain[0, o].copy()
             inter = {'reinit': reinit.astype(np.int64)} if mixed else {}
             if full or (mixed and qn):
-                d = take(qn * 4).reshape(qn, 4)[:m].astype(np.float32)
-                idx = take(qn)[:m].astype(np.int64)
-                sel_out = take(qn * 2).reshape(qn, 2)[:m].astype(np.float32)
-                logits = take(qn * len(ob.ref_info['poses'])).reshape(qn, -1)[:m].astype(np.float32)
+                d = take(qn * 4).reshape(qn, 4)[pick].astype(np.float32)
+                idx = take(qn)[pick].astype(np.int64)
+                sel_out = take(qn * 2).reshape(qn, 2)[pick].astype(np.float32)
+                logits = take(qn * len(ob.ref_info['poses'])).reshape(qn, -1)[pick].astype(np.float32)
                 inter.update({'det_position': d[:, :2].copy(), 'det_scale_r2q': d[:, 2].copy(), 'det_score': d[:, 3].copy(),
-                              'det_que_img': crops[o, :m].copy(), 'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': logits,
+                              'det_que_img': crops[o, pick].copy(), 'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': logits,
                               'sel_ref_idx': idx})
             inter['refine_poses'] = [first] + refined
             inter['bbox_pts'] = ring_h[o, np.arange(S), count_h[o] - 1].copy()

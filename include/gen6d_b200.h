@@ -64,6 +64,18 @@ int g6d_warp_perspective_u8(const g6d_warp_job* jobs, int n_jobs, uint8_t* out, 
 /* cv2.warpAffine(src, M, (w, h), flags=INTER_LINEAR), same conventions: the detection crop of
  * estimator.py:184 (utils/base_utils.py:646-655 transformation_crop). */
 int g6d_warp_affine_u8(const g6d_warp_job* jobs, int n_jobs, uint8_t* out, int h, int w, g6d_stream_t stream);
+/* Frames of different sizes as one zero-padded canvas (the `frames` argument of the g6d_glue_* kernels): frame i is
+ * the uint8 [rows, cols, 3] image at packed + offset, and canvas [n, H, W, 3] gets it in its top-left corner and 0 in
+ * every other byte (every byte is written).  A crop cut from the canvas with rows = H, cols = W equals the crop cut from
+ * the frame itself, bit for bit (taps outside a frame read the zero border either way).  host_table: HOST array [n],
+ * validated (rows <= H, cols <= W, each frame inside packed_bytes) and passed by value, n <= G6D_FRAMES_MAX. */
+#define G6D_FRAMES_MAX 1024
+typedef struct g6d_frame_entry {
+    long long offset;              /* byte offset of the frame in the packed buffer */
+    int rows, cols;
+} g6d_frame_entry;
+int g6d_frames_canvas(const uint8_t* packed, long long packed_bytes, const g6d_frame_entry* host_table, int n, uint8_t* canvas,
+                      int H, int W, g6d_stream_t stream);
 
 /* ---- camera algebra between the stages, on the device (estimator.py:176-214; utils/pose_utils.py:12-58,104-111,
  * 217-244; utils/database_utils.py:8-25,54-139; dataset/database.py:400-404,667-694).  With these four launches a
