@@ -17,7 +17,8 @@ G6D_GLUE_MAX_OBJECTS = 16                   # objects per g6d_glue_*_objects lau
 G6D_DET_MAX_INSTANCES = 16                  # instances per map of g6d_det_parse_peaks
 G6D_DET_MAX_PEAK_RADIUS = 3
 G6D_ATTENTION_MAX_SMEM_FLOATS = 12288 - 32  # n + C/heads of a g6d_attention call
-G6D_FRAMES_MAX = 1024                       # frames per g6d_frames_canvas launch
+G6D_FRAMES_MAX = 1024                       # frames per g6d_frames_canvas / g6d_frames_gather launch
+G6D_FRAME_RGB, G6D_FRAME_NV12 = 0, 1        # g6d_device_frame.format
 PRO_NONE, PRO_AFFINE, PRO_AFFINE_RELU, PRO_CORR = 0, 1, 2, 3
 ACT_NONE, ACT_RELU, ACT_LEAKY01 = 0, 1, 2
 TC_TF32, TC_F16 = 0, 1
@@ -59,6 +60,9 @@ _SIGNATURES = {
     'g6d_warp_perspective_u8': [P, I, P, I, I, P],
     'g6d_warp_affine_u8': [P, I, P, I, I, P],
     'g6d_frames_canvas': [P, L, P, I, P, I, I, P],
+    'g6d_frames_table_check': [P, I, L],
+    'g6d_frames_gather': [P, I, I, I, P, L, P],
+    'g6d_frames_gather_host': [P, I, P, L],
     'g6d_glue_detection_jobs': [P, P, I, I, I, I, P, P],
     'g6d_glue_detection_jobs_host': [P, P, I, I, I, I, P],
     'g6d_glue_initial_poses': [P, P, P, C.POINTER(GlueRefs), P, I, P, P],

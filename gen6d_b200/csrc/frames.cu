@@ -9,7 +9,11 @@
 // The canvas is written in one launch from the frames packed back to back.  Every byte is written, padding included,
 // so a graph replay never depends on what the canvas held before.  The table is a kernel parameter: it is fixed by the
 // frame sizes, which every captured graph of the canvas keys on.
+//
+// Frames already on the device (row f14) reach the packed layout through g6d_frames_gather below: a pitched copy for
+// RGB, OpenCV's NV12 conversion for decoder surfaces (frames_math.cuh).
 #include "common.cuh"
+#include "frames_math.cuh"
 
 namespace g6d {
 
@@ -51,7 +55,104 @@ int launch_canvas(const uint8_t* packed, const g6d_frame_entry* host_table, int 
     return G6D_OK;
 }
 
+// ------------------------------------------------------------------------------------------ device frames (row f14)
+// The first node of a captured graph over frames that are already on the device: the table (a graph input, uploaded per
+// call) holds their pointers and pitches, so the same graph serves every allocation and pitch of the same size pattern.
+
+constexpr int kGatherThreads = 128;
+
+// the conditions g6d_frames_table_check enforces on one entry; the kernel skips an entry that breaks them rather than
+// write outside `packed`
+__device__ __forceinline__ bool frame_ok(const g6d_device_frame& fe, long long packed_bytes) {
+    if (fe.rows <= 0 || fe.cols <= 0 || fe.offset < 0 || frames::frame_end(fe) > packed_bytes) return false;
+    if (fe.format == G6D_FRAME_NV12) return (fe.rows & 1) == 0 && (fe.cols & 1) == 0;
+    return fe.format == G6D_FRAME_RGB;
+}
+
+// grid (ceil(ceil(max_cols/2) / 128), ceil(max_rows/2), n): one 2x2 pixel block per thread, consecutive threads on
+// consecutive blocks of a row pair.  CTA (0, 0, i) also zeroes the bytes after frame i that no frame covers.
+__global__ void __launch_bounds__(kGatherThreads)
+frames_gather_kernel(const g6d_device_frame* __restrict__ table, int n, uint8_t* __restrict__ packed, long long packed_bytes) {
+    const int i = blockIdx.z;
+    const g6d_device_frame fe = table[i];
+    if (!frame_ok(fe, packed_bytes)) return;
+    if (blockIdx.x == 0 && blockIdx.y == 0) {
+        __shared__ long long runs[4];
+        if (threadIdx.x == 0) frames::gap_runs(table, n, i, packed_bytes, &runs[0], &runs[1], &runs[2], &runs[3]);
+        __syncthreads();
+        for (int r = 0; r < 2; ++r)
+            for (long long x = runs[2 * r] + threadIdx.x; x < runs[2 * r + 1]; x += kGatherThreads) packed[x] = 0;
+    }
+    const int bx = blockIdx.x * kGatherThreads + threadIdx.x, by = blockIdx.y;
+    if (2 * bx >= fe.cols || 2 * by >= fe.rows) return;
+    frames::gather_block(fe, bx, by, packed);
+}
+
 }  // namespace g6d
+
+static int check_table(const char* name, const g6d_device_frame* t, int n, long long packed_bytes) {
+    G6D_REQUIRE(t, "%s: null table", name);
+    G6D_REQUIRE(n > 0 && n <= G6D_FRAMES_MAX, "%s: n = %d frames, need 1..%d", name, n, G6D_FRAMES_MAX);
+    G6D_REQUIRE(packed_bytes > 0, "%s: packed_bytes = %lld", name, packed_bytes);
+    for (int i = 0; i < n; ++i) {
+        const g6d_device_frame& e = t[i];
+        G6D_REQUIRE(e.format == G6D_FRAME_RGB || e.format == G6D_FRAME_NV12, "%s: frame %d has unknown format %d (RGB %d, NV12 %d)",
+                    name, i, e.format, G6D_FRAME_RGB, G6D_FRAME_NV12);
+        G6D_REQUIRE(e.rows > 0 && e.cols > 0 && e.rows <= 131070, "%s: frame %d is %d x %d", name, i, e.rows, e.cols);
+        G6D_REQUIRE(e.plane0 && (e.format == G6D_FRAME_RGB || e.plane1), "%s: frame %d has a null plane", name, i);
+        if (e.format == G6D_FRAME_NV12) {
+            G6D_REQUIRE(e.rows % 2 == 0 && e.cols % 2 == 0, "%s: NV12 frame %d is %d x %d; NV12 needs an even height and width",
+                        name, i, e.rows, e.cols);
+            G6D_REQUIRE(e.pitch0 >= e.cols && e.pitch1 >= e.cols,
+                        "%s: NV12 frame %d has row pitches %lld (Y) and %lld (UV) below its width %d", name, i, e.pitch0, e.pitch1,
+                        e.cols);
+        } else {
+            G6D_REQUIRE(e.pitch0 >= 3LL * e.cols, "%s: RGB frame %d has row pitch %lld below 3 x its width %d", name, i, e.pitch0,
+                        e.cols);
+        }
+        G6D_REQUIRE(e.offset >= 0 && g6d::frames::frame_end(e) <= packed_bytes,
+                    "%s: frame %d (offset %lld, %d x %d) lies outside the %lld-byte packed buffer", name, i, e.offset, e.rows,
+                    e.cols, packed_bytes);
+    }
+    for (int i = 0; i < n; ++i)                 // no two packed images overlap (n <= G6D_FRAMES_MAX: at most 2^19 pairs)
+        for (int j = i + 1; j < n; ++j)
+            G6D_REQUIRE(t[i].offset >= g6d::frames::frame_end(t[j]) || t[j].offset >= g6d::frames::frame_end(t[i]),
+                        "%s: the packed images of frames %d and %d overlap", name, i, j);
+    return G6D_OK;
+}
+
+extern "C" int g6d_frames_table_check(const g6d_device_frame* host_table, int n, long long packed_bytes) {
+    return check_table("g6d_frames_table_check", host_table, n, packed_bytes);
+}
+
+extern "C" int g6d_frames_gather(const g6d_device_frame* table, int n, int max_rows, int max_cols, uint8_t* packed,
+                                 long long packed_bytes, g6d_stream_t stream) {
+    G6D_REQUIRE(table && packed && packed_bytes > 0, "g6d_frames_gather: null table or buffer, or empty packed buffer");
+    G6D_REQUIRE(n > 0 && n <= G6D_FRAMES_MAX, "g6d_frames_gather: n = %d frames, need 1..%d", n, G6D_FRAMES_MAX);
+    G6D_REQUIRE(max_rows > 0 && max_cols > 0 && max_rows <= 131070, "g6d_frames_gather: bad frame bound %d x %d", max_rows,
+                max_cols);
+    const long long blocks_x = ((long long)(max_cols + 1) / 2 + g6d::kGatherThreads - 1) / g6d::kGatherThreads;
+    dim3 grid((unsigned)blocks_x, (max_rows + 1) / 2, n);
+    g6d::frames_gather_kernel<<<grid, g6d::kGatherThreads, 0, g6d::as_stream(stream)>>>(table, n, packed, packed_bytes);
+    G6D_CHECK_LAUNCH("g6d_frames_gather");
+    return G6D_OK;
+}
+
+extern "C" int g6d_frames_gather_host(const g6d_device_frame* host_table, int n, uint8_t* packed, long long packed_bytes) {
+    const int rc = check_table("g6d_frames_gather_host", host_table, n, packed_bytes);
+    if (rc != G6D_OK) return rc;
+    G6D_REQUIRE(packed, "g6d_frames_gather_host: null packed buffer");
+    for (int i = 0; i < n; ++i) {
+        const g6d_device_frame& fe = host_table[i];
+        long long run[4];
+        g6d::frames::gap_runs(host_table, n, i, packed_bytes, &run[0], &run[1], &run[2], &run[3]);
+        for (int r = 0; r < 2; ++r)
+            for (long long x = run[2 * r]; x < run[2 * r + 1]; ++x) packed[x] = 0;
+        for (int by = 0; 2 * by < fe.rows; ++by)
+            for (int bx = 0; 2 * bx < fe.cols; ++bx) g6d::frames::gather_block(fe, bx, by, packed);
+    }
+    return G6D_OK;
+}
 
 extern "C" int g6d_frames_canvas(const uint8_t* packed, long long packed_bytes, const g6d_frame_entry* host_table, int n,
                                  uint8_t* canvas, int H, int W, g6d_stream_t stream) {

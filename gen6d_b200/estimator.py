@@ -109,7 +109,9 @@ class Gen6DEstimator:
                 'ref_ids': ref_ids, 'vert': vert, 'ids_all': ids_all}
 
     def predict(self, que_img, que_K, pose_init=None):
-        """estimator.py:173-216.  que_img uint8 [h,w,3], que_K [3,3] -> (pose [3,4], inter_results)."""
+        """estimator.py:173-216.  que_img uint8 [h,w,3], que_K [3,3] -> (pose [3,4], inter_results).  A numpy frame only:
+        frames on the GPU go through predict_batch (TypeError)."""
+        F.host_only([que_img], 'predict()')
         inter = {}
         res = self.cfg['ref_resolution']
         host_warps = self.cfg['host_warps']
@@ -149,11 +151,18 @@ class Gen6DEstimator:
         and device->host reads for the whole batch instead of per frame -- with the small per-frame camera
         algebra on the host in between.  Same results as predict() frame by frame.  Frames of different sizes take the
         device-glue path only (row f13: detection per size, the crops cut from one zero-padded canvas).
-        que_imgs: list / array of uint8 [h,w,3]; que_Ks: [qn,3,3].  Returns (poses [qn,3,4], inter dict of lists)."""
+        que_imgs: list / array of uint8 [h,w,3]; que_Ks: [qn,3,3].  Returns (poses [qn,3,4], inter dict of lists).
+        On the device-glue path que_imgs may instead be device frames (row f14; frames.as_frames): CUDA uint8 RGB tensors
+        [h,w,3] with any row pitch (or one [qn,h,w,3] tensor) and frames.NV12 decoder surfaces, mixed freely, with the
+        numpy path's results on the same RGB bytes.  They must be ready on the current stream; the call ends in its
+        synchronising read, after which they may be overwritten or freed."""
         qn, res = len(que_imgs), self.cfg['ref_resolution']
         que_Ks = [np.asarray(K) for K in que_Ks]
         device = self.cfg['device_glue'] and pose_inits is None and self._glue_possible()
-        imgs = [np.asarray(f) for f in que_imgs]
+        imgs = F.as_frames(que_imgs, 'predict_batch', self.detector,
+                           None if device else "predict_batch with pose_inits, cfg['device_glue'] off or cfg['host_warps'] on")
+        if F.is_device(imgs):                        # frames already on the GPU: gathered in the graph (row f14)
+            return self._predict_batch_device(None, que_Ks, F.check_frames(imgs, que_Ks, 'predict_batch'))
         if F.is_mixed(imgs):                         # frames of different sizes: the device glue path only (row f13)
             if not device:
                 F.require_one_size(imgs, "predict_batch with pose_inits, cfg['device_glue'] off or cfg['host_warps'] on")
@@ -319,7 +328,8 @@ class Gen6DEstimator:
         'refine_poses' a list of [qn,M,3,4], 'instance_valid' bool [qn,M] and 'instance_count' [qn].  Instance 0 is
         predict_batch's detection.  Rows of instances that were not found are computed too (on a repeat of instance 0's
         detection, so the graph keeps its shapes) and returned, masked by instance_valid: use only the valid rows.
-        One captured graph per (qn, frame shape, max_instances, peak_radius, nms_iou, min_score), one read per call."""
+        One captured graph per (qn, frame shape, max_instances, peak_radius, nms_iou, min_score), one read per call.
+        que_imgs may be device frames, with predict_batch's rules (row f14)."""
         from .objects import require_device_pipeline
         require_device_pipeline(self, 'predict_instances')
         key = instances.check_args(max_instances, nms_iou, peak_radius, min_score)
@@ -327,7 +337,7 @@ class Gen6DEstimator:
         qn, res = len(que_imgs), self.cfg['ref_resolution']
         if qn == 0 or len(que_Ks) != qn:
             raise ValueError(f'predict_instances: {qn} frames and {len(que_Ks)} intrinsics; need one K per frame and at least one frame')
-        imgs = [np.asarray(f) for f in que_imgs]
+        imgs = F.as_frames(que_imgs, 'predict_instances', self.detector)
         if F.is_mixed(imgs):
             F.check_frames(imgs, que_Ks, 'predict_instances')
         st = self._glue_state()
@@ -420,8 +430,10 @@ class Gen6DEstimator:
         at a time through predict_batch (batch = 1: plain predict), so one batch's host geometry overlaps
         another batch's kernels.  Same results as predict(); returns [(pose, inter)] (inter of a batched
         frame holds that frame's slices).  With batch > 1 the frames are grouped by size (in order of first
-        appearance) before they are cut into batches, so every batch has frames of one size."""
+        appearance) before they are cut into batches, so every batch has frames of one size.  Numpy frames only (TypeError
+        for frames on the GPU: predict_batch takes them)."""
         from concurrent.futures import ThreadPoolExecutor
+        F.host_only(que_imgs, 'predict_many')
         if len(que_imgs) == 0:
             return []
         # The clones share weights / reference features by reference and own captured graphs over them:

@@ -14,21 +14,140 @@ order into one buffer, each group at a 256-byte-aligned offset, and uploaded wit
 (h, w) of every frame) goes into every graph name: the graph caches key on input shapes only, and two patterns with the
 same packed length would otherwise share a graph.  A batch of one size takes none of this: the caller keeps its
 single-size path and graphs.
+
+Frames already on the GPU (row f14): a call's frames may instead all be device frames, CUDA uint8 RGB tensors [h, w, 3]
+with pitched rows or NV12 decoder surfaces (NV12), in any mix of sizes.  Their bytes never cross PCIe: the graph input
+is a device table of g6d_device_frame rows (plane pointers, pitches, size, format, offset in the packed layout), and
+the graph's first node, g6d_frames_gather, writes the packed layout of FramePlan from them (converting NV12 as
+cv2.cvtColor(COLOR_YUV2RGB_NV12) does).  From the packed buffer on, the graph is the numpy path's: the [qn, h, w, 3]
+view for one size, on_canvas for several.  Pointers and pitches live in the table, so a device-frame graph keys on the
+size pattern only, one size included ('device' in the name keeps it apart from the numpy graphs of that pattern), and a
+new allocation or pitch replays the same graph.
 """
+import ctypes as C
 import threading
 from contextlib import contextmanager
 
 import numpy as np
 import torch
 
-from . import ops
+from . import _lib, ops
 
 ALIGN = 256          # byte alignment of every size group in the packed input
 
+_DEVICE_PIPELINE = "device frames (CUDA tensors, NV12) go through the device pipeline only (cfg['device_glue'] on, cfg['host_warps'] off)"
+
+
+class NV12:
+    """An NV12 frame on the device, as GPU decoders hand it over: y the uint8 CUDA luma plane [h, w], uv the interleaved
+    (U, V) chroma plane [h/2, w], each with unit column stride and any row pitch >= w; h and w even.  It is converted as
+    cv2.cvtColor(np.vstack([y, uv]), cv2.COLOR_YUV2RGB_NV12) converts it (BT.601 limited range), bit for bit.  A decoder
+    surface t of [h*3/2, pitch] bytes is NV12(t[:h, :w], t[h:, :w])."""
+    __slots__ = ('y', 'uv')
+
+    def __init__(self, y, uv):
+        self.y, self.uv = y, uv
+
+    @property
+    def shape(self):
+        """(h, w, 3): the shape of the RGB frame it converts to."""
+        return (int(self.y.shape[0]), int(self.y.shape[1]), 3)
+
+    def __repr__(self):
+        return f'NV12({self.shape[0]}x{self.shape[1]}, {self.y.device})'
+
+
+def _gpu_frame(f):
+    return isinstance(f, NV12) or (isinstance(f, torch.Tensor) and f.is_cuda)
+
+
+def is_device(frames):
+    """True when the frames are device frames: a tensor, or a sequence holding a tensor or an NV12 frame."""
+    return isinstance(frames, torch.Tensor) or any(isinstance(f, (torch.Tensor, NV12)) for f in frames)
+
+
+def host_only(que_imgs, what):
+    """TypeError if any frame is on the GPU, on a path that takes numpy frames only (raised before anything is launched)."""
+    if isinstance(que_imgs, torch.Tensor) and que_imgs.is_cuda or any(_gpu_frame(f) for f in que_imgs):
+        raise TypeError(f'{what} takes numpy uint8 [h, w, 3] frames only: {_DEVICE_PIPELINE}')
+
+
+def as_frames(que_imgs, what, module, host_path=None):
+    """The frames of a call as a list: numpy arrays (np.asarray of each, the host upload path) or, when they are device
+    frames, RGB tensors [h, w, 3] and NV12 frames checked to be on module.device, the network's device, which is read
+    for device frames only (a [qn, h, w, 3] tensor counts as qn frames).
+    ValueError for a mix of numpy and device frames or a malformed device frame, before anything is enqueued.
+    host_path: None on the device pipeline, else the name of the numpy-only path the call takes (TypeError for frames
+    on the GPU)."""
+    if host_path is not None:
+        host_only(que_imgs, host_path)
+    elif is_device(que_imgs):
+        frames = list(que_imgs.unbind(0)) if isinstance(que_imgs, torch.Tensor) and que_imgs.dim() == 4 else list(que_imgs)
+        if isinstance(que_imgs, torch.Tensor) and que_imgs.dim() != 4:
+            raise ValueError(f'{what}: a frames tensor must be [qn, h, w, 3], got {list(que_imgs.shape)}')
+        for i, f in enumerate(frames):
+            _check_device_frame(f, i, what, torch.device(module.device))
+        return frames
+    return [np.asarray(f) for f in que_imgs]
+
+
+def _check_device_frame(f, i, what, device):
+    def plane(t, name, rows, cols, ch):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f'{what}: frame {i}: {name} is {type(t).__name__}, not a torch tensor; a call\'s frames are all numpy '
+                             'arrays or all device frames (CUDA tensors, NV12)')
+        if t.device != device:
+            raise ValueError(f'{what}: frame {i}: {name} is on {t.device}; device frames must be on {device}, the estimator\'s '
+                             'device (numpy arrays take the host upload path)')
+        if t.dtype != torch.uint8:
+            raise ValueError(f'{what}: frame {i}: {name} is {t.dtype}; device frames are uint8')
+        shape = [rows, cols] + ([ch] if ch else [])
+        if list(t.shape) != shape or rows < 1 or cols < 1:
+            raise ValueError(f'{what}: frame {i}: {name} is {list(t.shape)}, need {shape}')
+        unit = 3 if ch else 1
+        if (ch and t.stride(2) != 1) or (cols > 1 and t.stride(1) != unit) or (rows > 1 and t.stride(0) < unit * cols):
+            raise ValueError(f'{what}: frame {i}: {name} has strides {list(t.stride())}; need unit column steps '
+                             f'({"stride(2) == 1, stride(1) == 3" if ch else "stride(1) == 1"}) and a row pitch >= '
+                             f'{unit} x width')
+
+    if isinstance(f, NV12):
+        h, w = int(f.y.shape[0]) if f.y.dim() == 2 else -1, int(f.y.shape[1]) if f.y.dim() == 2 else -1
+        if h < 2 or w < 2 or h % 2 or w % 2:
+            raise ValueError(f'{what}: frame {i}: an NV12 Y plane must be [h, w] with h and w even, got {list(f.y.shape)}')
+        plane(f.y, 'the NV12 Y plane', h, w, 0)
+        plane(f.uv, 'the NV12 UV plane', h // 2, w, 0)
+    elif isinstance(f, torch.Tensor):
+        if f.dim() != 3:
+            raise ValueError(f'{what}: frame {i} is {list(f.shape)}; an RGB device frame is uint8 [h, w, 3]')
+        plane(f, 'the RGB frame', int(f.shape[0]), int(f.shape[1]), 3)
+    else:
+        raise ValueError(f'{what}: frame {i} is {type(f).__name__}; a call\'s frames are all numpy arrays or all device frames '
+                         '(CUDA tensors, NV12)')
+
+
+def device_table(frames, plan):
+    """Device frames + their FramePlan -> the HOST table (ctypes array of ops.DeviceFrame), checked by
+    g6d_frames_table_check: plane pointers, row pitches, size, format and the frame's offset in the packed layout."""
+    rows = []
+    for f, (off, h, w) in zip(frames, plan.table):
+        if isinstance(f, NV12):
+            rows.append(ops.DeviceFrame(f.y.data_ptr(), f.uv.data_ptr(), f.y.stride(0) if h > 1 else w, f.uv.stride(0) if h > 2 else w,
+                                        h, w, _lib.G6D_FRAME_NV12, off))
+        else:
+            rows.append(ops.DeviceFrame(f.data_ptr(), None, f.stride(0) if h > 1 else 3 * w, 0, h, w, _lib.G6D_FRAME_RGB, off))
+    table = (ops.DeviceFrame * len(rows))(*rows)
+    ops.frames_table_check(table, plan.nbytes)
+    return table
+
 
 def check_frames(que_imgs, que_Ks, what):
-    """-> the frames as numpy arrays; ValueError unless there is at least one frame, one K per frame and every frame is
-    uint8 [h, w, 3]."""
+    """-> the frames as numpy arrays (device frames, checked by as_frames, as they are); ValueError unless there is at
+    least one frame, one K per frame and every numpy frame is uint8 [h, w, 3]."""
+    if is_device(que_imgs):
+        frames = list(que_imgs)
+        if not frames or len(que_Ks) != len(frames):
+            raise ValueError(f'{what}: {len(frames)} frames and {len(que_Ks)} intrinsics; need one K per frame and at least one frame')
+        return frames
     frames = [np.asarray(f) for f in que_imgs]
     if not frames or len(que_Ks) != len(frames):
         raise ValueError(f'{what}: {len(frames)} frames and {len(que_Ks)} intrinsics; need one K per frame and at least one frame')
@@ -85,15 +204,47 @@ class FramePlan:
         offsets = [self.table[i][0] for _, _, idx, _ in self.groups for i in idx]
         return [module.upload_packed(arrays, offsets, self.nbytes), module._to_dev(self.order)]
 
+    def device_key(self, name):
+        """The graph name of `name` (the numpy path's name of this pattern) for device frames of this size pattern."""
+        return ('device', name, self.pattern)
 
-def stage(module, name, fn, frames, plan=None):
-    """A graph body fn(frames u8 [qn,h,w,3], *rest) and the numpy frames -> (graph name, graph body, frame inputs) for
-    StageCache.run(name, fn, frame inputs + rest).  One size: (name, fn, [the frames uploaded as [qn,h,w,3]]), exactly
-    the single-size path; several: the pattern's name, on_canvas(fn) and the packed upload."""
-    plan = plan or FramePlan(size_pattern(frames))
+    def device_upload(self, module, frames):
+        """Device frames -> graph inputs [table u8 [qn*56]] (one size) or [table, order int64 [qn]] (several): the checked
+        g6d_device_frame rows, uploaded like any small input.  The frames themselves are not copied."""
+        table = np.frombuffer(bytes(device_table(frames, self)), np.uint8)
+        return [module._to_dev(table)] + ([module._to_dev(self.order)] if self.mixed else [])
+
+    def gathered(self, fn):
+        """A graph body fn(frames u8 [qn,h,w,3], *rest) -> g(table, *rest) for device frames: g6d_frames_gather writes the
+        packed layout from the table, then fn runs on its [qn,h,w,3] view (one size) or through on_canvas (several)."""
+        qn, (h, w) = len(self.pattern), self.pattern[0]
+        body = on_canvas(fn, self) if self.mixed else fn
+
+        def g(table, *rest):
+            packed = ops.frames_gather(table, qn, self.H, self.W, self.nbytes)
+            return body(packed, *rest) if self.mixed else body(packed[:qn * h * w * 3].view(qn, h, w, 3), *rest)
+        return g
+
+
+def bind(module, name, fn, frames, plan):
+    """A graph name as the numpy path names it (the pattern's key for several sizes), its body fn(frames u8 [qn,h,w,3],
+    *rest) and the frames -> (graph name, graph body, frame inputs) for StageCache.run(name, body, frame inputs + rest).
+    Numpy frames of one size: (name, fn, [the frames uploaded as [qn,h,w,3]]), exactly the single-size path; of several:
+    on_canvas(fn) and the packed upload; device frames: the pattern's device key, the gather body and the table."""
+    if is_device(frames):
+        return plan.device_key(name), plan.gathered(fn), plan.device_upload(module, frames)
     if not plan.mixed:
         return name, fn, [module.upload_frame(frames)]
-    return plan.key(name), on_canvas(fn, plan), plan.upload(module, frames)
+    return name, on_canvas(fn, plan), plan.upload(module, frames)
+
+
+def stage(module, name, fn, frames, plan=None):
+    """A graph body fn(frames u8 [qn,h,w,3], *rest) and the frames (numpy, or device frames from as_frames) -> (graph
+    name, graph body, frame inputs) for StageCache.run(name, fn, frame inputs + rest).  Numpy frames of one size: (name,
+    fn, [the frames uploaded as [qn,h,w,3]]), exactly the single-size path; several: the pattern's name, on_canvas(fn)
+    and the packed upload; device frames: bind's device graph."""
+    plan = plan or FramePlan(size_pattern(frames))
+    return bind(module, plan.key(name) if plan.mixed else name, fn, frames, plan)
 
 
 # ------------------------------------------------------------------------------------------ detection per size

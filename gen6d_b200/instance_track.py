@@ -265,7 +265,8 @@ class InstanceTracker:
 
     # -------------------------------------------------------------- one step
     def step(self, frames, Ks):
-        """frames: S uint8 [h,w,3] (of one size or several, row f13); Ks: [S,3,3].  Returns (poses float32 [S,M,3,4], smoothed float64 [S,M,3,4],
+        """frames: S uint8 [h,w,3] (of one size or several, row f13; or device frames, row f14, as Tracker.step takes them);
+        Ks: [S,3,3].  Returns (poses float32 [S,M,3,4], smoothed float64 [S,M,3,4],
         track_ids int64 [S,M] (-1: empty slot), inter): inter['refine_poses'] a list of [S,M,3,4] (entry 0 the starting
         poses, float64 on a re-detection step; a row whose chain is shorter repeats its final pose), 'bbox_pts' and
         'smoothed_pts' [S,M,8,2].  Empty slots' poses and points are NaN.  A re-detection step adds predict_instances'
@@ -286,7 +287,7 @@ class InstanceTracker:
         F = est.cfg['refine_iter']
         if detecting and F < 1:
             raise ValueError("instance tracking needs cfg['refine_iter'] >= 1 (a re-detection step smooths float32 poses)")
-        imgs = [np.asarray(f) for f in frames]
+        imgs = fr.as_frames(frames, 'step', est.detector)
         plan = fr.FramePlan(fr.size_pattern(imgs))
         if plan.mixed:
             fr.check_frames(imgs, Ks, 'step')
@@ -421,7 +422,8 @@ class ObjectInstanceTracker(InstanceTracker):
         return [tuple(np.concatenate([slots[m * K + o][i] for m in range(M)]) for i in range(3)) for o in range(K)]
 
     def step(self, frames, Ks):
-        """frames: S uint8 [h,w,3] (of one size or several, row f13); Ks: [S,3,3] (shared by all objects).  Returns {name: (poses float32
+        """frames: S uint8 [h,w,3] (of one size or several, row f13; or device frames, row f14); Ks: [S,3,3] (shared by all
+        objects).  Returns {name: (poses float32
         [S,M,3,4], smoothed float64 [S,M,3,4], track_ids int64 [S,M], inter)}: per object what InstanceTracker.step returns,
         'det_score' included on a re-detection step; 'dropped' lists that object's ids only.  Ids are unique over every
         object of the tracker."""

@@ -229,13 +229,14 @@ class ObjectSet:
     def predict(self, que_imgs, que_Ks):
         """Every object's pose on the same qn frames (uint8 [h,w,3], of one size or several: row f13; que_Ks [qn,3,3]).
         Returns {name: (poses [qn,3,4], inter)}: inter has the keys and shapes of predict_batch's device-glue inter, plus
-        'det_score' [qn], the maximum of that object's detection score map (is the object in the frame at all)."""
+        'det_score' [qn], the maximum of that object's detection score map (is the object in the frame at all).
+        que_imgs may be device frames (CUDA RGB tensors, frames.NV12), with predict_batch's rules (row f14)."""
         self._check()
         est = self.est
         qn, res, iters = len(que_imgs), est.cfg['ref_resolution'], est.cfg['refine_iter']
         if qn == 0 or len(que_Ks) != qn:
             raise ValueError(f'predict: {qn} frames and {len(que_Ks)} intrinsics; need one K per frame and at least one frame')
-        imgs = [np.asarray(f) for f in que_imgs]
+        imgs = F.as_frames(que_imgs, 'predict', est.detector)
         if F.is_mixed(imgs):
             F.check_frames(imgs, que_Ks, 'predict')
         det = est.detector
@@ -283,7 +284,8 @@ class ObjectSet:
         with the shared query pyramid and correlation of predict().  Slot (m, o) -- instance m of object o -- goes through
         its own crop and object o's selection; a refinement step over the K*M*qn rows is one refiner stage.  Returns
         {name: (poses [qn,M,3,4], inter)} with predict_instances' keys.  Rows of instances that were not found are computed
-        and returned, masked by inter['instance_valid'].  One captured graph per argument set and frame shape, one read."""
+        and returned, masked by inter['instance_valid'].  One captured graph per argument set and frame shape, one read.
+        que_imgs may be device frames, with predict_batch's rules (row f14)."""
         self._check()
         key = instances.check_args(max_instances, nms_iou, peak_radius, min_score)
         est = self.est
@@ -291,7 +293,7 @@ class ObjectSet:
         qn, res, iters = len(que_imgs), est.cfg['ref_resolution'], est.cfg['refine_iter']
         if qn == 0 or len(que_Ks) != qn:
             raise ValueError(f'predict_instances: {qn} frames and {len(que_Ks)} intrinsics; need one K per frame and at least one frame')
-        imgs = [np.asarray(f) for f in que_imgs]
+        imgs = F.as_frames(que_imgs, 'predict_instances', est.detector)
         if F.is_mixed(imgs):
             F.check_frames(imgs, que_Ks, 'predict_instances')
         det = est.detector

@@ -118,6 +118,35 @@ def frames_canvas(packed, table, H, W):
     return out
 
 
+class DeviceFrame(C.Structure):       # g6d_device_frame
+    _fields_ = [('plane0', C.c_void_p), ('plane1', C.c_void_p), ('pitch0', C.c_longlong), ('pitch1', C.c_longlong),
+                ('rows', C.c_int), ('cols', C.c_int), ('format', C.c_int), ('offset', C.c_longlong)]
+
+
+def frames_table_check(table, nbytes):
+    """A HOST array of DeviceFrame (ctypes) -> None; Gen6DLibraryError (G6D_EINVAL, with the message) unless every entry
+    is valid for a packed buffer of nbytes bytes (g6d_frames_table_check)."""
+    _call('g6d_frames_table_check', table, len(table), int(nbytes))
+
+
+def frames_gather(table, n, max_rows, max_cols, nbytes):
+    """table: the bytes of n DeviceFrame entries on the device (uint8 [n*sizeof]) -> packed u8 [nbytes]: every frame's RGB
+    image at its offset, 0 elsewhere (g6d_frames_gather)."""
+    if table.dtype != torch.uint8 or table.numel() != n * C.sizeof(DeviceFrame):
+        raise ValueError(f'frames_gather: table must be the packed bytes of {n} g6d_device_frame records')
+    out = torch.empty(int(nbytes), device=table.device, dtype=torch.uint8)
+    _call('g6d_frames_gather', _p(table, torch.uint8), n, max_rows, max_cols, _p(out, torch.uint8), int(nbytes), _stream())
+    return out
+
+
+def frames_gather_host(table, nbytes):
+    """g6d_frames_gather on the host: a HOST array of DeviceFrame over host planes -> numpy u8 [nbytes]."""
+    import numpy as np
+    out = np.empty(int(nbytes), np.uint8)
+    _call('g6d_frames_gather_host', table, len(table), out.ctypes.data_as(C.c_void_p), int(nbytes))
+    return out
+
+
 # ------------------------------------------------------------------------------- camera algebra between the stages
 def glue_detection_jobs(det_out, frames, size):
     """det_out [qn,4] (g6d_det_parse) + frames u8 [qn,h,w,3] -> packed g6d_warp_job records [qn*88] of the selector crops."""

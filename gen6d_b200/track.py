@@ -359,7 +359,9 @@ class Tracker:
 
     # -------------------------------------------------------------- one step
     def step(self, frames, Ks):
-        """frames: S uint8 [h,w,3] (of different sizes on the device path, row f13); Ks: [S,3,3].  Returns (raw poses float32 [S,3,4], smoothed poses float64
+        """frames: S uint8 [h,w,3] (of different sizes on the device path, row f13; or, on that path, device frames with
+        predict_batch's rules, row f14: CUDA RGB tensors and frames.NV12 surfaces, ready on the current stream and free to
+        reuse when step returns); Ks: [S,3,3].  Returns (raw poses float32 [S,3,4], smoothed poses float64
         [S,3,4], inter): inter['refine_poses'] is this step's chain, inter['bbox_pts'] the projected box corners
         [S,8,2], inter['smoothed_pts'] their weighted average [S,8,2]; a full-prediction step adds the detection and
         selection entries of predict_batch.  A mixed step (some sequences re-initialised by reset(sequences), or previous
@@ -372,11 +374,13 @@ class Tracker:
         Ks = np.stack([np.asarray(K) for K in Ks], 0)
         kind = self._kind()
         device = self._device_path()
+        host_path = "tracking with cfg['device_glue'] off or cfg['host_warps'] on"
+        imgs = fr.as_frames(frames, 'step', self.est.detector, None if device else host_path)
         if not device:
-            fr.require_one_size(frames, "tracking with cfg['device_glue'] off or cfg['host_warps'] on")
-        elif fr.is_mixed(frames):
-            fr.check_frames(frames, Ks, 'step')
-        out = self._step_device(frames, Ks, kind) if device else self._step_host(frames, Ks, kind)
+            fr.require_one_size(frames, host_path)
+        elif fr.is_mixed(imgs):
+            fr.check_frames(imgs, Ks, 'step')
+        out = self._step_device(imgs, Ks, kind) if device else self._step_host(frames, Ks, kind)
         self._pending[:] = False
         return out
 
@@ -476,7 +480,7 @@ class Tracker:
         st = est._glue_state()
         self._to(True)
         full = kind == 'full'
-        imgs = [np.asarray(f) for f in frames]
+        imgs = frames                                     # numpy or device frames (as_frames)
         plan, pick = fr.FramePlan(fr.size_pattern(imgs)), None
         with torch.no_grad():
             if full:
@@ -490,15 +494,15 @@ class Tracker:
                 outs = self.stages.run(name, fn, fin + [cams, self._prev, self._ring, self._count])
             else:
                 F, dev = est.cfg['refine_iter'], est.detector.device
-                fin = plan.upload(est.detector, imgs) if plan.mixed else [est.detector.upload_frame(imgs)]
-                cams = est.detector._to_dev(glue.cameras(Ks))
                 reinit, b, extra = _mixed_inputs(S, 1, self._pending, self._f32, F, self.refine_iter, dev, plan)
-                prev = self._prev if self._prev is not None else torch.zeros(S, 12, dtype=torch.float64, device=dev)
                 if plan.mixed:                   # one graph per size pattern and per-size buckets (row f13)
                     _, blocks, pick = _size_buckets(reinit, plan)
-                    name, fn = (plan.key('track_mixed'), tuple(blocks)), fr.on_canvas(self._mixed_fn(st, b, blocks), plan)
+                    name, fn = (plan.key('track_mixed'), tuple(blocks)), self._mixed_fn(st, b, blocks)
                 else:
                     name, fn = f'track_mixed{b}', self._mixed_fn(st, b)
+                name, fn, fin = fr.bind(est.detector, name, fn, imgs, plan)
+                cams = est.detector._to_dev(glue.cameras(Ks))
+                prev = self._prev if self._prev is not None else torch.zeros(S, 12, dtype=torch.float64, device=dev)
                 outs = self.stages.run(name, fn, fin + [cams, prev, self._ring, self._count] + extra)
             buf, poses_dev, ring, count = outs
             self._prev = poses_dev.clone()
@@ -722,7 +726,8 @@ class ObjectTracker:
                          objs[0].tables['tables']['ref_num'], self.est.refiner._refine_warped(128), smooth, blocks)
 
     def step(self, frames, Ks):
-        """frames: S uint8 [h,w,3] (of one size or several, row f13); Ks: [S,3,3] (shared by all objects).  Returns {name: (raw poses float32
+        """frames: S uint8 [h,w,3] (of one size or several, row f13; or device frames, row f14, as Tracker.step takes them);
+        Ks: [S,3,3] (shared by all objects).  Returns {name: (raw poses float32
         [S,3,4], smoothed poses float64 [S,3,4], inter)}: inter has Tracker.step's keys, and a full-prediction step adds
         those of ObjectSet.predict (det_score included); a mixed step adds 'reinit' and those entries for the
         re-initialised sequences, as Tracker.step does."""
@@ -735,7 +740,7 @@ class ObjectTracker:
             raise ValueError(f'step: Ks must be [{S},3,3], got {Ks.shape}')
         kind = self._kind()
         full, mixed = kind == 'full', kind == 'mixed'
-        imgs = [np.asarray(f) for f in frames]
+        imgs = fr.as_frames(frames, 'step', est.detector)
         plan, pick = fr.FramePlan(fr.size_pattern(imgs)), None
         if plan.mixed:
             fr.check_frames(imgs, Ks, 'step')
@@ -751,15 +756,15 @@ class ObjectTracker:
                 outs = self.stages.run(name, fn, fin + [cams, self._prev, self._ring, self._count])
             else:
                 dev = est.detector.device
-                fin = plan.upload(est.detector, imgs) if plan.mixed else [est.detector.upload_frame(imgs)]
-                cams = est.detector._to_dev(glue.cameras(Ks))
                 reinit, b, extra = _mixed_inputs(S, K, self._pending, self._f32, est.cfg['refine_iter'], self.refine_iter, dev, plan)
-                prev = self._prev if self._prev is not None else torch.zeros(K * S, 12, dtype=torch.float64, device=dev)
                 if plan.mixed:                   # one graph per size pattern and per-size buckets (row f13)
                     _, blocks, pick = _size_buckets(reinit, plan)
-                    name, fn = (plan.key('track_mixed'), tuple(blocks)), fr.on_canvas(self._mixed_fn(b, blocks), plan)
+                    name, fn = (plan.key('track_mixed'), tuple(blocks)), self._mixed_fn(b, blocks)
                 else:
                     name, fn = f'track_mixed{b}', self._mixed_fn(b)
+                name, fn, fin = fr.bind(est.detector, name, fn, imgs, plan)
+                cams = est.detector._to_dev(glue.cameras(Ks))
+                prev = self._prev if self._prev is not None else torch.zeros(K * S, 12, dtype=torch.float64, device=dev)
                 outs = self.stages.run(name, fn, fin + [cams, prev, self._ring, self._count] + extra)
             buf, poses_dev, ring, count = outs
             prev_f32 = bool(self._f32[0])

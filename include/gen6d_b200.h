@@ -76,6 +76,32 @@ typedef struct g6d_frame_entry {
 } g6d_frame_entry;
 int g6d_frames_canvas(const uint8_t* packed, long long packed_bytes, const g6d_frame_entry* host_table, int n, uint8_t* canvas,
                       int H, int W, g6d_stream_t stream);
+/* Frames already on the device (a decoder surface, a CUDA RGB tensor) into the packed layout of g6d_frames_canvas:
+ * frame i of the table becomes the tightly packed uint8 [rows, cols, 3] RGB image at packed + offset.
+ *   G6D_FRAME_RGB:  plane0 is the RGB image, pixel (y, x) at plane0 + y*pitch0 + 3*x (pitch0 >= 3*cols); a pitched copy.
+ *   G6D_FRAME_NV12: plane0 the Y plane [rows, cols] (row pitch pitch0 >= cols), plane1 the interleaved U,V plane
+ *                   [rows/2, cols] (pitch1 >= cols); rows and cols even.  Converted as cv2.cvtColor(COLOR_YUV2RGB_NV12)
+ *                   does, bit for bit: BT.601 limited range in OpenCV's 20-bit fixed point (csrc/frames_math.cuh).
+ * Planes need no alignment.  Every byte of packed is written: bytes no frame covers get 0, so a graph replay never
+ * depends on what packed held before.  g6d_frames_table_check validates a HOST copy of a table: formats, positive and
+ * (NV12) even sizes, non-null planes, pitches, every frame inside packed_bytes, no two frames overlapping, and
+ * 1 <= n <= G6D_FRAMES_MAX; G6D_EINVAL with a message otherwise.  g6d_frames_gather reads `table` from DEVICE memory
+ * (like g6d_warp_job arrays), so the pointers and pitches of a captured launch change with the table's contents; the
+ * caller checks the table before uploading it, and max_rows / max_cols bound every frame's size.  The frames must be
+ * ready on `stream`.  g6d_frames_gather_host runs the same code on a HOST table of host planes (checked first). */
+#define G6D_FRAME_RGB 0
+#define G6D_FRAME_NV12 1
+typedef struct g6d_device_frame {
+    const uint8_t* plane0;         /* RGB: the [rows, cols, 3] image; NV12: the Y plane */
+    const uint8_t* plane1;         /* NV12: the interleaved U,V plane; RGB: unused */
+    long long pitch0, pitch1;      /* row pitches in bytes */
+    int rows, cols, format;
+    long long offset;              /* byte offset of the frame's packed [rows, cols, 3] image */
+} g6d_device_frame;
+int g6d_frames_table_check(const g6d_device_frame* host_table, int n, long long packed_bytes);
+int g6d_frames_gather(const g6d_device_frame* table, int n, int max_rows, int max_cols, uint8_t* packed, long long packed_bytes,
+                      g6d_stream_t stream);
+int g6d_frames_gather_host(const g6d_device_frame* host_table, int n, uint8_t* packed, long long packed_bytes);
 
 /* ---- camera algebra between the stages, on the device (estimator.py:176-214; utils/pose_utils.py:12-58,104-111,
  * 217-244; utils/database_utils.py:8-25,54-139; dataset/database.py:400-404,667-694).  With these four launches a
