@@ -119,6 +119,39 @@ __device__ __forceinline__ void kblock_src(const ConvTcP& p, int sp, int it, int
     }
 }
 
+// The (tap, channel block) sequence of one chain, stepped K-block by K-block in kblock_src's order without its divides:
+// the split-input TMA thread issues every load of the CTA alone, so its per-K-block integer work is on the critical path
+// of the whole pipeline.  The tap is kept as (kx, ky, kz); start() pays the divides once per chain.
+struct KbIter {
+    int kx, ky, kz, cb;
+    __device__ __forceinline__ void start(const ConvTcP& p, int sp, int it) {
+        int tap;
+        kblock_src(p, sp, it, tap, cb);
+        kx = tap % p.kw;
+        const int tq = tap / p.kw;
+        ky = tq % p.kh;
+        kz = tq / p.kh;
+    }
+    __device__ __forceinline__ void next(const ConvTcP& p) {
+        if (p.reuse_order) {                                 // channel block, then kz, then (ky, kx)
+            if (++kx < p.kw) return;
+            kx = 0;
+            if (++ky < p.kh) return;
+            ky = 0;
+            if (++kz < p.kd) return;
+            kz = 0; ++cb;
+        } else {                                             // tap-major, channel blocks innermost
+            if (++cb < p.Cin / 64) return;
+            cb = 0;
+            if (++kx < p.kw) return;
+            kx = 0;
+            if (++ky < p.kh) return;
+            ky = 0; ++kz;
+        }
+    }
+    __device__ __forceinline__ int tap(const ConvTcP& p) const { return (kz * p.kh + ky) * p.kw + kx; }
+};
+
 // ------------------------------------------------------------------------------------------ operand split
 // fp16 pair (element 0 in the low half, as laid out in memory), saturating instead of overflowing to inf
 __device__ __forceinline__ uint32_t cvt_f16x2_sat(float e0, float e1) {
@@ -430,11 +463,6 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
             // the rank-5 map, see make_split_input_map.
             if (threadIdx.x == 0) {
                 const bool vol = p.D > 1 || p.kd > 1;
-                auto kcoord = [&](int sp, int it) {             // K coordinate of the weight tiles of a K-block
-                    int tap, cb;
-                    kblock_src(p, sp, it, tap, cb);
-                    return tap * p.Cin + cb * BK;
-                };
                 int g = 0;
                 int mt, nt, sp;
                 for (int j = 0; chain_of(j, mt, nt, sp); ++j) {
@@ -444,20 +472,23 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
                     const int yo = m % p.Ho; m /= p.Ho;
                     const int zo = m % p.Do;
                     const int b = m / p.Do;
-                    // L2 prefetch of the weight tiles PF K-blocks ahead, as the consumers' weight stream does
-                    for (int i = 0; i < min(nkb, PF - 1); ++i) {
-                        tma_prefetch_2d(&map_hi, kcoord(sp, i), nt * BN);
-                        tma_prefetch_2d(&map_lo, kcoord(sp, i), nt * BN);
-                    }
-                    for (int it = 0; it < nkb; ++it, ++g) {
-                        if (it + PF - 1 < nkb) {
-                            tma_prefetch_2d(&map_hi, kcoord(sp, it + PF - 1), nt * BN);
-                            tma_prefetch_2d(&map_lo, kcoord(sp, it + PF - 1), nt * BN);
-                        }
-                        int tap, cb;
-                        kblock_src(p, sp, it, tap, cb);
-                        const uint16_t ox = (uint16_t)(tap % p.kw), oy = (uint16_t)((tap / p.kw) % p.kh);
-                        const uint16_t oz = (uint16_t)(tap / (p.kw * p.kh));
+                    // L2 prefetch of the weight tiles PF K-blocks ahead, as the consumers' weight stream does: pf is the
+                    // next K-block to prefetch, k the one to load
+                    KbIter pf, k;
+                    pf.start(p, sp, 0);
+                    k = pf;
+                    auto prefetch = [&]() {
+                        const int kc = pf.tap(p) * p.Cin + pf.cb * BK;
+                        tma_prefetch_2d(&map_hi, kc, nt * BN);
+                        tma_prefetch_2d(&map_lo, kc, nt * BN);
+                        pf.next(p);
+                    };
+#pragma unroll 1
+                    for (int i = 0; i < min(nkb, PF - 1); ++i) prefetch();
+                    for (int it = 0; it < nkb; ++it, ++g, k.next(p)) {
+                        if (it + PF - 1 < nkb) prefetch();
+                        const int tap = k.tap(p), cb = k.cb;
+                        const uint16_t ox = (uint16_t)k.kx, oy = (uint16_t)k.ky, oz = (uint16_t)k.kz;
                         const int s = g % STAGES;
                         mbar_wait(empty(s), ((g / STAGES) & 1) ^ 1, 1, g);
                         mbar_expect_tx(full_b(s), 2 * Cfg::B_BYTES);
