@@ -100,6 +100,7 @@ struct ConvTcP {
     int split_in;                             // A tiles by TMA im2col from the pre-split input (see split_input_ok)
     int reuse_order;                          // K-blocks in the A-reuse kernel's order (G6D_TC_REUSE_IM2COL, see kblock_src)
     int fold;                                 // a work item is a tile whose K splits one CTA sums (G6D_TC_FOLD_SPLITS)
+    int xr, Wp, Mp, xr_rows;                  // one A box per row of taps (see xr_ok): padded width, rows, box pixels
 };
 
 // Filter tap (kz, ky, kx flattened) and 64-channel block of K-block `it` of split `sp` when the input is split
@@ -390,13 +391,27 @@ template <int BN> struct Tc2Cfg {
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
 };
 
+// One A box per row of taps (XR, see xr_ok): BOXES slots of hi / lo boxes of up to BOX_ROWS pixels (roundup8(128 + kw - 1)
+// for kw <= 17, a whole number of 1024-byte swizzle atoms), released after the last kx tap of their (cb, kz, ky) group,
+// and a ring of B_STAGES weight stages with their own barriers.
+template <int BN> struct Tc2XrCfg {
+    static constexpr int BOX_ROWS = 144;
+    static constexpr int BOX_BYTES = BOX_ROWS * 128;
+    static constexpr int BOXES = 3;
+    static constexpr int B_BYTES = BN * 128;
+    static constexpr int B_STAGES = 6;
+    static constexpr int SMEM_BYTES = BOXES * 2 * BOX_BYTES + B_STAGES * 2 * B_BYTES + 1024 + 256;
+};
+static_assert(Tc2XrCfg<64>::SMEM_BYTES <= 227 * 1024, "x-reuse rings of BN 64");
+
 struct Tc2Work { int m_tiles, n_tiles, total; };
 
-template <int BN, int KIND, bool FOLD>
+template <int BN, int KIND, bool FOLD, bool XR>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUtensorMap map_hi,
                 const __grid_constant__ CUtensorMap map_lo, const __grid_constant__ CUtensorMap map_a) {
     using Cfg = Tc2Cfg<BN>;
+    using XC = Tc2XrCfg<BN>;
     using KC = KindCfg<KIND>;
     constexpr int NPW = TC_PRODUCER_WARPS;
     constexpr int STAGES = Cfg::STAGES;
@@ -416,9 +431,33 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
     auto full_a = [&](int s) { return bar_base + 8 * s; };
     auto full_b = [&](int s) { return bar_base + 8 * (STAGES + s); };
     auto empty = [&](int s) { return bar_base + 8 * (2 * STAGES + s); };
+    // XR layout: the box slots, then the weight stages, then their barriers
+    auto box_hi = [&](int s) { return base + s * 2 * XC::BOX_BYTES; };
+    auto box_lo = [&](int s) { return base + s * 2 * XC::BOX_BYTES + XC::BOX_BYTES; };
+    const uint32_t xb_base = base + XC::BOXES * 2 * XC::BOX_BYTES;
+    auto xb_hi = [&](int s) { return xb_base + s * 2 * XC::B_BYTES; };
+    auto xb_lo = [&](int s) { return xb_base + s * 2 * XC::B_BYTES + XC::B_BYTES; };
+    const uint32_t xbar = xb_base + XC::B_STAGES * 2 * XC::B_BYTES;
+    auto box_full = [&](int s) { return xbar + 8 * s; };
+    auto box_empty = [&](int s) { return xbar + 8 * (XC::BOXES + s); };
+    auto xb_full = [&](int s) { return xbar + 8 * (2 * XC::BOXES + s); };
+    auto xb_empty = [&](int s) { return xbar + 8 * (2 * XC::BOXES + XC::B_STAGES + s); };
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == TC_ISSUER) {
+    if (XR && threadIdx.x == TC_ISSUER) {
+        for (int s = 0; s < XC::BOXES; ++s) {
+            mbar_init(box_full(s), 1);
+            mbar_init(box_empty(s), TC_CONSUMER_WARPS);
+        }
+        for (int s = 0; s < XC::B_STAGES; ++s) {
+            mbar_init(xb_full(s), 1);
+            mbar_init(xb_empty(s), TC_CONSUMER_WARPS);
+        }
+        fence_barrier_init();
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_hi) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_lo) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
+    } else if (threadIdx.x == TC_ISSUER) {
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(full_a(s), p.split_in ? 1 : NPW);   // the A TMA transaction, or the producer warps
             mbar_init(full_b(s), 1);          // the TMA transaction
@@ -453,7 +492,58 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
 
     if (warp < NPW) {
         setmaxnreg_dec<FOLD ? TC_FOLD_PRODUCER_REGS : TC_PRODUCER_REGS>();
-        if (FOLD || p.split_in) {
+        if (XR && threadIdx.x == 0) {
+            // One box pair per (cb, kz, ky) group of kw consecutive K-blocks (the A-reuse K order starts every chain at
+            // kx = 0), over the padded enumeration of Wp columns: tile row j + kx of the box is tap kx of row j.  The
+            // weight tiles go to their own ring, one stage per K-block.
+            const bool vol = p.D > 1 || p.kd > 1;
+            const uint32_t box_tx = 2u * p.xr_rows * 128u;
+            int g = 0, gb = 0;                               // K-blocks, boxes
+            int mt, nt, sp;
+            for (int j = 0; chain_of(j, mt, nt, sp); ++j) {
+                const int nkb = kblocks_of(sp);
+                int m = mt * TC_BM;
+                const int xo = m % p.Wp; m /= p.Wp;
+                const int yo = m % p.Ho; m /= p.Ho;
+                const int zo = m % p.Do;
+                const int b = m / p.Do;
+                KbIter pf, k;
+                pf.start(p, sp, 0);
+                k = pf;
+                auto prefetch = [&]() {
+                    const int kc = pf.tap(p) * p.Cin + pf.cb * BK;
+                    tma_prefetch_2d(&map_hi, kc, nt * BN);
+                    tma_prefetch_2d(&map_lo, kc, nt * BN);
+                    pf.next(p);
+                };
+#pragma unroll 1
+                for (int i = 0; i < min(nkb, PF - 1); ++i) prefetch();
+                for (int it = 0; it < nkb; ++it, ++g, k.next(p)) {
+                    if (it + PF - 1 < nkb) prefetch();
+                    if (k.kx == 0) {
+                        const int s = gb % XC::BOXES;
+                        const uint16_t oy = (uint16_t)k.ky, oz = (uint16_t)k.kz;
+                        mbar_wait(box_empty(s), ((gb / XC::BOXES) & 1) ^ 1, 6, gb);
+                        mbar_expect_tx(box_full(s), box_tx);
+                        if (vol) {
+                            tma_im2col_5d(box_hi(s), &map_a, box_full(s), 2 * BK * k.cb, xo - p.pw, yo - p.ph, zo - p.pd, b, 0, oy, oz);
+                            tma_im2col_5d(box_lo(s), &map_a, box_full(s), 2 * BK * k.cb + BK, xo - p.pw, yo - p.ph, zo - p.pd, b, 0, oy, oz);
+                        } else {
+                            tma_im2col_4d(box_hi(s), &map_a, box_full(s), 2 * BK * k.cb, xo - p.pw, yo - p.ph, b, 0, oy);
+                            tma_im2col_4d(box_lo(s), &map_a, box_full(s), 2 * BK * k.cb + BK, xo - p.pw, yo - p.ph, b, 0, oy);
+                        }
+                        ++gb;
+                    }
+                    const int s = g % XC::B_STAGES;
+                    mbar_wait(xb_empty(s), ((g / XC::B_STAGES) & 1) ^ 1, 1, g);
+                    mbar_expect_tx(xb_full(s), 2 * XC::B_BYTES);
+                    tma_load_2d(xb_hi(s), &map_hi, xb_full(s), k.tap(p) * p.Cin + k.cb * BK, nt * BN);
+                    tma_load_2d(xb_lo(s), &map_lo, xb_full(s), k.tap(p) * p.Cin + k.cb * BK, nt * BN);
+                }
+            }
+            return;
+        }
+        if (XR || FOLD || p.split_in) {
             // =========================== A by TMA im2col ===========================
             // The input is already split (hi / lo of channel block cb at channels [128 cb, 128 cb + 64) /
             // [128 cb + 64, 128 cb + 128) of each pixel, in f16_k_source order), so a K-block of tap (kx, ky)
@@ -461,7 +551,7 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
             // below would store.  One thread issues them, and the stage's weight tiles with them (the consumers
             // then issue no loads); the other producer warps have nothing to do.  Volumes (D > 1 or kd > 1) use
             // the rank-5 map, see make_split_input_map.
-            if (threadIdx.x == 0) {
+            if (!XR && threadIdx.x == 0) {
                 const bool vol = p.D > 1 || p.kd > 1;
                 int g = 0;
                 int mt, nt, sp;
@@ -611,7 +701,7 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
         setmaxnreg_inc<FOLD ? TC_FOLD_CONSUMER_REGS : TC_CONSUMER_REGS>();
         const int cw = warp - NPW;                     // consumer warp: rows 16 cw .. 16 cw + 15 of the tile
         const uint32_t a_row = (cw >> 2) * 64 * 128;   // this warpgroup's 64 rows of the A tiles
-        const bool issuer = !FOLD && threadIdx.x == TC_ISSUER && !p.split_in;      // with the split input, the A issuer loads B
+        const bool issuer = !FOLD && !XR && threadIdx.x == TC_ISSUER && !p.split_in;   // with the split input, the A issuer loads B
         // weight-tile stream of the issuer: the next global K-block lg = K-block lit of work item lw
         int lw = blockIdx.x, lit = 0, lg = 0;
         auto load_next = [&]() {
@@ -655,10 +745,48 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
         float cross[BN / 2];
         float run[FOLD ? BN / 2 : 1];                  // FOLD: the tile's sum of its splits so far
         int g = 0;
+        int gb = 0, rb = 0;                            // XR: boxes awaited, boxes released
+        // XR: the weight stage of K-block g is free, and with it the box of a group whose last tap it was
+        auto xr_release = [&](int g, bool box_done) {
+            __syncwarp();
+            if (lane == 0) {
+                mbar_arrive(xb_empty(g % XC::B_STAGES));
+                if (box_done) mbar_arrive(box_empty(rb % XC::BOXES));
+            }
+            if (box_done) ++rb;
+        };
         int mt, nt, sp;
         for (int j = 0; chain_of(j, mt, nt, sp); ++j) {
             const int nkb = kblocks_of(sp);
             zero_acc<BN, NMAIN>(acc, cross);
+            if constexpr (XR) {
+                // tap kx of a (cb, kz, ky) group reads the group's box shifted by kx rows
+                int kx = 0;
+                bool box_done = false;
+                for (int it0 = 0; it0 < nkb; it0 += NMAIN) {
+#pragma unroll
+                    for (int a = 0; a < NMAIN; ++a) {
+                        const int it = it0 + a;
+                        if (it < nkb) {
+                            if (kx == 0) {
+                                mbar_wait(box_full(gb % XC::BOXES), (gb / XC::BOXES) & 1, 7, gb);
+                                ++gb;
+                            }
+                            const int s = g % XC::B_STAGES, sb = (gb - 1) % XC::BOXES;
+                            mbar_wait(xb_full(s), (g / XC::B_STAGES) & 1, 5, g);
+                            const uint32_t sh = a_row + kx * 128;
+                            mma_stage<BN, KIND>(acc[a], cross, box_hi(sb) + sh, box_lo(sb) + sh, xb_hi(s), xb_lo(s));
+                            wgmma_wait<1>();
+                            if (it > 0) xr_release(g - 1, box_done);
+                            box_done = kx == p.kw - 1;
+                            ++g;
+                            if (++kx == p.kw) kx = 0;
+                        }
+                    }
+                }
+                wgmma_wait<0>();
+                if (nkb > 0) xr_release(g - 1, true);
+            } else {
             for (int it0 = 0; it0 < nkb; it0 += NMAIN) {
 #pragma unroll
                 for (int a = 0; a < NMAIN; ++a) {              // K-block it uses main accumulator it % NMAIN
@@ -676,6 +804,7 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
             }
             wgmma_wait<0>();
             if (nkb > 0) release(g - 1);
+            }
 
             sum_chains<BN, KIND>(acc, cross, nkb < NMAIN ? nkb : NMAIN);
             if constexpr (FOLD) {
@@ -695,7 +824,18 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
             // 64-bit stores need 8-byte aligned column pairs
             const bool vec2 = partial ? (p.Cout & 1) == 0
                                       : ((p.ocs & 1) == 0 && (p.oco & 1) == 0 && (reinterpret_cast<uintptr_t>(p.y) & 7) == 0);
-            store_tile<BN>(cross, m0 < p.M ? out + m0 * ld : nullptr, m1 < p.M ? out + m1 * ld : nullptr, n_base, p.Cout, p.bias,
+            // XR: m0 / m1 count the padded enumeration; its columns xp >= Wo are never written (no fused moments either:
+            // XR plans take them from y, see g6d_conv_tc_ex)
+            auto dst = [&](int m) -> float* {
+                if constexpr (XR) {
+                    if (m >= p.Mp) return nullptr;
+                    const int q = m / p.Wp, xp = m - q * p.Wp;
+                    return xp < p.Wo ? out + ((long long)q * p.Wo + xp) * ld : nullptr;
+                } else {
+                    return m < p.M ? out + m * ld : nullptr;
+                }
+            };
+            store_tile<BN>(cross, dst(m0), dst(m1), n_base, p.Cout, p.bias,
                            p.act, partial, vec2, p.stats, (long long)(mt * TC_BM + 16 * cw) / p.stats_rows, lane);
         }
     }
@@ -893,7 +1033,7 @@ static EncodeIm2colFn get_encode_im2col_fn() {
 // (D > 1 or kd > 1, the same test as the kernel's) get the rank-5 map over [B, D, H, W, 2 Cin].
 static bool split_input_rank5(const g6d_conv_desc* d) { return d->D > 1 || d->kd > 1; }
 
-static int make_split_input_map(CUtensorMap* map, const void* xs, const g6d_conv_desc* d) {
+static int make_split_input_map(CUtensorMap* map, const void* xs, const g6d_conv_desc* d, int xr_rows) {
     EncodeIm2colFn enc = get_encode_im2col_fn();
     if (!enc) { set_error("g6d_conv_tc: cuTensorMapEncodeIm2col unavailable"); return G6D_ECUDA; }
     const cuuint64_t C2 = 2ull * d->Cin;
@@ -902,9 +1042,10 @@ static int make_split_input_map(CUtensorMap* map, const void* xs, const g6d_conv
     cuuint64_t strides[4] = {C2 * 2, C2 * 2 * d->W, C2 * 2 * d->W * d->H, C2 * 2 * d->W * d->H * d->D};
     if (rank == 4) dims[3] = d->B;
     int lower[3] = {-d->pw, -d->ph, -d->pd};
-    int upper[3] = {d->pw - (d->kw - 1), d->ph - (d->kh - 1), d->pd - (d->kd - 1)};
+    int upper[3] = {d->pw - (xr_rows ? 0 : d->kw - 1), d->ph - (d->kh - 1), d->pd - (d->kd - 1)};
     cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(xs), dims, strides, lower, upper, 64, TC_BM, estr,
+    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(xs), dims, strides, lower, upper, 64,
+                     xr_rows ? xr_rows : TC_BM, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error("g6d_conv_tc: cuTensorMapEncodeIm2col failed (%d)", (int)r); return G6D_ECUDA; }
@@ -974,21 +1115,21 @@ static int fill_tc_params(const g6d_conv_desc* d, int kind, ConvTcP& p) {
     return G6D_OK;
 }
 
-template <int BN, int KIND, bool FOLD>
+template <int BN, int KIND, bool FOLD, bool XR>
 static int launch_tc2(const ConvTcP& p, const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& ma, cudaStream_t st) {
-    using Cfg = Tc2Cfg<BN>;
+    constexpr int SMEM = XR ? Tc2XrCfg<BN>::SMEM_BYTES : Tc2Cfg<BN>::SMEM_BYTES;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN, KIND, FOLD>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
-        if (e != cudaSuccess) { set_error("g6d_conv_tc: cannot opt in to %d B of shared memory: %s", Cfg::SMEM_BYTES, cudaGetErrorString(e)); return G6D_ECUDA; }
+        cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN, KIND, FOLD, XR>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
+        if (e != cudaSuccess) { set_error("g6d_conv_tc: cannot opt in to %d B of shared memory: %s", SMEM, cudaGetErrorString(e)); return G6D_ECUDA; }
         configured = true;
     }
     Tc2Work wk;
-    wk.m_tiles = ceil_div(p.M, TC_BM); wk.n_tiles = ceil_div(p.Cout, BN);
+    wk.m_tiles = ceil_div(XR ? p.Mp : p.M, TC_BM); wk.n_tiles = ceil_div(p.Cout, BN);
     const long long total = (long long)wk.m_tiles * wk.n_tiles * (FOLD ? 1 : p.splits);
     wk.total = (int)total;
     const int grid = total < kNumSMs ? (int)total : kNumSMs;
-    conv_tc2_kernel<BN, KIND, FOLD><<<grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(p, wk, mh, ml, ma);
+    conv_tc2_kernel<BN, KIND, FOLD, XR><<<grid, TC_THREADS, SMEM, st>>>(p, wk, mh, ml, ma);
     G6D_CHECK_LAUNCH("g6d_conv_tc");
     return G6D_OK;
 }
@@ -1460,6 +1601,20 @@ static bool split_input_ok(const g6d_conv_desc* d, int kind, int flags, bool use
     return (flags & G6D_TC_REUSE_IM2COL) && corners_ok(d->kw, d->pw) && corners_ok(d->kh, d->ph) && corners_ok(d->kd, d->pd);
 }
 
+// One A box per row of taps: in the A-reuse kernel's K order the kw taps of a (channel block, kz, ky) group are kw
+// consecutive K-blocks, and over an enumeration of Wp = Wo + kw - 1 columns per output row, row j + kx of ONE im2col box
+// of roundup8(128 + kw - 1) pixels at kx = 0 is tap kx of row j (a real column xp < Wo never wraps past Wp).  So the
+// TMA thread loads one box pair per group instead of one per K-block (kw times fewer A bytes, with (kw - 1) / Wp more
+// rows), the consumers read tap kx through a descriptor shifted by kx rows, and the epilogue drops the padded columns.
+// Every real output element sums the same products in the same order.  Measured on an H100 (DESIGN.md section 5), the
+// saved A traffic pays for the padding at BN 64, where the weight tile is small and A is two thirds of the operand
+// bytes; at BN 128 it did not.
+static bool xr_ok(const g6d_conv_desc* d, const ConvPlan& pl) {
+    if (!pl.tc.split_in || !pl.tc.reuse_order || pl.bn != 64 || d->kw < 2 || d->kw > 17) return false;
+    if (split_input_rank5(d) && d->pw > 15) return false;     // the rank-5 map's upper W corner becomes pw
+    return (long long)pl.tc.M / pl.tc.Wo * (pl.tc.Wo + d->kw - 1) < (1ll << 31);
+}
+
 static int make_plan(const g6d_conv_desc* d, int kind, int flags, ConvPlan& pl) {
     G6D_REQUIRE((flags & ~(G6D_TC_PRENORM | G6D_TC_REUSE_IM2COL | G6D_TC_FOLD_SPLITS)) == 0, "g6d_conv_tc: bad flags %d", flags);
     const int rc = fill_tc_params(d, kind, pl.tc);
@@ -1477,6 +1632,12 @@ static int make_plan(const g6d_conv_desc* d, int kind, int flags, ConvPlan& pl) 
     pl.splits = pl.use_flat ? pl.flat.splits : pl.tc.splits;
     pl.tc.split_in = split_input_ok(d, kind, flags, pl.use_flat) ? 1 : 0;
     pl.tc.fold = (flags & G6D_TC_FOLD_SPLITS) && fold_ok(pl) ? 1 : 0;
+    pl.tc.xr = xr_ok(d, pl) ? 1 : 0;
+    if (pl.tc.xr) {
+        pl.tc.Wp = pl.tc.Wo + d->kw - 1;
+        pl.tc.Mp = (int)((long long)pl.tc.M / pl.tc.Wo * pl.tc.Wp);
+        pl.tc.xr_rows = (TC_BM + d->kw - 1 + 7) / 8 * 8;
+    }
     const long long partials =
         pl.splits > 1 && !pl.tc.fold ? (long long)pl.splits * pl.tc.M * pl.tc.Cout * (long long)sizeof(float) : 0;
     pl.split_in_off = (partials + 255) / 256 * 256;
@@ -1504,9 +1665,13 @@ static void bind_tensors(P& p, const float* x, const float* bias, const float* p
 template <int BN, int KIND>
 static int launch_plan(const ConvPlan& pl, const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& ma, cudaStream_t st) {
     if (pl.use_flat) return launch_flat<BN, KIND>(pl.flat, pl.flat_smem, mh, ml, st);
-    if constexpr (KIND == G6D_TC_F16)                      // the split input, hence folding, is fp16 only
-        if (pl.tc.fold) return launch_tc2<BN, KIND, true>(pl.tc, mh, ml, ma, st);
-    return launch_tc2<BN, KIND, false>(pl.tc, mh, ml, ma, st);
+    if constexpr (KIND == G6D_TC_F16) {                    // the split input, hence folding and x reuse, is fp16 only
+        if constexpr (BN == 64)
+            if (pl.tc.xr) return pl.tc.fold ? launch_tc2<BN, KIND, true, true>(pl.tc, mh, ml, ma, st)
+                                            : launch_tc2<BN, KIND, false, true>(pl.tc, mh, ml, ma, st);
+        if (pl.tc.fold) return launch_tc2<BN, KIND, true, false>(pl.tc, mh, ml, ma, st);
+    }
+    return launch_tc2<BN, KIND, false, false>(pl.tc, mh, ml, ma, st);
 }
 template <int KIND>
 static int dispatch(const ConvPlan& pl, const CUtensorMap& mh, const CUtensorMap& ml, const CUtensorMap& ma, cudaStream_t st) {
@@ -1520,7 +1685,7 @@ static int dispatch(const ConvPlan& pl, const CUtensorMap& mh, const CUtensorMap
 using namespace g6d;
 
 // Debug aid: copies the 8-int timeout record (0 = no timeout; else [1]=waiter role 1 A-producer/empty,
-// 3 weight-TMA issuer/empty, 4 MMA/full_a, 5 MMA/full_b; [2]=iteration;
+// 3 weight-TMA issuer/empty, 4 MMA/full_a, 5 MMA/full_b, 6 x-reuse box TMA/box empty, 7 x-reuse MMA/box full; [2]=iteration;
 // [3]=parity; [4..6]=block; [7]=thread) and clears it.  Synchronises the device.
 extern "C" int g6d_conv_tc_debug(int* host_out8) {
     G6D_REQUIRE(host_out8 != nullptr, "g6d_conv_tc_debug: null");
@@ -1570,8 +1735,8 @@ extern "C" int g6d_conv_tc_plan_v2(const g6d_conv_desc* desc, int kind, int flag
     ConvPlan pl{};
     const int rc = make_plan(desc, kind, flags, pl);
     if (rc != G6D_OK) return rc;
-    const int v[5] = {pl.use_flat ? 1 : 0, pl.bn, pl.splits, pl.tc.split_in, pl.tc.fold};
-    for (int i = 0; i < n && i < 5; ++i) out[i] = v[i];
+    const int v[6] = {pl.use_flat ? 1 : 0, pl.bn, pl.splits, pl.tc.split_in, pl.tc.fold, pl.tc.xr};
+    for (int i = 0; i < n && i < 6; ++i) out[i] = v[i];
     return G6D_OK;
 }
 
@@ -1608,7 +1773,7 @@ extern "C" int g6d_conv_tc_ex(const g6d_conv_desc* desc, const float* x, const v
     memset(&ma, 0, sizeof(ma));
     if (p.split_in) {
         __half* xs = reinterpret_cast<__half*>(static_cast<char*>(ws) + pl.split_in_off);
-        if ((rc = make_split_input_map(&ma, xs, desc)) != G6D_OK) return rc;
+        if ((rc = make_split_input_map(&ma, xs, desc, p.xr ? p.xr_rows : 0)) != G6D_OK) return rc;
         const long long plane = (long long)p.D * p.H * p.W, rows = p.B * plane, n = rows * (p.Cin / 8);
         split_input_f16_kernel<<<ceil_div(n, 256), 256, 0, st>>>(x, p.ics, p.ico, p.Cin, rows, plane, p.pro, pro_scale,
                                                                   pro_shift, p.group_rows, xs);

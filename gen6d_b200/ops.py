@@ -623,14 +623,15 @@ def conv(x, pc, prologue=PRO_NONE, pro_scale=None, pro_shift=None, group_rows=1,
         if fuse:
             stats = torch.empty(M // stats_rows, pc.cout, 2, device=x.device, dtype=torch.float64)
         def tag(d=d, kind=pc.kind, flags=flags):        # formatted by collect_profile, outside the timed launches
-            plan = (C.c_int * 5)()
-            _lib.check(_lib.lib().g6d_conv_tc_plan_v2(C.byref(d), kind, flags, plan, 5), 'g6d_conv_tc_plan_v2')
+            plan = (C.c_int * 6)()
+            _lib.check(_lib.lib().g6d_conv_tc_plan_v2(C.byref(d), kind, flags, plan, 6), 'g6d_conv_tc_plan_v2')
             a_op = (' prenorm' if prologue != PRO_NONE else ' im2col') if plan[3] else ''
             if flags & _lib.TC_REUSE_IM2COL and plan[3]:       # '-ro': taken from the A-reuse kernel, in its K order
                 plain = (C.c_int * 4)()
                 _lib.check(_lib.lib().g6d_conv_tc_plan_ex(C.byref(d), kind, flags & ~_lib.TC_REUSE_IM2COL, plain),
                            'g6d_conv_tc_plan_ex')
                 a_op += '-ro' if plain[0] else ''
+            a_op += '-xr' if plan[5] else ''       # one A box per row of taps
             return (f'M={M} N={pc.cout} K={kd * kh * kw * pc.cin} k={kd}x{kh}x{kw} s={s} pro={prologue} '
                     f'{"reuse" if plan[0] else "persist"} BN={plan[1]} splits={plan[2]}{" fold" if plan[4] else ""}{a_op}')
         _call('g6d_conv_tc_ex', C.byref(d), _p(x), _p(pc.w_hi, pc.w_hi.dtype), _p(pc.w_lo, pc.w_lo.dtype), pc.w_hi.shape[0],

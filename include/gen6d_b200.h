@@ -425,7 +425,9 @@ int g6d_conv_tc(const g6d_conv_desc* desc, const float* x, const void* w_hi, con
 #define G6D_TC_REUSE_IM2COL 4
 #define G6D_TC_FOLD_SPLITS 32
 int g6d_conv_tc_plan_ex(const g6d_conv_desc* desc, int kind, int flags, int* out4);
-/* g6d_conv_tc_plan_ex's four values, then folded (1: G6D_TC_FOLD_SPLITS applies); the first min(n, 5) are written. */
+/* g6d_conv_tc_plan_ex's four values, then folded (1: G6D_TC_FOLD_SPLITS applies), then x reuse (1: one im2col A box per
+ * row of kw taps, read through row-shifted descriptors; planned for the A-reuse K order at BN 64); the first min(n, 6)
+ * are written. */
 int g6d_conv_tc_plan_v2(const g6d_conv_desc* desc, int kind, int flags, int* out, int n);
 long long g6d_conv_tc_workspace_bytes_ex(const g6d_conv_desc* desc, int kind, int flags);
 int g6d_conv_tc_ex(const g6d_conv_desc* desc, const float* x, const void* w_hi, const void* w_lo, int w_rows, int kind,
