@@ -63,6 +63,9 @@ _SIGNATURES = {
     'g6d_frames_table_check': [P, I, L],
     'g6d_frames_gather': [P, I, I, I, P, L, P],
     'g6d_frames_gather_host': [P, I, P, L],
+    'g6d_frames_resized_table_check': [P, I, L],
+    'g6d_frames_gather_resized': [P, I, I, I, P, L, P],
+    'g6d_frames_gather_resized_host': [P, I, P, L],
     'g6d_glue_detection_jobs': [P, P, I, I, I, I, P, P],
     'g6d_glue_detection_jobs_host': [P, P, I, I, I, I, P],
     'g6d_glue_initial_poses': [P, P, P, C.POINTER(GlueRefs), P, I, P, P],

@@ -11,7 +11,7 @@ LIB = os.path.join(HERE, 'libgen6d_b200.so')
 STAMP = os.path.join(HERE, '.libgen6d_b200.hash')
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC']
-NO_FMA = ('glue.cu', 'track.cu')
+NO_FMA = ('glue.cu', 'track.cu', 'frames.cu')
 
 
 def sources():
@@ -42,7 +42,7 @@ def build(force=False, verbose=False):
     for src in sources():
         obj = os.path.join(objdir, os.path.basename(src)[:-3] + '.o')
         objs.append(obj)
-        extra = ['-fmad=false'] if os.path.basename(src) in NO_FMA else []      # numpy-like rounding (glue_math.cuh)
+        extra = ['-fmad=false'] if os.path.basename(src) in NO_FMA else []      # numpy / OpenCV rounding (glue_math.cuh, frames_math.cuh)
         cmd = [nvcc] + NVCC_FLAGS + extra + (['-Xptxas', '-v'] if verbose else []) + ['-c', src, '-o', obj]
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
     failed = False

@@ -23,6 +23,12 @@ cv2.cvtColor(COLOR_YUV2RGB_NV12) does).  From the packed buffer on, the graph is
 view for one size, on_canvas for several.  Pointers and pitches live in the table, so a device-frame graph keys on the
 size pattern only, one size included ('device' in the name keeps it apart from the numpy graphs of that pattern), and a
 new allocation or pitch replays the same graph.
+
+Device frames at a working resolution (row f15): a device frame wrapped in Resized is resized (and rotated) to its
+working size as predict.py's video2image does on the host, bit for bit with cv2.resize + cv2.rotate, by the graph's
+first node, g6d_frames_gather_resized.  A call holding one takes that gather for all its frames (plain ones as identity
+rows of its g6d_resized_frame table) under a 'device-resized' key on the working size pattern; the sources live in the
+table, so a new decoder resolution with the same working sizes replays the same graph.
 """
 import ctypes as C
 import threading
@@ -57,13 +63,89 @@ class NV12:
         return f'NV12({self.shape[0]}x{self.shape[1]}, {self.y.device})'
 
 
+_ROTATIONS = (0, 90, 180, 270)
+
+
+class Resized:
+    """A device frame (a CUDA uint8 RGB tensor [h, w, 3] with any row pitch, or an NV12 frame) resized and rotated to its
+    working size inside the graph's first node (row f15), bit for bit as
+        cv2.rotate(cv2.resize(rgb, (w', h'), interpolation=cv2.INTER_LINEAR), code)
+    with rgb the frame's RGB bytes (an NV12 frame's cv2.cvtColor(COLOR_YUV2RGB_NV12) conversion).  Downscales and the
+    identity only: ValueError for a working size larger than the frame on either axis.
+
+    max_side: prepare.video2image's rule, ratio = max_side / max(h, w) and (h', w') = (int(ratio*h), int(ratio*w)) in
+    Python floats; or size=(h', w'), the resized size before the rotation.  Exactly one of them.
+    rotate: 0, 90, 180 or 270 degrees clockwise after the resize (cv2.ROTATE_90_CLOCKWISE, ROTATE_180,
+    ROTATE_90_COUNTERCLOCKWISE).  predict.py's --transpose is rotate=180 with OpenCV >= 4.5 (flip(0) then flip(1)) and
+    rotate=90 before (transpose then flip(1)).
+
+    .shape is the working (rows, cols, 3) after the rotation: every call sees the frame at that size, and a new source
+    resolution, pitch or allocation with the same working sizes replays the same graph."""
+    __slots__ = ('frame', 'size', 'rotate')
+
+    def __init__(self, frame, max_side=None, size=None, rotate=0):
+        if not isinstance(frame, (torch.Tensor, NV12)):
+            raise ValueError(f'Resized: frame is {type(frame).__name__}; need a CUDA uint8 RGB tensor [h, w, 3] or an NV12 frame '
+                             '(numpy frames are resized on the host, as predict.py does)')
+        shape = tuple(frame.shape) if isinstance(frame, torch.Tensor) else tuple(getattr(frame.y, 'shape', ())) + (3,)
+        if len(shape) != 3 or shape[2] != 3 or shape[0] < 1 or shape[1] < 1:
+            raise ValueError(f'Resized: frame is {list(shape)}; need [h, w, 3]')
+        h, w = int(shape[0]), int(shape[1])
+        if (max_side is None) == (size is None):
+            raise ValueError('Resized: give exactly one of max_side and size')
+        if max_side is not None:
+            if not max_side > 0:
+                raise ValueError(f'Resized: max_side = {max_side}, need > 0')
+            ratio = max_side / max(h, w)
+            size = (int(ratio * h), int(ratio * w))
+        size = tuple(int(s) for s in size)
+        if len(size) != 2 or min(size) < 1:
+            raise ValueError(f'Resized: working size {size} of a {h} x {w} frame; need (rows, cols) >= (1, 1)')
+        if size[0] > h or size[1] > w:
+            raise ValueError(f'Resized: {h} x {w} -> {size[0]} x {size[1]} upscales; only downscales and the identity are '
+                             'resized on the device')
+        if rotate not in _ROTATIONS:
+            raise ValueError(f'Resized: rotate = {rotate}; need one of {_ROTATIONS} degrees clockwise')
+        self.frame, self.size, self.rotate = frame, size, int(rotate)
+
+    @property
+    def shape(self):
+        """(rows, cols, 3): the working size, after the rotation."""
+        h, w = self.size
+        return (w, h, 3) if self.rotate in (90, 270) else (h, w, 3)
+
+    def intrinsics(self, K):
+        """A camera matrix K [3, 3] of the source frame -> the matrix that projects the same camera points into the working
+        frame: OpenCV's pixel-centre convention x' = (x + 0.5) * w'/w - 0.5 (rows alike), then the rotation.  With a
+        rotation the result M is not upper triangular: M = K_w @ Rz, with Rz the turn about the optical axis (the 2x2
+        linear part of the pixel rotation, e.g. -I for 180) and K_w upper triangular (for a K without skew).  The
+        estimator takes K_w (M @ Rz.T); its poses are then those of the camera turned by Rz.  predict.py's pseudo-K is
+        built from the working size and needs no mapping."""
+        h, w = int(self.frame.shape[0]), int(self.frame.shape[1])
+        (rh, rw), sx, sy = self.size, self.size[1] / w, self.size[0] / h
+        A = np.array([[sx, 0, 0.5 * sx - 0.5], [0, sy, 0.5 * sy - 0.5], [0, 0, 1]])
+        R = {0: np.eye(3),
+             90: np.array([[0, -1, rh - 1], [1, 0, 0], [0, 0, 1]], np.float64),
+             180: np.array([[-1, 0, rw - 1], [0, -1, rh - 1], [0, 0, 1]], np.float64),
+             270: np.array([[0, 1, 0], [-1, 0, rw - 1], [0, 0, 1]], np.float64)}[self.rotate]
+        return R @ A @ np.asarray(K, np.float64)
+
+    def __repr__(self):
+        return f'Resized({self.frame!r} -> {self.size[0]}x{self.size[1]}, rotate={self.rotate})'
+
+
 def _gpu_frame(f):
-    return isinstance(f, NV12) or (isinstance(f, torch.Tensor) and f.is_cuda)
+    return isinstance(f, (NV12, Resized)) or (isinstance(f, torch.Tensor) and f.is_cuda)
 
 
 def is_device(frames):
-    """True when the frames are device frames: a tensor, or a sequence holding a tensor or an NV12 frame."""
-    return isinstance(frames, torch.Tensor) or any(isinstance(f, (torch.Tensor, NV12)) for f in frames)
+    """True when the frames are device frames: a tensor, or a sequence holding a tensor, an NV12 or a Resized frame."""
+    return isinstance(frames, torch.Tensor) or any(isinstance(f, (torch.Tensor, NV12, Resized)) for f in frames)
+
+
+def has_resized(frames):
+    """True when a sequence of device frames holds a Resized frame (the call takes the resized gather, row f15)."""
+    return not isinstance(frames, torch.Tensor) and any(isinstance(f, Resized) for f in frames)
 
 
 def host_only(que_imgs, what):
@@ -110,7 +192,9 @@ def _check_device_frame(f, i, what, device):
                              f'({"stride(2) == 1, stride(1) == 3" if ch else "stride(1) == 1"}) and a row pitch >= '
                              f'{unit} x width')
 
-    if isinstance(f, NV12):
+    if isinstance(f, Resized):                   # its size and rotation were checked when it was built
+        _check_device_frame(f.frame, i, what, device)
+    elif isinstance(f, NV12):
         h, w = int(f.y.shape[0]) if f.y.dim() == 2 else -1, int(f.y.shape[1]) if f.y.dim() == 2 else -1
         if h < 2 or w < 2 or h % 2 or w % 2:
             raise ValueError(f'{what}: frame {i}: an NV12 Y plane must be [h, w] with h and w even, got {list(f.y.shape)}')
@@ -137,6 +221,25 @@ def device_table(frames, plan):
             rows.append(ops.DeviceFrame(f.data_ptr(), None, f.stride(0) if h > 1 else 3 * w, 0, h, w, _lib.G6D_FRAME_RGB, off))
     table = (ops.DeviceFrame * len(rows))(*rows)
     ops.frames_table_check(table, plan.nbytes)
+    return table
+
+
+def resized_table(frames, plan):
+    """Device frames, at least one of them Resized, + their FramePlan (of working sizes) -> the HOST table (ctypes array
+    of ops.ResizedFrame), checked by g6d_frames_resized_table_check: a plain frame is an identity row (working size =
+    source size, no rotation)."""
+    rows = []
+    for f, (off, _, _) in zip(frames, plan.table):
+        (rh, rw), rot, f = (f.size, f.rotate, f.frame) if isinstance(f, Resized) else (f.shape[:2], 0, f)
+        h, w = int(f.shape[0]), int(f.shape[1])
+        if isinstance(f, NV12):
+            rows.append(ops.ResizedFrame(f.y.data_ptr(), f.uv.data_ptr(), f.y.stride(0) if h > 1 else w, f.uv.stride(0) if h > 2 else w,
+                                         h, w, _lib.G6D_FRAME_NV12, rh, rw, rot, off))
+        else:
+            rows.append(ops.ResizedFrame(f.data_ptr(), None, f.stride(0) if h > 1 else 3 * w, 0, h, w, _lib.G6D_FRAME_RGB, rh, rw,
+                                         rot, off))
+    table = (ops.ResizedFrame * len(rows))(*rows)
+    ops.frames_resized_table_check(table, plan.nbytes)
     return table
 
 
@@ -204,24 +307,28 @@ class FramePlan:
         offsets = [self.table[i][0] for _, _, idx, _ in self.groups for i in idx]
         return [module.upload_packed(arrays, offsets, self.nbytes), module._to_dev(self.order)]
 
-    def device_key(self, name):
-        """The graph name of `name` (the numpy path's name of this pattern) for device frames of this size pattern."""
-        return ('device', name, self.pattern)
+    def device_key(self, name, resized=False):
+        """The graph name of `name` (the numpy path's name of this pattern) for device frames of this size pattern;
+        resized: the frames hold a Resized frame (the pattern is of working sizes, and the sources live in the table)."""
+        return ('device-resized' if resized else 'device', name, self.pattern)
 
-    def device_upload(self, module, frames):
+    def device_upload(self, module, frames, resized=False):
         """Device frames -> graph inputs [table u8 [qn*56]] (one size) or [table, order int64 [qn]] (several): the checked
-        g6d_device_frame rows, uploaded like any small input.  The frames themselves are not copied."""
-        table = np.frombuffer(bytes(device_table(frames, self)), np.uint8)
+        g6d_device_frame rows (g6d_resized_frame rows of 64 bytes when resized), uploaded like any small input.  The
+        frames themselves are not copied."""
+        table = np.frombuffer(bytes(resized_table(frames, self) if resized else device_table(frames, self)), np.uint8)
         return [module._to_dev(table)] + ([module._to_dev(self.order)] if self.mixed else [])
 
-    def gathered(self, fn):
-        """A graph body fn(frames u8 [qn,h,w,3], *rest) -> g(table, *rest) for device frames: g6d_frames_gather writes the
-        packed layout from the table, then fn runs on its [qn,h,w,3] view (one size) or through on_canvas (several)."""
+    def gathered(self, fn, resized=False):
+        """A graph body fn(frames u8 [qn,h,w,3], *rest) -> g(table, *rest) for device frames: g6d_frames_gather (or, when
+        resized, g6d_frames_gather_resized) writes the packed layout from the table, then fn runs on its [qn,h,w,3] view
+        (one size) or through on_canvas (several)."""
         qn, (h, w) = len(self.pattern), self.pattern[0]
         body = on_canvas(fn, self) if self.mixed else fn
+        gather = ops.frames_gather_resized if resized else ops.frames_gather
 
         def g(table, *rest):
-            packed = ops.frames_gather(table, qn, self.H, self.W, self.nbytes)
+            packed = gather(table, qn, self.H, self.W, self.nbytes)
             return body(packed, *rest) if self.mixed else body(packed[:qn * h * w * 3].view(qn, h, w, 3), *rest)
         return g
 
@@ -230,9 +337,11 @@ def bind(module, name, fn, frames, plan):
     """A graph name as the numpy path names it (the pattern's key for several sizes), its body fn(frames u8 [qn,h,w,3],
     *rest) and the frames -> (graph name, graph body, frame inputs) for StageCache.run(name, body, frame inputs + rest).
     Numpy frames of one size: (name, fn, [the frames uploaded as [qn,h,w,3]]), exactly the single-size path; of several:
-    on_canvas(fn) and the packed upload; device frames: the pattern's device key, the gather body and the table."""
+    on_canvas(fn) and the packed upload; device frames: the pattern's device key, the gather body and the table (the
+    'device-resized' key, the resized gather and its table when a frame is Resized, row f15)."""
     if is_device(frames):
-        return plan.device_key(name), plan.gathered(fn), plan.device_upload(module, frames)
+        r = has_resized(frames)
+        return plan.device_key(name, r), plan.gathered(fn, r), plan.device_upload(module, frames, r)
     if not plan.mixed:
         return name, fn, [module.upload_frame(frames)]
     return name, on_canvas(fn, plan), plan.upload(module, frames)

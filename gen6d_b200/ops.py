@@ -147,6 +147,38 @@ def frames_gather_host(table, nbytes):
     return out
 
 
+class ResizedFrame(C.Structure):      # g6d_resized_frame
+    _fields_ = [('plane0', C.c_void_p), ('plane1', C.c_void_p), ('pitch0', C.c_longlong), ('pitch1', C.c_longlong),
+                ('src_rows', C.c_int), ('src_cols', C.c_int), ('format', C.c_int), ('rows', C.c_int), ('cols', C.c_int),
+                ('rotate', C.c_int), ('offset', C.c_longlong)]
+
+
+def frames_resized_table_check(table, nbytes):
+    """A HOST array of ResizedFrame (ctypes) -> None; Gen6DLibraryError (G6D_EINVAL, with the message) unless every entry
+    is valid for a packed buffer of nbytes bytes (g6d_frames_resized_table_check)."""
+    _call('g6d_frames_resized_table_check', table, len(table), int(nbytes))
+
+
+def frames_gather_resized(table, n, max_rows, max_cols, nbytes):
+    """table: the bytes of n ResizedFrame entries on the device (uint8 [n*sizeof]) -> packed u8 [nbytes]: every frame's
+    resized, rotated RGB image at its offset, 0 elsewhere (g6d_frames_gather_resized).  max_rows / max_cols bound the
+    working (rotated) sizes."""
+    if table.dtype != torch.uint8 or table.numel() != n * C.sizeof(ResizedFrame):
+        raise ValueError(f'frames_gather_resized: table must be the packed bytes of {n} g6d_resized_frame records')
+    out = torch.empty(int(nbytes), device=table.device, dtype=torch.uint8)
+    _call('g6d_frames_gather_resized', _p(table, torch.uint8), n, max_rows, max_cols, _p(out, torch.uint8), int(nbytes),
+          _stream())
+    return out
+
+
+def frames_gather_resized_host(table, nbytes):
+    """g6d_frames_gather_resized on the host: a HOST array of ResizedFrame over host planes -> numpy u8 [nbytes]."""
+    import numpy as np
+    out = np.empty(int(nbytes), np.uint8)
+    _call('g6d_frames_gather_resized_host', table, len(table), out.ctypes.data_as(C.c_void_p), int(nbytes))
+    return out
+
+
 # ------------------------------------------------------------------------------- camera algebra between the stages
 def glue_detection_jobs(det_out, frames, size):
     """det_out [qn,4] (g6d_det_parse) + frames u8 [qn,h,w,3] -> packed g6d_warp_job records [qn*88] of the selector crops."""

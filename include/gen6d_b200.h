@@ -102,6 +102,31 @@ int g6d_frames_table_check(const g6d_device_frame* host_table, int n, long long 
 int g6d_frames_gather(const g6d_device_frame* table, int n, int max_rows, int max_cols, uint8_t* packed, long long packed_bytes,
                       g6d_stream_t stream);
 int g6d_frames_gather_host(const g6d_device_frame* host_table, int n, uint8_t* packed, long long packed_bytes);
+/* Device frames resized and rotated to a working size on the way into the packed layout: frame i becomes
+ *   cv2.rotate(cv2.resize(rgb, (cols, rows), interpolation=cv2.INTER_LINEAR), code)
+ * bit for bit, as x86 OpenCV computes it, with rgb the RGB image of its source planes (src_rows x src_cols, planes,
+ * pitches and format as in g6d_device_frame, NV12 converted as g6d_frames_gather converts it) and code the rotation
+ * (0 none, 90 ROTATE_90_CLOCKWISE, 180 ROTATE_180, 270 ROTATE_90_COUNTERCLOCKWISE).  Downscales and identity only:
+ * 1 <= rows <= src_rows and 1 <= cols <= src_cols.  The same size is a copy, exactly half the size in both axes
+ * OpenCV's INTER_AREA switch, anything else its 11-bit fixed-point INTER_LINEAR (csrc/frames_math.cuh).  The packed
+ * image at offset is the working [rows, cols, 3] image, [cols, rows, 3] for 90 and 270.  Every byte of packed is
+ * written, as by g6d_frames_gather.  g6d_frames_resized_table_check validates a HOST table like g6d_frames_table_check
+ * (plus the rotation and the working size, <= 65535 on each axis); g6d_frames_gather_resized reads the table from DEVICE
+ * memory, max_rows / max_cols bounding every frame's working size (<= 65535); g6d_frames_gather_resized_host runs the
+ * same code on a HOST table of host planes (checked first). */
+typedef struct g6d_resized_frame {
+    const uint8_t* plane0;         /* as g6d_device_frame */
+    const uint8_t* plane1;
+    long long pitch0, pitch1;
+    int src_rows, src_cols, format;
+    int rows, cols;                /* the resized size, before the rotation */
+    int rotate;                    /* degrees clockwise: 0, 90, 180 or 270 */
+    long long offset;              /* byte offset of the frame's packed working image */
+} g6d_resized_frame;
+int g6d_frames_resized_table_check(const g6d_resized_frame* host_table, int n, long long packed_bytes);
+int g6d_frames_gather_resized(const g6d_resized_frame* table, int n, int max_rows, int max_cols, uint8_t* packed,
+                              long long packed_bytes, g6d_stream_t stream);
+int g6d_frames_gather_resized_host(const g6d_resized_frame* host_table, int n, uint8_t* packed, long long packed_bytes);
 
 /* ---- camera algebra between the stages, on the device (estimator.py:176-214; utils/pose_utils.py:12-58,104-111,
  * 217-244; utils/database_utils.py:8-25,54-139; dataset/database.py:400-404,667-694).  With these four launches a
