@@ -28,7 +28,8 @@ TC_PRENORM, TC_REUSE_IM2COL, TC_FOLD_SPLITS = 1, 4, 32     # g6d_conv_tc_ex flag
 class ConvDesc(C.Structure):
     _fields_ = [(n, C.c_int) for n in ('B', 'D', 'H', 'W', 'Cin', 'in_cstride', 'in_coff', 'Cout', 'kd', 'kh', 'kw',
                                        'stride', 'pd', 'ph', 'pw', 'Do', 'Ho', 'Wo', 'out_cstride', 'out_coff',
-                                       'prologue')] + [('group_rows', C.c_longlong), ('act', C.c_int), ('max_chain_k', C.c_int)]
+                                       'prologue')] + [('group_rows', C.c_longlong), ('act', C.c_int), ('max_chain_k', C.c_int),
+                                                      ('plan_rows', C.c_int)]
 
 
 class DetMaps(C.Structure):

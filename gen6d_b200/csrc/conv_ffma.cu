@@ -359,14 +359,16 @@ static int fill_params(const g6d_conv_desc* d, ConvP& p) {
     const long long M = (long long)d->B * Do * Ho * Wo;
     const long long K = (long long)d->kd * d->kh * d->kw * d->Cin;
     G6D_REQUIRE(M < (1ll << 31) && K < (1ll << 31), "g6d_conv: problem too large");
+    G6D_REQUIRE(d->plan_rows == 0 || (d->plan_rows > 0 && Do > 0 && Ho > 0 && Wo > 0 && d->plan_rows % ((long long)Do * Ho * Wo) == 0),
+                "g6d_conv: plan_rows (%d) must be a multiple of the %d output rows of one image", d->plan_rows, Do * Ho * Wo);
     p.B = d->B; p.D = d->D; p.H = d->H; p.W = d->W; p.Cin = d->Cin; p.ics = d->in_cstride; p.ico = d->in_coff;
     p.Cout = d->Cout; p.ldw = (d->Cout + 3) & ~3; p.kd = d->kd; p.kh = d->kh; p.kw = d->kw; p.stride = d->stride;
     p.pd = d->pd; p.ph = d->ph; p.pw = d->pw; p.Do = Do; p.Ho = Ho; p.Wo = Wo; p.ocs = d->out_cstride;
     p.oco = d->out_coff; p.pro = d->prologue; p.act = d->act; p.group_rows = d->group_rows > 0 ? d->group_rows : 1;
     p.M = (int)M; p.K = (int)K; p.ktiles = (int)((K + BK - 1) / BK);
-    // split-K heuristic: fill ~2 CTAs per SM when the MN grid alone cannot
+    // split-K heuristic: fill ~2 CTAs per SM when the MN grid alone cannot (of plan_rows rows, see g6d_conv_desc)
     const int bn = d->Cout > 64 ? 128 : (d->Cout > 32 ? 64 : 32);
-    const long long ctas = (long long)ceil_div(M, BM) * ceil_div(d->Cout, bn);
+    const long long ctas = (long long)ceil_div(d->plan_rows > 0 ? d->plan_rows : M, BM) * ceil_div(d->Cout, bn);
     int splits = 1;
     if (ctas < kNumSMs && p.ktiles >= 16) {
         splits = (int)((2 * kNumSMs + ctas - 1) / ctas);

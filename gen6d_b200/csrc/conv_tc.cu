@@ -1081,13 +1081,16 @@ static int fill_tc_params(const g6d_conv_desc* d, int kind, ConvTcP& p) {
     const long long M = (long long)d->B * Do * Ho * Wo;
     const long long K = (long long)d->kd * d->kh * d->kw * d->Cin;
     G6D_REQUIRE(M < (1ll << 31) && K < (1ll << 31), "g6d_conv_tc: problem too large");
+    G6D_REQUIRE(d->plan_rows >= 0 && d->plan_rows % ((long long)Do * Ho * Wo) == 0,
+                "g6d_conv_tc: plan_rows (%d) must be a multiple of the %d output rows of one image", d->plan_rows, Do * Ho * Wo);
     p.B = d->B; p.D = d->D; p.H = d->H; p.W = d->W; p.Cin = d->Cin; p.ics = d->in_cstride; p.ico = d->in_coff;
     p.Cout = d->Cout; p.kd = d->kd; p.kh = d->kh; p.kw = d->kw; p.stride = d->stride; p.pd = d->pd; p.ph = d->ph;
     p.pw = d->pw; p.Do = Do; p.Ho = Ho; p.Wo = Wo; p.ocs = d->out_cstride; p.oco = d->out_coff; p.pro = d->prologue;
     p.act = d->act; p.group_rows = d->group_rows > 0 ? d->group_rows : 1;
     p.M = (int)M; p.K = (int)K; p.kblocks = (int)(K / bk);
     const int bn = tc_block_n(d->Cout);
-    const long long ctas = (long long)ceil_div(M, TC_BM) * ceil_div(d->Cout, bn);
+    const long long plan_m = d->plan_rows > 0 ? d->plan_rows : M;     // the rows the K splits are planned for
+    const long long ctas = (long long)ceil_div(plan_m, TC_BM) * ceil_div(d->Cout, bn);
     const int min_kb = 256 / bk;                     // never split below 256 K-elements per item
     int splits = 1;
     if (ctas < kNumSMs && p.kblocks >= 2 * min_kb) {
@@ -1490,7 +1493,8 @@ static bool fill_flat_params(const g6d_conv_desc* d, int kind, ConvFlatP& p, int
     p.a_stages = a_st; p.b_stages = b_st;
     *smem_bytes = (int)(a_st * a_stage) + b_st * b_stage + 256 + tab_bytes + 1024 + 64;
     // split over channel blocks when the tile grid cannot fill the machine, or to bound accumulate chains
-    const long long ctas = (long long)d->B * Do * p.tiles_per_plane * ((d->Cout + bn - 1) / bn);
+    const long long plan_b = d->plan_rows > 0 ? d->plan_rows / ((long long)Do * Ho * Wo) : d->B;  // see g6d_conv_desc
+    const long long ctas = plan_b * Do * p.tiles_per_plane * ((d->Cout + bn - 1) / bn);
     const long long K = (long long)d->Cin * d->kd * d->kh * d->kw;
     int splits = 1;
     if (ctas < kNumSMs && p.cblocks >= 2) splits = (int)((kNumSMs + ctas - 1) / ctas);

@@ -36,6 +36,12 @@ class LocalComm:
 
 
 FEAT_PAD = 516  # 512 correlation features + 3 similarity scores, padded to a multiple of 4
+# Queries per batched selection call.  What a chunk holds grows with it: at 64 references x 5 angles a query's
+# level-0 16x16 64-channel output is 21 MB, and each batched layer also keeps its input's fp16 hi/lo split copy (the same
+# bytes), so the level-0 16x16 layer holds about 63 MB per query, the 8x8 layers about 31 MB and cat_buf 16 MB.  The
+# per-query q (.) ref layers' 168 MB split copy of the reference stack is not replicated.  Ten queries fill the waves of
+# the 8x8 and 4x4 layers (12.1 of 13 and 6.1 of 7).
+SEL_QUERY_CHUNK = 10
 
 
 @dataclass
@@ -165,7 +171,7 @@ class ViewpointSelector(PackedModule):
         return torch.zeros(3 * refs.shape[0] * refs.shape[1], device=device, dtype=torch.int32)
 
     def comm_stats(self):
-        """Collectives issued per query by the sharded path (counted on the last eager / capture pass)."""
+        """Collectives issued by the sharded path (counted on the last eager / capture pass)."""
         return dict(getattr(self.comm, 'calls', {}))
 
     def _s2_counters(self):
@@ -184,64 +190,79 @@ class ViewpointSelector(PackedModule):
         exact, not per-shard."""
         return ops.instnorm_finalize(self.comm.all_reduce_sum(ws), rows_total, IN_EPS)
 
-    def _tower(self, level, ref, scale, shift, cat_buf, S, refs):
-        """corr_conv_list[level] (selector.py:27-69) on the implicit correlation volume.  Every layer has a
-        prologue; prenorm applies it in a split pass over the input, so the A operand arrives by TMA instead of a
-        per-tap gather.  The 16x16 level-0 layers, which the A-reuse kernel would take, run on the persistent kernel
-        in that kernel's K order (reuse_im2col), so the result is the same bit for bit."""
-        convs = self.packed()['towers'][level]
-        x, pro, ps, pb = ref, ops.PRO_CORR, scale, shift
-        for i, (pc, post) in enumerate(convs):
-            last = i + 1 == len(convs)
-            if last:
-                ops.conv(x, pc, prologue=pro, pro_scale=ps, pro_shift=pb, group_rows=S, out=cat_buf, out_coff=256 * level,
-                         prenorm=True, reuse_im2col=True, fold_splits=True)
-                break
-            rows = x.shape[0] * x.shape[1] * x.shape[2]                   # stride-1 same-size convolution
-            y, ws = ops.conv(x, pc, prologue=pro, pro_scale=ps, pro_shift=pb, group_rows=S, stats_rows=rows, prenorm=True,
-                             reuse_im2col=True, fold_splits=True)
-            # InstanceNorm3d statistics over (S, h, w) of the raw conv output; the normalisation
-            # itself (and the ReLU) is applied by the next conv's loader.  MaxPool commutes with
-            # the positive-slope affine, so pooling the raw tensor first is exact.
-            ps, pb = self._finalize(ws, rows // refs.shape[0] * refs.rfn_total)
-            pro = ops.PRO_AFFINE_RELU if 'r' in post else ops.PRO_AFFINE
-            x = ops.maxpool2x2(y) if 'p' in post else y
+    def _tower_conv(self, level, i, st, Q, S, cat_buf):
+        """Convolution i of corr_conv_list[level] (selector.py:27-69) for the Q queries of a batched selection.  st holds
+        the tower's input x, prologue and its operands.  Every layer has a prologue; prenorm applies it in a split pass
+        over the input, so the A operand arrives by TMA instead of a per-tap gather.  The 16x16 level-0 layers, which
+        the A-reuse kernel would take, run on the persistent kernel in that kernel's K order (reuse_im2col), so the
+        result is the same bit for bit.
+        The first layer forms q (.) ref from the one reference stack: one call per query, each writing its query's rows
+        of the batched output and its group of the moments.  Every later layer is one call over the Q*S images, the
+        queries' InstanceNorm groups of S images each, with the K splits planned for one query's rows (plan_rows), so
+        every query's output is the bits a call of that query alone gives.  -> (y, moments [Q, Cout, 2], rows per
+        query), or None for the last layer (written into cat_buf)."""
+        pc, post = self.packed()['towers'][level][i]
+        x = st['x']
+        kw = dict(prenorm=True, reuse_im2col=True, fold_splits=True)
+        if i == 0:
+            rows = x.shape[0] * x.shape[1] * x.shape[2]                # stride-1 same-size convolution, one query
+            y = torch.empty(Q * x.shape[0], x.shape[1], x.shape[2], pc.cout, device=x.device, dtype=torch.float32)
+            ws = [ops.conv(x, pc, prologue=ops.PRO_CORR, pro_scale=st['ps'][q], pro_shift=st['pb'][q], group_rows=S,
+                           out=y[q * S:(q + 1) * S], stats_rows=rows, **kw)[1] for q in range(Q)]
+            return y, (ws[0] if Q == 1 else torch.cat(ws, 0)), rows
+        rows = x.shape[0] * x.shape[1] * x.shape[2] // Q
+        if i + 1 == len(self.packed()['towers'][level]):
+            ops.conv(x, pc, prologue=st['pro'], pro_scale=st['ps'], pro_shift=st['pb'], group_rows=S, out=cat_buf,
+                     out_coff=256 * level, plan_rows=rows, **kw)
+            return None
+        return ops.conv(x, pc, prologue=st['pro'], pro_scale=st['ps'], pro_shift=st['pb'], group_rows=S, stats_rows=rows,
+                        plan_rows=rows, **kw) + (rows,)
 
-    def _towers_sharded(self, q_feats, cat_buf, S, S_total, refs):
+    @staticmethod
+    def _tower_next(st, post, y, ps, pb):
+        """The normalisation (and ReLU) of InstanceNorm3d is applied by the next conv's loader.  MaxPool commutes with
+        the positive-slope affine, so pooling the raw tensor first is exact."""
+        st['ps'], st['pb'] = ps, pb
+        st['pro'] = ops.PRO_AFFINE_RELU if 'r' in post else ops.PRO_AFFINE
+        st['x'] = ops.maxpool2x2(y) if 'p' in post else y
+
+    def _tower_state(self, q, ref, s1, s2, S_total):
+        """A tower's input: the reference stack and each query's q (.) ref prologue (first InstanceNorm3d folded in)."""
+        Q, h, w, c = q.shape
+        pro = [ops.sel_corr_prologue(q[i].reshape(h * w, c), s1, s2, S_total, IN_EPS) for i in range(Q)]
+        return {'x': ref, 'ps': [a for a, _ in pro], 'pb': [b for _, b in pro]}
+
+    def _tower(self, level, st, Q, cat_buf, S, refs):
+        """corr_conv_list[level] on the implicit correlation volume of Q queries, one layer after the other."""
+        convs = self.packed()['towers'][level]
+        for i, (_, post) in enumerate(convs):
+            res = self._tower_conv(level, i, st, Q, S, cat_buf)
+            if res is None:
+                break
+            y, ws, rows = res
+            # InstanceNorm3d statistics over (S, h, w) of the raw conv output, per query
+            ps, pb = self._finalize(ws, rows // refs.shape[0] * refs.rfn_total)
+            self._tower_next(st, post, y, ps, pb)
+
+    def _towers_sharded(self, q_feats, cat_buf, Q, S, S_total, refs):
         """The three towers with the reference axis sharded over GPUs, ROUND-synchronous: round r runs the
         r-th convolution of every tower that still has one (concurrently, on branch streams), then ONE
-        all-reduce carries the InstanceNorm moments of all of them (5 rounds for the 6 + 4 + 2 convolutions
-        instead of 9 per-layer all-reduces; SURVEY 8e).  Same arithmetic as _tower."""
+        all-reduce carries the InstanceNorm moments of all of them and of all Q queries (5 rounds for the 6 + 4 + 2
+        convolutions instead of 9 per-layer all-reduces; SURVEY 8e).  Same arithmetic as _tower."""
         towers = self.packed()['towers']
         nbr = 3 if self.comm.capturable else 1
-        state, keep = [], []
-        for l, (q, ref, (s1, s2)) in enumerate(zip(q_feats, refs.feats_cache, refs.sums)):
-            h, w, c = q.shape
-            scale, shift = ops.sel_corr_prologue(q.reshape(h * w, c), s1, s2, S_total, IN_EPS)
-            state.append({'x': ref, 'pro': ops.PRO_CORR, 'ps': scale, 'pb': shift, 'i': 0})
-        for _ in range(max(len(t) for t in towers)):
+        state = [self._tower_state(q, ref, s1, s2, S_total)
+                 for q, ref, (s1, s2) in zip(q_feats, refs.feats_cache, refs.sums)]
+        keep = []
+        for i in range(max(len(t) for t in towers)):
             br = Branches(nbr)          # forks from the main stream: after the previous round's finalize / pool kernels
             pend = []
             for l, st in enumerate(state):
-                convs = towers[l]
-                if st['i'] >= len(convs):
+                if i >= len(towers[l]):
                     continue
-                pc, post = convs[st['i']]
-                last = st['i'] + 1 == len(convs)
-
-                def step(l=l, st=st, pc=pc, last=last):
-                    if last:
-                        ops.conv(st['x'], pc, prologue=st['pro'], pro_scale=st['ps'], pro_shift=st['pb'], group_rows=S,
-                                 out=cat_buf, out_coff=256 * l, prenorm=True, reuse_im2col=True,
-                                 fold_splits=True)
-                        return None
-                    rows = st['x'].shape[0] * st['x'].shape[1] * st['x'].shape[2]
-                    return ops.conv(st['x'], pc, prologue=st['pro'], pro_scale=st['ps'], pro_shift=st['pb'], group_rows=S,
-                                    stats_rows=rows, prenorm=True, reuse_im2col=True, fold_splits=True) + (rows,)
-                res = br.run(l, step)
-                st['i'] += 1
+                res = br.run(l, lambda l=l, st=st: self._tower_conv(l, i, st, Q, S, cat_buf))
                 if res is not None:
-                    pend.append((st, post, res))
+                    pend.append((st, towers[l][i][1], res))
             br.join()
             if not pend:
                 continue
@@ -253,96 +274,108 @@ class ViewpointSelector(PackedModule):
                 ps, pb = ops.instnorm_finalize(flat[o:o + n].reshape(ws.shape), rows // refs.shape[0] * refs.rfn_total, IN_EPS)
                 o += n
                 keep.append((y, ws))
-                st['ps'], st['pb'] = ps, pb
-                st['pro'] = ops.PRO_AFFINE_RELU if 'r' in post else ops.PRO_AFFINE
-                st['x'] = ops.maxpool2x2(y) if 'p' in post else y
+                self._tower_next(st, post, y, ps, pb)
 
-    def _select_one(self, q_feats, refs=None, counters=None):
-        """selector.py:177-215 for one query.  q_feats: 3 x [h, w, 512].  -> logits [rfn], angles [rfn]
-        refs: the SelectorRefs to select against (default: the module's own); with any other record, `counters` are
-        that record's own S2 counters (s2_counters_for), never the module's or another record's."""
-        p = self.packed()
+    def _select_batch(self, q_feats, refs=None, counters=None):
+        """selector.py:177-215 for Q queries against one reference record.  q_feats: 3 x [Q, h, w, 512].
+        -> logits [Q, rfn], angles [Q, rfn], S2 scores [Q, 3, S].  Queries run in chunks of SEL_QUERY_CHUNK: the layers
+        after each tower's first run once per chunk over all its queries, each query's rows bit for bit what a chunk of
+        that query alone gives.  refs: the SelectorRefs to select against (default: the module's own); with any other
+        record, `counters` are that record's own S2 counters (s2_counters_for), never the module's or another record's."""
         if refs is None:
             refs, counters = self.refs, self._s2_counters()
         rfn, an = refs.shape
+        if counters is None or counters.numel() != 3 * rfn * an:
+            raise ValueError('_select_batch: a reference record other than the module\'s needs its own S2 counters [3*S]')
+        Q = q_feats[0].shape[0]
+        if Q <= SEL_QUERY_CHUNK:
+            return self._select_chunk(q_feats, refs, counters)
+        parts = [self._select_chunk([f[q0:q0 + SEL_QUERY_CHUNK] for f in q_feats], refs, counters)
+                 for q0 in range(0, Q, SEL_QUERY_CHUNK)]
+        return tuple(torch.cat(t, 0) for t in zip(*parts))
+
+    def _select_chunk(self, q_feats, refs, counters):
+        p = self.packed()
+        Q = q_feats[0].shape[0]
+        rfn, an = refs.shape
         S = rfn * an
         S_total = refs.rfn_total * an
-        if counters is None or counters.numel() != 3 * S:
-            raise ValueError('_select_one: a reference record other than the module\'s needs its own S2 counters [3*S]')
         dev = self.device
-        cat_buf = torch.empty(S, 4, 4, 768, device=dev, dtype=torch.float32)
-        feats = torch.empty(S, FEAT_PAD, device=dev, dtype=torch.float32)      # cols 0-511: cf3, 512-514 + pad: vp_norm
-        scores = ops.sel_corr_score3([r.reshape(S, -1, r.shape[-1]) for r in refs.feats_cache],
-                                     [q.reshape(-1, q.shape[-1]) for q in q_feats], counters=counters)
+        cat_buf = torch.empty(Q * S, 4, 4, 768, device=dev, dtype=torch.float32)
+        feats = torch.empty(Q * S, FEAT_PAD, device=dev, dtype=torch.float32)  # cols 0-511: cf3, 512-514 + pad: vp_norm
+        scores = torch.empty(Q, 3, S, device=dev, dtype=torch.float32)
+        ref_rows = [r.reshape(S, -1, r.shape[-1]) for r in refs.feats_cache]
+        for q in range(Q):
+            ops.sel_corr_score3(ref_rows, [f[q].reshape(-1, f.shape[-1]) for f in q_feats], counters=counters, out=scores[q])
         if self.comm.world == 1:
             br = Branches(3)                                # the three towers only meet in cat_buf
             keep = []
 
             def one_level(l, q, ref, s1, s2):
-                h, w, c = q.shape
-                scale, shift = ops.sel_corr_prologue(q.reshape(h * w, c), s1, s2, S_total, IN_EPS)
-                keep.append((scale, shift))
-                self._tower(l, ref, scale, shift, cat_buf, S, refs)
+                st = self._tower_state(q, ref, s1, s2, S_total)
+                keep.append(st)
+                self._tower(l, st, Q, cat_buf, S, refs)
 
             for l, (q, ref, (s1, s2)) in enumerate(zip(q_feats, refs.feats_cache, refs.sums)):
                 br.run(l, lambda l=l, q=q, ref=ref, s1=s1, s2=s2: one_level(l, q, ref, s1, s2))
             br.join()
         else:
-            self._towers_sharded(q_feats, cat_buf, S, S_total, refs)
+            self._towers_sharded(q_feats, cat_buf, Q, S, S_total, refs)
         # corr_feats_conv (selector.py:71-77): 1x1 768->512, IN, ReLU, 1x1 512->512, AvgPool(4,4).
         # The second 1x1 conv is linear, so the 4x4 average is taken first (16x less work).
-        y, ws = ops.conv(cat_buf, p['cf0'], stats_rows=S * 16)
+        y, ws = ops.conv(cat_buf, p['cf0'], stats_rows=S * 16, plan_rows=S * 16)
         ps, pb = self._finalize(ws, S_total * 16)
-        y = ops.avgpool_affine(y.reshape(S * 16, 512), 16, ps, pb, rows_per_group=S * 16, act=ops.ACT_RELU)
-        ops.conv(y.reshape(S, 1, 1, 512), p['cf3'], out=feats.reshape(S, 1, 1, FEAT_PAD), out_coff=0)
+        y = ops.avgpool_affine(y.reshape(Q * S * 16, 512), 16, ps, pb, rows_per_group=S * 16, act=ops.ACT_RELU)
+        ops.conv(y.reshape(Q * S, 1, 1, 512), p['cf3'], out=feats.reshape(Q * S, 1, 1, FEAT_PAD), out_coff=0, plan_rows=S)
         if self.comm.world == 1:
-            ops.sel_vp_norm(scores, feats, 512, IN_EPS)                 # vp_norm, selector.py:201
+            for q in range(Q):
+                ops.sel_vp_norm(scores[q], feats[q * S:(q + 1) * S], 512, IN_EPS)         # vp_norm, selector.py:201
         else:   # InstanceNorm2d over ALL (rfn, an): gather the 3*S_total scores, normalise, keep our rows
-            all_scores = self.comm.all_gather_cat(scores, dim=1).contiguous()
-            tmp = torch.empty(S_total, 4, device=dev, dtype=torch.float32)
-            ops.sel_vp_norm(all_scores, tmp, 0, IN_EPS)
+            all_scores = self.comm.all_gather_cat(scores, dim=2).contiguous()
+            tmp = torch.empty(Q, S_total, 4, device=dev, dtype=torch.float32)
+            for q in range(Q):
+                ops.sel_vp_norm(all_scores[q], tmp[q], 0, IN_EPS)
             r0, _ = self.comm.shard_range(refs.rfn_total)
-            feats[:, 512:516] = tmp[r0 * an:r0 * an + S]
-        x = ops.conv(feats.reshape(S, 1, 1, FEAT_PAD), p['sp0'], act=ops.ACT_RELU)
-        x = ops.conv(x, p['sp2']).reshape(rfn, an, 512)
-        sf = ops.sel_max_angle_add(x, refs.pose_embed)                  # selector.py:203-204
+            feats.reshape(Q, S, FEAT_PAD)[:, :, 512:516] = tmp[:, r0 * an:r0 * an + S]
+        x = ops.conv(feats.reshape(Q * S, 1, 1, FEAT_PAD), p['sp0'], act=ops.ACT_RELU, plan_rows=S)
+        x = ops.conv(x, p['sp2'], plan_rows=S).reshape(Q * rfn, an, 512)
+        sf = torch.empty(Q * rfn, 512, device=dev, dtype=torch.float32)
+        for q in range(Q):                                              # selector.py:203-204
+            ops.sel_max_angle_add(x[q * rfn:(q + 1) * rfn], refs.pose_embed, out=sf[q * rfn:(q + 1) * rfn])
         # everything below couples all references (attention, InstanceNorm1d over rfn): gather the
-        # per-reference score features once ([rfn,512] = 128 KB at 64 refs) and run the tail replicated
-        sf = self.comm.all_gather_cat(sf, dim=0).contiguous()
+        # per-reference score features once ([rfn,512] = 128 KB per query at 64 refs) and run the tail replicated
+        sf = self.comm.all_gather_cat(sf.reshape(Q, rfn, 512), dim=1).contiguous()
         rfn_local, rfn = rfn, refs.rfn_total
+        sf = sf.reshape(Q * rfn, 512)
         for att, (m0, m3) in zip(p['atts'], p['mlps']):
-            x4 = sf.reshape(rfn, 1, 1, 512)
-            qv = ops.conv(x4, att['conv_query']).reshape(rfn, 512)
-            kv = ops.conv(x4, att['conv_key']).reshape(rfn, 512)
-            vv = ops.conv(x4, att['conv_feats']).reshape(rfn, 512)
-            msg = ops.attention(qv, kv, vv, heads=8, head_major=True)
-            msg = ops.conv(msg.reshape(rfn, 1, 1, 512), att['conv_merge']).reshape(rfn, 512)
+            x4 = sf.reshape(Q * rfn, 1, 1, 512)
+            qv = ops.conv(x4, att['conv_query'], plan_rows=rfn).reshape(Q * rfn, 512)
+            kv = ops.conv(x4, att['conv_key'], plan_rows=rfn).reshape(Q * rfn, 512)
+            vv = ops.conv(x4, att['conv_feats'], plan_rows=rfn).reshape(Q * rfn, 512)
+            msg = torch.empty_like(qv)
+            for q in range(Q):
+                r = slice(q * rfn, (q + 1) * rfn)
+                ops.attention(qv[r], kv[r], vv[r], heads=8, head_major=True, out=msg[r])
+            msg = ops.conv(msg.reshape(Q * rfn, 1, 1, 512), att['conv_merge'], plan_rows=rfn).reshape(Q * rfn, 512)
             msg = ops.layernorm(msg, att['ln_w'], att['ln_b'], 1e-5)
-            y = ops.conv(torch.cat([sf, msg], 1).reshape(rfn, 1, 1, 1024), m0)
-            ps, pb = ops.instnorm_stats(y, rows_per_group=rfn, eps=IN_EPS)      # InstanceNorm1d over rfn
-            y = ops.conv(y, m3, prologue=ops.PRO_AFFINE_RELU, pro_scale=ps, pro_shift=pb, group_rows=rfn)
+            y = ops.conv(torch.cat([sf, msg], 1).reshape(Q * rfn, 1, 1, 1024), m0, plan_rows=rfn)
+            ps, pb = ops.instnorm_stats(y, rows_per_group=rfn, eps=IN_EPS)      # InstanceNorm1d over rfn, per query
+            y = ops.conv(y, m3, prologue=ops.PRO_AFFINE_RELU, pro_scale=ps, pro_shift=pb, group_rows=rfn, plan_rows=rfn)
             ps, pb = ops.instnorm_stats(y, rows_per_group=rfn, eps=IN_EPS)
-            y = ops.affine_act(y.reshape(rfn, 512), ps, pb, rows_per_group=rfn, act=ops.ACT_RELU)
+            y = ops.affine_act(y.reshape(Q * rfn, 512), ps, pb, rows_per_group=rfn, act=ops.ACT_RELU)
             sf = ops.add(y, sf)
-        x = ops.conv(sf.reshape(rfn, 1, 1, 512), p['score_predict'][0], act=ops.ACT_RELU)
-        logits = ops.conv(x, p['score_predict'][1]).reshape(rfn)
-        x = feats.reshape(rfn_local, 1, 1, an * FEAT_PAD)               # angles are per-reference: local
+        x = ops.conv(sf.reshape(Q * rfn, 1, 1, 512), p['score_predict'][0], act=ops.ACT_RELU, plan_rows=rfn)
+        logits = ops.conv(x, p['score_predict'][1], plan_rows=rfn).reshape(Q, rfn)
+        x = feats.reshape(Q * rfn_local, 1, 1, an * FEAT_PAD)           # angles are per-reference: local
         for i, pc in enumerate(p['angle_predict']):
-            x = ops.conv(x, pc, act=ops.ACT_RELU if i < 2 else ops.ACT_NONE)
-        angles = self.comm.all_gather_cat(x.reshape(rfn_local), dim=0)
+            x = ops.conv(x, pc, act=ops.ACT_RELU if i < 2 else ops.ACT_NONE, plan_rows=rfn_local)
+        angles = self.comm.all_gather_cat(x.reshape(Q, rfn_local), dim=1)
         return logits, angles, scores
 
     def _select_nhwc(self, que_norm4):
         if self.ref_feats_cache is None:
             raise RuntimeError('ViewpointSelector: load_ref_imgs / extract_ref_feats must be called first')
-        feats = self._feats(que_norm4)
-        logits, angles, taps = [], [], []
-        for qi in range(que_norm4.shape[0]):
-            lg, ang, sc = self._select_one([f[qi] for f in feats])
-            logits.append(lg)
-            angles.append(ang)
-            taps.append(sc)
-        return torch.stack(logits, 0), torch.stack(angles, 0), torch.stack(taps, 0)
+        return self._select_batch(self._feats(que_norm4))
 
     def _select_u8(self, u8):
         """uint8 crop(s) on the device -> (ref_idx [qn], (angle, logit) [qn,2], logits [qn,rfn])."""

@@ -155,13 +155,8 @@ class ObjectSet:
             poses, sels = [], []
             for s in range(S):
                 ob = objs[s % K]
-                lg, ang = [], []
-                for qi in range(qn):
-                    l, a, _ = sel._select_one([f[s * qn + qi] for f in feats], ob.sel, ob.counters)
-                    lg.append(l)
-                    ang.append(a)
-                logits = torch.stack(lg, 0)
-                idx, sel_out = ops.sel_parse(logits, torch.stack(ang, 0))
+                logits, angles, _ = sel._select_batch([rows(f, s) for f in feats], ob.sel, ob.counters)
+                idx, sel_out = ops.sel_parse(logits, angles)
                 sels.append((idx, sel_out, logits))
                 poses.append(ops.glue_initial_poses(rows(det, s), idx, sel_out, ob.tables['refs'], cams))
             return cat(poses), det, sels, crop                                       # poses [S*qn,12], slot-major

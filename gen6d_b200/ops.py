@@ -612,7 +612,8 @@ def transpose_to_packed(x2d):
 
 
 def conv(x, pc, prologue=PRO_NONE, pro_scale=None, pro_shift=None, group_rows=1, act=ACT_NONE,
-         in_coff=0, out=None, out_coff=0, stats_rows=None, prenorm=False, reuse_im2col=False, fold_splits=False):
+         in_coff=0, out=None, out_coff=0, stats_rows=None, prenorm=False, reuse_im2col=False, fold_splits=False,
+         plan_rows=0):
     """x [B, D, H, W, cs] or [B, H, W, cs]; returns [B, Do, Ho, Wo, Cout] (or 4-D for 4-D input).
     stats_rows: also return the InstanceNorm moments of the OUTPUT, (y, ws) with ws float64
     [groups, Cout, 2] = per group of `stats_rows` consecutive output rows (sum y, sum y^2) -- fused into the
@@ -624,7 +625,9 @@ def conv(x, pc, prologue=PRO_NONE, pro_scale=None, pro_shift=None, group_rows=1,
     kernel) get the split input on the persistent kernel, in the A-reuse kernel's K order (same result bit for bit).
     fold_splits: G6D_TC_FOLD_SPLITS -- a split-input layer whose tiles keep the GPU about as busy without the K splits'
     parallelism sums its splits inside the convolution instead of through fp32 partials and a reduce pass (same result
-    bit for bit, smaller workspace)."""
+    bit for bit, smaller workspace).
+    plan_rows: choose the K splits as for a call of plan_rows output rows (0: this call's own).  A call over Q groups of
+    plan_rows rows (Q queries against one reference stack) then gives each group the bits a call of that group alone gives."""
     four = x.dim() == 4
     if four:
         B, H, W, cs = x.shape
@@ -640,7 +643,8 @@ def conv(x, pc, prologue=PRO_NONE, pro_scale=None, pro_shift=None, group_rows=1,
         out = torch.empty(shape, device=x.device, dtype=torch.float32)
     d = _lib.ConvDesc(B=B, D=D, H=H, W=W, Cin=pc.cin, in_cstride=cs, in_coff=in_coff, Cout=pc.cout, kd=kd, kh=kh,
                       kw=kw, stride=s, pd=pd, ph=ph, pw=pw, Do=Do, Ho=Ho, Wo=Wo, out_cstride=out.shape[-1],
-                      out_coff=out_coff, prologue=prologue, group_rows=group_rows, act=act, max_chain_k=pc.max_chain_k)
+                      out_coff=out_coff, prologue=prologue, group_rows=group_rows, act=act, max_chain_k=pc.max_chain_k,
+                      plan_rows=plan_rows)
     work = 2.0 * B * Do * Ho * Wo * pc.cout * kd * kh * kw * pc.cin
     M = B * Do * Ho * Wo
     stats = None
@@ -796,12 +800,13 @@ def sel_corr_score(ref, q, out=None):
     return out
 
 
-def sel_corr_score3(refs, qs, counters=None):
-    """refs: 3 x [S, P_l, C]; qs: 3 x [P_l, C] -> score [3, S] in one streaming pass.
+def sel_corr_score3(refs, qs, counters=None, out=None):
+    """refs: 3 x [S, P_l, C]; qs: 3 x [P_l, C] -> score [3, S] in one streaming pass (into `out` when given).
     counters: int32 [3*S], zero (the kernel leaves it zero): one launch; None: dots + finish kernels."""
     S, Cc = refs[0].shape[0], refs[0].shape[2]
     Ps = [r.shape[1] for r in refs]
-    out = torch.empty(3, S, device=refs[0].device, dtype=torch.float32)
+    if out is None:
+        out = torch.empty(3, S, device=refs[0].device, dtype=torch.float32)
     ws = torch.empty(_lib.lib().g6d_sel_corr_score3_workspace_bytes(S, *Ps) // 4, device=refs[0].device, dtype=torch.float32)
     _call('g6d_sel_corr_score3', _p(refs[0]), _p(refs[1]), _p(refs[2]), _p(qs[0]), _p(qs[1]), _p(qs[2]), S, Ps[0], Ps[1],
           Ps[2], Cc, _p(out), _p(ws), _p(counters, torch.int32), _stream(), work=4.0 * (S * sum(Ps) * Cc + sum(Ps) * Cc + 3 * S))
@@ -813,18 +818,20 @@ def sel_vp_norm(score, feats, coff, eps=1e-5):
     _call('g6d_sel_vp_norm', _p(score), Ln, n, eps, _p(feats), feats.shape[-1], coff, _stream())
 
 
-def sel_max_angle_add(x, embed):
+def sel_max_angle_add(x, embed, out=None):
     rfn, an, Cc = x.shape
-    out = torch.empty(rfn, Cc, device=x.device, dtype=torch.float32)
+    if out is None:
+        out = torch.empty(rfn, Cc, device=x.device, dtype=torch.float32)
     _call('g6d_sel_max_angle_add', _p(x), _p(embed), _p(out), rfn, an, Cc, _stream())
     return out
 
 
-def attention(q, k, v, heads, head_major=False):
-    """q, k, v [n, C] -> [n, C].  head_major=False: the reference's channel order c = d*heads + head;
-    True: c = head*D + d (the tiled kernel; producers / consumer permuted at pack time)."""
+def attention(q, k, v, heads, head_major=False, out=None):
+    """q, k, v [n, C] -> [n, C] (into `out` when given).  head_major=False: the reference's channel order
+    c = d*heads + head; True: c = head*D + d (the tiled kernel; producers / consumer permuted at pack time)."""
     n, Cc = q.shape
-    out = torch.empty_like(q)
+    if out is None:
+        out = torch.empty_like(q)
     _call('g6d_attention_headmajor' if head_major else 'g6d_attention', _p(q), _p(k), _p(v), _p(out), n, Cc, heads, _stream())
     return out
 

@@ -367,6 +367,10 @@ typedef struct g6d_conv_desc {
                                  accumulator (longer problems are split and summed in fp32 round-to-nearest).  The tensor
                                  core truncates on every accumulate, which biases long chains of SAME-SIGN products
                                  (detector correlation: post-ReLU features x post-ReLU features) by ~5e-8 per step. */
+    int plan_rows;            /* 0 = M.  > 0: every K-split count that depends on the number of output rows (the tensor-core
+                                 kernels' fill-the-GPU splits, the FFMA split-K heuristic) is chosen as for a call of
+                                 plan_rows rows, a multiple of Do*Ho*Wo.  A call over Q groups of rows then sums every
+                                 output element in the same chains as the call over one group (bit-identical). */
 } g6d_conv_desc;
 
 #define G6D_PRO_NONE 0

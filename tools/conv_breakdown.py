@@ -52,10 +52,9 @@ CLASSES = (
     ('Detector', '_features', 'detector VGG'),
     ('Detector', '_raw_correlation', 'detector correlation'),
     ('Detector', '_raw_correlation_objects', 'detector correlation'),
-    ('ViewpointSelector', '_select_one', 'selector 1x1 layers'),
+    ('ViewpointSelector', '_select_chunk', 'selector 1x1 layers'),
     ('ViewpointSelector', '_feats', 'selector crop VGG'),
-    ('ViewpointSelector', '_tower', 'selector towers'),
-    ('ViewpointSelector', '_towers_sharded', 'selector towers'),
+    ('ViewpointSelector', '_tower_conv', 'selector towers'),
     ('VolumeRefiner', '_feature_net', 'refiner crop VGG'),
     ('VolumeRefiner', '_volume_net', 'refiner volume net + feature branches'),
     ('VolumeRefiner', '_conv_in_conv', 'refiner volume net + feature branches'),
