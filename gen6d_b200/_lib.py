@@ -19,6 +19,7 @@ G6D_DET_MAX_PEAK_RADIUS = 3
 G6D_ATTENTION_MAX_SMEM_FLOATS = 12288 - 32  # n + C/heads of a g6d_attention call
 G6D_FRAMES_MAX = 1024                       # frames per g6d_frames_canvas / g6d_frames_gather launch
 G6D_FRAME_RGB, G6D_FRAME_NV12 = 0, 1        # g6d_device_frame.format
+G6D_DRAW_MAX_BOXES = 16                     # boxes per destination of g6d_draw_boxes
 PRO_NONE, PRO_AFFINE, PRO_AFFINE_RELU, PRO_CORR = 0, 1, 2, 3
 ACT_NONE, ACT_RELU, ACT_LEAKY01 = 0, 1, 2
 TC_TF32, TC_F16 = 0, 1
@@ -87,6 +88,11 @@ _SIGNATURES = {
     'g6d_track_smooth_host': [P, I, P, P, P, P, I, P, I, P, P],
     'g6d_track_smooth_objects': [P, I, P, I, I, P, P, P, I, P, P, P, P],
     'g6d_track_smooth_objects_host': [P, I, P, I, I, P, P, P, I, P, P, P],
+    'g6d_draw_check': [P, I, P, I, P, I, I, I, I, I],
+    'g6d_draw_boxes': [P, P, I, P, P, P, P, P, I, P, I, I, I, P],
+    'g6d_draw_boxes_host': [P, P, I, P, I, P, I, P, I, P, I, P, I, P, I],
+    'g6d_rgb_to_nv12': [P, L, I, I, P, L, P, L, P],
+    'g6d_rgb_to_nv12_host': [P, L, I, I, P, L, P, L],
     'g6d_instances_associate': [I, I, I, I, P, P, P, P, D, D, D, D, D, I, P, P, P, P, P, P, P, P, I, P, P, P, P, P, P, P],
     'g6d_instances_associate_host': [I, I, I, I, P, P, P, P, D, D, D, D, D, I, P, P, P, P, P, P, P, P, I, P, P, P, P, P, P],
     'g6d_instances_associate_objects': [I, I, I, I, I, P, P, P, P, P, D, D, I, P, P, P, P, P, P, P, P, I, P, P, P, P, P, P, P],

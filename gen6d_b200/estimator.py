@@ -354,29 +354,34 @@ class Gen6DEstimator:
         return instances.inter_of(chain, *parts, rd.crops.reshape(n, res, res, 3), M, qn)
 
     # ------------------------------------------------------------------ video tracking (predict.py)
-    def tracker(self, num_sequences=1, refine_iter=1, smooth_num=5, smooth_std=2.5, bbox_3d=None):
+    def tracker(self, num_sequences=1, refine_iter=1, smooth_num=5, smooth_std=2.5, bbox_3d=None, draw=None, draw_color=(0, 0, 255)):
         """A Tracker for `num_sequences` videos stepped in lockstep (gen6d_b200/track.py): the first step is a full
         prediction with cfg['refine_iter'] refinements, every later step `refine_iter` refinements from the previous
         frame's pose, each followed by predict.py's box smoothing (`smooth_num` frames, `smooth_std`; defaults of
         predict.py's --num / --std).  bbox_3d: the object's 8 box corners [8,3]; None: from the database's point cloud.
+        draw: 'raw', 'smoothed' or ('raw', 'smoothed'): every step also draws predict.py's images_out /
+        images_out_smooth frames on the device, the box edges in draw_color (R, G, B) (Tracker.step, row f16).
         cfg['refine_iter'] is left untouched."""
         from .track import Tracker
         return Tracker(self, num_sequences, refine_iter=refine_iter, smooth_num=smooth_num, smooth_std=smooth_std,
-                       bbox_3d=bbox_3d)
+                       bbox_3d=bbox_3d, draw=draw, draw_color=draw_color)
 
     def instance_tracker(self, num_sequences=1, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
-                         min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bbox_3d=None):
+                         min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bbox_3d=None, draw=None,
+                         draw_color=(0, 0, 255)):
         """An InstanceTracker (gen6d_b200/instance_track.py): every instance of the object, up to `max_instances` per frame,
         followed through `num_sequences` videos in lockstep.  The first step (and the one after reset() / redetect(), and
         every `redetect_every`-th step after the last re-detection) detects predict_instances' instances (min_score,
         nms_iou, peak_radius) and associates them with the live tracks: the greedy matching of the smallest
         |projected object centre - detected position| / (ref_resolution * detected scale) below `gate`; a track unmatched
         more than `max_misses` re-detections in a row is dropped, and unmatched detections start new tracks.  Every other
-        step refines each track `refine_iter` times from its previous pose.  Both smooth as tracker() does."""
+        step refines each track `refine_iter` times from its previous pose.  Both smooth as tracker() does.  draw /
+        draw_color: as for tracker(); every live slot (track id >= 0) is drawn, in slot order."""
         from .instance_track import InstanceTracker
         return InstanceTracker(self, num_sequences, max_instances=max_instances, refine_iter=refine_iter,
                                redetect_every=redetect_every, gate=gate, max_misses=max_misses, min_score=min_score, nms_iou=nms_iou,
-                               peak_radius=peak_radius, smooth_num=smooth_num, smooth_std=smooth_std, bbox_3d=bbox_3d)
+                               peak_radius=peak_radius, smooth_num=smooth_num, smooth_std=smooth_std, bbox_3d=bbox_3d,
+                               draw=draw, draw_color=draw_color)
 
     def track(self, que_imgs, que_K, **tracker_kwargs):
         """predict.py's loop over one video: que_imgs uint8 [h,w,3] frames of one size, que_K [3,3] (or one per frame).

@@ -29,12 +29,13 @@ import numpy as np
 import torch
 
 from . import _lib
+from . import draw as dr
 from . import frames as fr
 from . import glue
 from . import instances
 from . import ops
 from .graphs import StageCache
-from .track import _sequences, check_bbox, object_bbox, object_bboxes, smoothing_weights
+from .track import _sequences, check_bbox, draw_inputs, object_bbox, object_bboxes, smoothing_weights
 
 
 def host_associate(det, valid, init, cams, center, ref_resolution, gate, max_misses, F, r, prev, live, ids, misses, next_id,
@@ -118,7 +119,8 @@ class InstanceTracker:
     readback of the selections (_take_selections)."""
 
     def __init__(self, est, num_sequences, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
-                 min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bbox_3d=None):
+                 min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bbox_3d=None, draw=None,
+                 draw_color=dr.DEFAULT_COLOR):
         from .objects import require_device_pipeline
         require_device_pipeline(est, 'instance tracking')
         key = check_args(num_sequences, max_instances, refine_iter, redetect_every, gate, max_misses, min_score, nms_iou,
@@ -129,9 +131,11 @@ class InstanceTracker:
                 raise ValueError('the database has no object point cloud: pass bbox_3d (the 8 corners of the object box)')
         self.bbox = check_bbox(bbox_3d)
         self._gen = est._generation()
-        self._setup(est, key, [self.bbox], num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std)
+        self._setup(est, key, [self.bbox], num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std,
+                    draw, [draw_color])
 
-    def _setup(self, est, key, boxes, num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std):
+    def _setup(self, est, key, boxes, num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std,
+               draw=None, colors=None):
         """The tracker's constants and device state for K = len(boxes) objects with M = key[0] slots each."""
         self.est, self.key = est, key
         self.K, self.S, self.M, self.refine_iter = len(boxes), int(num_sequences), key[0], int(refine_iter)
@@ -153,6 +157,11 @@ class InstanceTracker:
                        'ring': torch.zeros(n, self.num, 8, 2, dtype=torch.float32, device=dev),
                        'count': torch.zeros(n, dtype=torch.int32, device=dev)}
         self._pending, self._since = True, 0
+        # drawing (row f16): every live slot (track id >= 0) of a sequence on its frame, in row (slot group) order
+        kinds = self.draw = dr.parse_kinds(draw)
+        G = self.M * self.K
+        self._drawer = dr.StepDrawer(kinds, colors, np.stack(boxes, 0), [g % self.K for g in range(G)], self.S, dev,
+                                     live=True) if kinds else None
 
     # -------------------------------------------------------------- state
     def reset(self, sequences=None):
@@ -213,13 +222,13 @@ class InstanceTracker:
         return [(rd.take(n), rd.take(n * 2), rd.take(n * len(self.est.ref_info['poses'])))]
 
     # -------------------------------------------------------------- the graphs
-    def _detect_fn(self, st):
+    def _detect_fn(self, st, draw=None):
         est, G, S, r = self.est, self.M * self.K, self.S, self.refine_iter
         F, c, n = est.cfg['refine_iter'], self._dev, self.M * self.K * self.S
         views, R = self._groups(st)
         initial, associate, refine = self._detection(st), self._associate(), est.refiner._refine_warped(128)
 
-        def fn(frames, cams, prev, park, live, ids, misses, next_id, ring, count):
+        def fn(frames, cams, prev, park, live, ids, misses, next_id, ring, count, *dt):
             init, det, crop, sels, valid, inst_count = initial(frames, cams)
             work, flags0, lists, det_slot, spawned, dropped = associate(det, valid, init, cams, prev, live, ids, misses, next_id,
                                                                         park, ring, count)
@@ -234,18 +243,21 @@ class InstanceTracker:
                 ops.glue_apply_refinements_rows(views, 2 * S, que_pose, que_K, rect, out, rows, work)
                 chain.append(real())
             poses = chain[-1]
-            smoothed, avg = ops.track_smooth_objects(poses, True, c['bboxes'], cams[:, :9].contiguous(), ring, count, c['weights'])
+            Ks = cams[:, :9].contiguous()
+            smoothed, avg = ops.track_smooth_objects(poses, True, c['bboxes'], Ks, ring, count, c['weights'])
+            if dt:
+                draw(frames, poses, True, smoothed, Ks, dt[0], ids)
             buf = instances.pack([torch.stack(chain, 0), smoothed, avg, ring, count, ids, det, *sels, valid, inst_count, det_slot,
                                   spawned, dropped], crop)
             return buf, poses, park, live, ids, misses, next_id, ring, count
         return fn
 
-    def _refine_fn(self, st):
+    def _refine_fn(self, st, draw=None):
         est, S, r, c, n = self.est, self.S, self.refine_iter, self._dev, self.M * self.K * self.S
         views, R = self._groups(st)
         refine = est.refiner._refine_warped(128)
 
-        def fn(frames, cams, prev, park, live, ids, ring, count):
+        def fn(frames, cams, prev, park, live, ids, ring, count, *dt):
             work = torch.where((live != 0)[:, None], prev, park)                 # empty slots restart from their parking pose
             flags0 = live.to(torch.uint8)                                        # tracks hold float32 values, parking poses not
             rows = torch.arange(n, device=live.device, dtype=torch.int32)
@@ -257,24 +269,28 @@ class InstanceTracker:
                 ops.glue_apply_refinements_rows(views, S, que_pose, que_K, rect, out, rows, work)
                 chain.append(work.clone())
             poses = chain[-1]
-            smoothed, avg = ops.track_smooth_objects(poses, True, c['bboxes'], cams[:, :9].contiguous(), ring, count, c['weights'])
+            Ks = cams[:, :9].contiguous()
+            smoothed, avg = ops.track_smooth_objects(poses, True, c['bboxes'], Ks, ring, count, c['weights'])
+            if dt:
+                draw(frames, poses, True, smoothed, Ks, dt[0], ids)
             buf = instances.pack([torch.stack(chain, 0), smoothed, avg, ring, count, ids], torch.empty(0, dtype=torch.uint8,
                                                                                                      device=live.device))
             return buf, poses, ring, count
         return fn
 
     # -------------------------------------------------------------- one step
-    def step(self, frames, Ks):
+    def step(self, frames, Ks, out=None):
         """frames: S uint8 [h,w,3] (of one size or several, row f13; or device frames, row f14, as Tracker.step takes them);
-        Ks: [S,3,3].  Returns (poses float32 [S,M,3,4], smoothed float64 [S,M,3,4],
+        Ks: [S,3,3]; out: drawing destinations as Tracker.step takes them (a tracker made with draw= draws every live slot
+        of a sequence on its frame, in slot order; without out= inter['drawn'] holds tracker-owned frames).  Returns (poses float32 [S,M,3,4], smoothed float64 [S,M,3,4],
         track_ids int64 [S,M] (-1: empty slot), inter): inter['refine_poses'] a list of [S,M,3,4] (entry 0 the starting
         poses, float64 on a re-detection step; a row whose chain is shorter repeats its final pose), 'bbox_pts' and
         'smoothed_pts' [S,M,8,2].  Empty slots' poses and points are NaN.  A re-detection step adds predict_instances'
         keys led by [S,M], 'det_slot' int64 [S,M] (the slot detection m went to, -1: discarded), 'spawned' bool [S,M]
         (the slots that started a track) and 'dropped' (the ids removed this step, ascending)."""
-        return self._step(frames, Ks)[0]
+        return self._step(frames, Ks, out)[0]
 
-    def _step(self, frames, Ks):
+    def _step(self, frames, Ks, out=None):
         """One step -> the decoded results of every object, in object order."""
         self._check()
         est, S = self.est, self.S
@@ -292,20 +308,21 @@ class InstanceTracker:
         if plan.mixed:
             fr.check_frames(imgs, Ks, 'step')
         stt, x = self._tables(), self._state
+        draw, dt, drawn, named = draw_inputs(self._drawer, est.detector, plan, out)
         with torch.no_grad():
             if detecting:
-                name, fn, fin = fr.stage(est.detector, 'detect', self._detect_fn(stt), imgs, plan)
+                name, fn, fin = fr.stage(est.detector, named('detect'), self._detect_fn(stt, draw), imgs, plan)
                 cams = est.detector._to_dev(glue.cameras(Ks))
                 outs = self.stages.run(name, fn, fin + [cams, x['prev'], x['park'], x['live'], x['ids'], x['misses'], self._next_id,
-                                                        x['ring'], x['count']])
+                                                        x['ring'], x['count']] + dt)
                 buf, poses, park, live, ids, misses, next_id, ring, count = outs
                 for k, v in (('park', park), ('live', live), ('ids', ids), ('misses', misses)):
                     x[k].copy_(v)
                 self._next_id.copy_(next_id)
             else:
-                name, fn, fin = fr.stage(est.detector, 'refine', self._refine_fn(stt), imgs, plan)
+                name, fn, fin = fr.stage(est.detector, named('refine'), self._refine_fn(stt, draw), imgs, plan)
                 cams = est.detector._to_dev(glue.cameras(Ks))
-                outs = self.stages.run(name, fn, fin + [cams, x['prev'], x['park'], x['live'], x['ids'], x['ring'], x['count']])
+                outs = self.stages.run(name, fn, fin + [cams, x['prev'], x['park'], x['live'], x['ids'], x['ring'], x['count']] + dt)
                 buf, poses, ring, count = outs
             x['prev'].copy_(poses)
             x['ring'].copy_(ring)
@@ -313,7 +330,11 @@ class InstanceTracker:
             host = est.detector._to_host(buf)                        # the step's one synchronising read
         self._pending = False
         self._since = 1 if detecting else self._since + 1
-        return self._decode(host, detecting)
+        res = self._decode(host, detecting)
+        if drawn is not None:
+            for r in res:
+                r[3]['drawn'] = drawn
+        return res
 
     def _decode(self, host, detecting):
         est, S, M, K, num = self.est, self.S, self.M, self.K, self.num
@@ -376,14 +397,16 @@ class ObjectInstanceTracker(InstanceTracker):
     sequence s.  reset(sequences) drops those sequences' tracks for every object."""
 
     def __init__(self, objs, num_sequences, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
-                 min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bboxes=None):
+                 min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bboxes=None, draw=None,
+                 draw_colors=None):
         key = check_args(num_sequences, max_instances, refine_iter, redetect_every, gate, max_misses, min_score, nms_iou,
                          peak_radius, smooth_num, smooth_std)
         objs._check()
         boxes = object_bboxes(objs, bboxes)
         self.objs, self.names, self.bboxes = objs, objs.names, np.ascontiguousarray(np.stack(boxes, 0))
         self._membership = objs.membership
-        self._setup(objs.est, key, boxes, num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std)
+        self._setup(objs.est, key, boxes, num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std,
+                    draw, dr.object_colors(self.names, draw_colors))
         centers = np.stack([np.asarray(ob.ref_info['center'], np.float64).reshape(3) for ob in objs._objects.values()], 0)
         self._dev['centers'] = torch.from_numpy(np.ascontiguousarray(centers)).to(self.est.detector.device)
 
@@ -421,10 +444,10 @@ class ObjectInstanceTracker(InstanceTracker):
         slots = [(rd.take(S), rd.take(S * 2), rd.take(S * n_sel[g % K])) for g in range(M * K)]
         return [tuple(np.concatenate([slots[m * K + o][i] for m in range(M)]) for i in range(3)) for o in range(K)]
 
-    def step(self, frames, Ks):
+    def step(self, frames, Ks, out=None):
         """frames: S uint8 [h,w,3] (of one size or several, row f13; or device frames, row f14); Ks: [S,3,3] (shared by all
-        objects).  Returns {name: (poses float32
+        objects); out: drawing destinations as InstanceTracker.step takes them, every live slot of every object drawn.  Returns {name: (poses float32
         [S,M,3,4], smoothed float64 [S,M,3,4], track_ids int64 [S,M], inter)}: per object what InstanceTracker.step returns,
         'det_score' included on a re-detection step; 'dropped' lists that object's ids only.  Ids are unique over every
         object of the tracker."""
-        return dict(zip(self.names, self._step(frames, Ks)))
+        return dict(zip(self.names, self._step(frames, Ks, out)))

@@ -324,6 +324,47 @@ def glue_apply_refinements_rows(views_structs, rows_per_obj, que_pose, que_K, re
     return poses
 
 
+class DrawSrc(C.Structure):           # g6d_draw_src
+    _fields_ = [('offset', C.c_longlong), ('pitch', C.c_longlong), ('rows', C.c_int), ('cols', C.c_int)]
+
+
+class DrawBox(C.Structure):           # g6d_draw_box
+    _fields_ = [('dst', C.c_int), ('pose', C.c_int), ('K', C.c_int), ('bbox', C.c_int), ('pose_f32', C.c_int), ('valid', C.c_int),
+                ('color', C.c_uint8 * 4)]
+
+
+def draw_check(srcs, boxes, dsts, n_poses, n_Ks, n_bboxes, n_ids=0):
+    """HOST ctypes arrays of DrawSrc, DrawBox and DeviceFrame -> None; Gen6DLibraryError unless they are valid for arrays of
+    n_poses poses, n_Ks intrinsics, n_bboxes boxes and n_ids track ids (g6d_draw_check)."""
+    _call('g6d_draw_check', srcs, len(srcs), boxes, len(boxes), dsts, len(dsts), int(n_poses), int(n_Ks), int(n_bboxes), int(n_ids))
+
+
+def draw_boxes(src, srcs, n_src, poses, Ks, bboxes, boxes, n_boxes, dsts, n_dst, max_rows, max_cols, ids=None):
+    """predict.py's draw_bbox_3d into every destination (g6d_draw_boxes): src the device address the source frames are
+    offset from (srcs: n_src DrawSrc rows on the device), poses float64 [n,12], Ks float64 [m,9], bboxes
+    float32 [k,8,3], boxes n_boxes DrawBox rows and dsts n_dst DeviceFrame rows on the device (checked by draw_check); ids:
+    int64 track ids a box with valid >= 0 reads (drawn when ids[valid] >= 0)."""
+    for t, n, cls in ((srcs, n_src, DrawSrc), (boxes, n_boxes, DrawBox), (dsts, n_dst, DeviceFrame)):
+        if t.dtype != torch.uint8 or t.numel() != n * C.sizeof(cls):
+            raise ValueError(f'draw_boxes: a table of {n} {cls.__name__} rows must be uint8 [{n * C.sizeof(cls)}]')
+    _call('g6d_draw_boxes', C.c_void_p(int(src)), _p(srcs, torch.uint8), n_src, _p(poses, torch.float64), _p(Ks, torch.float64),
+          _p(bboxes), _p(ids, torch.int64), _p(boxes, torch.uint8) if n_boxes else None, n_boxes, _p(dsts, torch.uint8), n_dst, max_rows, max_cols, _stream())
+
+
+def rgb_to_nv12(rgb, y, uv):
+    """cv2.cvtColor(rgb, COLOR_RGB2YUV_I420) with U and V interleaved, into the planes y uint8 [h,w] and uv [h/2,w] (any
+    row pitches; g6d_rgb_to_nv12): rgb a CUDA uint8 [h,w,3] tensor with unit column steps, h and w even."""
+    h, w = int(rgb.shape[0]), int(rgb.shape[1])
+    if rgb.dtype != torch.uint8 or rgb.dim() != 3 or rgb.shape[2] != 3 or rgb.stride(2) != 1 or rgb.stride(1) != 3:
+        raise ValueError(f'rgb_to_nv12: rgb must be uint8 [h,w,3] with unit column steps, got {rgb.dtype} {list(rgb.shape)}')
+    if tuple(y.shape) != (h, w) or tuple(uv.shape) != (h // 2, w) or y.stride(1) != 1 or uv.stride(1) != 1:
+        raise ValueError(f'rgb_to_nv12: planes {list(y.shape)} and {list(uv.shape)} for a {h} x {w} frame')
+    if not (rgb.is_cuda and y.is_cuda and uv.is_cuda and y.dtype == uv.dtype == torch.uint8):
+        raise ValueError('rgb_to_nv12: rgb, y and uv must be CUDA uint8 tensors')
+    _call('g6d_rgb_to_nv12', C.c_void_p(rgb.data_ptr()), rgb.stride(0), h, w, C.c_void_p(y.data_ptr()), y.stride(0),
+          C.c_void_p(uv.data_ptr()), uv.stride(0), _stream())
+
+
 def track_smooth_objects(poses, poses_are_f32, bboxes, Ks, ring, count, weights):
     """track_smooth for K objects through S sequences in one launch, rows object-major: poses float64 [K*S,12] (row o*S + s
     is object o on sequence s), bboxes float32 [K,8,3], Ks float64 [S,9], ring float32 [K*S,num,8,2] and count int32 [K*S]

@@ -18,6 +18,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from . import draw as dr
 from . import frames as fr
 from . import glue
 from . import ops
@@ -198,13 +199,14 @@ def _mixed_inputs(S, K, pending, f32, F, r, device, plan=None):
     return reinit, b, inputs
 
 
-def _mixed_fn(K, S, b, F, r, initial, views, R, refine, smooth, blocks=None):
+def _mixed_fn(K, S, b, F, r, initial, views, R, refine, smooth, blocks=None, draw=None):
     """The mixed step's graph body.  initial(frames, cams) -> (poses [K*b,12], crops, [tensors packed after the smoothing]);
     smooth(poses [K*S,12], Ks [S,9], ring, count) -> (smoothed, averaged corners).  blocks: the gathered rows per size
-    group of frames of different sizes (_size_buckets), detected per size."""
+    group of frames of different sizes (_size_buckets), detected per size.  draw(frames, raw, raw_f32, smoothed, Ks,
+    table): the draw node (row f16), run after the smoothing when the body is given a destination table."""
     n, lens = S + b, _iter_lengths(S, b, F, r)
 
-    def fn(frames, cams, prev, ring, count, seq, tgt, flags0, lists):
+    def fn(frames, cams, prev, ring, count, seq, tgt, flags0, lists, *dt):
         if b:
             gf, gc = frames.index_select(0, seq), cams.index_select(0, seq)
             if blocks is None:
@@ -230,10 +232,24 @@ def _mixed_fn(K, S, b, F, r, initial, views, R, refine, smooth, blocks=None):
                 ops.glue_apply_refinements_rows(views, n, que_pose, que_K, rect, out, idx, work)
             chain.append(real())
         poses = chain[-1]
-        smoothed, avg = smooth(poses, cams[:, :9].contiguous(), ring, count)
+        Ks = cams[:, :9].contiguous()
+        smoothed, avg = smooth(poses, Ks, ring, count)
+        if dt:
+            draw(frames, poses, True, smoothed, Ks, dt[0])
         packed = torch.cat([t.reshape(-1).to(torch.float64) for t in [torch.stack(chain, 0), smoothed, avg, ring, count] + extras])
         return (torch.cat([packed.view(torch.uint8), crop.reshape(-1)]) if b else packed.view(torch.uint8)), poses, ring, count
     return fn
+
+
+def draw_inputs(drawer, module, plan, out):
+    """A step's drawing (row f16) -> (draw hook for the graph body or None, [destination table] graph inputs, inter['drawn']
+    or None, graph name map).  The destinations are checked here, before anything is enqueued."""
+    if drawer is None:
+        if out is not None:
+            raise ValueError('step: out= names drawing destinations; create the tracker with draw=')
+        return None, [], None, (lambda n: n)
+    table, drawn = drawer.destinations(module, plan, out)
+    return (lambda *a: drawer.node(module, plan, *a)), [table], drawn, drawer.name
 
 
 def _sequences(S, sequences):
@@ -251,7 +267,9 @@ def _sequences(S, sequences):
 class Tracker:
     """S sequences tracked in lockstep (one frame each per step); see Gen6DEstimator.tracker()."""
 
-    def __init__(self, est, num_sequences, refine_iter=1, smooth_num=5, smooth_std=2.5, bbox_3d=None):
+    def __init__(self, est, num_sequences, refine_iter=1, smooth_num=5, smooth_std=2.5, bbox_3d=None, draw=None,
+                 draw_color=dr.DEFAULT_COLOR):
+        kinds, draw_color = dr.parse_kinds(draw), dr.parse_color(draw_color)
         if int(num_sequences) < 1:
             raise ValueError(f'num_sequences must be >= 1, got {num_sequences}')
         if int(refine_iter) < 1:
@@ -274,6 +292,8 @@ class Tracker:
         self._gen = est._generation()
         self.stages = StageCache()       # this tracker's step graphs (they capture its device state)
         self._dev = None                 # device copies of bbox / weights
+        self.draw = kinds                # the kinds each step draws (row f16); None: no drawing
+        self._drawer = dr.StepDrawer(kinds, [draw_color], self.bbox, [0], self.S, est.detector.device) if kinds else None
         self.reset()
 
     # -------------------------------------------------------------- state
@@ -358,7 +378,7 @@ class Tracker:
         return 'mixed'
 
     # -------------------------------------------------------------- one step
-    def step(self, frames, Ks):
+    def step(self, frames, Ks, out=None):
         """frames: S uint8 [h,w,3] (of different sizes on the device path, row f13; or, on that path, device frames with
         predict_batch's rules, row f14: CUDA RGB tensors and frames.NV12 surfaces, ready on the current stream and free to
         reuse when step returns); Ks: [S,3,3].  Returns (raw poses float32 [S,3,4], smoothed poses float64
@@ -367,22 +387,33 @@ class Tracker:
         selection entries of predict_batch.  A mixed step (some sequences re-initialised by reset(sequences), or previous
         poses of different dtypes) adds inter['reinit'] (the re-initialised sequences, ascending) with the detection and
         selection entries of those sequences in that order, and its chain has 1 + max(cfg['refine_iter'], refine_iter)
-        entries [S,3,4]: entry 0 the starting poses (float64), a row whose chain is shorter repeating its final pose."""
+        entries [S,3,4]: entry 0 the starting poses (float64), a row whose chain is shorter repeating its final pose.
+
+        A tracker made with draw= (row f16) draws predict.py's box into every frame inside the step's graph, as its last
+        node: inter['drawn'] = {kind: S CUDA uint8 [h, w, 3] views of tracker-owned buffers at each frame's working size,
+        overwritten by the next step}.  out={kind: S destinations} (CUDA uint8 RGB tensors of the working size with any
+        row pitch, or frames.NV12 of an even working size) writes into the caller's buffers instead; they are written on
+        the current stream."""
         self._check()
         if len(frames) != self.S or len(Ks) != self.S:
             raise ValueError(f'step: this tracker follows {self.S} sequences, got {len(frames)} frames and {len(Ks)} Ks')
+        if out is not None and self._drawer is None:
+            raise ValueError('step: out= names drawing destinations; create the tracker with draw=')
         Ks = np.stack([np.asarray(K) for K in Ks], 0)
         kind = self._kind()
         device = self._device_path()
+        if self._drawer is not None and not device:
+            raise ValueError("drawing (draw=) runs inside the device pipeline's step graph only (cfg['device_glue'] on, "
+                             "cfg['host_warps'] off)")
         host_path = "tracking with cfg['device_glue'] off or cfg['host_warps'] on"
         imgs = fr.as_frames(frames, 'step', self.est.detector, None if device else host_path)
         if not device:
             fr.require_one_size(frames, host_path)
         elif fr.is_mixed(imgs):
             fr.check_frames(imgs, Ks, 'step')
-        out = self._step_device(imgs, Ks, kind) if device else self._step_host(frames, Ks, kind)
+        res = self._step_device(imgs, Ks, kind, out) if device else self._step_host(frames, Ks, kind)
         self._pending[:] = False
-        return out
+        return res
 
     def _step_host(self, frames, Ks, kind):
         est, S = self.est, self.S
@@ -435,22 +466,25 @@ class Tracker:
             self._dev = {'bbox': torch.from_numpy(self.bbox).to(dev), 'weights': torch.from_numpy(self.weights.copy()).to(dev)}
         return self._dev
 
-    def _full_fn(self, st):
+    def _full_fn(self, st, draw=None):
         predict, c = self.est._predict_device_fn(st), self._device_consts()
 
-        def fn(frames, cams, ring, count):
+        def fn(frames, cams, ring, count, *dt):
             chain, det, crop, idx, sel_out, logits = predict(frames, cams)
             poses = chain[-1]
-            smoothed, avg = ops.track_smooth(poses, chain.shape[0] > 1, c['bbox'], cams[:, :9].contiguous(), ring, count, c['weights'])
+            Ks = cams[:, :9].contiguous()
+            smoothed, avg = ops.track_smooth(poses, chain.shape[0] > 1, c['bbox'], Ks, ring, count, c['weights'])
+            if dt:
+                draw(frames, poses, chain.shape[0] > 1, smoothed, Ks, dt[0])
             packed = torch.cat([t.reshape(-1).to(torch.float64) for t in (chain, smoothed, avg, ring, count, det, idx, sel_out, logits)])
             return torch.cat([packed.view(torch.uint8), crop.reshape(-1)]), poses, ring, count
         return fn
 
-    def _refine_fn(self, st, first_f32):
+    def _refine_fn(self, st, first_f32, draw=None):
         est, iters, c = self.est, self.refine_iter, self._device_consts()
         R, refine = st['tables']['ref_num'], est.refiner._refine_warped(128)
 
-        def fn(frames, cams, prev, ring, count):
+        def fn(frames, cams, prev, ring, count, *dt):
             poses, chain = prev, [prev]
             for it in range(iters):
                 jobs, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems(st['views'], R, cams, frames, poses,
@@ -458,12 +492,15 @@ class Tracker:
                 out = refine(jobs, que_K, que_pose, ref_Ks, ref_poses)
                 poses = ops.glue_apply_refinements(st['views'], que_pose, que_K, rect, out)
                 chain.append(poses)
-            smoothed, avg = ops.track_smooth(poses, True, c['bbox'], cams[:, :9].contiguous(), ring, count, c['weights'])
+            Ks = cams[:, :9].contiguous()
+            smoothed, avg = ops.track_smooth(poses, True, c['bbox'], Ks, ring, count, c['weights'])
+            if dt:
+                draw(frames, poses, True, smoothed, Ks, dt[0])
             packed = torch.cat([t.reshape(-1).to(torch.float64) for t in (torch.stack(chain, 0), smoothed, avg, ring, count)])
             return packed.view(torch.uint8), poses, ring, count
         return fn
 
-    def _mixed_fn(self, st, b, blocks=None):
+    def _mixed_fn(self, st, b, blocks=None, draw=None):
         est, c = self.est, self._device_consts()
         initial = est._initial_poses_device_fn(st)
 
@@ -473,37 +510,39 @@ class Tracker:
 
         smooth = lambda poses, Ks, ring, count: ops.track_smooth(poses, True, c['bbox'], Ks, ring, count, c['weights'])
         return _mixed_fn(1, self.S, b, est.cfg['refine_iter'], self.refine_iter, init, [st['views']], st['tables']['ref_num'],
-                         est.refiner._refine_warped(128), smooth, blocks)
+                         est.refiner._refine_warped(128), smooth, blocks, draw)
 
-    def _step_device(self, frames, Ks, kind):
+    def _step_device(self, frames, Ks, kind, out=None):
         est, S, num = self.est, self.S, self.num
         st = est._glue_state()
         self._to(True)
         full = kind == 'full'
         imgs = frames                                     # numpy or device frames (as_frames)
         plan, pick = fr.FramePlan(fr.size_pattern(imgs)), None
+        draw, dt, drawn, named = draw_inputs(self._drawer, est.detector, plan, out)
         with torch.no_grad():
             if full:
-                name, fn, fin = fr.stage(est.detector, 'track_full', self._full_fn(st), imgs, plan)
+                name, fn, fin = fr.stage(est.detector, named('track_full'), self._full_fn(st, draw), imgs, plan)
                 cams = est.detector._to_dev(glue.cameras(Ks))
-                outs = self.stages.run(name, fn, fin + [cams, self._ring, self._count])
+                outs = self.stages.run(name, fn, fin + [cams, self._ring, self._count] + dt)
             elif kind == 'refine':
                 prev_f32 = bool(self._f32[0])
-                name, fn, fin = fr.stage(est.detector, f'track_refine{int(prev_f32)}', self._refine_fn(st, prev_f32), imgs, plan)
+                name, fn, fin = fr.stage(est.detector, named(f'track_refine{int(prev_f32)}'), self._refine_fn(st, prev_f32, draw),
+                                         imgs, plan)
                 cams = est.detector._to_dev(glue.cameras(Ks))
-                outs = self.stages.run(name, fn, fin + [cams, self._prev, self._ring, self._count])
+                outs = self.stages.run(name, fn, fin + [cams, self._prev, self._ring, self._count] + dt)
             else:
                 F, dev = est.cfg['refine_iter'], est.detector.device
                 reinit, b, extra = _mixed_inputs(S, 1, self._pending, self._f32, F, self.refine_iter, dev, plan)
                 if plan.mixed:                   # one graph per size pattern and per-size buckets (row f13)
                     _, blocks, pick = _size_buckets(reinit, plan)
-                    name, fn = (plan.key('track_mixed'), tuple(blocks)), self._mixed_fn(st, b, blocks)
+                    name, fn = named((plan.key('track_mixed'), tuple(blocks))), self._mixed_fn(st, b, blocks, draw)
                 else:
-                    name, fn = f'track_mixed{b}', self._mixed_fn(st, b)
+                    name, fn = named(f'track_mixed{b}'), self._mixed_fn(st, b, draw=draw)
                 name, fn, fin = fr.bind(est.detector, name, fn, imgs, plan)
                 cams = est.detector._to_dev(glue.cameras(Ks))
                 prev = self._prev if self._prev is not None else torch.zeros(S, 12, dtype=torch.float64, device=dev)
-                outs = self.stages.run(name, fn, fin + [cams, prev, self._ring, self._count] + extra)
+                outs = self.stages.run(name, fn, fin + [cams, prev, self._ring, self._count] + extra + dt)
             buf, poses_dev, ring, count = outs
             self._prev = poses_dev.clone()
             self._ring.copy_(ring)
@@ -511,8 +550,13 @@ class Tracker:
             host = est.detector._to_host(buf)                        # the step's one synchronising read
         prev_f32 = bool(self._f32[0])
         self._f32[:] = True
-        if kind == 'mixed':
-            return self._decode_mixed(host, reinit, b, pick)
+        res = self._decode_mixed(host, reinit, b, pick) if kind == 'mixed' else self._decode(host, full, prev_f32)
+        if drawn is not None:
+            res[2]['drawn'] = drawn
+        return res
+
+    def _decode(self, host, full, prev_f32):
+        est, S, num = self.est, self.S, self.num
         n_chain = (est.cfg['refine_iter'] if full else self.refine_iter) + 1
         sizes = [('chain', n_chain * S * 12), ('smoothed', S * 12), ('avg', S * 16), ('ring', S * num * 16), ('count', S)]
         if full:
@@ -589,7 +633,9 @@ class ObjectTracker:
     g6d_glue_apply_refinements_objects), then g6d_track_smooth_objects, so the number of launches does not grow with
     K.  The previous poses [K*S,12], the corner histories and their counts stay on the device between steps."""
 
-    def __init__(self, objs, num_sequences, refine_iter=1, smooth_num=5, smooth_std=2.5, bboxes=None):
+    def __init__(self, objs, num_sequences, refine_iter=1, smooth_num=5, smooth_std=2.5, bboxes=None, draw=None,
+                 draw_colors=None):
+        kinds = dr.parse_kinds(draw)
         if int(num_sequences) < 1:
             raise ValueError(f'num_sequences must be >= 1, got {num_sequences}')
         if int(refine_iter) < 1:
@@ -610,6 +656,9 @@ class ObjectTracker:
         self.stages = StageCache()       # this tracker's step graphs (they capture its device state)
         dev = self.est.detector.device
         self._dev = {'bboxes': torch.from_numpy(self.bboxes).to(dev), 'weights': torch.from_numpy(self.weights.copy()).to(dev)}
+        self.draw = kinds
+        self._drawer = dr.StepDrawer(kinds, dr.object_colors(self.names, draw_colors), self.bboxes, range(self.K), self.S,
+                                     dev) if kinds else None
         self.reset()
 
     # -------------------------------------------------------------- state
@@ -676,15 +725,17 @@ class ObjectTracker:
         self.objs._check()
 
     # -------------------------------------------------------------- one step
-    def _full_fn(self):
+    def _full_fn(self, draw=None):
         predict, c, K = self.objs._predict_device_fn(), self._dev, self.K
 
-        def fn(frames, cams, ring, count):
+        def fn(frames, cams, ring, count, *dt):
             S = frames.shape[0]
             chain, det, sels, crop = predict(frames, cams)
             poses = chain[-1]
-            smoothed, avg = ops.track_smooth_objects(poses, chain.shape[0] > 1, c['bboxes'], cams[:, :9].contiguous(), ring, count,
-                                                     c['weights'])
+            Ks = cams[:, :9].contiguous()
+            smoothed, avg = ops.track_smooth_objects(poses, chain.shape[0] > 1, c['bboxes'], Ks, ring, count, c['weights'])
+            if dt:
+                draw(frames, poses, chain.shape[0] > 1, smoothed, Ks, dt[0])
             parts = [chain, smoothed, avg, ring, count]
             for o in range(K):
                 parts += [det[o * S:(o + 1) * S], *sels[o]]
@@ -692,12 +743,12 @@ class ObjectTracker:
             return torch.cat([packed.view(torch.uint8), crop.reshape(-1)]), poses, ring, count
         return fn
 
-    def _refine_fn(self, first_f32):
+    def _refine_fn(self, first_f32, draw=None):
         objs, iters, c = list(self.objs._objects.values()), self.refine_iter, self._dev
         views, R = [ob.tables['views'] for ob in objs], objs[0].tables['tables']['ref_num']
         refine = self.est.refiner._refine_warped(128)
 
-        def fn(frames, cams, prev, ring, count):
+        def fn(frames, cams, prev, ring, count, *dt):
             poses, chain = prev, [prev]
             for it in range(iters):
                 jobs, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems_objects(views, R, cams, frames, poses,
@@ -705,12 +756,15 @@ class ObjectTracker:
                 out = refine(jobs, que_K, que_pose, ref_Ks, ref_poses)           # one refiner stage for all K*S poses
                 poses = ops.glue_apply_refinements_objects(views, que_pose, que_K, rect, out)
                 chain.append(poses)
-            smoothed, avg = ops.track_smooth_objects(poses, True, c['bboxes'], cams[:, :9].contiguous(), ring, count, c['weights'])
+            Ks = cams[:, :9].contiguous()
+            smoothed, avg = ops.track_smooth_objects(poses, True, c['bboxes'], Ks, ring, count, c['weights'])
+            if dt:
+                draw(frames, poses, True, smoothed, Ks, dt[0])
             packed = torch.cat([t.reshape(-1).to(torch.float64) for t in (torch.stack(chain, 0), smoothed, avg, ring, count)])
             return packed.view(torch.uint8), poses, ring, count
         return fn
 
-    def _mixed_fn(self, b, blocks=None):
+    def _mixed_fn(self, b, blocks=None, draw=None):
         objs, c, K = list(self.objs._objects.values()), self._dev, self.K
         initial = self.objs._initial_poses_device_fn()
 
@@ -723,11 +777,12 @@ class ObjectTracker:
 
         smooth = lambda poses, Ks, ring, count: ops.track_smooth_objects(poses, True, c['bboxes'], Ks, ring, count, c['weights'])
         return _mixed_fn(K, self.S, b, self.est.cfg['refine_iter'], self.refine_iter, init, [ob.tables['views'] for ob in objs],
-                         objs[0].tables['tables']['ref_num'], self.est.refiner._refine_warped(128), smooth, blocks)
+                         objs[0].tables['tables']['ref_num'], self.est.refiner._refine_warped(128), smooth, blocks, draw)
 
-    def step(self, frames, Ks):
+    def step(self, frames, Ks, out=None):
         """frames: S uint8 [h,w,3] (of one size or several, row f13; or device frames, row f14, as Tracker.step takes them);
-        Ks: [S,3,3] (shared by all objects).  Returns {name: (raw poses float32
+        Ks: [S,3,3] (shared by all objects); out: drawing destinations as Tracker.step takes them, every object's box
+        drawn on its sequence's frame in object order (each step's result then also holds inter['drawn'] without out=).  Returns {name: (raw poses float32
         [S,3,4], smoothed poses float64 [S,3,4], inter)}: inter has Tracker.step's keys, and a full-prediction step adds
         those of ObjectSet.predict (det_score included); a mixed step adds 'reinit' and those entries for the
         re-initialised sequences, as Tracker.step does."""
@@ -744,28 +799,30 @@ class ObjectTracker:
         plan, pick = fr.FramePlan(fr.size_pattern(imgs)), None
         if plan.mixed:
             fr.check_frames(imgs, Ks, 'step')
+        draw, dt, drawn, named = draw_inputs(self._drawer, est.detector, plan, out)
         with torch.no_grad():
             if full:
-                name, fn, fin = fr.stage(est.detector, 'track_full', self._full_fn(), imgs, plan)
+                name, fn, fin = fr.stage(est.detector, named('track_full'), self._full_fn(draw), imgs, plan)
                 cams = est.detector._to_dev(glue.cameras(Ks))
-                outs = self.stages.run(name, fn, fin + [cams, self._ring, self._count])
+                outs = self.stages.run(name, fn, fin + [cams, self._ring, self._count] + dt)
             elif not mixed:
                 prev_f32 = bool(self._f32[0])
-                name, fn, fin = fr.stage(est.detector, f'track_refine{int(prev_f32)}', self._refine_fn(prev_f32), imgs, plan)
+                name, fn, fin = fr.stage(est.detector, named(f'track_refine{int(prev_f32)}'), self._refine_fn(prev_f32, draw), imgs,
+                                         plan)
                 cams = est.detector._to_dev(glue.cameras(Ks))
-                outs = self.stages.run(name, fn, fin + [cams, self._prev, self._ring, self._count])
+                outs = self.stages.run(name, fn, fin + [cams, self._prev, self._ring, self._count] + dt)
             else:
                 dev = est.detector.device
                 reinit, b, extra = _mixed_inputs(S, K, self._pending, self._f32, est.cfg['refine_iter'], self.refine_iter, dev, plan)
                 if plan.mixed:                   # one graph per size pattern and per-size buckets (row f13)
                     _, blocks, pick = _size_buckets(reinit, plan)
-                    name, fn = (plan.key('track_mixed'), tuple(blocks)), self._mixed_fn(b, blocks)
+                    name, fn = named((plan.key('track_mixed'), tuple(blocks))), self._mixed_fn(b, blocks, draw)
                 else:
-                    name, fn = f'track_mixed{b}', self._mixed_fn(b)
+                    name, fn = named(f'track_mixed{b}'), self._mixed_fn(b, draw=draw)
                 name, fn, fin = fr.bind(est.detector, name, fn, imgs, plan)
                 cams = est.detector._to_dev(glue.cameras(Ks))
                 prev = self._prev if self._prev is not None else torch.zeros(K * S, 12, dtype=torch.float64, device=dev)
-                outs = self.stages.run(name, fn, fin + [cams, prev, self._ring, self._count] + extra)
+                outs = self.stages.run(name, fn, fin + [cams, prev, self._ring, self._count] + extra + dt)
             buf, poses_dev, ring, count = outs
             prev_f32 = bool(self._f32[0])
             self._prev = poses_dev.clone()
@@ -798,7 +855,7 @@ class ObjectTracker:
         avg = take(n * 16).reshape(K, S, 8, 2)
         ring_h = take(n * num * 16).reshape(K, S, num, 8, 2).astype(np.float32)
         count_h = take(n).reshape(K, S).astype(np.int64)
-        out = {}
+        res = {}
         for o, (name, ob) in enumerate(self.objs._objects.items()):
             refined = [c.astype(np.float32) for c in chain[1:, o]]
             first = chain[0, o].astype(np.float32) if (kind == 'refine' and prev_f32) else chain[0, o].copy()
@@ -814,5 +871,7 @@ class ObjectTracker:
             inter['refine_poses'] = [first] + refined
             inter['bbox_pts'] = ring_h[o, np.arange(S), count_h[o] - 1].copy()
             inter['smoothed_pts'] = avg[o].copy()
-            out[name] = (refined[-1] if refined else first), smoothed[o].copy(), inter
-        return out
+            if drawn is not None:
+                inter['drawn'] = drawn
+            res[name] = (refined[-1] if refined else first), smoothed[o].copy(), inter
+        return res

@@ -250,6 +250,43 @@ int g6d_track_smooth_objects(const double* poses, int poses_are_f32, const float
 int g6d_track_smooth_objects_host(const double* poses, int poses_are_f32, const float* bboxes, int n_obj, int rows_per_obj,
                                   const double* Ks, float* ring, int* count, int num, const double* weights, double* smoothed,
                                   double* avg_pts);
+/* ---- drawn frames (predict.py:61-72 with utils/draw_utils.py:94-103,274-294 draw_bbox_3d): each destination frame is
+ * its source frame with the 3-D boxes of its g6d_draw_box entries drawn one after the other, bit for bit as
+ *   img = draw_bbox_3d(img, np.round(project_points(bbox, pose, K)) ..., color)
+ * with OpenCV's 8-bit drawing (8 filled red dots of radius 2, then 12 edges of thickness 2; csrc/draw_math.cuh).
+ * Source frame i is the uint8 RGB image [rows, cols, 3] at src + offset with row pitch `pitch` (>= 3*cols).  Destination
+ * d (a g6d_device_frame row: RGB with any pitch, or NV12 planes with an even size, converted as
+ * cv2.cvtColor(COLOR_RGB2YUV_I420) with U and V interleaved; its `offset` is unused) shows source d % n_src and has its
+ * size.  Box b projects bboxes[bbox] (float32 [8,3]) with poses[pose] (float64 values [12]; pose_f32: float32 values,
+ * projected in float32 as the smoothing projects them, else in float64) and Ks[K] (float64 values [9]); valid >= 0
+ * draws it only when ids[valid] >= 0 (a live track of an instance tracker), valid = -1 always; at most
+ * G6D_DRAW_MAX_BOXES boxes per destination, drawn in table order.  g6d_draw_check validates HOST copies of the tables
+ * (n_poses, n_Ks, n_bboxes, n_ids: the rows each array holds); g6d_draw_boxes reads srcs, boxes and dsts from DEVICE memory
+ * (checked by the caller before the upload; max_rows / max_cols bound every destination) and writes every byte of every
+ * destination's image; g6d_draw_boxes_host runs the same code on HOST tables and buffers (checked first).
+ * g6d_rgb_to_nv12 / _host convert without drawing: the RGB image [rows, cols, 3] (row pitch `pitch`) to the NV12 planes
+ * y [rows, cols] (pitch_y) and uv [rows/2, cols] (pitch_uv), rows and cols even. */
+#define G6D_DRAW_MAX_BOXES 16
+typedef struct g6d_draw_src {
+    long long offset, pitch;       /* byte offset from src, row pitch in bytes */
+    int rows, cols;
+} g6d_draw_src;
+typedef struct g6d_draw_box {
+    int dst, pose, K, bbox, pose_f32, valid;
+    uint8_t color[4];              /* the edges' (R, G, B); [3] unused */
+} g6d_draw_box;
+int g6d_draw_check(const g6d_draw_src* host_srcs, int n_src, const g6d_draw_box* host_boxes, int n_boxes,
+                   const g6d_device_frame* host_dsts, int n_dst, int n_poses, int n_Ks, int n_bboxes, int n_ids);
+int g6d_draw_boxes(const uint8_t* src, const g6d_draw_src* srcs, int n_src, const double* poses, const double* Ks,
+                   const float* bboxes, const long long* ids, const g6d_draw_box* boxes, int n_boxes,
+                   const g6d_device_frame* dsts, int n_dst, int max_rows, int max_cols, g6d_stream_t stream);
+int g6d_draw_boxes_host(const uint8_t* src, const g6d_draw_src* host_srcs, int n_src, const double* poses, int n_poses,
+                        const double* Ks, int n_Ks, const float* bboxes, int n_bboxes, const long long* ids, int n_ids,
+                        const g6d_draw_box* host_boxes, int n_boxes, const g6d_device_frame* host_dsts, int n_dst);
+int g6d_rgb_to_nv12(const uint8_t* rgb, long long pitch, int rows, int cols, uint8_t* y, long long pitch_y, uint8_t* uv,
+                    long long pitch_uv, g6d_stream_t stream);
+int g6d_rgb_to_nv12_host(const uint8_t* rgb, long long pitch, int rows, int cols, uint8_t* y, long long pitch_y, uint8_t* uv,
+                         long long pitch_uv);
 /* ---- the re-detection step of the multi-instance tracker (gen6d_b200/instance_track.py): M slots per sequence, rows
  * instance-major (row m*S + s is slot m of sequence s; 1 <= M <= G6D_DET_MAX_INSTANCES).  Per sequence s:
  *  1. the track point of each live slot: the object centre (cx, cy, cz) projected with prev[row] [12] and cams[s].K in
