@@ -8,6 +8,7 @@ object's 3-D box drawn by utils/draw_utils.py draw_bbox_3d, bit for bit with Ope
 The raw box is projected with the raw float32 pose in float32 (the corners inter['bbox_pts'] holds), the smoothed box
 with the float64 smoothed pose in float64 (predict.py's pts__), then rounded as np.round(...).astype(np.int32).
 """
+import copy
 import ctypes as C
 
 import numpy as np
@@ -87,7 +88,7 @@ class StepDrawer:
         if self.G > _lib.G6D_DRAW_MAX_BOXES:
             raise ValueError(f'draw: {self.G} boxes per frame (objects x instance slots); at most {_lib.G6D_DRAW_MAX_BOXES} are drawn')
         self.bboxes = torch.from_numpy(np.ascontiguousarray(bboxes, np.float32).reshape(-1, 8, 3)).to(device)
-        self._srcs, self._boxes, self._own = {}, {}, {}
+        self._srcs, self._boxes, self._own, self._subs = {}, {}, {}, {}
 
     def name(self, base):
         """The graph name of a drawing step: apart from the non-drawing graph `base`."""
@@ -116,22 +117,37 @@ class StepDrawer:
             t = self._boxes[raw_f32] = (module._to_dev(_bytes(rows, ops.DrawBox)), rows)
         return t
 
-    def destinations(self, module, plan, out):
+    def for_sequences(self, S):
+        """The drawer of a compact batch of S sequences (a partial step, row f17): this drawer's kinds, boxes and colours,
+        its own tables and buffers; made once per S."""
+        sub = self._subs.get(S)
+        if sub is None:
+            sub = self._subs[S] = copy.copy(self)
+            sub.S, sub._srcs, sub._boxes, sub._own, sub._subs = S, {}, {}, {}, {}
+        return sub
+
+    def destinations(self, module, plan, out, real=None):
         """-> (the DeviceFrame table on the device, inter['drawn'] or None), checked before anything is enqueued.  out
-        None: tracker-owned RGB buffers per size pattern (their table is made once)."""
+        None: tracker-owned RGB buffers per size pattern (their table is made once).  real: out holds destinations for
+        the first `real` sequences only (a partial step's listed ones); the others (its padding) draw into the
+        tracker-owned buffers as scratch."""
         S, pattern = self.S, plan.pattern
-        if out is None:
+        real = S if real is None else real
+        if out is None or real < S:
             own = self._own.get(pattern)
             if own is None:
                 bufs = {k: [torch.empty(h, w, 3, dtype=torch.uint8, device=self.device) for h, w in pattern] for k in self.kinds}
                 own = self._own[pattern] = (self._table(module, plan, bufs), bufs)
-            return own[0], {k: list(v) for k, v in own[1].items()}
+            if out is None:
+                return own[0], {k: list(v) for k, v in own[1].items()}
         if not isinstance(out, dict) or set(out) != set(self.kinds):
             raise ValueError(f'step: out must be a dict with exactly the drawn kinds {list(self.kinds)}, got '
                              f'{sorted(out) if isinstance(out, dict) else type(out).__name__}')
         for k in self.kinds:
-            if len(out[k]) != S:
-                raise ValueError(f'step: out[{k!r}] holds {len(out[k])} destinations, need one per sequence ({S})')
+            if len(out[k]) != real:
+                raise ValueError(f'step: out[{k!r}] holds {len(out[k])} destinations, need one per sequence ({real})')
+        if real < S:
+            out = {k: list(out[k]) + own[1][k][real:] for k in self.kinds}
         return self._table(module, plan, out), None
 
     def _table(self, module, plan, dests):

@@ -13,7 +13,12 @@ glue and smoothing launches (the g6d_*_objects entry points) and refiner stage c
 
 reset(sequences) / start(poses, sequences) re-initialise or restart single sequences while the others keep tracking;
 the step after them is the mixed step below, also one graph and one read.
+
+step(..., sequences=[...]) steps a subset of the sequences and leaves the others untouched (the partial step below), so
+streams at different frame rates, or that pause, share one tracker; S is then its capacity.
 """
+import copy
+
 import numpy as np
 import torch
 
@@ -241,14 +246,15 @@ def _mixed_fn(K, S, b, F, r, initial, views, R, refine, smooth, blocks=None, dra
     return fn
 
 
-def draw_inputs(drawer, module, plan, out):
+def draw_inputs(drawer, module, plan, out, real=None):
     """A step's drawing (row f16) -> (draw hook for the graph body or None, [destination table] graph inputs, inter['drawn']
-    or None, graph name map).  The destinations are checked here, before anything is enqueued."""
+    or None, graph name map).  The destinations are checked here, before anything is enqueued.  real: the leading
+    sequences of a compact batch that out= covers (a partial step, row f17; the others are padding)."""
     if drawer is None:
         if out is not None:
             raise ValueError('step: out= names drawing destinations; create the tracker with draw=')
         return None, [], None, (lambda n: n)
-    table, drawn = drawer.destinations(module, plan, out)
+    table, drawn = drawer.destinations(module, plan, out, real)
     return (lambda *a: drawer.node(module, plan, *a)), [table], drawn, drawer.name
 
 
@@ -261,6 +267,108 @@ def _sequences(S, sequences):
     if bad:
         raise ValueError(f'sequences {bad} are outside [0, {S})')
     return np.asarray(seqs, np.int64)
+
+
+def _step_kind(pending, f32, F):
+    """'full', 'refine' or 'mixed': the graph a step over sequences with these pending and float32 flags replays (F:
+    cfg['refine_iter'])."""
+    if pending.all():
+        return 'full'
+    if not pending.any() and (f32.all() or not f32.any()):
+        return 'refine'
+    if pending.any() and F < 1:
+        raise ValueError("re-initialising some sequences while others track needs cfg['refine_iter'] >= 1 (the step "
+                         'smooths float32 poses)')
+    return 'mixed'
+
+
+# ------------------------------------------------------------------------------------------ the partial step
+# A step over a subset of the sequences (row f17): the a listed sequences, sorted and padded to b = _bucket(a, S) by
+# repeating the last, run the unchanged step body of a b-sequence tracker on compact copies of their state rows, gathered
+# inside the graph; only the a real rows are copied back.  The gather and scatter rows are graph inputs, so every list of
+# one bucket (and step kind, size pattern and drawing) replays one graph.
+class PartialStep:
+    """The host plan of a partial step.  sequences: the caller's list (int64); seq: the compact batch's sequences [b],
+    ascending, then padding; pos[i]: the compact row of sequences[i]; pending / f32: the compact rows' flags; kind: the
+    step kind from them; gather int64 [K*b]: the tracker rows (object-major, o*S + s) of the compact rows o*b + j;
+    scatter int64 [K*b]: where compact row o*b + j goes in [tracker rows; compact rows], its tracker row when real, its
+    own copy (K*S + o*b + j) when padding; lockstep: every sequence is listed (the step is the lockstep step, reordered)."""
+
+    def __init__(self, S, K, sequences, pending, f32, F):
+        self.sequences = _sequences(S, sequences)
+        if not len(self.sequences):
+            raise ValueError('step: sequences lists no sequence; list at least one (or pass None for all)')
+        order = np.argsort(self.sequences, kind='stable')
+        self.S, self.K, self.a = S, K, len(order)
+        self.lockstep = self.a == S
+        self.b = S if self.lockstep else _bucket(self.a, S)
+        self.order = np.concatenate([order, np.full(self.b - self.a, order[-1])])      # caller index of each compact row
+        self.seq = self.sequences[self.order]
+        self.pos = np.empty(self.a, np.int64)
+        self.pos[order] = np.arange(self.a)
+        self.pending, self.f32 = pending[self.seq].copy(), f32[self.seq].copy()
+        self.kind = _step_kind(self.pending, self.f32, F)
+        j = np.arange(self.b)
+        self.gather = np.concatenate([o * S + self.seq for o in range(K)])
+        self.scatter = np.concatenate([np.where(j < self.a, o * S + self.seq, K * S + o * self.b + j) for o in range(K)])
+
+    def name(self, base):
+        """The graph name of the compact batch's step `base` (a lockstep name): apart from every lockstep graph."""
+        return (base, 'rows', self.b)
+
+    def check(self, frames, Ks, out=None):
+        """ValueError unless frames, Ks and every out= list hold one entry per listed sequence."""
+        n = [len(frames), len(Ks)] + ([len(v) for v in out.values()] if isinstance(out, dict) else [])
+        if any(m != self.a for m in n):
+            raise ValueError(f'step: sequences lists {self.a} sequences; frames, Ks and every out= list need one entry each, '
+                             f'got {len(frames)} frames, {len(Ks)} Ks' +
+                             (f', out {({k: len(v) for k, v in out.items()})}' if isinstance(out, dict) else ''))
+
+    def compact(self, items):
+        """The caller's per-sequence entries in compact row order (padding repeats the last listed sequence's)."""
+        return [items[i] for i in self.order]
+
+    def compact_out(self, out):
+        return None if out is None else {k: [v[i] for i in self.order[:self.a]] for k, v in out.items()}
+
+    def graph_inputs(self, device):
+        up = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.int64)).to(device)
+        return [up(self.gather), up(self.scatter)]
+
+    def results(self, raw, smoothed, inter):
+        """A step's results over the compact rows (ascending, padding last) -> the listed sequences' in the caller's order.
+        A mixed step's 'reinit' becomes tracker-wide sequences (ascending) with their detection entries in that order."""
+        pos = self.pos
+        take = lambda v, idx: v[idx] if isinstance(v, np.ndarray) else [v[i] for i in idx]
+        res = {}
+        if 'reinit' in inter:
+            r = np.asarray(inter['reinit'], np.int64)
+            m = int((r < self.a).sum())                    # the real re-initialised rows come first (ascending)
+        for k, v in inter.items():
+            if k == 'reinit':
+                res[k] = self.seq[r[:m]]
+            elif k == 'drawn':
+                res[k] = {kind: take(d, pos) for kind, d in v.items()}
+            elif k == 'refine_poses':
+                res[k] = [c[pos] for c in v]
+            elif 'reinit' in inter and k not in ('bbox_pts', 'smoothed_pts'):
+                res[k] = take(v, range(m))
+            else:
+                res[k] = take(v, pos)
+        res['sequences'] = self.sequences.copy()
+        return raw[pos], smoothed[pos], res
+
+
+def _compact_fn(fn, full):
+    """A lockstep step body fn(frames, cams, [prev,] ring, count, *rest) of the compact batch -> the partial step's graph
+    body g(frames, cams, prev, ring, count, gather, scatter, *rest) on the tracker's whole state: gather the compact rows,
+    run fn, copy its real rows back (padding rows land in their scratch copies, dropped)."""
+    def g(frames, cams, prev, ring, count, gather, scatter, *rest):
+        sub = [t.index_select(0, gather) for t in ((ring, count) if full else (prev, ring, count))]
+        buf, poses, ring_c, count_c = fn(frames, cams, *sub, *rest)
+        put = lambda t, c: torch.cat([t, c], 0).index_copy_(0, scatter, c)[:t.shape[0]]
+        return buf, put(prev, poses), put(ring, ring_c), put(count, count_c)
+    return g
 
 
 # ------------------------------------------------------------------------------------------ the tracker
@@ -368,17 +476,18 @@ class Tracker:
 
     def _kind(self):
         """'full', 'refine' or 'mixed': the graph the next step replays."""
-        if self._pending.all():
-            return 'full'
-        if not self._pending.any() and (self._f32.all() or not self._f32.any()):
-            return 'refine'
-        if self._pending.any() and self.est.cfg['refine_iter'] < 1:
-            raise ValueError("re-initialising some sequences while others track needs cfg['refine_iter'] >= 1 (the step "
-                             'smooths float32 poses)')
-        return 'mixed'
+        return _step_kind(self._pending, self._f32, self.est.cfg['refine_iter'])
+
+    def _partial(self, frames, Ks, out, sequences):
+        """The plan of a step over `sequences` (row f17), its arguments checked before anything is enqueued."""
+        part = PartialStep(self.S, getattr(self, 'K', 1), sequences, self._pending, self._f32, self.est.cfg['refine_iter'])
+        part.check(frames, Ks, out)
+        if out is not None and self._drawer is None:
+            raise ValueError('step: out= names drawing destinations; create the tracker with draw=')
+        return part
 
     # -------------------------------------------------------------- one step
-    def step(self, frames, Ks, out=None):
+    def step(self, frames, Ks, out=None, sequences=None):
         """frames: S uint8 [h,w,3] (of different sizes on the device path, row f13; or, on that path, device frames with
         predict_batch's rules, row f14: CUDA RGB tensors and frames.NV12 surfaces, ready on the current stream and free to
         reuse when step returns); Ks: [S,3,3].  Returns (raw poses float32 [S,3,4], smoothed poses float64
@@ -393,14 +502,30 @@ class Tracker:
         node: inter['drawn'] = {kind: S CUDA uint8 [h, w, 3] views of tracker-owned buffers at each frame's working size,
         overwritten by the next step}.  out={kind: S destinations} (CUDA uint8 RGB tensors of the working size with any
         row pitch, or frames.NV12 of an even working size) writes into the caller's buffers instead; they are written on
-        the current stream."""
+        the current stream.
+
+        sequences (row f17): step only these sequences (distinct, in any order, at least one); frames, Ks and out's lists
+        then hold one entry per listed sequence in that order, and every result (poses [n,3,4], each inter array, the
+        drawn frames) comes back in that order, with inter['sequences'] echoing the list and a mixed step's
+        inter['reinit'] holding tracker-wide sequences.  Each listed sequence takes exactly the step it would take in
+        lockstep (a full prediction if pending, else refinement from its start or previous pose, then the smoothing over
+        its own history); the others are untouched: no computation, their state and pending flags kept as they are.  The
+        listed sequences run as a compact batch of _bucket(n, S) sequences (the last repeated as padding), one captured
+        graph per bucket, step kind, size pattern and drawing, so results equal those of a tracker of that many
+        sequences.  Listing every sequence is the lockstep step."""
         self._check()
-        if len(frames) != self.S or len(Ks) != self.S:
+        part = None
+        if sequences is not None:
+            part = self._partial(frames, Ks, out, sequences)
+            frames, Ks, out = part.compact(frames), part.compact(Ks), part.compact_out(out)
+            if part.lockstep:
+                return part.results(*self.step(frames, Ks, out))
+        elif len(frames) != self.S or len(Ks) != self.S:
             raise ValueError(f'step: this tracker follows {self.S} sequences, got {len(frames)} frames and {len(Ks)} Ks')
         if out is not None and self._drawer is None:
             raise ValueError('step: out= names drawing destinations; create the tracker with draw=')
         Ks = np.stack([np.asarray(K) for K in Ks], 0)
-        kind = self._kind()
+        kind = self._kind() if part is None else part.kind
         device = self._device_path()
         if self._drawer is not None and not device:
             raise ValueError("drawing (draw=) runs inside the device pipeline's step graph only (cfg['device_glue'] on, "
@@ -411,8 +536,28 @@ class Tracker:
             fr.require_one_size(frames, host_path)
         elif fr.is_mixed(imgs):
             fr.check_frames(imgs, Ks, 'step')
-        res = self._step_device(imgs, Ks, kind, out) if device else self._step_host(frames, Ks, kind)
-        self._pending[:] = False
+        if part is None:
+            res = self._step_device(imgs, Ks, kind, out) if device else self._step_host(frames, Ks, kind)
+            self._pending[:] = False
+            return res
+        res = self._step_device(imgs, Ks, kind, out, part) if device else self._step_host_partial(frames, Ks, kind, part)
+        self._pending[part.seq] = False
+        return part.results(*res)
+
+    def _step_host_partial(self, frames, Ks, kind, part):
+        """A partial step on the host path: _step_host on a view of this tracker holding the listed sequences' rows only
+        (ascending, no padding), whose state is copied back."""
+        self._to(False)
+        seqs, a = part.seq[:part.a], part.a
+        sub = copy.copy(self)
+        sub.S, sub._pending, sub._f32 = a, part.pending[:a].copy(), part.f32[:a].copy()
+        sub._prev = None if self._prev is None else self._prev[seqs]
+        sub._ring, sub._count = self._ring[seqs], self._count[seqs]
+        res = sub._step_host(frames[:a], Ks[:a], kind)
+        if self._prev is None:
+            self._prev = np.zeros((self.S, 3, 4))
+        self._prev[seqs], self._f32[seqs] = sub._prev, sub._f32
+        self._ring[seqs], self._count[seqs] = sub._ring, sub._count
         return res
 
     def _step_host(self, frames, Ks, kind):
@@ -500,7 +645,7 @@ class Tracker:
             return packed.view(torch.uint8), poses, ring, count
         return fn
 
-    def _mixed_fn(self, st, b, blocks=None, draw=None):
+    def _mixed_fn(self, st, b, blocks=None, draw=None, S=None):
         est, c = self.est, self._device_consts()
         initial = est._initial_poses_device_fn(st)
 
@@ -509,54 +654,66 @@ class Tracker:
             return poses, crop, [det, idx, sel_out, logits]
 
         smooth = lambda poses, Ks, ring, count: ops.track_smooth(poses, True, c['bbox'], Ks, ring, count, c['weights'])
-        return _mixed_fn(1, self.S, b, est.cfg['refine_iter'], self.refine_iter, init, [st['views']], st['tables']['ref_num'],
-                         est.refiner._refine_warped(128), smooth, blocks, draw)
+        return _mixed_fn(1, S or self.S, b, est.cfg['refine_iter'], self.refine_iter, init, [st['views']],
+                         st['tables']['ref_num'], est.refiner._refine_warped(128), smooth, blocks, draw)
 
-    def _step_device(self, frames, Ks, kind, out=None):
-        est, S, num = self.est, self.S, self.num
+    def _step_device(self, frames, Ks, kind, out=None, part=None):
+        """One step's graph.  part: a partial step (row f17), whose compact batch of part.b sequences runs the same bodies
+        on gathered state rows (_compact_fn) under the names part.name(...)."""
+        est = self.est
         st = est._glue_state()
         self._to(True)
+        S, pending, f32 = (self.S, self._pending, self._f32) if part is None else (part.b, part.pending, part.f32)
+        rows = (lambda n: n) if part is None else part.name
+        drawer = self._drawer if part is None or self._drawer is None else self._drawer.for_sequences(part.b)
         full = kind == 'full'
         imgs = frames                                     # numpy or device frames (as_frames)
         plan, pick = fr.FramePlan(fr.size_pattern(imgs)), None
-        draw, dt, drawn, named = draw_inputs(self._drawer, est.detector, plan, out)
+        draw, dt, drawn, named = draw_inputs(drawer, est.detector, plan, out, None if part is None else part.a)
+        dev = est.detector.device
+        if self._prev is None and (part is not None or kind == 'mixed'):
+            self._prev = torch.zeros(self.S, 12, dtype=torch.float64, device=dev)
+        wrap, extra = (lambda fn: fn), []
+        if part is not None:
+            wrap = lambda fn: _compact_fn(fn, full)
         with torch.no_grad():
             if full:
-                name, fn, fin = fr.stage(est.detector, named('track_full'), self._full_fn(st, draw), imgs, plan)
-                cams = est.detector._to_dev(glue.cameras(Ks))
-                outs = self.stages.run(name, fn, fin + [cams, self._ring, self._count] + dt)
+                name, fn, fin = fr.stage(est.detector, named(rows('track_full')), wrap(self._full_fn(st, draw)), imgs, plan)
             elif kind == 'refine':
-                prev_f32 = bool(self._f32[0])
-                name, fn, fin = fr.stage(est.detector, named(f'track_refine{int(prev_f32)}'), self._refine_fn(st, prev_f32, draw),
-                                         imgs, plan)
-                cams = est.detector._to_dev(glue.cameras(Ks))
-                outs = self.stages.run(name, fn, fin + [cams, self._prev, self._ring, self._count] + dt)
+                prev_f32 = bool(f32[0])
+                name, fn, fin = fr.stage(est.detector, named(rows(f'track_refine{int(prev_f32)}')),
+                                         wrap(self._refine_fn(st, prev_f32, draw)), imgs, plan)
             else:
-                F, dev = est.cfg['refine_iter'], est.detector.device
-                reinit, b, extra = _mixed_inputs(S, 1, self._pending, self._f32, F, self.refine_iter, dev, plan)
+                F = est.cfg['refine_iter']
+                reinit, b, extra = _mixed_inputs(S, 1, pending, f32, F, self.refine_iter, dev, plan)
                 if plan.mixed:                   # one graph per size pattern and per-size buckets (row f13)
                     _, blocks, pick = _size_buckets(reinit, plan)
-                    name, fn = named((plan.key('track_mixed'), tuple(blocks))), self._mixed_fn(st, b, blocks, draw)
+                    name, fn = named(rows((plan.key('track_mixed'), tuple(blocks)))), self._mixed_fn(st, b, blocks, draw, S)
                 else:
-                    name, fn = named(f'track_mixed{b}'), self._mixed_fn(st, b, draw=draw)
-                name, fn, fin = fr.bind(est.detector, name, fn, imgs, plan)
-                cams = est.detector._to_dev(glue.cameras(Ks))
-                prev = self._prev if self._prev is not None else torch.zeros(S, 12, dtype=torch.float64, device=dev)
-                outs = self.stages.run(name, fn, fin + [cams, prev, self._ring, self._count] + extra + dt)
-            buf, poses_dev, ring, count = outs
+                    name, fn = named(rows(f'track_mixed{b}')), self._mixed_fn(st, b, draw=draw, S=S)
+                name, fn, fin = fr.bind(est.detector, name, wrap(fn), imgs, plan)
+            if part is not None:
+                state = [self._prev, self._ring, self._count] + part.graph_inputs(dev)
+            else:
+                state = [self._ring, self._count] if full else [self._prev, self._ring, self._count]
+            cams = est.detector._to_dev(glue.cameras(Ks))
+            buf, poses_dev, ring, count = self.stages.run(name, fn, fin + [cams] + state + extra + dt)
             self._prev = poses_dev.clone()
             self._ring.copy_(ring)
             self._count.copy_(count)
             host = est.detector._to_host(buf)                        # the step's one synchronising read
-        prev_f32 = bool(self._f32[0])
-        self._f32[:] = True
-        res = self._decode_mixed(host, reinit, b, pick) if kind == 'mixed' else self._decode(host, full, prev_f32)
+        prev_f32 = bool(f32[0])
+        if part is None:
+            self._f32[:] = True
+        else:
+            self._f32[part.seq] = True
+        res = self._decode_mixed(host, reinit, b, pick, S) if kind == 'mixed' else self._decode(host, full, prev_f32, S)
         if drawn is not None:
             res[2]['drawn'] = drawn
         return res
 
-    def _decode(self, host, full, prev_f32):
-        est, S, num = self.est, self.S, self.num
+    def _decode(self, host, full, prev_f32, S=None):
+        est, S, num = self.est, S or self.S, self.num
         n_chain = (est.cfg['refine_iter'] if full else self.refine_iter) + 1
         sizes = [('chain', n_chain * S * 12), ('smoothed', S * 12), ('avg', S * 16), ('ring', S * num * 16), ('count', S)]
         if full:
@@ -588,9 +745,10 @@ class Tracker:
         inter['smoothed_pts'] = vals['avg'].reshape(S, 8, 2).copy()
         return (refined[-1] if refined else first), vals['smoothed'].reshape(S, 3, 4).copy(), inter
 
-    def _decode_mixed(self, host, reinit, b, pick=None):
-        """pick: the gathered row of each re-initialised sequence (per-size buckets); None: the first m rows."""
-        est, S, num, m = self.est, self.S, self.num, len(reinit)
+    def _decode_mixed(self, host, reinit, b, pick=None, S=None):
+        """pick: the gathered row of each re-initialised sequence (per-size buckets); None: the first m rows.  S: the
+        step's sequences (a partial step's compact batch); default all."""
+        est, S, num, m = self.est, S or self.S, self.num, len(reinit)
         pick = slice(0, m) if pick is None else pick
         n_chain = max(est.cfg['refine_iter'], self.refine_iter) + 1
         res = est.cfg['ref_resolution']
@@ -764,7 +922,7 @@ class ObjectTracker:
             return packed.view(torch.uint8), poses, ring, count
         return fn
 
-    def _mixed_fn(self, b, blocks=None, draw=None):
+    def _mixed_fn(self, b, blocks=None, draw=None, S=None):
         objs, c, K = list(self.objs._objects.values()), self._dev, self.K
         initial = self.objs._initial_poses_device_fn()
 
@@ -776,61 +934,96 @@ class ObjectTracker:
             return poses, crop, extras
 
         smooth = lambda poses, Ks, ring, count: ops.track_smooth_objects(poses, True, c['bboxes'], Ks, ring, count, c['weights'])
-        return _mixed_fn(K, self.S, b, self.est.cfg['refine_iter'], self.refine_iter, init, [ob.tables['views'] for ob in objs],
+        return _mixed_fn(K, S or self.S, b, self.est.cfg['refine_iter'], self.refine_iter, init, [ob.tables['views'] for ob in objs],
                          objs[0].tables['tables']['ref_num'], self.est.refiner._refine_warped(128), smooth, blocks, draw)
 
-    def step(self, frames, Ks, out=None):
+    _partial = Tracker._partial
+
+    def step(self, frames, Ks, out=None, sequences=None):
         """frames: S uint8 [h,w,3] (of one size or several, row f13; or device frames, row f14, as Tracker.step takes them);
         Ks: [S,3,3] (shared by all objects); out: drawing destinations as Tracker.step takes them, every object's box
         drawn on its sequence's frame in object order (each step's result then also holds inter['drawn'] without out=).  Returns {name: (raw poses float32
         [S,3,4], smoothed poses float64 [S,3,4], inter)}: inter has Tracker.step's keys, and a full-prediction step adds
         those of ObjectSet.predict (det_score included); a mixed step adds 'reinit' and those entries for the
-        re-initialised sequences, as Tracker.step does."""
+        re-initialised sequences, as Tracker.step does.  sequences: step only these sequences, every object on each, as
+        Tracker.step does (row f17); every object's results then hold one row per listed sequence in that order."""
         self._check()
-        K, S, num, est = self.K, self.S, self.num, self.est
+        part = None
+        if sequences is not None:
+            part = self._partial(frames, Ks, out, sequences)
+            frames, Ks, out = part.compact(frames), part.compact(Ks), part.compact_out(out)
+            if part.lockstep:
+                return {name: part.results(*r) for name, r in self.step(frames, Ks, out).items()}
+        K, S, est = self.K, self.S if part is None else part.b, self.est
         if len(frames) != S or len(Ks) != S:
             raise ValueError(f'step: this tracker follows {S} sequences, got {len(frames)} frames and {len(Ks)} Ks')
         Ks = np.stack([np.asarray(k) for k in Ks], 0)
         if Ks.shape != (S, 3, 3):
             raise ValueError(f'step: Ks must be [{S},3,3], got {Ks.shape}')
-        kind = self._kind()
-        full, mixed = kind == 'full', kind == 'mixed'
+        kind = self._kind() if part is None else part.kind
         imgs = fr.as_frames(frames, 'step', est.detector)
-        plan, pick = fr.FramePlan(fr.size_pattern(imgs)), None
+        plan = fr.FramePlan(fr.size_pattern(imgs))
         if plan.mixed:
             fr.check_frames(imgs, Ks, 'step')
-        draw, dt, drawn, named = draw_inputs(self._drawer, est.detector, plan, out)
+        res = self._step_device(imgs, Ks, kind, plan, out, part)
+        if part is None:
+            self._pending[:] = False
+            return res
+        self._pending[part.seq] = False
+        return {name: part.results(*r) for name, r in res.items()}
+
+    def _step_device(self, imgs, Ks, kind, plan, out=None, part=None):
+        """One step's graph; part: a partial step (row f17), as in Tracker._step_device."""
+        K, est = self.K, self.est
+        S, pending, f32 = (self.S, self._pending, self._f32) if part is None else (part.b, part.pending, part.f32)
+        rows = (lambda n: n) if part is None else part.name
+        drawer = self._drawer if part is None or self._drawer is None else self._drawer.for_sequences(part.b)
+        full, mixed = kind == 'full', kind == 'mixed'
+        pick = None
+        draw, dt, drawn, named = draw_inputs(drawer, est.detector, plan, out, None if part is None else part.a)
+        dev = est.detector.device
+        if self._prev is None and (part is not None or mixed):
+            self._prev = torch.zeros(K * self.S, 12, dtype=torch.float64, device=dev)
+        wrap, extra = (lambda fn: fn), []
+        if part is not None:
+            wrap = lambda fn: _compact_fn(fn, full)
         with torch.no_grad():
             if full:
-                name, fn, fin = fr.stage(est.detector, named('track_full'), self._full_fn(draw), imgs, plan)
-                cams = est.detector._to_dev(glue.cameras(Ks))
-                outs = self.stages.run(name, fn, fin + [cams, self._ring, self._count] + dt)
+                name, fn, fin = fr.stage(est.detector, named(rows('track_full')), wrap(self._full_fn(draw)), imgs, plan)
             elif not mixed:
-                prev_f32 = bool(self._f32[0])
-                name, fn, fin = fr.stage(est.detector, named(f'track_refine{int(prev_f32)}'), self._refine_fn(prev_f32, draw), imgs,
-                                         plan)
-                cams = est.detector._to_dev(glue.cameras(Ks))
-                outs = self.stages.run(name, fn, fin + [cams, self._prev, self._ring, self._count] + dt)
+                prev_f32 = bool(f32[0])
+                name, fn, fin = fr.stage(est.detector, named(rows(f'track_refine{int(prev_f32)}')),
+                                         wrap(self._refine_fn(prev_f32, draw)), imgs, plan)
             else:
-                dev = est.detector.device
-                reinit, b, extra = _mixed_inputs(S, K, self._pending, self._f32, est.cfg['refine_iter'], self.refine_iter, dev, plan)
+                reinit, b, extra = _mixed_inputs(S, K, pending, f32, est.cfg['refine_iter'], self.refine_iter, dev, plan)
                 if plan.mixed:                   # one graph per size pattern and per-size buckets (row f13)
                     _, blocks, pick = _size_buckets(reinit, plan)
-                    name, fn = named((plan.key('track_mixed'), tuple(blocks))), self._mixed_fn(b, blocks, draw)
+                    name, fn = named(rows((plan.key('track_mixed'), tuple(blocks)))), self._mixed_fn(b, blocks, draw, S)
                 else:
-                    name, fn = named(f'track_mixed{b}'), self._mixed_fn(b, draw=draw)
-                name, fn, fin = fr.bind(est.detector, name, fn, imgs, plan)
-                cams = est.detector._to_dev(glue.cameras(Ks))
-                prev = self._prev if self._prev is not None else torch.zeros(K * S, 12, dtype=torch.float64, device=dev)
-                outs = self.stages.run(name, fn, fin + [cams, prev, self._ring, self._count] + extra + dt)
-            buf, poses_dev, ring, count = outs
-            prev_f32 = bool(self._f32[0])
+                    name, fn = named(rows(f'track_mixed{b}')), self._mixed_fn(b, draw=draw, S=S)
+                name, fn, fin = fr.bind(est.detector, name, wrap(fn), imgs, plan)
+            if part is not None:
+                state = [self._prev, self._ring, self._count] + part.graph_inputs(dev)
+            else:
+                state = [self._ring, self._count] if full else [self._prev, self._ring, self._count]
+            cams = est.detector._to_dev(glue.cameras(Ks))
+            buf, poses_dev, ring, count = self.stages.run(name, fn, fin + [cams] + state + extra + dt)
+            prev_f32 = bool(f32[0])
             self._prev = poses_dev.clone()
             self._ring.copy_(ring)
             self._count.copy_(count)
             host = est.detector._to_host(buf)                        # the step's one synchronising read
-        self._pending[:] = False
-        self._f32[:] = True
+        if part is None:
+            self._f32[:] = True
+        else:
+            self._f32[part.seq] = True
+        if not mixed:
+            reinit, b = None, None
+        return self._decode(host, kind, S, reinit, b, pick, prev_f32, drawn)
+
+    def _decode(self, host, kind, S, reinit, b, pick, prev_f32, drawn):
+        K, num, est = self.K, self.num, self.est
+        full, mixed = kind == 'full', kind == 'mixed'
         n = K * S
         if mixed:
             n_chain, qn, m = max(est.cfg['refine_iter'], self.refine_iter) + 1, b, len(reinit)
