@@ -6,6 +6,10 @@
 // pin it against a numpy restatement.  The translation unit is compiled with -fmad=false: products and sums round
 // separately.
 //
+// A step in which only some sequences re-detect (g6d_instances_associate_sequences) gives each sequence its row j in a
+// detection batch of D rows per slot group (det_index[s], -1: the sequence does not detect): the detecting pairs run the
+// association on detection rows g*D + j, the others only set up their refinement, as a refine-only step does.
+//
 // Layout: K objects with M instance slots each over S sequences; slot group g = m*K + o is instance slot m of object o,
 // and row g*S + s is that slot on sequence s.  A single object (g6d_instances_associate) is K = 1, where g = m and every
 // row index, work row and id is the one of the single-object layout.
@@ -42,7 +46,20 @@ struct Args {
     int* det_slot;                 // [M*K*S] out
     int* spawned;                  // [M*K*S] out
     long long* dropped;            // [M*K*S] out
+    const int* det_index;          // [S] each sequence's detection row j < D, -1: no detection; null: every s detects at s, D = S
+    int D;                         // detection rows per slot group (det, valid, init are [M*K*D,...], row g*D + j)
 };
+
+G6D_HD int det_rows(const Args& a) { return a.det_index ? a.D : a.S; }
+
+// The entry of lists for slot t (slot group g = t*K + o) at iteration it: iterations it < r list every row of the
+// M*K*S (entry (it*M*K + g)*S + s); iterations r <= it < F follow with the M*K*D rows of the detecting sequences only
+// (entry r*M*K*S + ((it - r)*M*K + g)*D + j).  With det_index null (D = S, j = s) both are (it*M*K + g)*S + s.
+G6D_HD long long list_entry(const Args& a, int it, int g, int s, int j) {
+    const long long G = (long long)a.M * a.K;
+    if (it < a.r) return ((long long)it * G + g) * a.S + s;
+    return (long long)a.r * G * a.S + ((long long)(it - a.r) * G + g) * det_rows(a) + j;
+}
 
 // The object centre projected with a track's previous pose and the frame's K, in fp64 and in this order:
 //   p_i = ((P[i,0]*cx + P[i,1]*cy) + P[i,2]*cz) + P[i,3],  q_j = (K[j,0]*p_0 + K[j,1]*p_1) + K[j,2]*p_2,  u = q_0/q_2, v = q_1/q_2.
@@ -70,9 +87,14 @@ G6D_HD void copy12(double* dst, const double* src) {
 // Everything of sequence s and object o except the new tracks' ids; returns the number of tracks it spawns.  The pair's
 // slot t is row base + t*stride (base = o*S + s, stride = K*S: slot group g = t*K + o) and matches only its object's
 // detection rows, with its object's centre.
+G6D_HD int setup_refinement(int s, int o, const Args& a);
+
 G6D_HD int associate_sequence(int s, int o, const Args& a) {
     const int S = a.S, M = a.M;
+    const int jd = a.det_index ? a.det_index[s] : s;                   // the sequence's row in the detection batch
+    if (jd < 0) return setup_refinement(s, o, a);
     const long long base = (long long)o * S + s, stride = (long long)a.K * S;
+    const long long dbase = (long long)o * det_rows(a) + jd, dstride = (long long)a.K * det_rows(a);
     const double* K = a.cams + (long long)s * 20;
     const double* c = a.centers ? a.centers + (long long)o * 3 : a.center1;
     const double cx = c[0], cy = c[1], cz = c[2];
@@ -92,7 +114,7 @@ G6D_HD int associate_sequence(int s, int o, const Args& a) {
         for (int t = 0; t < M; ++t) {
             if (!ok[t] || match[t] >= 0) continue;
             for (int d = 0; d < M; ++d) {
-                const long long j = base + d * stride;
+                const long long j = dbase + d * dstride;
                 if (!a.valid[j] || det_of[d] >= 0) continue;
                 const double cost = pair_cost(u[t], v[t], a.det + j * 4, a.ref_resolution);
                 if (cost < a.gate && (bt < 0 || cost < bc)) { bt = t; bd = d; bc = cost; }
@@ -124,13 +146,13 @@ G6D_HD int associate_sequence(int s, int o, const Args& a) {
     // unmatched valid detections, in peak order, take the lowest empty slots
     int n_new = 0, t_free = 0;
     for (int d = 0; d < M; ++d) {
-        const long long j = base + d * stride;
-        if (!a.valid[j]) { a.det_slot[j] = -1; continue; }
-        if (det_of[d] >= 0) { a.det_slot[j] = det_of[d]; continue; }
+        const long long j = dbase + d * dstride, q = base + d * stride;     // detection d's batch row and its det_slot row
+        if (!a.valid[j]) { a.det_slot[q] = -1; continue; }
+        if (det_of[d] >= 0) { a.det_slot[q] = det_of[d]; continue; }
         while (t_free < M && a.live[base + t_free * stride]) ++t_free;
-        if (t_free == M) { a.det_slot[j] = -1; continue; }
+        if (t_free == M) { a.det_slot[q] = -1; continue; }
         const long long i = base + t_free * stride;
-        a.det_slot[j] = t_free;
+        a.det_slot[q] = t_free;
         a.live[i] = 1;
         a.misses[i] = 0;
         is_new[t_free] = true;
@@ -145,7 +167,7 @@ G6D_HD int associate_sequence(int s, int o, const Args& a) {
         const long long i = base + t * stride, real = real_row(t);
         a.spawned[i] = is_new[t];
         if (!a.live[i]) {
-            copy12(a.park + i * 12, a.init + i * 12);
+            copy12(a.park + i * 12, a.init + (dbase + t * dstride) * 12);
             a.ids[i] = -1;
         }
         double* w = a.work + real * 12;
@@ -158,8 +180,46 @@ G6D_HD int associate_sequence(int s, int o, const Args& a) {
     const int n_it = a.F > a.r ? a.F : a.r;
     for (int it = 0; it < n_it; ++it)
         for (int t = 0; t < M; ++t)
-            a.lists[(long long)it * M * stride + base + t * stride] = (int)real_row(t) + (it < chain[t] ? 0 : S);
+            a.lists[list_entry(a, it, t * a.K + o, s, jd)] = (int)real_row(t) + (it < chain[t] ? 0 : S);
     return n_new;
+}
+
+// A pair that does not detect this step: the set-up of a refine-only step (work row = live ? prev : park and its scratch
+// copy, flags0 = live, chain r, listed in iterations it < r), spawned 0, dropped and det_slot -1; the slot state is not
+// touched.
+G6D_HD int setup_refinement(int s, int o, const Args& a) {
+    const int S = a.S;
+    const long long base = (long long)o * S + s, stride = (long long)a.K * S;
+    for (int t = 0; t < a.M; ++t) {
+        const long long i = base + t * stride, real = (long long)(t * a.K + o) * 2 * S + s;
+        double* w = a.work + real * 12;
+        copy12(w, a.live[i] ? a.prev + i * 12 : a.park + i * 12);
+        copy12(w + (long long)S * 12, w);
+        a.flags0[real] = a.flags0[real + S] = (uint8_t)a.live[i];
+        a.spawned[i] = 0;
+        a.dropped[i] = -1;
+        a.det_slot[i] = -1;
+        for (int it = 0; it < a.r; ++it) a.lists[list_entry(a, it, t * a.K + o, s, -1)] = (int)real;
+    }
+    return 0;
+}
+
+// Detection row j < D that no sequence uses (padding of the detection batch): in iterations r <= it < F its M*K list
+// entries point at the scratch rows of the rank-th non-detecting sequence, rank = j's rank among the unused rows.  Those
+// rows are free (a non-detecting chain ends at r) and there are enough of them (D - #detecting <= S - #detecting), so a
+// padding entry never refines a real row nor shares a row with another entry.
+G6D_HD void pad_lists(int j, const Args& a) {
+    int below = 0;
+    for (int s = 0; s < a.S; ++s) {
+        if (a.det_index[s] == j) return;
+        below += a.det_index[s] >= 0 && a.det_index[s] < j;
+    }
+    int rank = j - below, s = 0;
+    for (; s < a.S; ++s)
+        if (a.det_index[s] < 0 && rank-- == 0) break;
+    const int n_it = a.F > a.r ? a.F : a.r;
+    for (int it = a.r; it < n_it; ++it)
+        for (int g = 0; g < a.M * a.K; ++g) a.lists[list_entry(a, it, g, s, j)] = g * 2 * a.S + a.S + s;
 }
 
 }  // namespace assoc

@@ -36,7 +36,9 @@ __global__ void __launch_bounds__(32) track_smooth_objects_kernel(const double* 
 // (sequence, object) pair, pairs object-major (pair p = o*S + s); phase 2 numbers the spawned tracks in ascending
 // (object, sequence, slot) order -- which is (object, sequence, detection) order, since a pair's unmatched detections take
 // its empty slots in ascending order -- by an exclusive block scan of the pairs' spawn counts, chunk by chunk; thread 0
-// then advances the counter.  Pair p's slot t is row p + t*K*S.
+// then advances the counter.  Pair p's slot t is row p + t*K*S.  With a det_index (a step in which only some sequences
+// detect) non-detecting pairs spawn nothing, and the threads also fill the list entries of the detection batch's padding
+// rows.
 constexpr int kAssocThreads = 256;
 
 __global__ void __launch_bounds__(kAssocThreads) instances_associate_kernel(assoc::Args a, long long* next_id) {
@@ -46,6 +48,8 @@ __global__ void __launch_bounds__(kAssocThreads) instances_associate_kernel(asso
     const int P = a.K * a.S;
     const long long stride = (long long)a.K * a.S;
     for (int p = tid; p < P; p += kAssocThreads) assoc::associate_sequence(p % a.S, p / a.S, a);
+    if (a.det_index)
+        for (int j = tid; j < a.D; j += kAssocThreads) assoc::pad_lists(j, a);
     if (tid == 0) s_base = *next_id;
     __syncthreads();
     for (int p0 = 0; p0 < P; p0 += kAssocThreads) {
@@ -87,7 +91,9 @@ static int associate_ok(const char* name, const assoc::Args& a, const long long*
                 "%s: need F, r >= 0 with max(F, r) >= 1, num >= 1 and max_misses >= 0 (got F=%d, r=%d, num=%d, max_misses=%d)", name,
                 a.F, a.r, a.num, a.max_misses);
     G6D_REQUIRE(a.gate > 0. && a.gate < INFINITY && a.ref_resolution > 0., "%s: need a finite gate > 0 and ref_resolution > 0", name);
-    G6D_REQUIRE(a.det && a.valid && a.init && a.cams && a.prev && a.live && a.ids && a.misses && a.park && a.ring && a.count && a.work &&
+    const bool detects = !a.det_index || a.D > 0;
+    G6D_REQUIRE(!a.det_index || (a.D >= 0 && a.D <= a.S), "%s: need 0 <= D <= S (got D=%d, S=%d)", name, a.D, a.S);
+    G6D_REQUIRE(((a.det && a.valid && a.init) || !detects) && a.cams && a.prev && a.live && a.ids && a.misses && a.park && a.ring && a.count && a.work &&
                 a.flags0 && a.lists && a.det_slot && a.spawned && a.dropped && next_id, "%s: null pointer", name);
     return G6D_OK;
 }
@@ -95,6 +101,8 @@ static int associate_ok(const char* name, const assoc::Args& a, const long long*
 static void associate_host(const assoc::Args& a, long long* next_id) {
     const long long stride = (long long)a.K * a.S;
     for (int p = 0; p < a.K * a.S; ++p) assoc::associate_sequence(p % a.S, p / a.S, a);
+    if (a.det_index)
+        for (int j = 0; j < a.D; ++j) assoc::pad_lists(j, a);
     for (int p = 0; p < a.K * a.S; ++p)
         for (int m = 0; m < a.M; ++m)
             if (a.spawned[p + m * stride]) a.ids[p + m * stride] = (*next_id)++;
@@ -157,6 +165,51 @@ extern "C" int g6d_instances_associate_objects_host(int S, int K, int M, int F, 
     const assoc::Args a{S, K, M, F, r, num, max_misses, det, valid, init, reinterpret_cast<const double*>(cams), centers, {0., 0., 0.},
                         ref_resolution, gate, prev, live, ids, misses, park, ring, count, work, flags0, lists, det_slot, spawned, dropped};
     const int rc = associate_ok("g6d_instances_associate_objects_host", a, next_id);
+    if (rc != G6D_OK) return rc;
+    associate_host(a, next_id);
+    return G6D_OK;
+}
+
+// det_index [S] on the host: every entry -1 or a row j < D, no row twice.
+static int det_index_ok(const char* name, const int* det_index, int S, int D) {
+    G6D_REQUIRE(det_index, "%s: null pointer (det_index)", name);
+    G6D_REQUIRE(D >= 0 && D <= S, "%s: need 0 <= D <= S (got D=%d, S=%d)", name, D, S);
+    for (int s = 0; s < S; ++s) {
+        G6D_REQUIRE(det_index[s] >= -1 && det_index[s] < D, "%s: det_index[%d] = %d is outside [-1, %d)", name, s, det_index[s], D);
+        for (int q = 0; q < s; ++q)
+            G6D_REQUIRE(det_index[s] < 0 || det_index[q] != det_index[s], "%s: det_index[%d] and det_index[%d] are both %d", name, q, s,
+                        det_index[s]);
+    }
+    return G6D_OK;
+}
+
+extern "C" int g6d_instances_associate_sequences(int S, int K, int M, int F, int r, int D, const int* det_index, const float* det,
+                                                 const int* valid, const double* init, const g6d_glue_camera* cams, const double* centers,
+                                                 double ref_resolution, double gate, int max_misses, const double* prev, int* live,
+                                                 long long* ids, int* misses, long long* next_id, double* park, float* ring, int* count,
+                                                 int num, double* work, uint8_t* flags0, int* lists, int* det_slot, int* spawned,
+                                                 long long* dropped, g6d_stream_t stream) {
+    G6D_REQUIRE(centers && det_index, "g6d_instances_associate_sequences: null pointer (centers, det_index)");
+    const assoc::Args a{S, K, M, F, r, num, max_misses, det, valid, init, reinterpret_cast<const double*>(cams), centers, {0., 0., 0.},
+                        ref_resolution, gate, prev, live, ids, misses, park, ring, count, work, flags0, lists, det_slot, spawned, dropped,
+                        det_index, D};
+    return associate_launch("g6d_instances_associate_sequences", a, next_id, stream);
+}
+
+extern "C" int g6d_instances_associate_sequences_host(int S, int K, int M, int F, int r, int D, const int* det_index, const float* det,
+                                                      const int* valid, const double* init, const g6d_glue_camera* cams,
+                                                      const double* centers, double ref_resolution, double gate, int max_misses,
+                                                      const double* prev, int* live, long long* ids, int* misses, long long* next_id,
+                                                      double* park, float* ring, int* count, int num, double* work, uint8_t* flags0,
+                                                      int* lists, int* det_slot, int* spawned, long long* dropped) {
+    const char* name = "g6d_instances_associate_sequences_host";
+    G6D_REQUIRE(centers, "%s: null pointer (centers)", name);
+    int rc = det_index_ok(name, det_index, S, D);
+    if (rc != G6D_OK) return rc;
+    const assoc::Args a{S, K, M, F, r, num, max_misses, det, valid, init, reinterpret_cast<const double*>(cams), centers, {0., 0., 0.},
+                        ref_resolution, gate, prev, live, ids, misses, park, ring, count, work, flags0, lists, det_slot, spawned, dropped,
+                        det_index, D};
+    rc = associate_ok(name, a, next_id);
     if (rc != G6D_OK) return rc;
     associate_host(a, next_id);
     return G6D_OK;

@@ -368,7 +368,7 @@ class Gen6DEstimator:
 
     def instance_tracker(self, num_sequences=1, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
                          min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bbox_3d=None, draw=None,
-                         draw_color=(0, 0, 255)):
+                         draw_color=(0, 0, 255), schedule='lockstep'):
         """An InstanceTracker (gen6d_b200/instance_track.py): every instance of the object, up to `max_instances` per frame,
         followed through `num_sequences` videos in lockstep.  The first step (and the one after reset() / redetect(), and
         every `redetect_every`-th step after the last re-detection) detects predict_instances' instances (min_score,
@@ -376,12 +376,15 @@ class Gen6DEstimator:
         |projected object centre - detected position| / (ref_resolution * detected scale) below `gate`; a track unmatched
         more than `max_misses` re-detections in a row is dropped, and unmatched detections start new tracks.  Every other
         step refines each track `refine_iter` times from its previous pose.  Both smooth as tracker() does.  draw /
-        draw_color: as for tracker(); every live slot (track id >= 0) is drawn, in slot order."""
+        draw_color: as for tracker(); every live slot (track id >= 0) is drawn, in slot order.
+        schedule (row f18): 'lockstep' (every sequence re-detects on the same steps), 'per_sequence' (each sequence has its
+        own re-detection flag and counter; reset / redetect take sequences, and step takes sequences= to step any subset)
+        or 'staggered' ('per_sequence' with the periodic re-detections spread over the steps; needs redetect_every)."""
         from .instance_track import InstanceTracker
         return InstanceTracker(self, num_sequences, max_instances=max_instances, refine_iter=refine_iter,
                                redetect_every=redetect_every, gate=gate, max_misses=max_misses, min_score=min_score, nms_iou=nms_iou,
                                peak_radius=peak_radius, smooth_num=smooth_num, smooth_std=smooth_std, bbox_3d=bbox_3d,
-                               draw=draw, draw_color=draw_color)
+                               draw=draw, draw_color=draw_color, schedule=schedule)
 
     def track(self, que_imgs, que_K, **tracker_kwargs):
         """predict.py's loop over one video: que_imgs uint8 [h,w,3] frames of one size, que_K [3,3] (or one per frame).

@@ -24,6 +24,19 @@ g = m*K + o is instance slot m of object o (row g*S + s, the layout of ObjectSet
 re-detection step runs the set's shared pyramid and correlation and g6d_instances_associate_objects (each object's
 tracks matched against its own peaks, one id counter), and every refinement iteration is still ONE refiner stage over
 all M*K*S poses.  Both trackers are the class below, parameterised by the per-group tables and the detection.
+
+Re-detection schedules (row f18, schedule=): 'lockstep' re-detects every sequence on the same steps.  'per_sequence'
+gives every sequence its own pending flag and re-detection counter (host-side, so planning a step reads nothing from the
+device): reset(sequences) / redetect(sequences) mark only those sequences, and step(..., sequences=[...]) steps any
+subset as Tracker.step does (row f17).  'staggered' is 'per_sequence' whose periodic re-detections are spread over the
+steps: a detection leaves a sequence's counter at 1 (the lockstep count), except one it was marked for (its first, or
+after reset / redetect), which leaves it at 1 + floor(s*E/S); sequence s then re-detects every E steps from E - floor(s*E/S)
+steps on, so in lockstep stepping at most ceil(S/E) sequences re-detect on any later step (Schedule).  Each step is still one
+graph and one read: with b the stepped batch (all S, or the listed sequences padded to f17's bucket) and d the bucket of
+its re-detecting sequences, d = 0 replays the refine body, d = b the re-detection body, and anything between the mixed
+instance step (_mixed_fn): the re-detecting sequences' frames are gathered and detected as a batch of d,
+g6d_instances_associate_sequences associates them and sets up every other pair's refinement, and the iterations past
+refine_iter run one refiner stage over the re-detecting sequences' slots only.
 """
 import numpy as np
 import torch
@@ -35,7 +48,67 @@ from . import glue
 from . import instances
 from . import ops
 from .graphs import StageCache
-from .track import _sequences, check_bbox, draw_inputs, object_bbox, object_bboxes, smoothing_weights
+from .track import (PartialStep, _bucket, _gather_rows, _scatter_rows, _sequences, _size_buckets, check_bbox, draw_inputs,
+                    object_bbox, object_bboxes, smoothing_weights)
+
+
+def staggered_phases(S, E):
+    """Each sequence's phase under schedule='staggered': floor(s*E/S) for sequence s."""
+    return (np.arange(S) * int(E)) // int(S)
+
+
+class Schedule:
+    """The host plan of a per-sequence schedule (row f18): per sequence a pending flag (marked by the first step, reset and
+    redetect) and `count`, the steps since its last detection counting the step of that detection as 1, as the lockstep
+    tracker counts.  A sequence re-detects when pending or when count >= E (redetect_every).  After a detection it was
+    marked for, its count restarts at 1 + phase (phase 0 under 'per_sequence', floor(s*E/S) under 'staggered', so a
+    sequence of phase p re-detects periodically E - p steps later); after a periodic one, at 1."""
+
+    def __init__(self, S, E, staggered):
+        self.S, self.E = S, E
+        self.pending, self.count = np.ones(S, bool), np.zeros(S, np.int64)
+        self.phase = staggered_phases(S, E) if staggered else np.zeros(S, np.int64)
+
+    def due(self):
+        """bool [S]: the sequences that re-detect on their next step."""
+        return self.pending | ((self.count >= self.E) if self.E is not None else False)
+
+    def plan(self, seqs, n_real):
+        """The stepped batch seqs [b] (its first n_real rows real, the rest padding) -> (det_seq bool [b], kind): the rows
+        that re-detect (padding never does, so it spawns no ids) and the body the step runs ('refine': none, 'detect':
+        every row, else 'mixed')."""
+        det_seq = self.due()[seqs]
+        det_seq[n_real:] = False
+        m = int(det_seq.sum())
+        return det_seq, 'refine' if m == 0 else 'detect' if m == len(seqs) else 'mixed'
+
+    def advance(self, stepped):
+        """The counters after a step of the distinct sequences `stepped`."""
+        hit, restart = self.due()[stepped], self.pending[stepped]
+        self.count[stepped] = np.where(hit, np.where(restart, 1 + self.phase[stepped], 1), self.count[stepped] + 1)
+        self.pending[stepped] = False
+
+
+def plan_mixed(det_seq, plan):
+    """A mixed step's detection batch -> (gathered sequences [d], per-size blocks or None, det_index [b] (each sequence's
+    row in the batch, -1: none), d, the graph key of the batch).  One size: the re-detecting sequences ascending, padded to
+    d = _bucket(m, b) by repeating the last; several sizes (plan.mixed): _size_buckets' per-size blocks."""
+    S, det = len(det_seq), np.flatnonzero(det_seq)
+    if plan is not None and plan.mixed:
+        seq, blocks, pick = _size_buckets(det, plan)
+        d, key = len(seq), tuple(blocks)
+    else:
+        d = _bucket(len(det), S)
+        seq, blocks, pick, key = np.concatenate([det, np.full(d - len(det), det[-1])]), None, np.arange(len(det)), d
+    det_index = np.full(S, -1, np.int64)
+    det_index[det] = pick
+    check_det_index(det_index, S, d)
+    return seq, blocks, det_index, d, key
+
+
+def mixed_name(b, key):
+    """The graph name of the mixed instance step over b sequences with detection batch `key` (d, or per-size blocks)."""
+    return ('instance_mixed', b, key)
 
 
 def host_associate(det, valid, init, cams, center, ref_resolution, gate, max_misses, F, r, prev, live, ids, misses, next_id,
@@ -90,10 +163,65 @@ def host_associate_objects(det, valid, init, cams, centers, ref_resolution, gate
     return work, flags0, lists, det_slot, spawned, dropped
 
 
+def check_det_index(det_index, S, D):
+    """ValueError unless det_index [S] holds -1 (the sequence does not detect) or distinct rows j < D, with 0 <= D <= S."""
+    det_index = np.asarray(det_index).reshape(-1)
+    if len(det_index) != S or not 0 <= int(D) <= S:
+        raise ValueError(f'det_index: need {S} entries and 0 <= D <= {S}, got {len(det_index)} entries and D = {D}')
+    bad = det_index[(det_index < -1) | (det_index >= D)]
+    if len(bad):
+        raise ValueError(f'det_index: entries {bad.tolist()} are outside [-1, {D})')
+    rows = det_index[det_index >= 0]
+    if len(np.unique(rows)) != len(rows):
+        raise ValueError(f'det_index: {det_index.tolist()} lists a detection row twice')
+
+
+def list_length(G, S, D, F, r):
+    """Entries of the row lists of g6d_instances_associate_sequences for G slot groups: r iterations over every row, then
+    max(F - r, 0) over the detecting sequences' D rows per group."""
+    return r * G * S + max(F - r, 0) * G * D
+
+
+def host_associate_sequences(det_index, det, valid, init, cams, centers, ref_resolution, gate, max_misses, F, r, prev, live, ids,
+                             misses, next_id, park, ring, count):
+    """g6d_instances_associate_sequences_host on numpy arrays: det_index int [S] (-1: the sequence does not detect, else its
+    row j < D in the detection batch; D = len(det) // (M*K)), det [M*K*D,4], valid [M*K*D], init [M*K*D,12], the rest as
+    host_associate_objects.  live, ids, misses, next_id, park, ring and count are updated in place.  Returns (work, flags0,
+    lists, det_slot, spawned, dropped) as numpy arrays."""
+    c = lambda a, dt: np.ascontiguousarray(a, dt)
+    centers = c(centers, np.float64).reshape(-1, 3)
+    n, S, K = len(live), len(cams), len(centers)
+    G, num = n // max(K * S, 1) * K, ring.shape[1]
+    D = len(det) // max(G, 1)
+    for a, dt in ((live, np.int32), (ids, np.int64), (misses, np.int32), (next_id, np.int64), (park, np.float64),
+                  (ring, np.float32), (count, np.int32)):
+        if a.dtype != dt or not a.flags.c_contiguous:
+            raise ValueError(f'host_associate_sequences: the state arrays must be contiguous {dt.__name__} arrays (updated in place)')
+    det_index, det, valid, init = c(det_index, np.int32), c(det, np.float32), c(valid, np.int32), c(init, np.float64)
+    cams, prev = c(cams, np.float64), c(prev, np.float64)
+    work, flags0 = np.zeros((2 * n, 12)), np.zeros(2 * n, np.uint8)
+    lists = np.zeros(list_length(G, S, D, int(F), int(r)), np.int32)
+    det_slot, spawned, dropped = np.zeros(n, np.int32), np.zeros(n, np.int32), np.zeros(n, np.int64)
+    _lib.check(_lib.lib().g6d_instances_associate_sequences_host(
+        S, K, n // max(K * S, 1), int(F), int(r), D, det_index.ctypes.data, det.ctypes.data, valid.ctypes.data, init.ctypes.data,
+        cams.ctypes.data, centers.ctypes.data, float(ref_resolution), float(gate), int(max_misses), prev.ctypes.data,
+        live.ctypes.data, ids.ctypes.data, misses.ctypes.data, next_id.ctypes.data, park.ctypes.data, ring.ctypes.data,
+        count.ctypes.data, num, work.ctypes.data, flags0.ctypes.data, lists.ctypes.data, det_slot.ctypes.data,
+        spawned.ctypes.data, dropped.ctypes.data), 'g6d_instances_associate_sequences_host')
+    return work, flags0, lists, det_slot, spawned, dropped
+
+
+SCHEDULES = ('lockstep', 'per_sequence', 'staggered')
+
+
 def check_args(num_sequences, max_instances, refine_iter, redetect_every, gate, max_misses, min_score, nms_iou, peak_radius,
-               smooth_num, smooth_std):
+               smooth_num, smooth_std, schedule='lockstep'):
     """-> the detection key of instances.check_args; ValueError for a bad argument."""
     key = instances.check_args(max_instances, nms_iou, peak_radius, min_score)
+    if schedule not in SCHEDULES:
+        raise ValueError(f'schedule={schedule!r}: need one of {SCHEDULES}')
+    if schedule == 'staggered' and redetect_every is None:
+        raise ValueError("schedule='staggered' spreads the periodic re-detections: it needs redetect_every")
     if int(num_sequences) < 1:
         raise ValueError(f'num_sequences must be >= 1, got {num_sequences}')
     if int(refine_iter) < 1:
@@ -120,11 +248,11 @@ class InstanceTracker:
 
     def __init__(self, est, num_sequences, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
                  min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bbox_3d=None, draw=None,
-                 draw_color=dr.DEFAULT_COLOR):
+                 draw_color=dr.DEFAULT_COLOR, schedule='lockstep'):
         from .objects import require_device_pipeline
         require_device_pipeline(est, 'instance tracking')
         key = check_args(num_sequences, max_instances, refine_iter, redetect_every, gate, max_misses, min_score, nms_iou,
-                         peak_radius, smooth_num, smooth_std)
+                         peak_radius, smooth_num, smooth_std, schedule)
         if bbox_3d is None:
             bbox_3d = object_bbox(est.refiner.ref_database)
             if bbox_3d is None:
@@ -132,12 +260,14 @@ class InstanceTracker:
         self.bbox = check_bbox(bbox_3d)
         self._gen = est._generation()
         self._setup(est, key, [self.bbox], num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std,
-                    draw, [draw_color])
+                    draw, [draw_color], schedule)
+        center = np.asarray(est.ref_info['center'], np.float64).reshape(1, 3)
+        self._dev['centers'] = torch.from_numpy(np.ascontiguousarray(center)).to(est.detector.device)
 
     def _setup(self, est, key, boxes, num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std,
-               draw=None, colors=None):
+               draw=None, colors=None, schedule='lockstep'):
         """The tracker's constants and device state for K = len(boxes) objects with M = key[0] slots each."""
-        self.est, self.key = est, key
+        self.est, self.key, self.schedule = est, key, schedule
         self.K, self.S, self.M, self.refine_iter = len(boxes), int(num_sequences), key[0], int(refine_iter)
         self.redetect_every = None if redetect_every is None else int(redetect_every)
         self.gate, self.max_misses = float(gate), int(max_misses)
@@ -157,6 +287,8 @@ class InstanceTracker:
                        'ring': torch.zeros(n, self.num, 8, 2, dtype=torch.float32, device=dev),
                        'count': torch.zeros(n, dtype=torch.int32, device=dev)}
         self._pending, self._since = True, 0
+        # per-sequence schedules (row f18): each sequence's pending flag and steps since its last detection, on the host
+        self._schedule = Schedule(self.S, self.redetect_every, schedule == 'staggered')
         # drawing (row f16): every live slot (track id >= 0) of a sequence on its frame, in row (slot group) order
         kinds = self.draw = dr.parse_kinds(draw)
         G = self.M * self.K
@@ -178,10 +310,25 @@ class InstanceTracker:
         st['ring'][rows] = 0
         st['count'][rows] = 0
         self._pending = True
+        self._schedule.pending[slice(None) if sequences is None else seqs] = True
 
-    def redetect(self):
-        """The next step re-detects: the live tracks are kept and associated with the new detections."""
-        self._pending = True
+    def redetect(self, sequences=None):
+        """The next step re-detects: the live tracks are kept and associated with the new detections.  sequences (the
+        per-sequence schedules only): mark only those sequences; each re-detects on its next step."""
+        if sequences is None:
+            self._pending = True
+            self._schedule.pending[:] = True
+            return
+        if self.schedule == 'lockstep':
+            raise ValueError("redetect(sequences): a lockstep tracker re-detects every sequence together; create it with "
+                             "schedule='per_sequence' or 'staggered' to re-detect single sequences")
+        self._schedule.pending[_sequences(self.S, sequences)] = True
+
+    def detecting(self):
+        """bool [S]: the sequences that re-detect on their next step."""
+        if self.schedule == 'lockstep':
+            return np.full(self.S, self._detecting())
+        return self._schedule.due()
 
     def _check(self):
         if self.est._generation() != self._gen:
@@ -216,15 +363,17 @@ class InstanceTracker:
             det, valid, init, cams, center, float(self.est.cfg['ref_resolution']), self.gate, self.max_misses,
             self.est.cfg['refine_iter'], self.refine_iter, *state)
 
-    def _take_selections(self, rd):
-        """-> per object (sel_idx [M*S], sel_out [M*S*2], logits [M*S*n_sel]) instance-major, read in packing order."""
-        n = self.M * self.S
+    def _take_selections(self, rd, S):
+        """-> per object (sel_idx [M*S], sel_out [M*S*2], logits [M*S*n_sel]) instance-major, read in packing order (S:
+        the detected frames)."""
+        n = self.M * S
         return [(rd.take(n), rd.take(n * 2), rd.take(n * len(self.est.ref_info['poses'])))]
 
     # -------------------------------------------------------------- the graphs
-    def _detect_fn(self, st, draw=None):
-        est, G, S, r = self.est, self.M * self.K, self.S, self.refine_iter
-        F, c, n = est.cfg['refine_iter'], self._dev, self.M * self.K * self.S
+    def _detect_fn(self, st, draw=None, S=None):
+        """The re-detection body for S sequences (default: the tracker's; a partial step's compact batch, row f18)."""
+        est, G, S, r = self.est, self.M * self.K, S or self.S, self.refine_iter
+        F, c, n = est.cfg['refine_iter'], self._dev, self.M * self.K * S
         views, R = self._groups(st)
         initial, associate, refine = self._detection(st), self._associate(), est.refiner._refine_warped(128)
 
@@ -252,8 +401,9 @@ class InstanceTracker:
             return buf, poses, park, live, ids, misses, next_id, ring, count
         return fn
 
-    def _refine_fn(self, st, draw=None):
-        est, S, r, c, n = self.est, self.S, self.refine_iter, self._dev, self.M * self.K * self.S
+    def _refine_fn(self, st, draw=None, S=None):
+        est, S, r, c = self.est, S or self.S, self.refine_iter, self._dev
+        n = self.M * self.K * S
         views, R = self._groups(st)
         refine = est.refiner._refine_warped(128)
 
@@ -278,8 +428,63 @@ class InstanceTracker:
             return buf, poses, ring, count
         return fn
 
+    def _mixed_fn(self, st, S, d, blocks=None, draw=None):
+        """The mixed instance step's body for S sequences of which some re-detect, their frames gathered into a batch of
+        d (blocks: per size group of frames of several sizes, as _size_buckets makes them)."""
+        est, G, r = self.est, self.M * self.K, self.refine_iter
+        F, c, n = est.cfg['refine_iter'], self._dev, self.M * self.K * S
+        views, R = self._groups(st)
+        initial, refine = self._detection(st), est.refiner._refine_warped(128)
+        ref_res = float(est.cfg['ref_resolution'])
+
+        def fn(frames, cams, prev, park, live, ids, misses, next_id, ring, count, seq, det_index, *dt):
+            gf, gc = frames.index_select(0, seq), cams.index_select(0, seq)
+            if blocks is None:
+                init, det, crop, sels, valid, inst_count = initial(gf, gc)
+            else:
+                with fr.gathered(frames, gf, seq, blocks):                       # detection on true-size frames (row f13)
+                    init, det, crop, sels, valid, inst_count = initial(gf, gc)
+            work, flags0, lists, det_slot, spawned, dropped = ops.instances_associate_sequences(
+                det_index, det, valid, init, cams, c['centers'], ref_res, self.gate, self.max_misses, F, r, prev, live, ids, misses,
+                next_id, park, ring, count)
+            frames_x, cams_x = torch.cat([frames, frames], 0), torch.cat([cams, cams], 0)
+            real = lambda: work.view(G, 2 * S, 12)[:, :S].reshape(n, 12).clone()
+            ones, chain, off = torch.ones_like(flags0), [real()], 0
+            for it in range(max(F, r)):
+                L = n if it < r else G * d                  # past refine_iter: the re-detecting sequences' slots only
+                rows = lists[off:off + L]
+                off += L
+                jobs, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems_rows(
+                    views, R, 2 * S, cams_x, frames_x, work, rows, flags0 if it == 0 else ones)
+                out = refine(jobs, que_K, que_pose, ref_Ks, ref_poses)
+                ops.glue_apply_refinements_rows(views, 2 * S, que_pose, que_K, rect, out, rows, work)
+                chain.append(real())
+            poses = chain[-1]
+            Ks = cams[:, :9].contiguous()
+            smoothed, avg = ops.track_smooth_objects(poses, True, c['bboxes'], Ks, ring, count, c['weights'])
+            if dt:
+                draw(frames, poses, True, smoothed, Ks, dt[0], ids)
+            buf = instances.pack([torch.stack(chain, 0), smoothed, avg, ring, count, ids, det, *sels, valid, inst_count, det_slot,
+                                  spawned, dropped], crop)
+            return buf, poses, park, live, ids, misses, next_id, ring, count
+        return fn
+
+    def _body(self, st, kind, S, d=None, blocks=None, draw=None):
+        """A per-sequence step's body on the whole slot state: fn(frames, cams, prev, park, live, ids, misses, next_id, ring,
+        count, *rest) -> (buf, prev, park, live, ids, misses, next_id, ring, count), kind 'detect', 'refine' or 'mixed'."""
+        if kind == 'detect':
+            return self._detect_fn(st, draw, S)
+        if kind == 'mixed':
+            return self._mixed_fn(st, S, d, blocks, draw)
+        refine = self._refine_fn(st, draw, S)
+
+        def fn(frames, cams, prev, park, live, ids, misses, next_id, ring, count, *dt):
+            buf, poses, ring, count = refine(frames, cams, prev, park, live, ids, ring, count, *dt)
+            return buf, poses, park, live, ids, misses, next_id, ring, count
+        return fn
+
     # -------------------------------------------------------------- one step
-    def step(self, frames, Ks, out=None):
+    def step(self, frames, Ks, out=None, sequences=None):
         """frames: S uint8 [h,w,3] (of one size or several, row f13; or device frames, row f14, as Tracker.step takes them);
         Ks: [S,3,3]; out: drawing destinations as Tracker.step takes them (a tracker made with draw= draws every live slot
         of a sequence on its frame, in slot order; without out= inter['drawn'] holds tracker-owned frames).  Returns (poses float32 [S,M,3,4], smoothed float64 [S,M,3,4],
@@ -287,12 +492,23 @@ class InstanceTracker:
         poses, float64 on a re-detection step; a row whose chain is shorter repeats its final pose), 'bbox_pts' and
         'smoothed_pts' [S,M,8,2].  Empty slots' poses and points are NaN.  A re-detection step adds predict_instances'
         keys led by [S,M], 'det_slot' int64 [S,M] (the slot detection m went to, -1: discarded), 'spawned' bool [S,M]
-        (the slots that started a track) and 'dropped' (the ids removed this step, ascending)."""
-        return self._step(frames, Ks, out)[0]
+        (the slots that started a track) and 'dropped' (the ids removed this step, ascending).
 
-    def _step(self, frames, Ks, out=None):
+        On the per-sequence schedules (row f18) inter['detected'] (bool [n]) marks the sequences that re-detected; when
+        any did, the re-detection keys cover every row, the others' filled with NaN, -1, False / 0 and zero crops, and
+        refine_poses has max(cfg['refine_iter'], refine_iter) + 1 entries.  sequences: step only these sequences, with
+        Tracker.step's contract (row f17): one frame, K and out= destination each, in any order; results in that order
+        with inter['sequences']; the others are not computed and keep their state and out= buffers."""
+        return self._step(frames, Ks, out, sequences)[0]
+
+    def _step(self, frames, Ks, out=None, sequences=None):
         """One step -> the decoded results of every object, in object order."""
         self._check()
+        if self.schedule != 'lockstep':
+            return self._step_sequences(frames, Ks, out, sequences)
+        if sequences is not None:
+            raise ValueError("step: sequences= needs schedule='per_sequence' or 'staggered'; a lockstep tracker's "
+                             're-detection schedule is tracker-wide')
         est, S = self.est, self.S
         if len(frames) != S or len(Ks) != S:
             raise ValueError(f'step: this tracker follows {S} sequences, got {len(frames)} frames and {len(Ks)} Ks')
@@ -300,57 +516,118 @@ class InstanceTracker:
         if Ks.shape != (S, 3, 3):
             raise ValueError(f'step: Ks must be [{S},3,3], got {Ks.shape}')
         detecting = self._detecting()
+        res = self._run(frames, Ks, out, 'detect' if detecting else 'refine')
+        self._pending = False
+        self._since = 1 if detecting else self._since + 1
+        return res
+
+    def _run(self, frames, Ks, out, kind, part=None, det_seq=None):
+        """One step's graph and read -> decoded results.  kind: 'detect', 'refine' or 'mixed'; part: a partial step (row
+        f17/f18) over its compact batch; det_seq: bool over the batch's sequences, those that re-detect (kind 'mixed')."""
+        est = self.est
+        S = self.S if part is None else part.b
         F = est.cfg['refine_iter']
-        if detecting and F < 1:
+        if kind != 'refine' and F < 1:
             raise ValueError("instance tracking needs cfg['refine_iter'] >= 1 (a re-detection step smooths float32 poses)")
         imgs = fr.as_frames(frames, 'step', est.detector)
         plan = fr.FramePlan(fr.size_pattern(imgs))
         if plan.mixed:
             fr.check_frames(imgs, Ks, 'step')
         stt, x = self._tables(), self._state
-        draw, dt, drawn, named = draw_inputs(self._drawer, est.detector, plan, out)
+        drawer = self._drawer if part is None or self._drawer is None else self._drawer.for_sequences(part.b)
+        draw, dt, drawn, named = draw_inputs(drawer, est.detector, plan, out, None if part is None else part.a)
+        dev = est.detector.device
+        det_rows, extra, D = None, [], S
+        if kind == 'mixed':
+            seq, blocks, det_rows, D, key = plan_mixed(det_seq, plan)
+            up = lambda a, dt_: torch.from_numpy(np.ascontiguousarray(a, dt_)).to(dev)
+            extra = [up(seq, np.int64), up(det_rows, np.int32)]
+            base, fn = mixed_name(S, key), self._body(stt, 'mixed', S, D, blocks, draw)
+        elif part is None:
+            base = kind
+            fn = self._detect_fn(stt, draw) if kind == 'detect' else self._refine_fn(stt, draw)
+        else:
+            base, fn = kind, self._body(stt, kind, S, draw=draw)
+        if part is not None:
+            base = part.name(base)
+            fn = _compact_state_fn(fn)
+            extra = part.graph_inputs(dev) + extra
         with torch.no_grad():
-            if detecting:
-                name, fn, fin = fr.stage(est.detector, named('detect'), self._detect_fn(stt, draw), imgs, plan)
-                cams = est.detector._to_dev(glue.cameras(Ks))
+            name, fn, fin = fr.stage(est.detector, named(base), fn, imgs, plan)
+            cams = est.detector._to_dev(glue.cameras(Ks))
+            if part is None and kind == 'refine':
+                outs = self.stages.run(name, fn, fin + [cams, x['prev'], x['park'], x['live'], x['ids'], x['ring'], x['count']] + dt)
+                buf, poses, ring, count = outs
+            else:
                 outs = self.stages.run(name, fn, fin + [cams, x['prev'], x['park'], x['live'], x['ids'], x['misses'], self._next_id,
-                                                        x['ring'], x['count']] + dt)
+                                                        x['ring'], x['count']] + extra + dt)
                 buf, poses, park, live, ids, misses, next_id, ring, count = outs
                 for k, v in (('park', park), ('live', live), ('ids', ids), ('misses', misses)):
                     x[k].copy_(v)
                 self._next_id.copy_(next_id)
-            else:
-                name, fn, fin = fr.stage(est.detector, named('refine'), self._refine_fn(stt, draw), imgs, plan)
-                cams = est.detector._to_dev(glue.cameras(Ks))
-                outs = self.stages.run(name, fn, fin + [cams, x['prev'], x['park'], x['live'], x['ids'], x['ring'], x['count']] + dt)
-                buf, poses, ring, count = outs
             x['prev'].copy_(poses)
             x['ring'].copy_(ring)
             x['count'].copy_(count)
             host = est.detector._to_host(buf)                        # the step's one synchronising read
-        self._pending = False
-        self._since = 1 if detecting else self._since + 1
-        res = self._decode(host, detecting)
+        res = self._decode(host, kind != 'refine', S, det_rows, D)
         if drawn is not None:
             for r in res:
                 r[3]['drawn'] = drawn
         return res
 
-    def _decode(self, host, detecting):
-        est, S, M, K, num = self.est, self.S, self.M, self.K, self.num
+    def _step_sequences(self, frames, Ks, out, sequences):
+        """A step on a per-sequence schedule (row f18): the stepped sequences' plan, one graph, their counters."""
+        S, sch = self.S, self._schedule
+        part = None
+        if sequences is not None:
+            part = PartialStep(S, self.M * self.K, sequences, sch.due(), np.ones(S, bool), 1)
+            part.check(frames, Ks, out)
+            if out is not None and self._drawer is None:
+                raise ValueError('step: out= names drawing destinations; create the tracker with draw=')
+            frames, Ks, out = part.compact(frames), part.compact(Ks), part.compact_out(out)
+            seqs, n_real = part.seq, part.a
+        else:
+            if len(frames) != S or len(Ks) != S:
+                raise ValueError(f'step: this tracker follows {S} sequences, got {len(frames)} frames and {len(Ks)} Ks')
+            seqs, n_real = np.arange(S), S
+        Ks = np.stack([np.asarray(k) for k in Ks], 0)
+        if Ks.shape != (len(seqs), 3, 3):
+            raise ValueError(f'step: Ks must be [{len(seqs)},3,3], got {Ks.shape}')
+        det_seq, kind = sch.plan(seqs, n_real)
+        res = self._run(frames, Ks, out, kind, None if part is None or part.lockstep else part, det_seq)
+        sch.advance(seqs[:n_real])
+        for r in res:
+            r[3]['detected'] = det_seq.copy()
+        if part is None:
+            return res
+        return [_reorder(r, part) for r in res]
+
+    def _decode(self, host, detecting, S=None, det_rows=None, D=None):
+        """det_rows: a mixed step's detection row of each sequence ([S], -1: not detecting) in its batch of D rows, whose
+        parts are spread over the S rows (the others filled); None: every sequence detected at its own row."""
+        est, M, K, num = self.est, self.M, self.K, self.num
+        S = S or self.S
+        D = S if D is None else D
         n = M * K * S
         n_chain = (max(est.cfg['refine_iter'], self.refine_iter) if detecting else self.refine_iter) + 1
         res = est.cfg['ref_resolution']
-        rd = instances.Unpacker(host, n * res * res * 3 if detecting else 0)
+        rd = instances.Unpacker(host, M * K * D * res * res * 3 if detecting else 0)
         chain = rd.take(n_chain * n * 12).reshape(n_chain, n, 12)
         smoothed, avg = rd.take(n * 12).reshape(n, 12), rd.take(n * 16).reshape(n, 16)
         ring_h, count_h = rd.take(n * num * 16).reshape(n, num, 8, 2).astype(np.float32), rd.take(n).astype(np.int64)
         ids = rd.take(n)
         if detecting:
-            det, sels = rd.take(n * 4).reshape(n, 4), self._take_selections(rd)
-            valid, inst_count = rd.take(n), rd.take(K * S).reshape(K, S)
+            nd = M * K * D
+            det, sels = rd.take(nd * 4).reshape(nd, 4), self._take_selections(rd, D)
+            valid, inst_count = rd.take(nd), rd.take(K * D).reshape(K, D)
             det_slot, spawned, dropped = rd.take(n), rd.take(n), rd.take(n)
-            crops = rd.crops.reshape(n, res, res, 3)
+            crops = rd.crops.reshape(nd, res, res, 3)
+            if det_rows is not None:
+                sp = lambda a, L, fill: _spread(a, L, D, det_rows, fill)
+                det, valid, crops = sp(det, M * K, np.nan), sp(valid, M * K, 0), sp(crops, M * K, 0)
+                inst_count = sp(inst_count.reshape(-1), K, 0).reshape(K, S)
+                sels = [(sp(i, M, -1), sp(so.reshape(M * D, 2), M, np.nan).reshape(-1), sp(lg.reshape(M * D, -1), M, np.nan).reshape(-1))
+                        for i, so, lg in sels]
 
         obj = lambda a, o: a.reshape(M, K, S, *a.shape[1:])[:, o].reshape(M * S, *a.shape[1:])      # object o, instance-major
         out = []
@@ -361,12 +638,12 @@ class InstanceTracker:
             if detecting:
                 det_parts = [obj(det, o), *sels[o], obj(valid, o), inst_count[o], obj(crops, o),
                              *(obj(a, o) for a in (det_slot, spawned, dropped))]
-            out.append(self._decode_object(c, *one, det_parts, o))
+            out.append(self._decode_object(c, *one, det_parts, o, S))
         return out
 
-    def _decode_object(self, chain, smoothed, avg, ring_h, count_h, ids, det_parts, o):
+    def _decode_object(self, chain, smoothed, avg, ring_h, count_h, ids, det_parts, o, S=None):
         """One object's instance-major rows (row m*S + s) -> (poses, smoothed, track_ids, inter) as step() returns them."""
-        S, M = self.S, self.M
+        S, M = S or self.S, self.M
         n = M * S
         ids = instances.frame_major(ids.astype(np.int64), M, S)
         empty = ids < 0
@@ -391,6 +668,44 @@ class InstanceTracker:
         return inter['refine_poses'][-1], nan(fm(smoothed.reshape(n, 3, 4))), ids, inter
 
 
+def _spread(a, L, D, det_rows, fill):
+    """Rows l*D + j of a detection batch -> rows l*S + s of the S sequences (j = det_rows[s]); rows of sequences that did
+    not detect (det_rows -1) are `fill`."""
+    S = len(det_rows)
+    a = a.reshape(L, D, *a.shape[1:])
+    out = np.full((L, S) + a.shape[2:], fill, a.dtype)
+    s = np.flatnonzero(det_rows >= 0)
+    out[:, s] = a[:, det_rows[s]]
+    return out.reshape(L * S, *a.shape[2:])
+
+
+def _compact_state_fn(fn):
+    """A per-sequence step body fn(frames, cams, prev, park, live, ids, misses, next_id, ring, count, *rest) of a compact
+    batch -> the partial step's body g(frames, cams, <the same state>, gather, scatter, *rest) on the tracker's whole slot
+    state (PartialStep's rows over the M*K slot groups): gather the compact rows, run fn, copy the real rows back."""
+    def g(frames, cams, prev, park, live, ids, misses, next_id, ring, count, gather, scatter, *rest):
+        state = (prev, park, live, ids, misses, ring, count)
+        p, pk, lv, i, ms, ring_c, count_c = _gather_rows(state, gather)
+        outs = fn(frames, cams, p, pk, lv, i, ms, next_id, ring_c, count_c, *rest)
+        buf, next_id = outs[0], outs[6]
+        new = outs[1:6] + outs[7:9]
+        return (buf, *[_scatter_rows(t, c, scatter) for t, c in zip(state[:5], new[:5])], next_id,
+                *[_scatter_rows(t, c, scatter) for t, c in zip(state[5:], new[5:])])
+    return g
+
+
+def _reorder(res, part):
+    """One object's results over a partial step's compact rows -> the listed sequences', in the caller's order, through
+    PartialStep.results; 'dropped' (ids, not rows) passes through."""
+    poses, smoothed, ids, inter = res
+    inter = dict(inter)
+    dropped = inter.pop('dropped', None)
+    poses, smoothed, inter = part.results(poses, smoothed, inter)
+    if dropped is not None:
+        inter['dropped'] = dropped
+    return poses, smoothed, ids[part.pos], inter
+
+
 class ObjectInstanceTracker(InstanceTracker):
     """Every instance of every object of an ObjectSet tracked through S sequences in lockstep; see
     ObjectSet.instance_tracker().  Slot group g = m*K + o is instance slot m of object o; row g*S + s is that slot on
@@ -398,15 +713,15 @@ class ObjectInstanceTracker(InstanceTracker):
 
     def __init__(self, objs, num_sequences, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
                  min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bboxes=None, draw=None,
-                 draw_colors=None):
+                 draw_colors=None, schedule='lockstep'):
         key = check_args(num_sequences, max_instances, refine_iter, redetect_every, gate, max_misses, min_score, nms_iou,
-                         peak_radius, smooth_num, smooth_std)
+                         peak_radius, smooth_num, smooth_std, schedule)
         objs._check()
         boxes = object_bboxes(objs, bboxes)
         self.objs, self.names, self.bboxes = objs, objs.names, np.ascontiguousarray(np.stack(boxes, 0))
         self._membership = objs.membership
         self._setup(objs.est, key, boxes, num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std,
-                    draw, dr.object_colors(self.names, draw_colors))
+                    draw, dr.object_colors(self.names, draw_colors), schedule)
         centers = np.stack([np.asarray(ob.ref_info['center'], np.float64).reshape(3) for ob in objs._objects.values()], 0)
         self._dev['centers'] = torch.from_numpy(np.ascontiguousarray(centers)).to(self.est.detector.device)
 
@@ -438,16 +753,16 @@ class ObjectInstanceTracker(InstanceTracker):
             det, valid, init, cams, centers, float(est.cfg['ref_resolution']), self.gate, self.max_misses, est.cfg['refine_iter'],
             self.refine_iter, *state)
 
-    def _take_selections(self, rd):
-        S, M, K = self.S, self.M, self.K
+    def _take_selections(self, rd, S):
+        M, K = self.M, self.K
         n_sel = [len(ob.ref_info['poses']) for ob in self.objs._objects.values()]
         slots = [(rd.take(S), rd.take(S * 2), rd.take(S * n_sel[g % K])) for g in range(M * K)]
         return [tuple(np.concatenate([slots[m * K + o][i] for m in range(M)]) for i in range(3)) for o in range(K)]
 
-    def step(self, frames, Ks, out=None):
+    def step(self, frames, Ks, out=None, sequences=None):
         """frames: S uint8 [h,w,3] (of one size or several, row f13; or device frames, row f14); Ks: [S,3,3] (shared by all
         objects); out: drawing destinations as InstanceTracker.step takes them, every live slot of every object drawn.  Returns {name: (poses float32
         [S,M,3,4], smoothed float64 [S,M,3,4], track_ids int64 [S,M], inter)}: per object what InstanceTracker.step returns,
         'det_score' included on a re-detection step; 'dropped' lists that object's ids only.  Ids are unique over every
-        object of the tracker."""
-        return dict(zip(self.names, self._step(frames, Ks, out)))
+        object of the tracker.  sequences (per-sequence schedules, row f18): step only these, as InstanceTracker.step."""
+        return dict(zip(self.names, self._step(frames, Ks, out, sequences)))

@@ -326,18 +326,21 @@ class ObjectSet:
 
     def instance_tracker(self, num_sequences=1, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
                          min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bboxes=None, draw=None,
-                         draw_colors=None):
+                         draw_colors=None, schedule='lockstep'):
         """An ObjectInstanceTracker (gen6d_b200/instance_track.py): every instance of every object of the set, up to
         `max_instances` per object and frame, followed through `num_sequences` videos in lockstep, with
         Gen6DEstimator.instance_tracker()'s semantics per object (each object's tracks are matched only to its own
         detections) and track ids unique over the whole tracker.  Re-detection steps share the set's query pyramid and
         correlation; each step is one captured graph and one synchronising read.  bboxes, draw, draw_colors: as for
-        tracker(); only live slots (track id >= 0) are drawn."""
+        tracker(); only live slots (track id >= 0) are drawn.
+        schedule (row f18): 'lockstep' (every sequence re-detects on the same steps), 'per_sequence' (each sequence has its
+        own re-detection flag and counter; reset / redetect take sequences, and step takes sequences= to step any subset)
+        or 'staggered' ('per_sequence' with the periodic re-detections spread over the steps; needs redetect_every)."""
         from .instance_track import ObjectInstanceTracker
         return ObjectInstanceTracker(self, num_sequences, max_instances=max_instances, refine_iter=refine_iter,
                                      redetect_every=redetect_every, gate=gate, max_misses=max_misses, min_score=min_score,
                                      nms_iou=nms_iou, peak_radius=peak_radius, smooth_num=smooth_num, smooth_std=smooth_std,
-                                     bboxes=bboxes, draw=draw, draw_colors=draw_colors)
+                                     bboxes=bboxes, draw=draw, draw_colors=draw_colors, schedule=schedule)
 
     def raw_correlation(self, que_imgs):
         """The detector's raw correlation maps for inspection: {name: [scale][level] float32 [qn, H, W, rfn]} (the maps

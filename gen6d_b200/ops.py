@@ -451,6 +451,40 @@ def instances_associate_objects(det, valid, init, cams, centers, ref_resolution,
     return work, flags0, lists, det_slot, spawned, dropped
 
 
+def instances_associate_sequences(det_index, det, valid, init, cams, centers, ref_resolution, gate, max_misses, F, r, prev, live, ids,
+                                  misses, next_id, park, ring, count):
+    """instances_associate_objects for a step in which only some sequences re-detect (g6d_instances_associate_sequences):
+    det_index int32 [S] (device) gives each sequence its row j in a detection batch of D rows per slot group, -1 when it
+    does not detect; det float32 [M*K*D,4], valid int32 [M*K*D], init float64 [M*K*D,12] (row g*D + j).  Detecting pairs
+    are associated as instances_associate_objects does; the others only set up their refinement, as a refine-only step.
+    Outside graph capture det_index is read back and checked (distinct rows in [0, D) or -1); inside a capture the caller
+    has checked the values it uploads.  Returns (work float64 [M*K*2S,12], flags0 uint8 [M*K*2S], lists int32 [r*M*K*S +
+    max(F-r,0)*M*K*D], det_slot int32, spawned int32, dropped int64 [M*K*S])."""
+    from .instance_track import check_det_index, list_length
+    n, S, K = live.shape[0], cams.shape[0], centers.shape[0]
+    M, num, dev = n // max(K * S, 1), ring.shape[1], live.device
+    D = det.shape[0] // max(M * K, 1)
+    if (K < 1 or centers.shape != (K, 3) or n != M * K * S or det_index.shape != (S,) or det.shape != (M * K * D, 4)
+            or valid.shape != (M * K * D,) or init.shape != (M * K * D, 12) or prev.shape != (n, 12) or park.shape != (n, 12)
+            or ids.shape != (n,) or misses.shape != (n,) or next_id.shape != (1,) or ring.shape != (n, num, 8, 2)
+            or count.shape != (n,)):
+        raise ValueError(f'instances_associate_sequences: inconsistent shapes for {n} rows over {K} objects and {S} sequences')
+    if not torch.cuda.is_current_stream_capturing():
+        check_det_index(det_index.cpu().numpy(), S, D)
+    work = torch.empty(2 * n, 12, device=dev, dtype=torch.float64)
+    flags0 = torch.empty(2 * n, device=dev, dtype=torch.uint8)
+    lists = torch.empty(list_length(M * K, S, D, int(F), int(r)), device=dev, dtype=torch.int32)
+    det_slot, spawned = torch.empty(n, device=dev, dtype=torch.int32), torch.empty(n, device=dev, dtype=torch.int32)
+    dropped = torch.empty(n, device=dev, dtype=torch.int64)
+    _call('g6d_instances_associate_sequences', S, K, M, int(F), int(r), D, _p(det_index, torch.int32), _p(det), _p(valid, torch.int32),
+          _p(init, torch.float64), _p(cams, torch.float64), _p(centers, torch.float64), float(ref_resolution), float(gate),
+          int(max_misses), _p(prev, torch.float64), _p(live, torch.int32), _p(ids, torch.int64), _p(misses, torch.int32),
+          _p(next_id, torch.int64), _p(park, torch.float64), _p(ring), _p(count, torch.int32), num, _p(work, torch.float64),
+          _p(flags0, torch.uint8), _p(lists, torch.int32), _p(det_slot, torch.int32), _p(spawned, torch.int32),
+          _p(dropped, torch.int64), _stream())
+    return work, flags0, lists, det_slot, spawned, dropped
+
+
 def imagenet_norm(x, out_c=4):
     out = torch.empty(*x.shape[:-1], out_c, device=x.device, dtype=torch.float32)
     _call('g6d_imagenet_norm', _p(x), _p(out), x.numel() // x.shape[-1], x.shape[-1], out_c, _stream())

@@ -359,14 +359,25 @@ class PartialStep:
         return raw[pos], smoothed[pos], res
 
 
+def _gather_rows(tensors, gather):
+    """The compact rows (PartialStep.gather) of every state tensor."""
+    return [t.index_select(0, gather) for t in tensors]
+
+
+def _scatter_rows(t, c, scatter):
+    """State tensor t with the compact rows c copied back (PartialStep.scatter: padding rows land in scratch copies,
+    dropped)."""
+    return torch.cat([t, c], 0).index_copy_(0, scatter, c)[:t.shape[0]]
+
+
 def _compact_fn(fn, full):
     """A lockstep step body fn(frames, cams, [prev,] ring, count, *rest) of the compact batch -> the partial step's graph
     body g(frames, cams, prev, ring, count, gather, scatter, *rest) on the tracker's whole state: gather the compact rows,
     run fn, copy its real rows back (padding rows land in their scratch copies, dropped)."""
     def g(frames, cams, prev, ring, count, gather, scatter, *rest):
-        sub = [t.index_select(0, gather) for t in ((ring, count) if full else (prev, ring, count))]
+        sub = _gather_rows((ring, count) if full else (prev, ring, count), gather)
         buf, poses, ring_c, count_c = fn(frames, cams, *sub, *rest)
-        put = lambda t, c: torch.cat([t, c], 0).index_copy_(0, scatter, c)[:t.shape[0]]
+        put = lambda t, c: _scatter_rows(t, c, scatter)
         return buf, put(prev, poses), put(ring, ring_c), put(count, count_c)
     return g
 

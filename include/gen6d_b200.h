@@ -340,6 +340,35 @@ int g6d_instances_associate_objects_host(int S, int K, int M, int F, int r, cons
                                          int max_misses, const double* prev, int* live, long long* ids, int* misses,
                                          long long* next_id, double* park, float* ring, int* count, int num, double* work,
                                          uint8_t* flags0, int* lists, int* det_slot, int* spawned, long long* dropped);
+/* The association of g6d_instances_associate_objects for a step in which only some sequences re-detect
+ * (gen6d_b200/instance_track.py, the per-sequence schedules).  det_index [S] int32 gives each sequence its row j in a
+ * detection batch of D rows per slot group (0 <= j < D, no row twice), or -1 when the sequence does not detect this
+ * step; det, valid and init are [M*K*D,...], row g*D + j.  A detecting (sequence, object) pair is associated exactly as
+ * g6d_instances_associate_objects does it.  A non-detecting pair only sets up its refinement, as a refine-only step
+ * does: its real work row is prev when the slot is live, else park, with its scratch copy; flags0 = live; its chain is r;
+ * spawned 0, dropped and det_slot -1; live, ids, misses, park, ring and count are untouched.  det_slot, spawned and
+ * dropped have M*K*S rows (det_slot row g*S + s: detection m of sequence s).  The spawned tracks are numbered in
+ * ascending (object, sequence, detection) order over the detecting pairs, continuing the shared counter.  In lists,
+ * iterations it < r list all M*K*S rows (entry (it*M*K + g)*S + s), then iterations r <= it < F
+ * list the M*K*D rows of the detecting sequences only (entry r*M*K*S + ((it - r)*M*K + g)*D + j), a finished chain
+ * replaced by its scratch row; a padding row j (used by no sequence) lists the scratch rows of the rank-th
+ * non-detecting sequence, rank its rank among the unused rows, so it never touches a row another entry lists.  lists
+ * thus has r*M*K*S + max(F - r, 0)*M*K*D entries.  det_index the identity with D = S is g6d_instances_associate_objects
+ * bit for bit; every entry -1 (D = 0; det, valid and init may be null) is a refine-only step's set-up.  det_index is
+ * device memory for the device call (the caller validates it) and host memory for the *_host one, which rejects
+ * out-of-range and repeated rows.  Needs 0 <= D <= S and centers [K,3]. */
+int g6d_instances_associate_sequences(int S, int K, int M, int F, int r, int D, const int* det_index, const float* det,
+                                      const int* valid, const double* init, const g6d_glue_camera* cams, const double* centers,
+                                      double ref_resolution, double gate, int max_misses, const double* prev, int* live,
+                                      long long* ids, int* misses, long long* next_id, double* park, float* ring, int* count,
+                                      int num, double* work, uint8_t* flags0, int* lists, int* det_slot, int* spawned,
+                                      long long* dropped, g6d_stream_t stream);
+int g6d_instances_associate_sequences_host(int S, int K, int M, int F, int r, int D, const int* det_index, const float* det,
+                                           const int* valid, const double* init, const g6d_glue_camera* cams, const double* centers,
+                                           double ref_resolution, double gate, int max_misses, const double* prev, int* live,
+                                           long long* ids, int* misses, long long* next_id, double* park, float* ring, int* count,
+                                           int num, double* work, uint8_t* flags0, int* lists, int* det_slot, int* spawned,
+                                           long long* dropped);
 /* (x - mean) / std on f32 [n_pixels, in_c] -> [n_pixels, out_c] (in_c, out_c in {3,4})
  * (network/detector.py:189, selector.py:115, refiner.py:65) */
 int g6d_imagenet_norm(const float* in, float* out, long long n_pixels, int in_c, int out_c, g6d_stream_t stream);
