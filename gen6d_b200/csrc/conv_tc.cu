@@ -378,8 +378,9 @@ __device__ __forceinline__ void epilogue_tile(float (&acc)[AccCfg<BN>::NMAIN][BN
 //     flight while K-block it is transformed and stored) and never drain the smem ring between tiles
 //     (one global K-block counter), so they fill the next tile's stages during the epilogue;
 //   * each of the two consumer warpgroups issues the wgmmas of its 64 rows of a stage, keeps one
-//     stage's group in flight while it waits for the next, releases each stage once its group has
-//     completed (a stage is free when all 8 consumer warps have released it) and runs the epilogue;
+//     stage's group in flight while it waits for the next (BN 128 with the split input: none, see
+//     `early`), releases each stage once its group has completed (a stage is free when all 8 consumer
+//     warps have released it) and runs the epilogue;
 //   * one consumer thread streams the weight tiles by TMA, STAGES K-blocks ahead of the MMAs.
 constexpr int TC2_PF_BYTES = 12 * 128;      // weight-tile L2 prefetch distance, in bytes of K per row
 
@@ -507,19 +508,9 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
                 const int yo = m % p.Ho; m /= p.Ho;
                 const int zo = m % p.Do;
                 const int b = m / p.Do;
-                KbIter pf, k;
-                pf.start(p, sp, 0);
-                k = pf;
-                auto prefetch = [&]() {
-                    const int kc = pf.tap(p) * p.Cin + pf.cb * BK;
-                    tma_prefetch_2d(&map_hi, kc, nt * BN);
-                    tma_prefetch_2d(&map_lo, kc, nt * BN);
-                    pf.next(p);
-                };
-#pragma unroll 1
-                for (int i = 0; i < min(nkb, PF - 1); ++i) prefetch();
+                KbIter k;                                    // no weight L2 prefetch, see below
+                k.start(p, sp, 0);
                 for (int it = 0; it < nkb; ++it, ++g, k.next(p)) {
-                    if (it + PF - 1 < nkb) prefetch();
                     if (k.kx == 0) {
                         const int s = gb % XC::BOXES;
                         const uint16_t oy = (uint16_t)k.ky, oz = (uint16_t)k.kz;
@@ -562,21 +553,13 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
                     const int yo = m % p.Ho; m /= p.Ho;
                     const int zo = m % p.Do;
                     const int b = m / p.Do;
-                    // L2 prefetch of the weight tiles PF K-blocks ahead, as the consumers' weight stream does: pf is the
-                    // next K-block to prefetch, k the one to load
-                    KbIter pf, k;
-                    pf.start(p, sp, 0);
-                    k = pf;
-                    auto prefetch = [&]() {
-                        const int kc = pf.tap(p) * p.Cin + pf.cb * BK;
-                        tma_prefetch_2d(&map_hi, kc, nt * BN);
-                        tma_prefetch_2d(&map_lo, kc, nt * BN);
-                        pf.next(p);
-                    };
-#pragma unroll 1
-                    for (int i = 0; i < min(nkb, PF - 1); ++i) prefetch();
+                    // No L2 prefetch of the weight tiles ahead of their loads (the consumers' weight stream below keeps
+                    // one): the TMA unit walks a prefetch box row by row like a load, so the two prefetches per K-block
+                    // were a third of the box rows it processed, and every bench shape ran faster without them
+                    // (DESIGN.md section 5).  The x-reuse thread above does without it for the same reason.
+                    KbIter k;
+                    k.start(p, sp, 0);
                     for (int it = 0; it < nkb; ++it, ++g, k.next(p)) {
-                        if (it + PF - 1 < nkb) prefetch();
                         const int tap = k.tap(p), cb = k.cb;
                         const uint16_t ox = (uint16_t)k.kx, oy = (uint16_t)k.ky, oz = (uint16_t)k.kz;
                         const int s = g % STAGES;
@@ -741,6 +724,11 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
         if (issuer)
             for (int i = 0; i < STAGES; ++i) load_next();
 
+        // Early release (BN 128 with the split input): only three 64 KB stages fit, and a consumer that keeps one
+        // group in flight holds two of them, which leaves the TMA thread one stage ahead.  These consumers instead
+        // wait for each stage's group and release the stage at once: two stages ahead, while the other warpgroup's
+        // wgmmas keep the tensor cores busy across the wait.  The wgmmas and their order are unchanged.
+        const bool early = BN == 128 && p.split_in;
         float acc[NMAIN][BN / 2];
         float cross[BN / 2];
         float run[FOLD ? BN / 2 : 1];                  // FOLD: the tile's sum of its splits so far
@@ -796,14 +784,19 @@ conv_tc2_kernel(const ConvTcP p, const Tc2Work wk, const __grid_constant__ CUten
                         mbar_wait(full_a(s), (g / STAGES) & 1, 4, g);
                         mbar_wait(full_b(s), (g / STAGES) & 1, 5, g);
                         mma_stage<BN, KIND>(acc[a], cross, a_hi(s) + a_row, a_lo(s) + a_row, b_hi(s), b_lo(s));
-                        wgmma_wait<1>();
-                        if (it > 0) release(g - 1);
+                        if (early) {
+                            wgmma_wait<0>();
+                            release(g);
+                        } else {
+                            wgmma_wait<1>();
+                            if (it > 0) release(g - 1);
+                        }
                         ++g;
                     }
                 }
             }
             wgmma_wait<0>();
-            if (nkb > 0) release(g - 1);
+            if (nkb > 0 && !early) release(g - 1);
             }
 
             sum_chains<BN, KIND>(acc, cross, nkb < NMAIN ? nkb : NMAIN);
