@@ -16,6 +16,7 @@ G6D_DET_MAX_SCALES = 8
 G6D_GLUE_MAX_OBJECTS = 16                   # objects per g6d_glue_*_objects launch
 G6D_DET_MAX_INSTANCES = 16                  # instances per map of g6d_det_parse_peaks
 G6D_DET_MAX_PEAK_RADIUS = 3
+G6D_DET_MAX_BOXES = 256                     # boxes per map of g6d_det_from_boxes
 G6D_ATTENTION_MAX_SMEM_FLOATS = 12288 - 32  # n + C/heads of a g6d_attention call
 G6D_FRAMES_MAX = 1024                       # frames per g6d_frames_canvas / g6d_frames_gather launch
 G6D_FRAME_RGB, G6D_FRAME_NV12 = 0, 1        # g6d_device_frame.format
@@ -134,6 +135,8 @@ _SIGNATURES = {
     'g6d_det_parse': [P, P, P, I, I, I, I, P, P, P],
     'g6d_det_parse_peaks': [P, P, P, I, I, I, I, I, I, F, F, F, P, P, P, P, P],
     'g6d_det_parse_peaks_host': [P, P, P, I, I, I, I, I, I, F, F, F, P, P, P, P],
+    'g6d_det_from_boxes': [P, P, I, I, I, F, P, P, P, P],
+    'g6d_det_from_boxes_host': [P, P, I, I, I, F, P, P, P],
     'g6d_det_corr_rowsum': [P, P, I, I, I, I, I, P],
     'g6d_det_corr_rowsum_objects': [P, P, I, I, I, I, I, I, P],
     'g6d_sel_ref_sums': [P, I, I, I, P, P, P],

@@ -450,6 +450,112 @@ __global__ void det_corr_rowsum_objects_kernel(const float4* __restrict__ partia
     out[i] = acc;
 }
 
+
+// ------------------------------------------------------------------------------------------ detections from boxes
+// A caller-supplied box (x0, y0, x1, y1, score) -> a detection record as g6d_det_parse_peaks writes one.  The box is
+// usable when all five values are finite and it has positive width and height.  The record is the square on the box's
+// longer side: (x0 + x1) * 0.5, (y0 + y1) * 0.5, max(w, h) * inv_box_size, score.  An add followed by a multiply has
+// no fused form, so host and device round every operation the same way.
+__host__ __device__ __forceinline__ bool box_usable(const float* b) {
+    return isfinite(b[0]) && isfinite(b[1]) && isfinite(b[2]) && isfinite(b[3]) && isfinite(b[4]) && b[2] > b[0] && b[3] > b[1];
+}
+
+__host__ __device__ __forceinline__ void box_record(const float* b, float inv_box_size, float* r) {
+    const float w = b[2] - b[0], h = b[3] - b[1];
+    r[0] = (b[0] + b[2]) * 0.5f;
+    r[1] = (b[1] + b[3]) * 0.5f;
+    r[2] = (w > h ? w : h) * inv_box_size;
+    r[3] = b[4];
+}
+
+// box a (score sa, index ia) comes before box b: score descending, ties to the lower index
+__host__ __device__ __forceinline__ bool box_before(float sa, int ia, float sb, int ib) {
+    return sa > sb || (sa == sb && ia < ib);
+}
+
+struct BoxArgs { int n_maps, N, max_inst; float inv_box_size; };
+
+__host__ __device__ __forceinline__ void box_write(const BoxArgs& a, int j, int m, const float* r, int valid, float* det_out,
+                                                   int* valid_out) {
+    const long long row = (long long)m * a.n_maps + j;
+    for (int k = 0; k < 4; ++k) det_out[row * 4 + k] = r[k];
+    valid_out[row] = valid;
+}
+
+// One block per map, one thread per box: a usable box's rank is the number of usable boxes before it; the boxes of rank
+// < max_inst are the valid rows.  Rows past the count repeat row 0 (the empty-map record when no box is usable).
+__global__ void __launch_bounds__(G6D_DET_MAX_BOXES) det_from_boxes_kernel(const float* __restrict__ boxes,
+                                                                           const int* __restrict__ counts, const BoxArgs a,
+                                                                           float* det_out, int* valid_out, int* count_out) {
+    __shared__ float sc[G6D_DET_MAX_BOXES];
+    __shared__ int use[G6D_DET_MAX_BOXES];
+    __shared__ float row0[4];
+    const int j = blockIdx.x, b = threadIdx.x;
+    const int n = min(max(counts[j], 0), a.N);
+    float box[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+    bool u = false;
+    if (b < n) {
+        const float* p = boxes + ((long long)j * a.N + b) * 5;
+        for (int k = 0; k < 5; ++k) box[k] = p[k];
+        u = box_usable(box);
+    }
+    sc[b] = box[4];
+    use[b] = u;
+    if (b == 0) { row0[0] = 0.f; row0[1] = 0.f; row0[2] = 1.f; row0[3] = -INFINITY; }
+    const int n_use = __syncthreads_count(u);
+    const int count = min(n_use, a.max_inst);
+    if (u) {
+        int rank = 0;
+        for (int i = 0; i < n; ++i) rank += use[i] && box_before(sc[i], i, box[4], b);
+        if (rank < a.max_inst) {
+            float r[4];
+            box_record(box, a.inv_box_size, r);
+            box_write(a, j, rank, r, 1, det_out, valid_out);
+            if (rank == 0)
+                for (int k = 0; k < 4; ++k) row0[k] = r[k];
+        }
+    }
+    __syncthreads();
+    if (b >= count && b < a.max_inst) box_write(a, j, b, row0, 0, det_out, valid_out);
+    if (b == 0) count_out[j] = count;
+}
+
+// the kernel's records for map j, serially on host memory
+static void det_from_boxes_map_host(const float* boxes, const int* counts, const BoxArgs& a, int j, float* det_out, int* valid_out,
+                                    int* count_out) {
+    const int n = counts[j] < 0 ? 0 : counts[j] > a.N ? a.N : counts[j];
+    const float* bj = boxes + (long long)j * a.N * 5;
+    float row0[4] = {0.f, 0.f, 1.f, -INFINITY};
+    int count = 0;
+    for (int b = 0; b < n; ++b) {
+        if (!box_usable(bj + b * 5)) continue;
+        int rank = 0;
+        for (int i = 0; i < n; ++i) rank += box_usable(bj + i * 5) && box_before(bj[i * 5 + 4], i, bj[b * 5 + 4], b);
+        if (rank >= a.max_inst) continue;
+        float r[4];
+        box_record(bj + b * 5, a.inv_box_size, r);
+        box_write(a, j, rank, r, 1, det_out, valid_out);
+        if (rank == 0)
+            for (int k = 0; k < 4; ++k) row0[k] = r[k];
+        ++count;
+    }
+    for (int m = count; m < a.max_inst; ++m) box_write(a, j, m, row0, 0, det_out, valid_out);
+    count_out[j] = count;
+}
+
+static int det_from_boxes_args(const char* name, const void* boxes, const void* counts, int n_maps, int N, int max_inst,
+                               float inv_box_size, const void* det_out, const void* valid_out, const void* count_out, BoxArgs* a) {
+    G6D_REQUIRE(boxes && counts && det_out && valid_out && count_out, "%s: null pointer", name);
+    G6D_REQUIRE(n_maps > 0, "%s: n_maps=%d must be positive", name, n_maps);
+    G6D_REQUIRE(N >= 1 && N <= G6D_DET_MAX_BOXES, "%s: N=%d outside [1, %d]", name, N, G6D_DET_MAX_BOXES);
+    G6D_REQUIRE(max_inst >= 1 && max_inst <= G6D_DET_MAX_INSTANCES, "%s: max_inst=%d outside [1, %d]", name, max_inst,
+                G6D_DET_MAX_INSTANCES);
+    G6D_REQUIRE(inv_box_size > 0.f && inv_box_size <= 3.0e38f, "%s: inv_box_size=%g must be positive and finite", name,
+                (double)inv_box_size);
+    *a = BoxArgs{n_maps, N, max_inst, inv_box_size};
+    return G6D_OK;
+}
+
 }  // namespace g6d
 
 using namespace g6d;
@@ -545,5 +651,27 @@ extern "C" int g6d_det_parse_peaks_host(const float* scores, const float* scales
                                         nms_iou, box_size, min_score, det_out, idx_out, valid_out, count_out, &a);
     if (rc != G6D_OK) return rc;
     for (int j = 0; j < n_maps; ++j) det_parse_peaks_map_host(scores, scales, offsets, a, j, det_out, idx_out, valid_out, count_out);
+    return G6D_OK;
+}
+
+extern "C" int g6d_det_from_boxes(const float* boxes, const int* counts, int n_maps, int N, int max_inst, float inv_box_size,
+                                  float* det_out, int* valid_out, int* count_out, g6d_stream_t stream) {
+    BoxArgs a;
+    const int rc = det_from_boxes_args("g6d_det_from_boxes", boxes, counts, n_maps, N, max_inst, inv_box_size, det_out, valid_out,
+                                       count_out, &a);
+    if (rc != G6D_OK) return rc;
+    const int threads = (max(N, max_inst) + 31) / 32 * 32;
+    det_from_boxes_kernel<<<n_maps, threads, 0, as_stream(stream)>>>(boxes, counts, a, det_out, valid_out, count_out);
+    G6D_CHECK_LAUNCH("g6d_det_from_boxes");
+    return G6D_OK;
+}
+
+extern "C" int g6d_det_from_boxes_host(const float* boxes, const int* counts, int n_maps, int N, int max_inst, float inv_box_size,
+                                       float* det_out, int* valid_out, int* count_out) {
+    BoxArgs a;
+    const int rc = det_from_boxes_args("g6d_det_from_boxes_host", boxes, counts, n_maps, N, max_inst, inv_box_size, det_out,
+                                       valid_out, count_out, &a);
+    if (rc != G6D_OK) return rc;
+    for (int j = 0; j < n_maps; ++j) det_from_boxes_map_host(boxes, counts, a, j, det_out, valid_out, count_out);
     return G6D_OK;
 }

@@ -12,6 +12,7 @@ import numpy as np
 import torch
 import yaml
 
+from . import boxes as B
 from . import frames as F
 from . import geometry as G
 from . import glue
@@ -145,7 +146,7 @@ class Gen6DEstimator:
         return pose, inter
 
 
-    def predict_batch(self, que_imgs, que_Ks, pose_inits=None):
+    def predict_batch(self, que_imgs, que_Ks, pose_inits=None, boxes=None):
         """predict() for a batch of independent frames (row f3): qn frames go through ONE
         detect stage, ONE select stage and ONE refine stage per iteration -- 2 + refine_iter graph launches
         and device->host reads for the whole batch instead of per frame -- with the small per-frame camera
@@ -155,7 +156,16 @@ class Gen6DEstimator:
         On the device-glue path que_imgs may instead be device frames (row f14; frames.as_frames): CUDA uint8 RGB tensors
         [h,w,3] with any row pitch (or one [qn,h,w,3] tensor) and frames.NV12 decoder surfaces, mixed freely, with the
         numpy path's results on the same RGB bytes.  They must be ready on the current stream; the call ends in its
-        synchronising read, after which they may be overwritten or freed."""
+        synchronising read, after which they may be overwritten or freed.
+
+        boxes (row f19): the object's box on every frame from another detector, exactly one per frame ([4] x0, y0, x1, y1
+        or [5] with a score, or [1, 4|5]; numpy or CUDA float32, in the frame's pixels; gen6d_b200/boxes.py).  The
+        detector does not run: the call is predict_instances(max_instances=1, boxes=) with its [:, 0] rows, and inter
+        also holds 'det_score' [qn], the box scores.  Needs the device pipeline, and pose_inits None.  Numpy boxes are
+        checked on the host (ValueError when non-finite or degenerate); a CUDA box is not read, and one that is not
+        usable gives the empty detection record (position (0, 0), scale 1, det_score -inf), whose pose is meaningless."""
+        if boxes is not None:
+            return self._predict_batch_boxes(que_imgs, que_Ks, pose_inits, boxes)
         qn, res = len(que_imgs), self.cfg['ref_resolution']
         que_Ks = [np.asarray(K) for K in que_Ks]
         device = self.cfg['device_glue'] and pose_inits is None and self._glue_possible()
@@ -185,6 +195,19 @@ class Gen6DEstimator:
         if self.refiner is not None:
             poses, inter['refine_poses'] = self._refine_batch_host(frames, que_Ks, poses, self.cfg['refine_iter'])
         return poses, inter
+
+    def _predict_batch_boxes(self, que_imgs, que_Ks, pose_inits, boxes):
+        """predict_batch(boxes=): predict_instances(max_instances=1, boxes=) in predict_batch's return contract."""
+        from .objects import require_device_pipeline
+        require_device_pipeline(self, 'predict_batch(boxes=)')
+        if pose_inits is not None:
+            raise ValueError('predict_batch: boxes= detects the initial poses; pass boxes or pose_inits, not both')
+        poses, inter = self.predict_instances(que_imgs, que_Ks, max_instances=1,
+                                              boxes=B.one_per_frame(boxes, len(que_imgs), 'predict_batch'))
+        keys = ('det_position', 'det_scale_r2q', 'det_score', 'det_que_img', 'sel_angle_r2q', 'sel_scores', 'sel_ref_idx')
+        one = {k: np.ascontiguousarray(inter[k][:, 0]) for k in keys}
+        one['refine_poses'] = [np.ascontiguousarray(c[:, 0]) for c in inter['refine_poses']]
+        return np.ascontiguousarray(poses[:, 0]), one
 
     def _refine_batch_host(self, frames, que_Ks, poses, iters):
         """`iters` host-sequenced batched refinements from poses [qn,3,4] -> (poses, [poses, refined 1, ..., refined iters])."""
@@ -300,11 +323,12 @@ class Gen6DEstimator:
         return (refined[-1] if refined else poses0), inter
 
     # ------------------------------------------------------------------ several instances per frame (instances.py)
-    def _instances_fn(self, st, M, radius, nms_iou, min_score):
+    def _instances_fn(self, st, M, radius, nms_iou, min_score, boxes=None):
         """frames u8 [qn,h,w,3], cams f64 [qn,20] -> packed results of predict_instances: the detector's maps, the peaks,
-        M*qn crops and selections, and refine_iter x (glue over M slots, ONE refiner stage over M*qn poses, glue)."""
+        M*qn crops and selections, and refine_iter x (glue over M slots, ONE refiner stage over M*qn poses, glue).
+        boxes: a boxes.Detect, the detection step from caller boxes instead of the maps and peaks."""
         iters, R = self.cfg['refine_iter'], st['tables']['ref_num']
-        detect, extra = self._peaks_detect_fn(M, radius, nms_iou, min_score)
+        detect, extra = (boxes, boxes.extra) if boxes is not None else self._peaks_detect_fn(M, radius, nms_iou, min_score)
         initial, refine = self._initial_poses_device_fn(st, detect), self.refiner._refine_warped(128)
         views = [st['views']] * M
 
@@ -319,7 +343,7 @@ class Gen6DEstimator:
             return instances.pack([torch.stack(chain, 0), det, idx, sel_out, logits] + extra, crop)
         return fn
 
-    def predict_instances(self, que_imgs, que_Ks, max_instances=4, min_score=None, nms_iou=0.3, peak_radius=1):
+    def predict_instances(self, que_imgs, que_Ks, max_instances=4, min_score=None, nms_iou=0.3, peak_radius=1, boxes=None):
         """Every instance of the object on qn frames (of one size or several, row f13): up to `max_instances` detections per frame, the peaks of
         the detector's score map (within `peak_radius` cells) kept by greedy non-maximum suppression of their
         ref_resolution * scale boxes at IoU > `nms_iou` (g6d_det_parse_peaks), each selected and refined as predict_batch
@@ -329,7 +353,17 @@ class Gen6DEstimator:
         predict_batch's detection.  Rows of instances that were not found are computed too (on a repeat of instance 0's
         detection, so the graph keeps its shapes) and returned, masked by instance_valid: use only the valid rows.
         One captured graph per (qn, frame shape, max_instances, peak_radius, nms_iou, min_score), one read per call.
-        que_imgs may be device frames, with predict_batch's rules (row f14)."""
+        que_imgs may be device frames, with predict_batch's rules (row f14).
+
+        boxes (row f19): the instances from another detector instead of the score map, one entry per frame: a numpy array
+        or CUDA float32 tensor [n, 4] (x0, y0, x1, y1) or [n, 5] (with a score), n >= 0, in the frame's pixels (a Resized
+        frame's working pixels); gen6d_b200/boxes.py.  The detector runs no kernel: g6d_det_from_boxes makes instance m
+        of a frame its m-th usable box by score (the square on the box's longer side, so scale = side / ref_resolution),
+        at most max_instances, and everything after the detection is unchanged.  det_score holds the box scores (0 for
+        [n, 4]), instance_valid / instance_count the boxes kept.  min_score, nms_iou and peak_radius do not apply to boxes
+        (the caller's detector thresholds and suppresses) and are not part of the box graphs' key: one graph per (qn,
+        frame shape, max_instances, box bucket N), N the next power of two of the longest list.  CUDA boxes must be
+        ready on the current stream."""
         from .objects import require_device_pipeline
         require_device_pipeline(self, 'predict_instances')
         key = instances.check_args(max_instances, nms_iou, peak_radius, min_score)
@@ -340,12 +374,19 @@ class Gen6DEstimator:
         imgs = F.as_frames(que_imgs, 'predict_instances', self.detector)
         if F.is_mixed(imgs):
             F.check_frames(imgs, que_Ks, 'predict_instances')
+        table = None if boxes is None else B.for_frames(boxes, qn, 'predict_instances', self.detector.device)
         st = self._glue_state()
         det = self.detector
         with torch.no_grad():
-            name, fn, fin = F.stage(det, ('instances',) + key, self._instances_fn(st, *key), imgs)
+            if table is None:
+                name, fn, tail = ('instances',) + key, self._instances_fn(st, *key), []
+            else:
+                dt = B.Detect(M, 1, qn, table.N, B.inv_box_size(res))
+                name, fn = B.graph_name(('instances', M), table.N), dt.bind(self._instances_fn(st, *key, boxes=dt))
+                tail = [table.upload(det)]
+            name, fn, fin = F.stage(det, name, fn, imgs)
             cams = det._to_dev(glue.cameras(np.stack([np.asarray(K) for K in que_Ks], 0)))
-            buf = self.stages.run(name, fn, fin + [cams])
+            buf = self.stages.run(name, fn, fin + [cams] + tail)
             host = det._to_host(buf)                                       # the call's one synchronising read
         n, n_sel = M * qn, len(self.ref_info['poses'])
         rd = instances.Unpacker(host, n * res * res * 3)
@@ -361,7 +402,8 @@ class Gen6DEstimator:
         predict.py's --num / --std).  bbox_3d: the object's 8 box corners [8,3]; None: from the database's point cloud.
         draw: 'raw', 'smoothed' or ('raw', 'smoothed'): every step also draws predict.py's images_out /
         images_out_smooth frames on the device, the box edges in draw_color (R, G, B) (Tracker.step, row f16).
-        cfg['refine_iter'] is left untouched."""
+        cfg['refine_iter'] is left untouched.  To start from another detector's boxes, pose the first frames with
+        predict_batch(boxes=) and pass those poses to the tracker's start(poses, sequences)."""
         from .track import Tracker
         return Tracker(self, num_sequences, refine_iter=refine_iter, smooth_num=smooth_num, smooth_std=smooth_std,
                        bbox_3d=bbox_3d, draw=draw, draw_color=draw_color)

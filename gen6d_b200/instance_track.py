@@ -37,11 +37,19 @@ its re-detecting sequences, d = 0 replays the refine body, d = b the re-detectio
 instance step (_mixed_fn): the re-detecting sequences' frames are gathered and detected as a batch of d,
 g6d_instances_associate_sequences associates them and sets up every other pair's refinement, and the iterations past
 refine_iter run one refiner stage over the re-detecting sequences' slots only.
+
+Boxes from another detector (row f19): step(..., boxes=) re-detects from caller boxes instead of the detector.  Their
+records (g6d_det_from_boxes) take the place of the peaks in the same bodies, under graph names of their own
+(boxes.graph_name) with the box buffer as the last graph input.  Lockstep: boxes for every sequence, and the step is a
+re-detection step.  Per-sequence schedules: exactly the stepped sequences given boxes re-detect (the mixed step when only
+some do), and their detection counts in the schedule as a detector detection does; a due sequence without boxes is not
+detected and stays due.
 """
 import numpy as np
 import torch
 
 from . import _lib
+from . import boxes as B
 from . import draw as dr
 from . import frames as fr
 from . import glue
@@ -73,20 +81,24 @@ class Schedule:
         """bool [S]: the sequences that re-detect on their next step."""
         return self.pending | ((self.count >= self.E) if self.E is not None else False)
 
-    def plan(self, seqs, n_real):
+    def plan(self, seqs, n_real, hit=None):
         """The stepped batch seqs [b] (its first n_real rows real, the rest padding) -> (det_seq bool [b], kind): the rows
         that re-detect (padding never does, so it spawns no ids) and the body the step runs ('refine': none, 'detect':
-        every row, else 'mixed')."""
-        det_seq = self.due()[seqs]
+        every row, else 'mixed').  hit bool [b]: the rows that re-detect whether due or not (a step with boxes: the rows
+        given boxes); None: the due rows."""
+        det_seq = self.due()[seqs] if hit is None else np.array(hit, bool)
         det_seq[n_real:] = False
         m = int(det_seq.sum())
         return det_seq, 'refine' if m == 0 else 'detect' if m == len(seqs) else 'mixed'
 
-    def advance(self, stepped):
-        """The counters after a step of the distinct sequences `stepped`."""
-        hit, restart = self.due()[stepped], self.pending[stepped]
+    def advance(self, stepped, hit=None):
+        """The counters after a step of the distinct sequences `stepped`, of which those in hit (bool, aligned; None: the
+        due ones) re-detected.  A sequence that re-detected counts as a detection; any other, due or not, as a step
+        without one (a due sequence stays due)."""
+        hit = self.due()[stepped] if hit is None else np.asarray(hit, bool)
+        restart = self.pending[stepped] & hit
         self.count[stepped] = np.where(hit, np.where(restart, 1 + self.phase[stepped], 1), self.count[stepped] + 1)
-        self.pending[stepped] = False
+        self.pending[stepped[hit]] = False
 
 
 def plan_mixed(det_seq, plan):
@@ -346,10 +358,11 @@ class InstanceTracker:
         """-> (the refiner's view table of every slot group, the reference views per table)."""
         return [st['views']] * self.M, st['tables']['ref_num']
 
-    def _detection(self, st):
+    def _detection(self, st, boxes=None):
         """-> fn(frames, cams) -> (initial poses [n,12], det [n,4], crops, the selections' tensors in packing order, valid
-        int32 [n], instance count int32 [K*S]): predict_instances' detection half on the S frames."""
-        detect, extra = self.est._peaks_detect_fn(*self.key)
+        int32 [n], instance count int32 [K*S]): predict_instances' detection half on the S frames (boxes: a boxes.Detect,
+        the detection from caller boxes)."""
+        detect, extra = (boxes, boxes.extra) if boxes is not None else self.est._peaks_detect_fn(*self.key)
         initial = self.est._initial_poses_device_fn(st, detect)
 
         def fn(frames, cams):
@@ -370,12 +383,13 @@ class InstanceTracker:
         return [(rd.take(n), rd.take(n * 2), rd.take(n * len(self.est.ref_info['poses'])))]
 
     # -------------------------------------------------------------- the graphs
-    def _detect_fn(self, st, draw=None, S=None):
-        """The re-detection body for S sequences (default: the tracker's; a partial step's compact batch, row f18)."""
+    def _detect_fn(self, st, draw=None, S=None, boxes=None):
+        """The re-detection body for S sequences (default: the tracker's; a partial step's compact batch, row f18); boxes:
+        a boxes.Detect, the detection from caller boxes (row f19)."""
         est, G, S, r = self.est, self.M * self.K, S or self.S, self.refine_iter
         F, c, n = est.cfg['refine_iter'], self._dev, self.M * self.K * S
         views, R = self._groups(st)
-        initial, associate, refine = self._detection(st), self._associate(), est.refiner._refine_warped(128)
+        initial, associate, refine = self._detection(st, boxes), self._associate(), est.refiner._refine_warped(128)
 
         def fn(frames, cams, prev, park, live, ids, misses, next_id, ring, count, *dt):
             init, det, crop, sels, valid, inst_count = initial(frames, cams)
@@ -428,17 +442,20 @@ class InstanceTracker:
             return buf, poses, ring, count
         return fn
 
-    def _mixed_fn(self, st, S, d, blocks=None, draw=None):
+    def _mixed_fn(self, st, S, d, blocks=None, draw=None, boxes=None):
         """The mixed instance step's body for S sequences of which some re-detect, their frames gathered into a batch of
-        d (blocks: per size group of frames of several sizes, as _size_buckets makes them)."""
+        d (blocks: per size group of frames of several sizes, as _size_buckets makes them; boxes: a boxes.Detect over the
+        S sequences' maps, gathered like the frames)."""
         est, G, r = self.est, self.M * self.K, self.refine_iter
         F, c, n = est.cfg['refine_iter'], self._dev, self.M * self.K * S
         views, R = self._groups(st)
-        initial, refine = self._detection(st), est.refiner._refine_warped(128)
+        initial, refine = self._detection(st, boxes), est.refiner._refine_warped(128)
         ref_res = float(est.cfg['ref_resolution'])
 
         def fn(frames, cams, prev, park, live, ids, misses, next_id, ring, count, seq, det_index, *dt):
             gf, gc = frames.index_select(0, seq), cams.index_select(0, seq)
+            if boxes is not None:
+                boxes.select(seq)
             if blocks is None:
                 init, det, crop, sels, valid, inst_count = initial(gf, gc)
             else:
@@ -469,13 +486,13 @@ class InstanceTracker:
             return buf, poses, park, live, ids, misses, next_id, ring, count
         return fn
 
-    def _body(self, st, kind, S, d=None, blocks=None, draw=None):
+    def _body(self, st, kind, S, d=None, blocks=None, draw=None, boxes=None):
         """A per-sequence step's body on the whole slot state: fn(frames, cams, prev, park, live, ids, misses, next_id, ring,
         count, *rest) -> (buf, prev, park, live, ids, misses, next_id, ring, count), kind 'detect', 'refine' or 'mixed'."""
         if kind == 'detect':
-            return self._detect_fn(st, draw, S)
+            return self._detect_fn(st, draw, S, boxes)
         if kind == 'mixed':
-            return self._mixed_fn(st, S, d, blocks, draw)
+            return self._mixed_fn(st, S, d, blocks, draw, boxes)
         refine = self._refine_fn(st, draw, S)
 
         def fn(frames, cams, prev, park, live, ids, misses, next_id, ring, count, *dt):
@@ -484,7 +501,7 @@ class InstanceTracker:
         return fn
 
     # -------------------------------------------------------------- one step
-    def step(self, frames, Ks, out=None, sequences=None):
+    def step(self, frames, Ks, out=None, sequences=None, boxes=None):
         """frames: S uint8 [h,w,3] (of one size or several, row f13; or device frames, row f14, as Tracker.step takes them);
         Ks: [S,3,3]; out: drawing destinations as Tracker.step takes them (a tracker made with draw= draws every live slot
         of a sequence on its frame, in slot order; without out= inter['drawn'] holds tracker-owned frames).  Returns (poses float32 [S,M,3,4], smoothed float64 [S,M,3,4],
@@ -498,14 +515,22 @@ class InstanceTracker:
         any did, the re-detection keys cover every row, the others' filled with NaN, -1, False / 0 and zero crops, and
         refine_poses has max(cfg['refine_iter'], refine_iter) + 1 entries.  sequences: step only these sequences, with
         Tracker.step's contract (row f17): one frame, K and out= destination each, in any order; results in that order
-        with inter['sequences']; the others are not computed and keep their state and out= buffers."""
-        return self._step(frames, Ks, out, sequences)[0]
+        with inter['sequences']; the others are not computed and keep their state and out= buffers.
 
-    def _step(self, frames, Ks, out=None, sequences=None):
+        boxes (row f19): re-detect from another detector's boxes instead of running the detector, one entry per stepped
+        sequence (in sequences= order, else 0..S-1): the boxes Gen6DEstimator.predict_instances(boxes=) takes for a frame
+        ([n, 4|5], n >= 0), or None for none.  The boxes' records go through the same association and refinement as a
+        detection; the detector runs no kernel.  Lockstep: every entry must be an array (an empty one: no detections),
+        and the step is a re-detection step that restarts the re-detection count.  Per-sequence schedules: exactly the
+        sequences given an array re-detect, and each counts as re-detected; a due sequence given None is not detected
+        and stays due (detecting()).  So redetect_every=None with boxes on the first step never runs the detector."""
+        return self._step(frames, Ks, out, sequences, boxes)[0]
+
+    def _step(self, frames, Ks, out=None, sequences=None, boxes=None):
         """One step -> the decoded results of every object, in object order."""
         self._check()
         if self.schedule != 'lockstep':
-            return self._step_sequences(frames, Ks, out, sequences)
+            return self._step_sequences(frames, Ks, out, sequences, boxes)
         if sequences is not None:
             raise ValueError("step: sequences= needs schedule='per_sequence' or 'staggered'; a lockstep tracker's "
                              're-detection schedule is tracker-wide')
@@ -515,15 +540,26 @@ class InstanceTracker:
         Ks = np.stack([np.asarray(k) for k in Ks], 0)
         if Ks.shape != (S, 3, 3):
             raise ValueError(f'step: Ks must be [{S},3,3], got {Ks.shape}')
-        detecting = self._detecting()
-        res = self._run(frames, Ks, out, 'detect' if detecting else 'refine')
+        table = None
+        if boxes is not None:
+            table, has = self._boxes(boxes, S)
+            if not has.all():
+                raise ValueError(f'step: a lockstep step with boxes re-detects every sequence; sequences '
+                                 f'{np.flatnonzero(~has).tolist()} have None (pass an empty [0, 4] array for no detections)')
+        detecting = table is not None or self._detecting()
+        res = self._run(frames, Ks, out, 'detect' if detecting else 'refine', boxes=table)
         self._pending = False
         self._since = 1 if detecting else self._since + 1
         return res
 
-    def _run(self, frames, Ks, out, kind, part=None, det_seq=None):
+    def _boxes(self, boxes, n):
+        """A step's boxes for n stepped sequences -> (boxes.Table of their maps, has bool [n])."""
+        return B.for_sequences(boxes, n, 'step', self.est.detector.device)
+
+    def _run(self, frames, Ks, out, kind, part=None, det_seq=None, boxes=None):
         """One step's graph and read -> decoded results.  kind: 'detect', 'refine' or 'mixed'; part: a partial step (row
-        f17/f18) over its compact batch; det_seq: bool over the batch's sequences, those that re-detect (kind 'mixed')."""
+        f17/f18) over its compact batch; det_seq: bool over the batch's sequences, those that re-detect (kind 'mixed');
+        boxes: a boxes.Table of the batch's maps, the detection of a 'detect' or 'mixed' step (row f19)."""
         est = self.est
         S = self.S if part is None else part.b
         F = est.cfg['refine_iter']
@@ -538,16 +574,22 @@ class InstanceTracker:
         draw, dt, drawn, named = draw_inputs(drawer, est.detector, plan, out, None if part is None else part.a)
         dev = est.detector.device
         det_rows, extra, D = None, [], S
+        dbox = tail = None
+        if boxes is not None and kind != 'refine':
+            dbox = B.Detect(self.M, self.K, boxes.n_maps, boxes.N, B.inv_box_size(est.cfg['ref_resolution']))
+            tail = [boxes.upload(est.detector)]
         if kind == 'mixed':
             seq, blocks, det_rows, D, key = plan_mixed(det_seq, plan)
             up = lambda a, dt_: torch.from_numpy(np.ascontiguousarray(a, dt_)).to(dev)
             extra = [up(seq, np.int64), up(det_rows, np.int32)]
-            base, fn = mixed_name(S, key), self._body(stt, 'mixed', S, D, blocks, draw)
+            base, fn = mixed_name(S, key), self._body(stt, 'mixed', S, D, blocks, draw, dbox)
         elif part is None:
             base = kind
-            fn = self._detect_fn(stt, draw) if kind == 'detect' else self._refine_fn(stt, draw)
+            fn = self._detect_fn(stt, draw, boxes=dbox) if kind == 'detect' else self._refine_fn(stt, draw)
         else:
-            base, fn = kind, self._body(stt, kind, S, draw=draw)
+            base, fn = kind, self._body(stt, kind, S, draw=draw, boxes=dbox)
+        if dbox is not None:
+            base, fn = B.graph_name(base, boxes.N), dbox.bind(fn)
         if part is not None:
             base = part.name(base)
             fn = _compact_state_fn(fn)
@@ -560,7 +602,7 @@ class InstanceTracker:
                 buf, poses, ring, count = outs
             else:
                 outs = self.stages.run(name, fn, fin + [cams, x['prev'], x['park'], x['live'], x['ids'], x['misses'], self._next_id,
-                                                        x['ring'], x['count']] + extra + dt)
+                                                        x['ring'], x['count']] + extra + dt + (tail or []))
                 buf, poses, park, live, ids, misses, next_id, ring, count = outs
                 for k, v in (('park', park), ('live', live), ('ids', ids), ('misses', misses)):
                     x[k].copy_(v)
@@ -575,8 +617,9 @@ class InstanceTracker:
                 r[3]['drawn'] = drawn
         return res
 
-    def _step_sequences(self, frames, Ks, out, sequences):
-        """A step on a per-sequence schedule (row f18): the stepped sequences' plan, one graph, their counters."""
+    def _step_sequences(self, frames, Ks, out, sequences, boxes=None):
+        """A step on a per-sequence schedule (row f18): the stepped sequences' plan, one graph, their counters.  boxes (row
+        f19): per stepped sequence an array or None; the sequences with an array re-detect, from them."""
         S, sch = self.S, self._schedule
         part = None
         if sequences is not None:
@@ -586,16 +629,24 @@ class InstanceTracker:
                 raise ValueError('step: out= names drawing destinations; create the tracker with draw=')
             frames, Ks, out = part.compact(frames), part.compact(Ks), part.compact_out(out)
             seqs, n_real = part.seq, part.a
+            if boxes is not None:
+                B.check_len(boxes, n_real, 'step', 'stepped sequence')
+                boxes = part.compact(list(boxes))[:n_real] + [None] * (part.b - n_real)       # padding rows never detect
         else:
             if len(frames) != S or len(Ks) != S:
                 raise ValueError(f'step: this tracker follows {S} sequences, got {len(frames)} frames and {len(Ks)} Ks')
             seqs, n_real = np.arange(S), S
+            if boxes is not None:
+                B.check_len(boxes, S, 'step', 'stepped sequence')
         Ks = np.stack([np.asarray(k) for k in Ks], 0)
         if Ks.shape != (len(seqs), 3, 3):
             raise ValueError(f'step: Ks must be [{len(seqs)},3,3], got {Ks.shape}')
-        det_seq, kind = sch.plan(seqs, n_real)
-        res = self._run(frames, Ks, out, kind, None if part is None or part.lockstep else part, det_seq)
-        sch.advance(seqs[:n_real])
+        table = hit = None
+        if boxes is not None:
+            table, hit = self._boxes(boxes, len(seqs))
+        det_seq, kind = sch.plan(seqs, n_real, hit)
+        res = self._run(frames, Ks, out, kind, None if part is None or part.lockstep else part, det_seq, table)
+        sch.advance(seqs[:n_real], det_seq[:n_real])
         for r in res:
             r[3]['detected'] = det_seq.copy()
         if part is None:
@@ -738,8 +789,8 @@ class ObjectInstanceTracker(InstanceTracker):
         objs = list(self.objs._objects.values())
         return [ob.tables['views'] for ob in objs] * self.M, objs[0].tables['tables']['ref_num']
 
-    def _detection(self, st):
-        detect, extra = self.objs._peaks_detect_fn(*self.key)
+    def _detection(self, st, boxes=None):
+        detect, extra = (boxes, boxes.extra) if boxes is not None else self.objs._peaks_detect_fn(*self.key)
         initial = self.objs._initial_poses_device_fn(detect)
 
         def fn(frames, cams):
@@ -753,16 +804,21 @@ class ObjectInstanceTracker(InstanceTracker):
             det, valid, init, cams, centers, float(est.cfg['ref_resolution']), self.gate, self.max_misses, est.cfg['refine_iter'],
             self.refine_iter, *state)
 
+    def _boxes(self, boxes, n):
+        return B.for_sequences(boxes, n, 'step', self.est.detector.device, self.names)
+
     def _take_selections(self, rd, S):
         M, K = self.M, self.K
         n_sel = [len(ob.ref_info['poses']) for ob in self.objs._objects.values()]
         slots = [(rd.take(S), rd.take(S * 2), rd.take(S * n_sel[g % K])) for g in range(M * K)]
         return [tuple(np.concatenate([slots[m * K + o][i] for m in range(M)]) for i in range(3)) for o in range(K)]
 
-    def step(self, frames, Ks, out=None, sequences=None):
+    def step(self, frames, Ks, out=None, sequences=None, boxes=None):
         """frames: S uint8 [h,w,3] (of one size or several, row f13; or device frames, row f14); Ks: [S,3,3] (shared by all
         objects); out: drawing destinations as InstanceTracker.step takes them, every live slot of every object drawn.  Returns {name: (poses float32
         [S,M,3,4], smoothed float64 [S,M,3,4], track_ids int64 [S,M], inter)}: per object what InstanceTracker.step returns,
         'det_score' included on a re-detection step; 'dropped' lists that object's ids only.  Ids are unique over every
-        object of the tracker.  sequences (per-sequence schedules, row f18): step only these, as InstanceTracker.step."""
-        return dict(zip(self.names, self._step(frames, Ks, out, sequences)))
+        object of the tracker.  sequences (per-sequence schedules, row f18): step only these, as InstanceTracker.step.
+        boxes (row f19): as InstanceTracker.step takes them, each entry a dict {object name: boxes} (an object missing from
+        it has no boxes on that frame) or None."""
+        return dict(zip(self.names, self._step(frames, Ks, out, sequences, boxes)))

@@ -19,6 +19,7 @@ each (gen6d_b200/instance_track.py ObjectInstanceTracker).
 import numpy as np
 import torch
 
+from . import boxes as B
 from . import frames as F
 from . import glue
 from . import instances
@@ -263,10 +264,11 @@ class ObjectSet:
             out[name] = (refined[-1] if refined else chain[0].copy(), inter)
         return out
 
-    def _instances_fn(self, M, radius, nms_iou, min_score):
+    def _instances_fn(self, M, radius, nms_iou, min_score, boxes=None):
         """frames u8 [qn,h,w,3], cams f64 [qn,20] -> packed results of predict_instances (the M*K slots' chain, detections,
-        per-slot selections, the peak masks and counts, then the crops)."""
-        detect, extra = self._peaks_detect_fn(M, radius, nms_iou, min_score)
+        per-slot selections, the peak masks and counts, then the crops).  boxes: a boxes.Detect, the detection step from
+        caller boxes instead of the maps and peaks."""
+        detect, extra = (boxes, boxes.extra) if boxes is not None else self._peaks_detect_fn(M, radius, nms_iou, min_score)
         stages = self._predict_device_fn(detect, M)
 
         def fn(frames, cams):
@@ -274,13 +276,17 @@ class ObjectSet:
             return instances.pack([chain, det] + [t for sel in sels for t in sel] + extra, crop)
         return fn
 
-    def predict_instances(self, que_imgs, que_Ks, max_instances=4, min_score=None, nms_iou=0.3, peak_radius=1):
+    def predict_instances(self, que_imgs, que_Ks, max_instances=4, min_score=None, nms_iou=0.3, peak_radius=1, boxes=None):
         """Every instance of every object on the same qn frames: Gen6DEstimator.predict_instances for each object of the set,
         with the shared query pyramid and correlation of predict().  Slot (m, o) -- instance m of object o -- goes through
         its own crop and object o's selection; a refinement step over the K*M*qn rows is one refiner stage.  Returns
         {name: (poses [qn,M,3,4], inter)} with predict_instances' keys.  Rows of instances that were not found are computed
         and returned, masked by inter['instance_valid'].  One captured graph per argument set and frame shape, one read.
-        que_imgs may be device frames, with predict_batch's rules (row f14)."""
+        que_imgs may be device frames, with predict_batch's rules (row f14).
+        boxes (row f19): every object's instances from another detector, one dict {object name: boxes} per frame, the
+        boxes as Gen6DEstimator.predict_instances takes them; an object missing from a frame's dict has no boxes there
+        (instance_count 0), and a name not in the set is a ValueError.  The detector runs no kernel; min_score, nms_iou
+        and peak_radius do not apply and are not part of the box graphs' key."""
         self._check()
         key = instances.check_args(max_instances, nms_iou, peak_radius, min_score)
         est = self.est
@@ -292,10 +298,17 @@ class ObjectSet:
         if F.is_mixed(imgs):
             F.check_frames(imgs, que_Ks, 'predict_instances')
         det = est.detector
+        table = None if boxes is None else B.for_objects(boxes, self.names, qn, 'predict_instances', det.device)
         with torch.no_grad():
-            name, fn, fin = F.stage(det, ('instances',) + key, self._instances_fn(*key), imgs)
+            if table is None:
+                name, fn, tail = ('instances',) + key, self._instances_fn(*key), []
+            else:
+                dt = B.Detect(M, K, K * qn, table.N, B.inv_box_size(res))
+                name, fn = B.graph_name(('instances', M), table.N), dt.bind(self._instances_fn(*key, boxes=dt))
+                tail = [table.upload(det)]
+            name, fn, fin = F.stage(det, name, fn, imgs)
             cams = det._to_dev(glue.cameras(np.stack([np.asarray(K_) for K_ in que_Ks], 0)))
-            buf = self.stages.run(name, fn, fin + [cams])
+            buf = self.stages.run(name, fn, fin + [cams] + tail)
             host = det._to_host(buf)                                       # the call's one synchronising read
         S = M * K
         rd = instances.Unpacker(host, S * qn * res * res * 3)

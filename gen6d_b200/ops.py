@@ -847,6 +847,20 @@ def det_parse_peaks(scores, scales, offsets, max_inst, radius=1, nms_iou=0.3, bo
     return det, idx, valid, count
 
 
+def det_from_boxes(boxes, counts, max_inst, inv_box_size):
+    """Detection records from caller boxes (g6d_det_from_boxes): boxes float32 [n_maps,N,5] (x0, y0, x1, y1, score),
+    counts int32 [n_maps] -> instance-major (det [max_inst,n_maps,4] = x,y,scale,score; valid int32 [max_inst,n_maps];
+    count int32 [n_maps]) in det_parse_peaks' layout."""
+    n, N, _ = boxes.shape
+    dev = boxes.device
+    det = torch.empty(max_inst, n, 4, device=dev, dtype=torch.float32)
+    valid = torch.empty(max_inst, n, device=dev, dtype=torch.int32)
+    count = torch.empty(n, device=dev, dtype=torch.int32)
+    _call('g6d_det_from_boxes', _p(boxes), _p(counts, torch.int32), n, N, max_inst, float(inv_box_size), _p(det),
+          _p(valid, torch.int32), _p(count, torch.int32), _stream())
+    return det, valid, count
+
+
 # ------------------------------------------------------------------------------- selector
 def sel_ref_sums(ref):
     """ref [S, P, C] -> (sum, sum of squares) over S, float64 [P, C]."""

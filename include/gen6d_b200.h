@@ -605,6 +605,23 @@ int g6d_det_parse_peaks(const float* scores, const float* scales, const float* o
 int g6d_det_parse_peaks_host(const float* scores, const float* scales, const float* offsets, int n_maps, int hs, int ws,
                              int pool_ratio, int max_inst, int radius, float nms_iou, float box_size, float min_score,
                              float* det_out, long long* idx_out, int* valid_out, int* count_out);
+/* Detections from caller-supplied boxes, in g6d_det_parse_peaks' layout, so another detector's boxes replace the score
+ * maps and peaks.  Map j (one (frame, object) pair, j = o*qn + f) has its own list boxes[j] of N rows (x0, y0, x1, y1,
+ * score), of which the first counts[j] (clamped to [0, N]) are read.  A box is usable when its five values are finite,
+ * x1 > x0 and y1 > y0; others are skipped.  The usable boxes are ordered by score descending, ties to the lower index,
+ * and the first max_inst become instances 0.. of map j, each the record (fp32, round to nearest, never contracted)
+ *   x = (x0 + x1) * 0.5, y = (y0 + y1) * 0.5, scale = max(x1 - x0, y1 - y0) * inv_box_size, score
+ * i.e. the square on the box's longer side, whose side is box_size * scale (inv_box_size = 1 / ref_resolution).  As in
+ * g6d_det_parse_peaks, the valid rows form a prefix, count_out[j] is their number and rows past it repeat row 0 with
+ * valid 0.  A map with no usable box gets row 0 = (0, 0, 1, -inf), valid 0, count 0.  Outputs are instance-major:
+ * det_out [max_inst, n_maps, 4], valid_out [max_inst, n_maps], count_out [n_maps].  1 <= N <= G6D_DET_MAX_BOXES,
+ * 1 <= max_inst <= G6D_DET_MAX_INSTANCES, inv_box_size > 0 and finite.  No workspace, no synchronisation.  The *_host
+ * variant writes the same bytes from host memory. */
+#define G6D_DET_MAX_BOXES 256
+int g6d_det_from_boxes(const float* boxes, const int* counts, int n_maps, int N, int max_inst, float inv_box_size,
+                       float* det_out, int* valid_out, int* count_out, g6d_stream_t stream);
+int g6d_det_from_boxes_host(const float* boxes, const int* counts, int n_maps, int N, int max_inst, float inv_box_size,
+                            float* det_out, int* valid_out, int* count_out);
 
 /* ------------------------------------------------------------------ selector ---------------- */
 /* Load-time sums over the reference stack ref [S, P, C]: sum_s ref and sum_s ref^2, as doubles
