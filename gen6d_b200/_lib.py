@@ -85,6 +85,10 @@ _SIGNATURES = {
     'g6d_glue_refine_problems_rows_host': [C.POINTER(GlueViews), I, I, P, P, I, I, P, P, I, P, P, P, P, P, P, P, P],
     'g6d_glue_apply_refinements_rows': [C.POINTER(GlueViews), I, I, P, P, P, P, P, I, P, P],
     'g6d_glue_apply_refinements_rows_host': [C.POINTER(GlueViews), I, I, P, P, P, P, P, I, P],
+    'g6d_verify_windows': [P, I, C.POINTER(GlueRefs), I, I, P, P, P],
+    'g6d_verify_windows_host': [P, I, C.POINTER(GlueRefs), I, I, P, P],
+    'g6d_verify_judge': [P, P, I, I, D, I, D, I, D, P, P, P],
+    'g6d_verify_judge_host': [P, P, I, I, D, I, D, I, D, P, P],
     'g6d_track_smooth': [P, I, P, P, P, P, I, P, I, P, P, P],
     'g6d_track_smooth_host': [P, I, P, P, P, P, I, P, I, P, P],
     'g6d_track_smooth_objects': [P, I, P, I, I, P, P, P, I, P, P, P, P],

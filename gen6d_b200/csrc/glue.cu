@@ -447,3 +447,94 @@ extern "C" int g6d_glue_apply_refinements_rows_host(const g6d_glue_views* views,
     for (int j = 0; j < n_sel; ++j) do_apply_rows(j, pk, rows_per_obj, row_idx, que_pose, que_K, rect, net_out, poses);
     return G6D_OK;
 }
+
+// ------------------------------------------------------------------------------------------ verification windows
+namespace g6d {
+struct GlueRefsPack {                  // by value: the objects' selector references of one launch
+    g6d_glue_refs r[G6D_GLUE_MAX_OBJECTS];
+};
+
+// row i = o * rows_per_obj + s: object o's pose on frame s
+G6D_HD void do_verify_window(int i, const GlueRefsPack& pk, int rows_per_obj, const g6d_glue_camera* cams, const double* poses,
+                             int in_f32, float* rec) {
+    const g6d_glue_refs& r = pk.r[i / rows_per_obj];
+    const g6d_glue_camera& c = cams[i % rows_per_obj];
+    window_from_pose(poses + (long long)i * 12, in_f32, r.center, c.K, c.Kinv, c.f, c.f_sq, r.dist[0], r.f[0], rec + (long long)i * 4);
+}
+
+__global__ void verify_windows_kernel(const GlueRefsPack pk, int rows_per_obj, const g6d_glue_camera* cams, const double* poses,
+                                      int in_f32, int n, float* rec) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) do_verify_window(i, pk, rows_per_obj, cams, poses, in_f32, rec);
+}
+
+__global__ void verify_judge_kernel(const float* rec, const float* det, int n, int window, double ref_resolution, int use_score,
+                                    double lost_score, int use_gate, double lost_gate, float* out, int* lost) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n)
+        lost[i] = verify_judge(rec + i * 4, det + i * 4, window, ref_resolution, use_score, lost_score, use_gate, lost_gate, out + i * 5);
+}
+
+static int verify_refs_ok(const char* name, const g6d_glue_refs* refs, int n_obj, int rows_per_obj, GlueRefsPack* pk) {
+    G6D_REQUIRE(refs, "%s: null refs", name);
+    G6D_REQUIRE(n_obj >= 1 && n_obj <= G6D_GLUE_MAX_OBJECTS, "%s: need 1 <= n_obj <= %d (got n_obj=%d)", name, G6D_GLUE_MAX_OBJECTS, n_obj);
+    G6D_REQUIRE(rows_per_obj >= 1, "%s: need rows_per_obj >= 1 (got %d)", name, rows_per_obj);
+    for (int o = 0; o < n_obj; ++o) {
+        G6D_REQUIRE(refs[o].f && refs[o].dist, "%s: object %d has no reference distances (f, dist)", name, o);
+        pk->r[o] = refs[o];
+    }
+    return G6D_OK;
+}
+
+static int judge_ok(const char* name, const float* rec, const float* det, int n, int window, double ref_resolution, int use_score,
+                    double lost_score, int use_gate, double lost_gate, const float* out, const int* lost) {
+    G6D_REQUIRE(rec && det && out && lost && n >= 1, "%s: bad args", name);
+    G6D_REQUIRE(window > 0 && ref_resolution > 0, "%s: need window > 0 and ref_resolution > 0 (got %d, %g)", name, window, ref_resolution);
+    G6D_REQUIRE(!use_score || lost_score == lost_score, "%s: lost_score is NaN", name);
+    G6D_REQUIRE(!use_gate || lost_gate == lost_gate, "%s: lost_gate is NaN", name);
+    return G6D_OK;
+}
+}  // namespace g6d
+
+extern "C" int g6d_verify_windows(const double* poses, int poses_are_f32, const g6d_glue_refs* refs, int n_obj, int rows_per_obj,
+                                  const g6d_glue_camera* cams, float* rec, g6d_stream_t stream) {
+    const char* name = "g6d_verify_windows";
+    GlueRefsPack pk;
+    const int rc = verify_refs_ok(name, refs, n_obj, rows_per_obj, &pk);
+    if (rc != G6D_OK) return rc;
+    G6D_REQUIRE(poses && cams && rec, "%s: bad args", name);
+    const int n = n_obj * rows_per_obj;
+    verify_windows_kernel<<<ceil_div(n, 32), 32, 0, as_stream(stream)>>>(pk, rows_per_obj, cams, poses, poses_are_f32, n, rec);
+    G6D_CHECK_LAUNCH(name);
+    return G6D_OK;
+}
+extern "C" int g6d_verify_windows_host(const double* poses, int poses_are_f32, const g6d_glue_refs* refs, int n_obj, int rows_per_obj,
+                                       const g6d_glue_camera* cams, float* rec) {
+    const char* name = "g6d_verify_windows_host";
+    GlueRefsPack pk;
+    const int rc = verify_refs_ok(name, refs, n_obj, rows_per_obj, &pk);
+    if (rc != G6D_OK) return rc;
+    G6D_REQUIRE(poses && cams && rec, "%s: bad args", name);
+    for (int i = 0; i < n_obj * rows_per_obj; ++i) do_verify_window(i, pk, rows_per_obj, cams, poses, poses_are_f32, rec);
+    return G6D_OK;
+}
+
+extern "C" int g6d_verify_judge(const float* rec, const float* det, int n, int window, double ref_resolution, int use_score,
+                                double lost_score, int use_gate, double lost_gate, float* out, int* lost, g6d_stream_t stream) {
+    const char* name = "g6d_verify_judge";
+    const int rc = judge_ok(name, rec, det, n, window, ref_resolution, use_score, lost_score, use_gate, lost_gate, out, lost);
+    if (rc != G6D_OK) return rc;
+    verify_judge_kernel<<<ceil_div(n, 32), 32, 0, as_stream(stream)>>>(rec, det, n, window, ref_resolution, use_score, lost_score,
+                                                                         use_gate, lost_gate, out, lost);
+    G6D_CHECK_LAUNCH(name);
+    return G6D_OK;
+}
+extern "C" int g6d_verify_judge_host(const float* rec, const float* det, int n, int window, double ref_resolution, int use_score,
+                                     double lost_score, int use_gate, double lost_gate, float* out, int* lost) {
+    const char* name = "g6d_verify_judge_host";
+    const int rc = judge_ok(name, rec, det, n, window, ref_resolution, use_score, lost_score, use_gate, lost_gate, out, lost);
+    if (rc != G6D_OK) return rc;
+    for (int i = 0; i < n; ++i)
+        lost[i] = verify_judge(rec + i * 4, det + i * 4, window, ref_resolution, use_score, lost_score, use_gate, lost_gate, out + i * 5);
+    return G6D_OK;
+}

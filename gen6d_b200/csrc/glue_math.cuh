@@ -289,5 +289,57 @@ G6D_HD void apply_refinement(const float* que_pose, const float* que_K, const fl
     }
 }
 
+// ------------------------------------------------------------------------------------------ E: pose -> detection window
+// The inverse of pose_from_similarity for one pose: the detection record (cx, cy, s, 1) that B would have turned into
+// this pose's centre and distance.  c = project_center(center, pose, K); s = ref_dist * que_f_ray / ref_f / que_dist
+// with que_dist = |camera centre - object centre| and que_f_ray computed at c as B computes it.  ref_dist / ref_f is the
+// same for every normalised reference view, so the caller passes row 0's.  in_f32: the pose holds float32 values (as
+// after a refinement) and is read rounded to float32; everything else is float64.  A pose whose centre is not in front
+// of the camera, or whose c or s is not finite in float32, gives the invalid record (0, 0, 1, 0).
+G6D_HD void window_from_pose(const double* pose_in, int in_f32, const double* center, const double* K, const double* Kinv,
+                             double f, double f_sq, double ref_dist, double ref_f, float* rec /* [4] */) {
+    double P[12];
+    for (int i = 0; i < 12; ++i) P[i] = in_f32 ? (double)(float)pose_in[i] : pose_in[i];
+    const double depth = (P[8] * center[0] + P[9] * center[1] + P[10] * center[2]) + P[11];
+    double px, py;
+    project_center(center, P, K, &px, &py);
+    double d[3];
+    for (int i = 0; i < 3; ++i) d[i] = -((P[i] * P[3] + P[4 + i] * P[7]) + P[8 + i] * P[11]) - center[i];
+    const double que_dist = sqrt((d[0] * d[0] + d[1] * d[1]) + d[2] * d[2]);
+    const double v[3] = {px, py, 1.0};
+    double bearing[3];
+    mat3_vec(Kinv, v, bearing);
+    const double bx = bearing[0] / bearing[2], by = bearing[1] / bearing[2];
+    const double n2 = sqrt((bx * f) * (bx * f) + (by * f) * (by * f));
+    const double que_f_ray = sqrt(f_sq + n2 * n2);
+    const double s = ref_dist * que_f_ray / ref_f / que_dist;
+    const float cx = (float)px, cy = (float)py, fs = (float)s;
+    if (depth > 0 && isfinite(cx) && isfinite(cy) && isfinite(fs) && fs > 0.f) {
+        rec[0] = cx; rec[1] = cy; rec[2] = fs; rec[3] = 1.f;
+    } else {
+        rec[0] = 0.f; rec[1] = 0.f; rec[2] = 1.f; rec[3] = 0.f;
+    }
+}
+
+// A detection (x, y, scale, score) in the window of record `rec` (size `window`) mapped back to the frame:
+// out = (cx + (x - window/2) s, cy + (y - window/2) s, scale s, score, offset), offset = |(x, y) - window/2| s /
+// (ref_resolution s), the distance of the detection from the pose's centre in reference sizes.  lost: the record is
+// invalid, or use_score and not score >= lost_score (NaN is lost), or use_gate and not offset <= lost_gate (NaN is
+// lost); both comparisons take the float32 values returned, so a tie with the threshold is kept.
+G6D_HD int verify_judge(const float* rec, const float* det, int window, double ref_resolution, int use_score, double lost_score,
+                        int use_gate, double lost_gate, float* out /* [5] */) {
+    const double cx = rec[0], cy = rec[1], s = rec[2], half = window / 2;
+    const double dx = ((double)det[0] - half) * s, dy = ((double)det[1] - half) * s;
+    out[0] = (float)(cx + dx);
+    out[1] = (float)(cy + dy);
+    out[2] = (float)((double)det[2] * s);
+    out[3] = det[3];
+    out[4] = (float)(sqrt(dx * dx + dy * dy) / (ref_resolution * s));
+    int lost = rec[3] == 0.f;
+    if (use_score && !((double)out[3] >= lost_score)) lost = 1;
+    if (use_gate && !((double)out[4] <= lost_gate)) lost = 1;
+    return lost;
+}
+
 }  // namespace glue
 }  // namespace g6d

@@ -394,8 +394,49 @@ class Gen6DEstimator:
         parts = [rd.take(n * 4), rd.take(n), rd.take(n * 2), rd.take(n * n_sel), rd.take(n), rd.take(qn)]
         return instances.inter_of(chain, *parts, rd.crops.reshape(n, res, res, 3), M, qn)
 
+    # ------------------------------------------------------------------ checking poses with the detector (row f20)
+    def _verify_fn(self, st, key):
+        """The verification nodes (verify.nodes) of this estimator's object."""
+        from . import verify
+        return verify.nodes(self, [st['refs']], [self.detector._detect_u8], key)
+
+    def verify_poses(self, frames, Ks, poses, lost_score=None, lost_gate=None):
+        """Check each pose with the detector on a window around the object (row f20; gen6d_b200/verify.py).  Pose i on
+        frame i (predict_batch's frame forms: numpy, of one size or several, CUDA RGB, frames.NV12, frames.Resized; Ks
+        [n,3,3]; poses [n,3,4], a float32 array read as float32 values, any other dtype as float64) becomes the detection
+        record that would have produced it: its projected object centre and scale.  A 2 x ref_resolution window is cut
+        there (the object at its reference size in the middle), the detector runs on the windows, and its detection is
+        mapped back to the frame.  Returns {'position' [n,2], 'scale' [n], 'score' [n] (the detector's raw score head),
+        'offset' [n] (|position - projected centre| / (ref_resolution * window_scale)), 'lost' bool [n], 'window_center'
+        [n,2], 'window_scale' [n]}.  lost: the pose's centre is not in front of the camera (or not finite), score <
+        lost_score (NaN is lost) or offset > lost_gate; a threshold of None is not applied.  The thresholds' meaning
+        depends on the checkpoint.  One captured graph per (n, frame pattern, pose dtype, thresholds), one read."""
+        from . import verify
+        from .objects import require_device_pipeline
+        require_device_pipeline(self, 'verify_poses')
+        key = verify.check_thresholds(lost_score, lost_gate)
+        poses = np.asarray(poses)
+        n = len(frames)
+        if n == 0 or len(Ks) != n or poses.shape != (n, 3, 4):
+            raise ValueError(f'verify_poses: {n} frames, {len(Ks)} intrinsics and poses {poses.shape}; need one K and one pose '
+                             '[3,4] per frame and at least one frame')
+        f32 = poses.dtype == np.float32
+        imgs = F.as_frames(frames, 'verify_poses', self.detector)
+        if F.is_mixed(imgs):
+            F.check_frames(imgs, Ks, 'verify_poses')
+        st = self._glue_state()
+        det = self.detector
+        nodes = self._verify_fn(st, key)
+        with torch.no_grad():
+            name, fn, fin = F.stage(det, ('verify_poses', int(f32)) + key, lambda u8, cams, p: nodes(u8, cams, p, f32), imgs)
+            cams = det._to_dev(glue.cameras(np.stack([np.asarray(K) for K in Ks], 0)))
+            p = det._to_dev(np.ascontiguousarray(poses, np.float64).reshape(n, 12))
+            host = det._to_host(self.stages.run(name, fn, fin + [cams, p]))      # the call's one synchronising read
+        return verify.decode(host, n)
+
     # ------------------------------------------------------------------ video tracking (predict.py)
-    def tracker(self, num_sequences=1, refine_iter=1, smooth_num=5, smooth_std=2.5, bbox_3d=None, draw=None, draw_color=(0, 0, 255)):
+    def tracker(self, num_sequences=1, refine_iter=1, smooth_num=5, smooth_std=2.5, bbox_3d=None, draw=None, draw_color=(0, 0, 255),
+                verify_every=None, lost_score=None, lost_gate=None):
         """A Tracker for `num_sequences` videos stepped in lockstep (gen6d_b200/track.py): the first step is a full
         prediction with cfg['refine_iter'] refinements, every later step `refine_iter` refinements from the previous
         frame's pose, each followed by predict.py's box smoothing (`smooth_num` frames, `smooth_std`; defaults of
@@ -403,10 +444,16 @@ class Gen6DEstimator:
         draw: 'raw', 'smoothed' or ('raw', 'smoothed'): every step also draws predict.py's images_out /
         images_out_smooth frames on the device, the box edges in draw_color (R, G, B) (Tracker.step, row f16).
         cfg['refine_iter'] is left untouched.  To start from another detector's boxes, pose the first frames with
-        predict_batch(boxes=) and pass those poses to the tracker's start(poses, sequences)."""
+        predict_batch(boxes=) and pass those poses to the tracker's start(poses, sequences).
+        verify_every (row f20; needs the device pipeline): a refine step in which a stepped sequence has taken
+        verify_every refine steps since its last full prediction, start(), reset() or verification also checks every
+        stepped sequence's final pose as verify_poses(lost_score, lost_gate) does, inside the step's graph, and returns
+        the result as inter['verify']; every sequence judged lost is then re-initialised as reset([s]) does.  Thresholds
+        None: verify and report, never reset."""
         from .track import Tracker
         return Tracker(self, num_sequences, refine_iter=refine_iter, smooth_num=smooth_num, smooth_std=smooth_std,
-                       bbox_3d=bbox_3d, draw=draw, draw_color=draw_color)
+                       bbox_3d=bbox_3d, draw=draw, draw_color=draw_color, verify_every=verify_every, lost_score=lost_score,
+                       lost_gate=lost_gate)
 
     def instance_tracker(self, num_sequences=1, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
                          min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bbox_3d=None, draw=None,

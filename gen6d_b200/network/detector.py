@@ -113,11 +113,12 @@ class Detector(PackedModule):
             out.append((ht, wt))
         return out
 
-    def _raw_correlation(self, que01):
-        """The three sliding inner products of detector.py:222-224 for one scale."""
+    def _raw_correlation(self, que01, kernels=None):
+        """The three sliding inner products of detector.py:222-224 for one scale (kernels: another object's
+        DetectorRefs.kernels; default the loaded object's)."""
         feats = self._features(que01)
         out = []
-        for f, pc in zip(feats, self.ref_kernels):
+        for f, pc in zip(feats, kernels or self.ref_kernels):
             y = ops.conv(f, pc, reuse_im2col=True, fold_splits=True)      # persistent kernel, TMA im2col A, the A-reuse kernel's K order
             rows = getattr(pc, 'rows', None)
             out.append(ops.det_corr_rowsum(y, *rows) if rows is not None else y)
@@ -181,9 +182,14 @@ class Detector(PackedModule):
             outs['scores_feats'] = feats
         return outs
 
-    def _detect_u8(self, u8):
-        """uint8 frame(s) on the device -> [qn,4] (x, y, scale, score); one capturable stage."""
-        o = self._detect_nhwc(ops.preprocess_u8(u8, out_c=3, imagenet_norm=False))
+    def _detect_u8(self, u8, refs=None):
+        """uint8 frame(s) on the device -> [qn,4] (x, y, scale, score); one capturable stage.  refs: another object's
+        DetectorRefs (make_refs_u8) to detect instead of the loaded object; the same launches as a detector loaded with it."""
+        que01 = ops.preprocess_u8(u8, out_c=3, imagenet_norm=False)
+        if refs is None:
+            o = self._detect_nhwc(que01)
+        else:
+            o = self._detect_maps(que01, lambda cur: self._raw_correlation(cur, refs.kernels), que01.shape[0], refs.rfn, False)
         out, _ = ops.det_parse(o['score_predict'], o['scale_predict'], o['offset_predict'], self.pool_ratio)
         return out
 

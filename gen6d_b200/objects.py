@@ -16,6 +16,8 @@ a contiguous slice whose row i is frame i, which is the layout the g6d_glue_* ke
 the set's objects through videos (gen6d_b200/track.py ObjectTracker), ObjectSet.instance_tracker() every instance of
 each (gen6d_b200/instance_track.py ObjectInstanceTracker).
 """
+from functools import partial
+
 import numpy as np
 import torch
 
@@ -24,6 +26,7 @@ from . import frames as F
 from . import glue
 from . import instances
 from . import ops
+from . import verify
 from .graphs import StageCache
 
 
@@ -327,15 +330,55 @@ class ObjectSet:
                                            valid[:, o], count[o], crops[:, o].reshape(M * qn, res, res, 3), M, qn)
         return out
 
-    def tracker(self, num_sequences=1, refine_iter=1, smooth_num=5, smooth_std=2.5, bboxes=None, draw=None, draw_colors=None):
+    def _verify_fn(self, key):
+        """The verification nodes (verify.nodes) of the set's objects, each object's windows detected against its own
+        references: the launches of Gen6DEstimator.verify_poses on an estimator built on that object."""
+        objs = list(self._objects.values())
+        det = self.est.detector
+        return verify.nodes(self.est, [ob.tables['refs'] for ob in objs], [partial(det._detect_u8, refs=ob.det) for ob in objs], key)
+
+    def verify_poses(self, que_imgs, que_Ks, poses, lost_score=None, lost_gate=None):
+        """Gen6DEstimator.verify_poses for every object of the set on the same qn frames: poses {name: [qn,3,4]} for every
+        object (one dtype for all) -> {name: verify_poses' dict}.  One captured graph, one read."""
+        self._check()
+        key = verify.check_thresholds(lost_score, lost_gate)
+        est, det = self.est, self.est.detector
+        qn = len(que_imgs)
+        missing, extra = [n for n in self.names if n not in poses], sorted(set(poses) - set(self.names))
+        if missing or extra:
+            raise ValueError(f'verify_poses: need poses for exactly the set\'s objects {self.names}; missing {missing}, unknown {extra}')
+        arrs = [np.asarray(poses[n]) for n in self.names]
+        if qn == 0 or len(que_Ks) != qn or any(a.shape != (qn, 3, 4) for a in arrs):
+            raise ValueError(f'verify_poses: {qn} frames, {len(que_Ks)} intrinsics and poses {[a.shape for a in arrs]}; need one K '
+                             'and, per object, one pose [3,4] per frame, and at least one frame')
+        if len({a.dtype for a in arrs}) != 1:
+            raise ValueError('verify_poses: the objects\' poses have different dtypes; pass one dtype (float32: float32 values)')
+        f32 = arrs[0].dtype == np.float32
+        imgs = F.as_frames(que_imgs, 'verify_poses', det)
+        if F.is_mixed(imgs):
+            F.check_frames(imgs, que_Ks, 'verify_poses')
+        nodes = self._verify_fn(key)
+        with torch.no_grad():
+            name, fn, fin = F.stage(det, ('verify_poses', int(f32)) + key, lambda u8, cams, p: nodes(u8, cams, p, f32), imgs)
+            cams = det._to_dev(glue.cameras(np.stack([np.asarray(K) for K in que_Ks], 0)))
+            p = det._to_dev(np.ascontiguousarray(np.concatenate(arrs, 0), np.float64).reshape(-1, 12))
+            host = det._to_host(self.stages.run(name, fn, fin + [cams, p]))      # the call's one synchronising read
+        res = verify.decode(host, len(arrs) * qn)
+        return {name: {k: v[o * qn:(o + 1) * qn] for k, v in res.items()} for o, name in enumerate(self.names)}
+
+    def tracker(self, num_sequences=1, refine_iter=1, smooth_num=5, smooth_std=2.5, bboxes=None, draw=None, draw_colors=None,
+                verify_every=None, lost_score=None, lost_gate=None):
         """An ObjectTracker (gen6d_b200/track.py): every object of the set followed through `num_sequences` videos in
         lockstep, with Tracker's semantics per object; each step is one captured graph and one synchronising read.
         bboxes: {name: 8 box corners [8,3]}; a missing name takes the box of the object's database point cloud.
         draw / draw_colors {name: (R, G, B)}: every step also draws every object's box on its sequence's frame, as
-        Gen6DEstimator.tracker(draw=) does (row f16)."""
+        Gen6DEstimator.tracker(draw=) does (row f16).  verify_every, lost_score, lost_gate: as for
+        Gen6DEstimator.tracker() (row f20), every object checked against its own references; a sequence is re-initialised
+        if any of its objects is judged lost."""
         from .track import ObjectTracker
         return ObjectTracker(self, num_sequences, refine_iter=refine_iter, smooth_num=smooth_num, smooth_std=smooth_std,
-                             bboxes=bboxes, draw=draw, draw_colors=draw_colors)
+                             bboxes=bboxes, draw=draw, draw_colors=draw_colors, verify_every=verify_every, lost_score=lost_score,
+                             lost_gate=lost_gate)
 
     def instance_tracker(self, num_sequences=1, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
                          min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bboxes=None, draw=None,

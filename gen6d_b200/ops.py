@@ -324,6 +324,32 @@ def glue_apply_refinements_rows(views_structs, rows_per_obj, que_pose, que_K, re
     return poses
 
 
+def verify_windows(refs_structs, cams, poses, poses_are_f32):
+    """K objects' poses float64 [K*qn,12] (object-major, row o*qn + s with refs_structs[o] and cams[s]) -> the detection
+    windows' records float32 [K*qn,4] (cx, cy, s, valid; g6d_verify_windows), one launch per G6D_GLUE_MAX_OBJECTS objects."""
+    K, qn = len(refs_structs), cams.shape[0]
+    if poses.shape != (K * qn, 12):
+        raise ValueError(f'verify_windows: poses {tuple(poses.shape)} for {K} objects x {qn} frames')
+    rec = torch.empty(K * qn, 4, device=poses.device, dtype=torch.float32)
+    for o0, o1 in _object_chunks(K):
+        r = slice(o0 * qn, o1 * qn)
+        refs = (_lib.GlueRefs * (o1 - o0))(*refs_structs[o0:o1])
+        _call('g6d_verify_windows', _p(poses[r], torch.float64), int(poses_are_f32), refs, o1 - o0, qn, _p(cams, torch.float64),
+              _p(rec[r]), _stream())
+    return rec
+
+
+def verify_judge(rec, det, window, ref_resolution, lost_score=None, lost_gate=None):
+    """Window records [n,4] + the detector's records on the windows [n,4] -> (out float32 [n,5] = x, y, scale, score,
+    offset in the frame; lost int32 [n]) (g6d_verify_judge).  A threshold of None is not applied."""
+    n = rec.shape[0]
+    out = torch.empty(n, 5, device=rec.device, dtype=torch.float32)
+    lost = torch.empty(n, device=rec.device, dtype=torch.int32)
+    _call('g6d_verify_judge', _p(rec), _p(det), n, int(window), float(ref_resolution), int(lost_score is not None),
+          float(lost_score or 0.0), int(lost_gate is not None), float(lost_gate or 0.0), _p(out), _p(lost, torch.int32), _stream())
+    return out, lost
+
+
 class DrawSrc(C.Structure):           # g6d_draw_src
     _fields_ = [('offset', C.c_longlong), ('pitch', C.c_longlong), ('rows', C.c_int), ('cols', C.c_int)]
 

@@ -16,6 +16,10 @@ the step after them is the mixed step below, also one graph and one read.
 
 step(..., sequences=[...]) steps a subset of the sequences and leaves the others untouched (the partial step below), so
 streams at different frame rates, or that pause, share one tracker; S is then its capacity.
+
+verify_every (row f20) makes every verify_every-th refine step of a sequence replay the verifying variant of the refine
+graph (gen6d_b200/verify.py): the same body, then the detector on a window around each final pose, in the same read;
+sequences judged lost are re-initialised as reset([s]) does.
 """
 import copy
 
@@ -27,6 +31,7 @@ from . import draw as dr
 from . import frames as fr
 from . import glue
 from . import ops
+from . import verify as V
 from .graphs import StageCache
 
 
@@ -351,6 +356,8 @@ class PartialStep:
                 res[k] = {kind: take(d, pos) for kind, d in v.items()}
             elif k == 'refine_poses':
                 res[k] = [c[pos] for c in v]
+            elif k == 'verify':
+                res[k] = {kk: vv[pos] for kk, vv in v.items()}
             elif 'reinit' in inter and k not in ('bbox_pts', 'smoothed_pts'):
                 res[k] = take(v, range(m))
             else:
@@ -385,12 +392,14 @@ def _compact_fn(fn, full):
 # ------------------------------------------------------------------------------------------ the tracker
 class Tracker:
     """S sequences tracked in lockstep (one frame each per step); see Gen6DEstimator.tracker()."""
+    _verify = V.Schedule()           # no verification (row f20)
 
     def __init__(self, est, num_sequences, refine_iter=1, smooth_num=5, smooth_std=2.5, bbox_3d=None, draw=None,
-                 draw_color=dr.DEFAULT_COLOR):
+                 draw_color=dr.DEFAULT_COLOR, verify_every=None, lost_score=None, lost_gate=None):
         kinds, draw_color = dr.parse_kinds(draw), dr.parse_color(draw_color)
         if int(num_sequences) < 1:
             raise ValueError(f'num_sequences must be >= 1, got {num_sequences}')
+        self._verify = V.Schedule(verify_every, lost_score, lost_gate)
         if int(refine_iter) < 1:
             raise ValueError(f'refine_iter must be >= 1, got {refine_iter}')
         if int(smooth_num) < 1:
@@ -421,6 +430,7 @@ class Tracker:
         and the smoothing histories restart.  sequences: only those sequences are re-initialised at the next step and
         restart their histories; the others keep tracking (that step is the mixed step)."""
         if sequences is None:
+            self._since = np.zeros(self.S, np.int64)  # refine steps since the last verification (row f20)
             self._prev = None                        # float64 previous poses ([S,12] on the device, [S,3,4] on the host)
             self._pending = np.ones(self.S, bool)    # a full prediction at the next step
             self._f32 = np.ones(self.S, bool)        # each row's previous pose holds float32 values
@@ -432,7 +442,9 @@ class Tracker:
         self._restart(seqs)
 
     def _restart(self, seqs):
-        """Restart the smoothing of `seqs`: count 0 and a zero ring, the bytes of a fresh tracker's history."""
+        """Restart the smoothing of `seqs`: count 0 and a zero ring, the bytes of a fresh tracker's history; and their
+        verification counts."""
+        self._since[seqs] = 0
         if len(seqs):
             idx = seqs if isinstance(self._ring, np.ndarray) else torch.from_numpy(seqs).to(self._ring.device)
             self._ring[idx] = 0
@@ -523,7 +535,10 @@ class Tracker:
         its own history); the others are untouched: no computation, their state and pending flags kept as they are.  The
         listed sequences run as a compact batch of _bucket(n, S) sequences (the last repeated as padding), one captured
         graph per bucket, step kind, size pattern and drawing, so results equal those of a tracker of that many
-        sequences.  Listing every sequence is the lockstep step."""
+        sequences.  Listing every sequence is the lockstep step.
+
+        A tracker made with verify_every (row f20) adds inter['verify'] to the refine steps that verify: verify_poses' keys
+        on the step's final poses, in the step's row order; the sequences it judges lost are pending afterwards."""
         self._check()
         part = None
         if sequences is not None:
@@ -541,19 +556,30 @@ class Tracker:
         if self._drawer is not None and not device:
             raise ValueError("drawing (draw=) runs inside the device pipeline's step graph only (cfg['device_glue'] on, "
                              "cfg['host_warps'] off)")
+        if self._verify.every is not None and not device:
+            raise ValueError("verification (verify_every=) runs inside the device pipeline's step graph only "
+                             "(cfg['device_glue'] on, cfg['host_warps'] off)")
         host_path = "tracking with cfg['device_glue'] off or cfg['host_warps'] on"
         imgs = fr.as_frames(frames, 'step', self.est.detector, None if device else host_path)
         if not device:
             fr.require_one_size(frames, host_path)
         elif fr.is_mixed(imgs):
             fr.check_frames(imgs, Ks, 'step')
+        stepped = np.arange(self.S) if part is None else part.seq[:part.a]
+        pending, check = self._pending[stepped].copy(), self._verify.due(kind, self._since[stepped])
         if part is None:
-            res = self._step_device(imgs, Ks, kind, out) if device else self._step_host(frames, Ks, kind)
+            res = self._step_device(imgs, Ks, kind, out, check=check) if device else self._step_host(frames, Ks, kind)
             self._pending[:] = False
-            return res
-        res = self._step_device(imgs, Ks, kind, out, part) if device else self._step_host_partial(frames, Ks, kind, part)
-        self._pending[part.seq] = False
-        return part.results(*res)
+        else:
+            res = self._step_device(imgs, Ks, kind, out, part, check) if device else self._step_host_partial(frames, Ks, kind, part)
+            self._pending[part.seq] = False
+            res = part.results(*res)
+        self._verify.advance(self._since, stepped, pending, check)
+        if check:
+            lost = self._verify.lost_sequences(stepped if part is None else part.sequences, res[2]['verify']['lost'])
+            if len(lost):
+                self.reset(lost)
+        return res
 
     def _step_host_partial(self, frames, Ks, kind, part):
         """A partial step on the host path: _step_host on a view of this tracker holding the listed sequences' rows only
@@ -668,9 +694,10 @@ class Tracker:
         return _mixed_fn(1, S or self.S, b, est.cfg['refine_iter'], self.refine_iter, init, [st['views']],
                          st['tables']['ref_num'], est.refiner._refine_warped(128), smooth, blocks, draw)
 
-    def _step_device(self, frames, Ks, kind, out=None, part=None):
+    def _step_device(self, frames, Ks, kind, out=None, part=None, check=False):
         """One step's graph.  part: a partial step (row f17), whose compact batch of part.b sequences runs the same bodies
-        on gathered state rows (_compact_fn) under the names part.name(...)."""
+        on gathered state rows (_compact_fn) under the names part.name(...).  check: a refine step replays its verifying
+        variant (row f20)."""
         est = self.est
         st = est._glue_state()
         self._to(True)
@@ -692,8 +719,11 @@ class Tracker:
                 name, fn, fin = fr.stage(est.detector, named(rows('track_full')), wrap(self._full_fn(st, draw)), imgs, plan)
             elif kind == 'refine':
                 prev_f32 = bool(f32[0])
-                name, fn, fin = fr.stage(est.detector, named(rows(f'track_refine{int(prev_f32)}')),
-                                         wrap(self._refine_fn(st, prev_f32, draw)), imgs, plan)
+                base, body = f'track_refine{int(prev_f32)}', self._refine_fn(st, prev_f32, draw)
+                if check:
+                    key = self._verify.key
+                    base, body = V.graph_name(base, key), V.verifying(body, est._verify_fn(st, key))
+                name, fn, fin = fr.stage(est.detector, named(rows(base)), wrap(body), imgs, plan)
             else:
                 F = est.cfg['refine_iter']
                 reinit, b, extra = _mixed_inputs(S, 1, pending, f32, F, self.refine_iter, dev, plan)
@@ -718,9 +748,13 @@ class Tracker:
             self._f32[:] = True
         else:
             self._f32[part.seq] = True
+        if check:
+            host, checked = V.split(host, S)
         res = self._decode_mixed(host, reinit, b, pick, S) if kind == 'mixed' else self._decode(host, full, prev_f32, S)
         if drawn is not None:
             res[2]['drawn'] = drawn
+        if check:
+            res[2]['verify'] = checked
         return res
 
     def _decode(self, host, full, prev_f32, S=None):
@@ -801,12 +835,14 @@ class ObjectTracker:
     captured graph: refine_iter x (g6d_glue_refine_problems_objects -> one refiner stage over all K*S poses ->
     g6d_glue_apply_refinements_objects), then g6d_track_smooth_objects, so the number of launches does not grow with
     K.  The previous poses [K*S,12], the corner histories and their counts stay on the device between steps."""
+    _verify = V.Schedule()
 
     def __init__(self, objs, num_sequences, refine_iter=1, smooth_num=5, smooth_std=2.5, bboxes=None, draw=None,
-                 draw_colors=None):
+                 draw_colors=None, verify_every=None, lost_score=None, lost_gate=None):
         kinds = dr.parse_kinds(draw)
         if int(num_sequences) < 1:
             raise ValueError(f'num_sequences must be >= 1, got {num_sequences}')
+        self._verify = V.Schedule(verify_every, lost_score, lost_gate)
         if int(refine_iter) < 1:
             raise ValueError(f'refine_iter must be >= 1, got {refine_iter}')
         if int(smooth_num) < 1:
@@ -838,6 +874,7 @@ class ObjectTracker:
         if sequences is None:
             self._prev = None
             self._pending, self._f32 = np.ones(self.S, bool), np.ones(self.S, bool)
+            self._since = np.zeros(self.S, np.int64)
             self._ring = torch.zeros(n, self.num, 8, 2, device=dev, dtype=torch.float32)
             self._count = torch.zeros(n, device=dev, dtype=torch.int32)
             return
@@ -851,6 +888,7 @@ class ObjectTracker:
         return torch.from_numpy(rows).to(self.est.detector.device)
 
     def _restart(self, seqs):
+        self._since[seqs] = 0
         if len(seqs):
             rows = self._rows(seqs)
             self._ring[rows] = 0
@@ -957,7 +995,10 @@ class ObjectTracker:
         [S,3,4], smoothed poses float64 [S,3,4], inter)}: inter has Tracker.step's keys, and a full-prediction step adds
         those of ObjectSet.predict (det_score included); a mixed step adds 'reinit' and those entries for the
         re-initialised sequences, as Tracker.step does.  sequences: step only these sequences, every object on each, as
-        Tracker.step does (row f17); every object's results then hold one row per listed sequence in that order."""
+        Tracker.step does (row f17); every object's results then hold one row per listed sequence in that order.
+        verify_every (row f20): a verifying refine step adds inter['verify'] to every object's results (its windows
+        detected against that object's references only), and a sequence is re-initialised if any of its objects is
+        judged lost."""
         self._check()
         part = None
         if sequences is not None:
@@ -976,15 +1017,24 @@ class ObjectTracker:
         plan = fr.FramePlan(fr.size_pattern(imgs))
         if plan.mixed:
             fr.check_frames(imgs, Ks, 'step')
-        res = self._step_device(imgs, Ks, kind, plan, out, part)
+        stepped = np.arange(self.S) if part is None else part.seq[:part.a]
+        pending, check = self._pending[stepped].copy(), self._verify.due(kind, self._since[stepped])
+        res = self._step_device(imgs, Ks, kind, plan, out, part, check)
         if part is None:
             self._pending[:] = False
-            return res
-        self._pending[part.seq] = False
-        return {name: part.results(*r) for name, r in res.items()}
+        else:
+            self._pending[part.seq] = False
+            res = {name: part.results(*r) for name, r in res.items()}
+        self._verify.advance(self._since, stepped, pending, check)
+        if check:
+            lost = np.any([r[2]['verify']['lost'] for r in res.values()], 0)
+            lost = self._verify.lost_sequences(stepped if part is None else part.sequences, lost)
+            if len(lost):
+                self.reset(lost)
+        return res
 
-    def _step_device(self, imgs, Ks, kind, plan, out=None, part=None):
-        """One step's graph; part: a partial step (row f17), as in Tracker._step_device."""
+    def _step_device(self, imgs, Ks, kind, plan, out=None, part=None, check=False):
+        """One step's graph; part: a partial step (row f17), check: verify (row f20), as in Tracker._step_device."""
         K, est = self.K, self.est
         S, pending, f32 = (self.S, self._pending, self._f32) if part is None else (part.b, part.pending, part.f32)
         rows = (lambda n: n) if part is None else part.name
@@ -1003,8 +1053,11 @@ class ObjectTracker:
                 name, fn, fin = fr.stage(est.detector, named(rows('track_full')), wrap(self._full_fn(draw)), imgs, plan)
             elif not mixed:
                 prev_f32 = bool(f32[0])
-                name, fn, fin = fr.stage(est.detector, named(rows(f'track_refine{int(prev_f32)}')),
-                                         wrap(self._refine_fn(prev_f32, draw)), imgs, plan)
+                base, body = f'track_refine{int(prev_f32)}', self._refine_fn(prev_f32, draw)
+                if check:
+                    key = self._verify.key
+                    base, body = V.graph_name(base, key), V.verifying(body, self.objs._verify_fn(key))
+                name, fn, fin = fr.stage(est.detector, named(rows(base)), wrap(body), imgs, plan)
             else:
                 reinit, b, extra = _mixed_inputs(S, K, pending, f32, est.cfg['refine_iter'], self.refine_iter, dev, plan)
                 if plan.mixed:                   # one graph per size pattern and per-size buckets (row f13)
@@ -1030,7 +1083,13 @@ class ObjectTracker:
             self._f32[part.seq] = True
         if not mixed:
             reinit, b = None, None
-        return self._decode(host, kind, S, reinit, b, pick, prev_f32, drawn)
+        if check:
+            host, checked = V.split(host, K * S)
+        res = self._decode(host, kind, S, reinit, b, pick, prev_f32, drawn)
+        if check:
+            for o, r in enumerate(res.values()):
+                r[2]['verify'] = {k: v[o * S:(o + 1) * S] for k, v in checked.items()}
+        return res
 
     def _decode(self, host, kind, S, reinit, b, pick, prev_f32, drawn):
         K, num, est = self.K, self.num, self.est

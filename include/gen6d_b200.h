@@ -227,6 +227,24 @@ int g6d_glue_apply_refinements_rows(const g6d_glue_views* views, int n_obj, int 
 int g6d_glue_apply_refinements_rows_host(const g6d_glue_views* views, int n_obj, int rows_per_obj, const float* que_pose,
                                          const float* que_K, const float* rect, const float* net_out, const int* row_idx, int n_sel,
                                          double* poses);
+/* ---- checking a pose with the detector on a window around the object (gen6d_b200/verify.py).
+ * verify_windows: poses [n_obj*rows_per_obj,12] (float64 storage; poses_are_f32: float32 values), object-major as the
+ * *_objects calls take them (row o*rows_per_obj + s with refs[o] and cams[s]; refs is a host array of n_obj <=
+ * G6D_GLUE_MAX_OBJECTS) -> rec [n,4] float32 in g6d_det_parse's layout: (cx, cy, s, 1), cx, cy the projected object centre
+ * and s the scale_r2q a detection there would need to give this pose (the inverse of g6d_glue_initial_poses, with
+ * refs[o].dist[0] / refs[o].f[0]); (0, 0, 1, 0) for a pose whose centre is not in front of the camera or whose values are
+ * not finite.  g6d_glue_detection_jobs(rec, frames, window) cuts the windows.
+ * verify_judge: rec [n,4] and the detector's records det [n,4] on those windows (x, y, scale, score) -> out [n,5] float32
+ * (x, y, scale in the frame, score, offset = |detection - window centre| / (ref_resolution * s)) and lost [n] int32: the
+ * record is invalid, use_score and not score >= lost_score, or use_gate and not offset <= lost_gate (NaN is lost). */
+int g6d_verify_windows(const double* poses, int poses_are_f32, const g6d_glue_refs* refs, int n_obj, int rows_per_obj,
+                       const g6d_glue_camera* cams, float* rec, g6d_stream_t stream);
+int g6d_verify_windows_host(const double* poses, int poses_are_f32, const g6d_glue_refs* refs, int n_obj, int rows_per_obj,
+                            const g6d_glue_camera* cams, float* rec);
+int g6d_verify_judge(const float* rec, const float* det, int n, int window, double ref_resolution, int use_score, double lost_score,
+                     int use_gate, double lost_gate, float* out, int* lost, g6d_stream_t stream);
+int g6d_verify_judge_host(const float* rec, const float* det, int n, int window, double ref_resolution, int use_score,
+                          double lost_score, int use_gate, double lost_gate, float* out, int* lost);
 /* ---- temporal smoothing of tracked poses (predict.py:18-26,61-70; utils/base_utils.py:256-265 project_points;
  * utils/pose_utils.py:246-279 pnp).  Per sequence s: project the object's bounding box bbox [8,3] (float32) with the raw
  * pose poses[s] [12] (float64 storage; poses_are_f32: float32 values, projected in float32 like numpy does with
