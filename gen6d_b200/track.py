@@ -9,7 +9,10 @@ previous poses and the corner histories stay on the device between steps.  Other
 with predict_batch's host path and runs the smoothing through g6d_track_smooth_host (same code, on the CPU).
 
 ObjectTracker (ObjectSet.tracker()) does the same for every object of an object set at once: one graph per step whose
-glue and smoothing launches (the g6d_*_objects entry points) and refiner stage cover all K objects' K*S rows.
+glue and smoothing launches (the g6d_*_objects entry points) and refiner stage cover all K objects' K*S rows.  It is
+Tracker's subclass: the state, the step driver (checks, partial steps, verification) and the decode of a step's read are
+Tracker's, written for K object-major rows per sequence (K = 1 for Tracker); each class supplies its graph bodies, its
+start() poses and its result shape.
 
 reset(sequences) / start(poses, sequences) re-initialise or restart single sequences while the others keep tracking;
 the step after them is the mixed step below, also one graph and one read.
@@ -211,9 +214,9 @@ def _mixed_inputs(S, K, pending, f32, F, r, device, plan=None):
 
 def _mixed_fn(K, S, b, F, r, initial, views, R, refine, smooth, blocks=None, draw=None):
     """The mixed step's graph body.  initial(frames, cams) -> (poses [K*b,12], crops, [tensors packed after the smoothing]);
-    smooth(poses [K*S,12], Ks [S,9], ring, count) -> (smoothed, averaged corners).  blocks: the gathered rows per size
-    group of frames of different sizes (_size_buckets), detected per size.  draw(frames, raw, raw_f32, smoothed, Ks,
-    table): the draw node (row f16), run after the smoothing when the body is given a destination table."""
+    smooth(poses [K*S,12], poses_are_f32, Ks [S,9], ring, count) -> (smoothed, averaged corners).  blocks: the gathered
+    rows per size group of frames of different sizes (_size_buckets), detected per size.  draw(frames, raw, raw_f32,
+    smoothed, Ks, table): the draw node (row f16), run after the smoothing when the body is given a destination table."""
     n, lens = S + b, _iter_lengths(S, b, F, r)
 
     def fn(frames, cams, prev, ring, count, seq, tgt, flags0, lists, *dt):
@@ -243,7 +246,7 @@ def _mixed_fn(K, S, b, F, r, initial, views, R, refine, smooth, blocks=None, dra
             chain.append(real())
         poses = chain[-1]
         Ks = cams[:, :9].contiguous()
-        smoothed, avg = smooth(poses, Ks, ring, count)
+        smoothed, avg = smooth(poses, True, Ks, ring, count)
         if dt:
             draw(frames, poses, True, smoothed, Ks, dt[0])
         packed = torch.cat([t.reshape(-1).to(torch.float64) for t in [torch.stack(chain, 0), smoothed, avg, ring, count] + extras])
@@ -391,12 +394,34 @@ def _compact_fn(fn, full):
 
 # ------------------------------------------------------------------------------------------ the tracker
 class Tracker:
-    """S sequences tracked in lockstep (one frame each per step); see Gen6DEstimator.tracker()."""
+    """S sequences tracked in lockstep (one frame each per step); see Gen6DEstimator.tracker().
+
+    The state, the step driver and the decode of a step's read are written for K objects per sequence (K = 1 here), rows
+    object-major (row o*S + s is object o on sequence s); ObjectTracker supplies an object set's graph bodies, start()
+    poses and result shape through the hooks at the end of this class."""
+    K = 1
+    _host = True                     # steps may take the host path; the state stays on the host until a device step
     _verify = V.Schedule()           # no verification (row f20)
 
     def __init__(self, est, num_sequences, refine_iter=1, smooth_num=5, smooth_std=2.5, bbox_3d=None, draw=None,
                  draw_color=dr.DEFAULT_COLOR, verify_every=None, lost_score=None, lost_gate=None):
         kinds, draw_color = dr.parse_kinds(draw), dr.parse_color(draw_color)
+        self._setup(est, num_sequences, refine_iter, smooth_num, smooth_std, verify_every, lost_score, lost_gate)
+        if est.refiner is None:
+            raise ValueError('tracking refines from the previous pose: the estimator needs a refiner')
+        if bbox_3d is None:
+            bbox_3d = object_bbox(est.refiner.ref_database)
+            if bbox_3d is None:
+                raise ValueError('the database has no object point cloud: pass bbox_3d (the 8 corners of the object box)')
+        self.bbox = check_bbox(bbox_3d)
+        self._gen = est._generation()
+        self._dev = None                 # device copies of bbox / weights
+        self.draw = kinds                # the kinds each step draws (row f16); None: no drawing
+        self._drawer = dr.StepDrawer(kinds, [draw_color], self.bbox, [0], self.S, est.detector.device) if kinds else None
+        self.reset()
+
+    def _setup(self, est, num_sequences, refine_iter, smooth_num, smooth_std, verify_every, lost_score, lost_gate):
+        """The arguments every tracker takes, checked, and the constants that do not depend on its objects."""
         if int(num_sequences) < 1:
             raise ValueError(f'num_sequences must be >= 1, got {num_sequences}')
         self._verify = V.Schedule(verify_every, lost_score, lost_gate)
@@ -406,83 +431,69 @@ class Tracker:
             raise ValueError(f'smooth_num must be >= 1, got {smooth_num}')
         if not float(smooth_std) > 0:
             raise ValueError(f'smooth_std must be > 0, got {smooth_std}')
-        if est.refiner is None:
-            raise ValueError('tracking refines from the previous pose: the estimator needs a refiner')
-        if bbox_3d is None:
-            bbox_3d = object_bbox(est.refiner.ref_database)
-            if bbox_3d is None:
-                raise ValueError('the database has no object point cloud: pass bbox_3d (the 8 corners of the object box)')
         self.est = est
         self.S, self.refine_iter = int(num_sequences), int(refine_iter)
         self.num, self.std = int(smooth_num), float(smooth_std)
-        self.bbox = check_bbox(bbox_3d)
         self.weights = smoothing_weights(self.num, self.std)
-        self._gen = est._generation()
         self.stages = StageCache()       # this tracker's step graphs (they capture its device state)
-        self._dev = None                 # device copies of bbox / weights
-        self.draw = kinds                # the kinds each step draws (row f16); None: no drawing
-        self._drawer = dr.StepDrawer(kinds, [draw_color], self.bbox, [0], self.S, est.detector.device) if kinds else None
-        self.reset()
 
     # -------------------------------------------------------------- state
     def reset(self, sequences=None):
-        """The next step is a full prediction (detect -> select -> cfg['refine_iter'] refinements) for every sequence,
-        and the smoothing histories restart.  sequences: only those sequences are re-initialised at the next step and
-        restart their histories; the others keep tracking (that step is the mixed step)."""
+        """The next step is a full prediction (detect -> select -> cfg['refine_iter'] refinements) for every object and
+        sequence, and the smoothing histories restart.  sequences: only those sequences (every object on them) are
+        re-initialised at the next step and restart their histories; the others keep tracking (that step is the mixed
+        step)."""
         if sequences is None:
+            n = self.K * self.S
             self._since = np.zeros(self.S, np.int64)  # refine steps since the last verification (row f20)
-            self._prev = None                        # float64 previous poses ([S,12] on the device, [S,3,4] on the host)
+            self._prev = None                        # float64 previous poses ([K*S,12] on the device, [S,3,4] on the host)
             self._pending = np.ones(self.S, bool)    # a full prediction at the next step
-            self._f32 = np.ones(self.S, bool)        # each row's previous pose holds float32 values
-            self._ring = np.zeros((self.S, self.num, 8, 2), np.float32)
-            self._count = np.zeros(self.S, np.int32)
+            self._f32 = np.ones(self.S, bool)        # each sequence's previous poses hold float32 values
+            self._ring = np.zeros((n, self.num, 8, 2), np.float32)
+            self._count = np.zeros(n, np.int32)
+            if not self._host:
+                self._to(True)
             return
         seqs = _sequences(self.S, sequences)
         self._pending[seqs] = True
         self._restart(seqs)
+
+    def _rows(self, seqs):
+        """The state rows of sequences `seqs`, every object's (object-major), as an index into the state arrays."""
+        rows = np.concatenate([o * self.S + seqs for o in range(self.K)])
+        return rows if isinstance(self._ring, np.ndarray) else torch.from_numpy(rows).to(self._ring.device)
 
     def _restart(self, seqs):
         """Restart the smoothing of `seqs`: count 0 and a zero ring, the bytes of a fresh tracker's history; and their
         verification counts."""
         self._since[seqs] = 0
         if len(seqs):
-            idx = seqs if isinstance(self._ring, np.ndarray) else torch.from_numpy(seqs).to(self._ring.device)
-            self._ring[idx] = 0
-            self._count[idx] = 0
+            rows = self._rows(seqs)
+            self._ring[rows] = 0
+            self._count[rows] = 0
 
     def start(self, poses, sequences=None):
         """Begin (or restart) every sequence from known poses [S,3,4]: the next step refines from them, and the
         smoothing histories restart.  sequences: poses [len(sequences),3,4] for those sequences only; the others are
         unaffected.  A float32 array marks its poses as float32 values (as after a refinement), any other dtype float64."""
-        poses = np.asarray(poses)
+        seqs, p64, f32 = self._start_poses(poses, sequences)
         if sequences is None:
-            if poses.shape != (self.S, 3, 4):
-                raise ValueError(f'start: expected poses [{self.S},3,4], got {poses.shape}')
             self.reset()
-            seqs = np.arange(self.S)
         else:
-            seqs = _sequences(self.S, sequences)
-            if poses.shape != (len(seqs), 3, 4):
-                raise ValueError(f'start: expected poses [{len(seqs)},3,4] for sequences {seqs.tolist()}, got {poses.shape}')
             self._restart(seqs)
-        p64 = np.asarray(poses, np.float64).reshape(len(seqs), 12)
         if self._prev is None:
             self._prev = np.zeros((self.S, 3, 4)) if isinstance(self._ring, np.ndarray) else \
-                torch.zeros(self.S, 12, dtype=torch.float64, device=self._ring.device)
+                torch.zeros(self.K * self.S, 12, dtype=torch.float64, device=self._ring.device)
+        rows = self._rows(seqs)
         if isinstance(self._prev, np.ndarray):
-            self._prev[seqs] = p64.reshape(-1, 3, 4)
+            self._prev[rows] = p64.reshape(-1, 3, 4)
         else:
-            self._prev[torch.from_numpy(seqs).to(self._prev.device)] = torch.from_numpy(p64).to(self._prev.device)
+            self._prev[rows] = torch.from_numpy(p64).to(self._prev.device)
         self._pending[seqs] = False
-        self._f32[seqs] = poses.dtype == np.float32
-
-    def _check(self):
-        if self.est._generation() != self._gen:
-            raise RuntimeError('this tracker is stale: the estimator was rebuilt (build() on another object) or its weights '
-                               'changed since the tracker was created; create a new one with est.tracker()')
+        self._f32[seqs] = f32
 
     def _device_path(self):
-        return bool(self.est.cfg['device_glue']) and self.est._glue_possible()
+        return not self._host or (bool(self.est.cfg['device_glue']) and self.est._glue_possible())
 
     def _to(self, device):
         """Move the previous poses and the histories to the device (torch tensors) or the host (numpy)."""
@@ -503,7 +514,7 @@ class Tracker:
 
     def _partial(self, frames, Ks, out, sequences):
         """The plan of a step over `sequences` (row f17), its arguments checked before anything is enqueued."""
-        part = PartialStep(self.S, getattr(self, 'K', 1), sequences, self._pending, self._f32, self.est.cfg['refine_iter'])
+        part = PartialStep(self.S, self.K, sequences, self._pending, self._f32, self.est.cfg['refine_iter'])
         part.check(frames, Ks, out)
         if out is not None and self._drawer is None:
             raise ValueError('step: out= names drawing destinations; create the tracker with draw=')
@@ -539,18 +550,25 @@ class Tracker:
 
         A tracker made with verify_every (row f20) adds inter['verify'] to the refine steps that verify: verify_poses' keys
         on the step's final poses, in the step's row order; the sequences it judges lost are pending afterwards."""
+        return self._results(self._step(frames, Ks, out, sequences))
+
+    def _step(self, frames, Ks, out, sequences):
+        """step() -> [(raw, smoothed, inter)] per object."""
         self._check()
         part = None
         if sequences is not None:
             part = self._partial(frames, Ks, out, sequences)
             frames, Ks, out = part.compact(frames), part.compact(Ks), part.compact_out(out)
             if part.lockstep:
-                return part.results(*self.step(frames, Ks, out))
+                return [part.results(*r) for r in self._step(frames, Ks, out, None)]
         elif len(frames) != self.S or len(Ks) != self.S:
             raise ValueError(f'step: this tracker follows {self.S} sequences, got {len(frames)} frames and {len(Ks)} Ks')
         if out is not None and self._drawer is None:
             raise ValueError('step: out= names drawing destinations; create the tracker with draw=')
+        S = self.S if part is None else part.b
         Ks = np.stack([np.asarray(K) for K in Ks], 0)
+        if Ks.shape != (S, 3, 3):
+            raise ValueError(f'step: Ks must be [{S},3,3], got {Ks.shape}')
         kind = self._kind() if part is None else part.kind
         device = self._device_path()
         if self._drawer is not None and not device:
@@ -568,15 +586,17 @@ class Tracker:
         stepped = np.arange(self.S) if part is None else part.seq[:part.a]
         pending, check = self._pending[stepped].copy(), self._verify.due(kind, self._since[stepped])
         if part is None:
-            res = self._step_device(imgs, Ks, kind, out, check=check) if device else self._step_host(frames, Ks, kind)
+            res = self._step_device(imgs, Ks, kind, out, check=check) if device else [self._step_host(frames, Ks, kind)]
             self._pending[:] = False
         else:
-            res = self._step_device(imgs, Ks, kind, out, part, check) if device else self._step_host_partial(frames, Ks, kind, part)
+            res = self._step_device(imgs, Ks, kind, out, part, check) if device else \
+                [self._step_host_partial(frames, Ks, kind, part)]
             self._pending[part.seq] = False
-            res = part.results(*res)
+            res = [part.results(*r) for r in res]
         self._verify.advance(self._since, stepped, pending, check)
-        if check:
-            lost = self._verify.lost_sequences(stepped if part is None else part.sequences, res[2]['verify']['lost'])
+        if check:                                          # a sequence is lost when any of its objects is
+            lost = np.any([r[2]['verify']['lost'] for r in res], 0)
+            lost = self._verify.lost_sequences(stepped if part is None else part.sequences, lost)
             if len(lost):
                 self.reset(lost)
         return res
@@ -642,91 +662,38 @@ class Tracker:
         inter['refine_poses'] = [chain[0]] + [c.astype(np.float32) for c in chain[1:]]
         return inter['refine_poses'][-1], inter
 
-    def _device_consts(self):
-        if self._dev is None:
-            dev = self.est.detector.device
-            self._dev = {'bbox': torch.from_numpy(self.bbox).to(dev), 'weights': torch.from_numpy(self.weights.copy()).to(dev)}
-        return self._dev
 
-    def _full_fn(self, st, draw=None):
-        predict, c = self.est._predict_device_fn(st), self._device_consts()
-
-        def fn(frames, cams, ring, count, *dt):
-            chain, det, crop, idx, sel_out, logits = predict(frames, cams)
-            poses = chain[-1]
-            Ks = cams[:, :9].contiguous()
-            smoothed, avg = ops.track_smooth(poses, chain.shape[0] > 1, c['bbox'], Ks, ring, count, c['weights'])
-            if dt:
-                draw(frames, poses, chain.shape[0] > 1, smoothed, Ks, dt[0])
-            packed = torch.cat([t.reshape(-1).to(torch.float64) for t in (chain, smoothed, avg, ring, count, det, idx, sel_out, logits)])
-            return torch.cat([packed.view(torch.uint8), crop.reshape(-1)]), poses, ring, count
-        return fn
-
-    def _refine_fn(self, st, first_f32, draw=None):
-        est, iters, c = self.est, self.refine_iter, self._device_consts()
-        R, refine = st['tables']['ref_num'], est.refiner._refine_warped(128)
-
-        def fn(frames, cams, prev, ring, count, *dt):
-            poses, chain = prev, [prev]
-            for it in range(iters):
-                jobs, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems(st['views'], R, cams, frames, poses,
-                                                                                             first_f32 or it > 0)
-                out = refine(jobs, que_K, que_pose, ref_Ks, ref_poses)
-                poses = ops.glue_apply_refinements(st['views'], que_pose, que_K, rect, out)
-                chain.append(poses)
-            Ks = cams[:, :9].contiguous()
-            smoothed, avg = ops.track_smooth(poses, True, c['bbox'], Ks, ring, count, c['weights'])
-            if dt:
-                draw(frames, poses, True, smoothed, Ks, dt[0])
-            packed = torch.cat([t.reshape(-1).to(torch.float64) for t in (torch.stack(chain, 0), smoothed, avg, ring, count)])
-            return packed.view(torch.uint8), poses, ring, count
-        return fn
-
-    def _mixed_fn(self, st, b, blocks=None, draw=None, S=None):
-        est, c = self.est, self._device_consts()
-        initial = est._initial_poses_device_fn(st)
-
-        def init(frames, cams):
-            poses, det, crop, idx, sel_out, logits = initial(frames, cams)
-            return poses, crop, [det, idx, sel_out, logits]
-
-        smooth = lambda poses, Ks, ring, count: ops.track_smooth(poses, True, c['bbox'], Ks, ring, count, c['weights'])
-        return _mixed_fn(1, S or self.S, b, est.cfg['refine_iter'], self.refine_iter, init, [st['views']],
-                         st['tables']['ref_num'], est.refiner._refine_warped(128), smooth, blocks, draw)
-
-    def _step_device(self, frames, Ks, kind, out=None, part=None, check=False):
-        """One step's graph.  part: a partial step (row f17), whose compact batch of part.b sequences runs the same bodies
-        on gathered state rows (_compact_fn) under the names part.name(...).  check: a refine step replays its verifying
-        variant (row f20)."""
-        est = self.est
-        st = est._glue_state()
+    def _step_device(self, imgs, Ks, kind, out=None, part=None, check=False):
+        """One step's graph -> [(raw, smoothed, inter)] per object.  part: a partial step (row f17), whose compact batch of
+        part.b sequences runs the same bodies on gathered state rows (_compact_fn) under the names part.name(...).
+        check: a refine step replays its verifying variant (row f20)."""
+        est, K = self.est, self.K
+        st = self._tables()
         self._to(True)
         S, pending, f32 = (self.S, self._pending, self._f32) if part is None else (part.b, part.pending, part.f32)
         rows = (lambda n: n) if part is None else part.name
         drawer = self._drawer if part is None or self._drawer is None else self._drawer.for_sequences(part.b)
         full = kind == 'full'
-        imgs = frames                                     # numpy or device frames (as_frames)
-        plan, pick = fr.FramePlan(fr.size_pattern(imgs)), None
+        plan, reinit, b, pick = fr.FramePlan(fr.size_pattern(imgs)), None, 0, None
         draw, dt, drawn, named = draw_inputs(drawer, est.detector, plan, out, None if part is None else part.a)
         dev = est.detector.device
         if self._prev is None and (part is not None or kind == 'mixed'):
-            self._prev = torch.zeros(self.S, 12, dtype=torch.float64, device=dev)
+            self._prev = torch.zeros(K * self.S, 12, dtype=torch.float64, device=dev)
         wrap, extra = (lambda fn: fn), []
         if part is not None:
             wrap = lambda fn: _compact_fn(fn, full)
         with torch.no_grad():
             if full:
-                name, fn, fin = fr.stage(est.detector, named(rows('track_full')), wrap(self._full_fn(st, draw)), imgs, plan)
+                name, fn, fin = fr.stage(est.detector, named(rows('track_full')), wrap(self._full_fn(st=st, draw=draw)), imgs, plan)
             elif kind == 'refine':
                 prev_f32 = bool(f32[0])
-                base, body = f'track_refine{int(prev_f32)}', self._refine_fn(st, prev_f32, draw)
+                base, body = f'track_refine{int(prev_f32)}', self._refine_fn(st=st, first_f32=prev_f32, draw=draw)
                 if check:
                     key = self._verify.key
-                    base, body = V.graph_name(base, key), V.verifying(body, est._verify_fn(st, key))
+                    base, body = V.graph_name(base, key), V.verifying(body, self._verify_fn(st, key))
                 name, fn, fin = fr.stage(est.detector, named(rows(base)), wrap(body), imgs, plan)
             else:
-                F = est.cfg['refine_iter']
-                reinit, b, extra = _mixed_inputs(S, 1, pending, f32, F, self.refine_iter, dev, plan)
+                reinit, b, extra = _mixed_inputs(S, K, pending, f32, est.cfg['refine_iter'], self.refine_iter, dev, plan)
                 if plan.mixed:                   # one graph per size pattern and per-size buckets (row f13)
                     _, blocks, pick = _size_buckets(reinit, plan)
                     name, fn = named(rows((plan.key('track_mixed'), tuple(blocks)))), self._mixed_fn(st, b, blocks, draw, S)
@@ -749,84 +716,168 @@ class Tracker:
         else:
             self._f32[part.seq] = True
         if check:
-            host, checked = V.split(host, S)
-        res = self._decode_mixed(host, reinit, b, pick, S) if kind == 'mixed' else self._decode(host, full, prev_f32, S)
-        if drawn is not None:
-            res[2]['drawn'] = drawn
-        if check:
-            res[2]['verify'] = checked
+            host, checked = V.split(host, K * S)
+        res = self._unpack(host, kind, S, prev_f32, reinit, b, pick)
+        for o, (_, _, inter) in enumerate(res):
+            if drawn is not None:
+                inter['drawn'] = drawn
+            if check:
+                inter['verify'] = {k: v[o * S:(o + 1) * S] for k, v in checked.items()}
         return res
 
-    def _decode(self, host, full, prev_f32, S=None):
-        est, S, num = self.est, S or self.S, self.num
-        n_chain = (est.cfg['refine_iter'] if full else self.refine_iter) + 1
-        sizes = [('chain', n_chain * S * 12), ('smoothed', S * 12), ('avg', S * 16), ('ring', S * num * 16), ('count', S)]
-        if full:
-            res = est.cfg['ref_resolution']
-            crop_bytes = S * res * res * 3
-            f64 = host[:len(host) - crop_bytes].view(np.float64)
-            crop = host[len(host) - crop_bytes:].reshape(S, res, res, 3)
-            sizes += [('det', S * 4), ('idx', S), ('sel_out', S * 2)]
-            sizes.append(('logits', len(f64) - sum(n for _, n in sizes)))
-        else:
-            f64 = host.view(np.float64)
-        vals, off = {}, 0
-        for name, n in sizes:
-            vals[name] = f64[off:off + n]
-            off += n
-        chain = vals['chain'].reshape(n_chain, S, 3, 4)
-        refined = [c.astype(np.float32) for c in chain[1:]]
-        first = chain[0].astype(np.float32) if (not full and prev_f32) else chain[0].copy()
-        inter = {}
-        if full:
-            det = vals['det'].reshape(S, 4).astype(np.float32)
-            sel_out = vals['sel_out'].reshape(S, 2).astype(np.float32)
-            inter.update({'det_position': det[:, :2].copy(), 'det_scale_r2q': det[:, 2].copy(), 'det_que_img': crop,
-                          'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': vals['logits'].reshape(S, -1).astype(np.float32),
-                          'sel_ref_idx': vals['idx'].astype(np.int64)})
-        ring_h, count_h = vals['ring'].reshape(S, num, 8, 2).astype(np.float32), vals['count'].astype(np.int64)
-        inter['refine_poses'] = [first] + refined
-        inter['bbox_pts'] = ring_h[np.arange(S), count_h - 1].copy()
-        inter['smoothed_pts'] = vals['avg'].reshape(S, 8, 2).copy()
-        return (refined[-1] if refined else first), vals['smoothed'].reshape(S, 3, 4).copy(), inter
-
-    def _decode_mixed(self, host, reinit, b, pick=None, S=None):
-        """pick: the gathered row of each re-initialised sequence (per-size buckets); None: the first m rows.  S: the
-        step's sequences (a partial step's compact batch); default all."""
-        est, S, num, m = self.est, S or self.S, self.num, len(reinit)
-        pick = slice(0, m) if pick is None else pick
-        n_chain = max(est.cfg['refine_iter'], self.refine_iter) + 1
+    def _unpack(self, host, kind, S, prev_f32=False, reinit=None, b=0, pick=None):
+        """A step's read -> [(raw poses float32 [S,3,4], smoothed poses float64 [S,3,4], inter)] per object.  S: the step's
+        sequences (a partial step's compact batch); prev_f32: a refine step's previous poses hold float32 values.  A mixed
+        step's reinit (the re-initialised sequences), b (its bucket, the gathered rows per object) and pick (the gathered
+        row of each re-initialised sequence, per-size buckets; None: the first len(reinit) rows)."""
+        est, K, num, n = self.est, self.K, self.num, self.K * S
+        full, mixed = kind == 'full', kind == 'mixed'
+        F, r = est.cfg['refine_iter'], self.refine_iter
+        n_chain = 1 + (max(F, r) if mixed else F if full else r)
+        qn = b if mixed else S if full else 0                   # detected rows per object
+        pick = slice(0, len(reinit) if mixed else qn) if pick is None else pick
         res = est.cfg['ref_resolution']
-        crop_bytes = b * res * res * 3
+        crop_bytes = K * qn * res * res * 3
         f64 = host[:len(host) - crop_bytes].view(np.float64)
+        crops = host[len(host) - crop_bytes:].reshape(K, qn, res, res, 3)
         off = 0
 
-        def take(n):
+        def take(m):
             nonlocal off
-            off += n
-            return f64[off - n:off]
-        chain = take(n_chain * S * 12).reshape(n_chain, S, 3, 4)
-        smoothed = take(S * 12).reshape(S, 3, 4).copy()
-        avg = take(S * 16).reshape(S, 8, 2).copy()
-        ring_h = take(S * num * 16).reshape(S, num, 8, 2).astype(np.float32)
-        count_h = take(S).astype(np.int64)
-        inter = {'reinit': reinit.astype(np.int64)}
-        if b:
-            det = take(b * 4).reshape(b, 4)[pick].astype(np.float32)
-            idx = take(b)[pick].astype(np.int64)
-            sel_out = take(b * 2).reshape(b, 2)[pick].astype(np.float32)
-            logits = f64[off:].reshape(b, -1)[pick].astype(np.float32)
-            crop = host[len(host) - crop_bytes:].reshape(b, res, res, 3)[pick].copy()
-            inter.update({'det_position': det[:, :2].copy(), 'det_scale_r2q': det[:, 2].copy(), 'det_que_img': crop,
-                          'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': logits, 'sel_ref_idx': idx})
-        inter['refine_poses'] = [chain[0].copy()] + [c.astype(np.float32) for c in chain[1:]]
-        inter['bbox_pts'] = ring_h[np.arange(S), count_h - 1].copy()
-        inter['smoothed_pts'] = avg
-        return inter['refine_poses'][-1], smoothed, inter
+            off += m
+            return f64[off - m:off]
+        chain = take(n_chain * n * 12).reshape(n_chain, K, S, 3, 4)
+        smoothed = take(n * 12).reshape(K, S, 3, 4)
+        avg = take(n * 16).reshape(K, S, 8, 2)
+        ring_h = take(n * num * 16).reshape(K, S, num, 8, 2).astype(np.float32)
+        count_h = take(n).reshape(K, S).astype(np.int64)
+        out = []
+        for o, n_sel in enumerate(self._ref_counts()):
+            refined = [c.astype(np.float32) for c in chain[1:, o]]
+            first = chain[0, o].astype(np.float32) if (kind == 'refine' and prev_f32) else chain[0, o].copy()
+            inter = {'reinit': reinit.astype(np.int64)} if mixed else {}
+            if qn:
+                d = take(qn * 4).reshape(qn, 4)[pick].astype(np.float32)
+                idx = take(qn)[pick].astype(np.int64)
+                sel_out = take(qn * 2).reshape(qn, 2)[pick].astype(np.float32)
+                logits = take(qn * n_sel).reshape(qn, -1)[pick].astype(np.float32)
+                inter.update({'det_position': d[:, :2].copy(), 'det_scale_r2q': d[:, 2].copy(), 'det_score': d[:, 3].copy(),
+                              'det_que_img': crops[o, pick].copy(), 'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': logits,
+                              'sel_ref_idx': idx})
+            inter['refine_poses'] = [first] + refined
+            inter['bbox_pts'] = ring_h[o, np.arange(S), count_h[o] - 1].copy()
+            inter['smoothed_pts'] = avg[o].copy()
+            out.append(((refined[-1] if refined else first), smoothed[o].copy(), inter))
+        return out
+
+    def _decode(self, host, full, prev_f32, S=None):
+        """step()'s result from the read of a full step (full true) or a refine step over S sequences (default: all)."""
+        return self._results(self._unpack(host, 'full' if full else 'refine', S or self.S, prev_f32))
+
+    def _decode_mixed(self, host, reinit, b, pick=None, S=None):
+        """step()'s result from the read of a mixed step over S sequences (default: all)."""
+        return self._results(self._unpack(host, 'mixed', S or self.S, False, reinit, b, pick))
+
+    def _mixed_fn(self, st, b, blocks=None, draw=None, S=None):
+        """The mixed step's graph body (_mixed_fn) for S sequences (default: the tracker's) and bucket b."""
+        views, R = self._groups(st)
+        return _mixed_fn(self.K, S or self.S, b, self.est.cfg['refine_iter'], self.refine_iter, self._initial(st), views, R,
+                         self.est.refiner._refine_warped(128), self._smoother(), blocks, draw)
+
+    # -------------------------------------------------------------- what differs between the estimator and an object set
+    def _check(self):
+        if self.est._generation() != self._gen:
+            raise RuntimeError('this tracker is stale: the estimator was rebuilt (build() on another object) or its weights '
+                               'changed since the tracker was created; create a new one with est.tracker()')
+
+    def _start_poses(self, poses, sequences):
+        """start()'s arguments -> (the sequences, their poses float64 [K*n,12] object-major, whether they are float32)."""
+        poses = np.asarray(poses)
+        if sequences is None:
+            if poses.shape != (self.S, 3, 4):
+                raise ValueError(f'start: expected poses [{self.S},3,4], got {poses.shape}')
+            seqs = np.arange(self.S)
+        else:
+            seqs = _sequences(self.S, sequences)
+            if poses.shape != (len(seqs), 3, 4):
+                raise ValueError(f'start: expected poses [{len(seqs)},3,4] for sequences {seqs.tolist()}, got {poses.shape}')
+        return seqs, np.asarray(poses, np.float64).reshape(len(seqs), 12), poses.dtype == np.float32
+
+    def _results(self, res):
+        """The per-object results -> step()'s: the one object's, with predict_batch's detection entries (no det_score)."""
+        (raw, smoothed, inter), = res
+        inter.pop('det_score', None)
+        return raw, smoothed, inter
+
+    def _ref_counts(self):
+        """The selector references of each object: the width of its sel_scores."""
+        return [len(self.est.ref_info['poses'])]
+
+    def _tables(self):
+        return self.est._glue_state()
+
+    def _groups(self, st):
+        """-> (the refiner's view table of each object, the reference views per table)."""
+        return [st['views']], st['tables']['ref_num']
+
+    def _smoother(self):
+        """-> smooth(poses, poses_are_f32, Ks, ring, count) -> (smoothed, averaged corners): the smoothing launch."""
+        if self._dev is None:
+            dev = self.est.detector.device
+            self._dev = {'bbox': torch.from_numpy(self.bbox).to(dev), 'weights': torch.from_numpy(self.weights.copy()).to(dev)}
+        c = self._dev
+        return lambda poses, f32, Ks, ring, count: ops.track_smooth(poses, f32, c['bbox'], Ks, ring, count, c['weights'])
+
+    def _initial(self, st):
+        """The mixed step's detection: fn(frames, cams) -> (initial poses [K*b,12], crops, [the detection and selection
+        tensors, in packing order])."""
+        initial = self.est._initial_poses_device_fn(st)
+
+        def fn(frames, cams):
+            poses, det, crop, idx, sel_out, logits = initial(frames, cams)
+            return poses, crop, [det, idx, sel_out, logits]
+        return fn
+
+    def _verify_fn(self, st, key):
+        return self.est._verify_fn(st, key)
+
+    def _full_fn(self, st, draw=None):
+        predict, smooth = self.est._predict_device_fn(st), self._smoother()
+
+        def fn(frames, cams, ring, count, *dt):
+            chain, det, crop, idx, sel_out, logits = predict(frames, cams)
+            poses = chain[-1]
+            Ks = cams[:, :9].contiguous()
+            smoothed, avg = smooth(poses, chain.shape[0] > 1, Ks, ring, count)
+            if dt:
+                draw(frames, poses, chain.shape[0] > 1, smoothed, Ks, dt[0])
+            packed = torch.cat([t.reshape(-1).to(torch.float64) for t in (chain, smoothed, avg, ring, count, det, idx, sel_out, logits)])
+            return torch.cat([packed.view(torch.uint8), crop.reshape(-1)]), poses, ring, count
+        return fn
+
+    def _refine_fn(self, st, first_f32, draw=None):
+        est, iters, smooth = self.est, self.refine_iter, self._smoother()
+        R, refine = st['tables']['ref_num'], est.refiner._refine_warped(128)
+
+        def fn(frames, cams, prev, ring, count, *dt):
+            poses, chain = prev, [prev]
+            for it in range(iters):
+                jobs, que_K, que_pose, rect, ref_Ks, ref_poses, _ = ops.glue_refine_problems(st['views'], R, cams, frames, poses,
+                                                                                             first_f32 or it > 0)
+                out = refine(jobs, que_K, que_pose, ref_Ks, ref_poses)
+                poses = ops.glue_apply_refinements(st['views'], que_pose, que_K, rect, out)
+                chain.append(poses)
+            Ks = cams[:, :9].contiguous()
+            smoothed, avg = smooth(poses, True, Ks, ring, count)
+            if dt:
+                draw(frames, poses, True, smoothed, Ks, dt[0])
+            packed = torch.cat([t.reshape(-1).to(torch.float64) for t in (torch.stack(chain, 0), smoothed, avg, ring, count)])
+            return packed.view(torch.uint8), poses, ring, count
+        return fn
 
 
 # ------------------------------------------------------------------------------------------ several objects
-class ObjectTracker:
+class ObjectTracker(Tracker):
     """Every object of an ObjectSet tracked through S sequences in lockstep; see ObjectSet.tracker().
 
     Per object the semantics are Tracker's: the first step (and the first after reset()) is the set's full prediction
@@ -834,31 +885,28 @@ class ObjectTracker:
     by predict.py's smoothing.  Rows are object-major (row o*S + s is object o on sequence s), and each step is ONE
     captured graph: refine_iter x (g6d_glue_refine_problems_objects -> one refiner stage over all K*S poses ->
     g6d_glue_apply_refinements_objects), then g6d_track_smooth_objects, so the number of launches does not grow with
-    K.  The previous poses [K*S,12], the corner histories and their counts stay on the device between steps."""
-    _verify = V.Schedule()
+    K.  The previous poses [K*S,12], the corner histories and their counts stay on the device between steps.
+
+    start(poses, sequences) takes {name: [S,3,4]} (every object of the set, one dtype for all; [len(sequences),3,4] each
+    with sequences).  step() takes Tracker.step's arguments, Ks [S,3,3] shared by all objects and out= drawing every
+    object's box on its sequence's frame in object order, and returns {name: (raw poses float32 [S,3,4], smoothed poses
+    float64 [S,3,4], inter)}: inter has Tracker.step's keys, and a full-prediction step adds those of ObjectSet.predict
+    (det_score included); a mixed step adds 'reinit' and those entries for the re-initialised sequences.  sequences=
+    steps every object on each listed sequence.  With verify_every, a verifying refine step adds inter['verify'] to every
+    object's results (its windows detected against that object's references only), and a sequence is re-initialised if
+    any of its objects is judged lost."""
+    _host = False                    # an object set runs on the device pipeline only
 
     def __init__(self, objs, num_sequences, refine_iter=1, smooth_num=5, smooth_std=2.5, bboxes=None, draw=None,
                  draw_colors=None, verify_every=None, lost_score=None, lost_gate=None):
         kinds = dr.parse_kinds(draw)
-        if int(num_sequences) < 1:
-            raise ValueError(f'num_sequences must be >= 1, got {num_sequences}')
-        self._verify = V.Schedule(verify_every, lost_score, lost_gate)
-        if int(refine_iter) < 1:
-            raise ValueError(f'refine_iter must be >= 1, got {refine_iter}')
-        if int(smooth_num) < 1:
-            raise ValueError(f'smooth_num must be >= 1, got {smooth_num}')
-        if not float(smooth_std) > 0:
-            raise ValueError(f'smooth_std must be > 0, got {smooth_std}')
+        self._setup(objs.est, num_sequences, refine_iter, smooth_num, smooth_std, verify_every, lost_score, lost_gate)
         objs._check()
         boxes = object_bboxes(objs, bboxes)
-        self.objs, self.est = objs, objs.est
-        self.names = objs.names
-        self.K, self.S, self.refine_iter = len(self.names), int(num_sequences), int(refine_iter)
-        self.num, self.std = int(smooth_num), float(smooth_std)
+        self.objs, self.names = objs, objs.names
+        self.K = len(self.names)
         self.bboxes = np.ascontiguousarray(np.stack(boxes, 0))
-        self.weights = smoothing_weights(self.num, self.std)
         self._membership = objs.membership
-        self.stages = StageCache()       # this tracker's step graphs (they capture its device state)
         dev = self.est.detector.device
         self._dev = {'bboxes': torch.from_numpy(self.bboxes).to(dev), 'weights': torch.from_numpy(self.weights.copy()).to(dev)}
         self.draw = kinds
@@ -866,38 +914,13 @@ class ObjectTracker:
                                      dev) if kinds else None
         self.reset()
 
-    # -------------------------------------------------------------- state
-    def reset(self, sequences=None):
-        """The next step is a full prediction for every object and sequence, and the smoothing histories restart.
-        sequences: only those sequences are re-initialised (for every object) and restart their histories."""
-        dev, n = self.est.detector.device, self.K * self.S
-        if sequences is None:
-            self._prev = None
-            self._pending, self._f32 = np.ones(self.S, bool), np.ones(self.S, bool)
-            self._since = np.zeros(self.S, np.int64)
-            self._ring = torch.zeros(n, self.num, 8, 2, device=dev, dtype=torch.float32)
-            self._count = torch.zeros(n, device=dev, dtype=torch.int32)
-            return
-        seqs = _sequences(self.S, sequences)
-        self._pending[seqs] = True
-        self._restart(seqs)
+    def _check(self):
+        if self.objs.membership != self._membership:
+            raise RuntimeError('this tracker is stale: objects were added to or removed from the set since it was created; '
+                               'create a new one with objs.tracker()')
+        self.objs._check()
 
-    def _rows(self, seqs):
-        """Object-major rows of sequences `seqs` for every object, on the device."""
-        rows = np.concatenate([o * self.S + seqs for o in range(self.K)])
-        return torch.from_numpy(rows).to(self.est.detector.device)
-
-    def _restart(self, seqs):
-        self._since[seqs] = 0
-        if len(seqs):
-            rows = self._rows(seqs)
-            self._ring[rows] = 0
-            self._count[rows] = 0
-
-    def start(self, poses, sequences=None):
-        """Begin (or restart) every object's sequences from known poses {name: [S,3,4]} (every object of the set, one
-        dtype for all): the next step refines from them, and the smoothing histories restart.  sequences: poses
-        {name: [len(sequences),3,4]} for those sequences only; the other sequences are unaffected."""
+    def _start_poses(self, poses, sequences):
         missing = [n for n in self.names if n not in poses]
         extra = sorted(set(poses) - set(self.names))
         if missing or extra:
@@ -911,48 +934,64 @@ class ObjectTracker:
         if len(dtypes) != 1:
             raise ValueError(f'start: the objects\' poses have different dtypes {sorted(str(d) for d in dtypes)}; the refinement '
                              'reads them all as float32 or all as float64, so pass one dtype')
-        if sequences is None:
-            self.reset()
-        else:
-            self._restart(seqs)
-        dev = self.est.detector.device
-        prev = torch.from_numpy(np.ascontiguousarray(np.concatenate(arrs, 0).astype(np.float64).reshape(-1, 12))).to(dev)
-        if self._prev is None:
-            self._prev = torch.zeros(self.K * self.S, 12, dtype=torch.float64, device=dev)
-        self._prev[self._rows(seqs)] = prev
-        self._pending[seqs] = False
-        self._f32[seqs] = arrs[0].dtype == np.float32
+        return seqs, np.concatenate(arrs, 0).astype(np.float64).reshape(-1, 12), arrs[0].dtype == np.float32
 
-    _kind = Tracker._kind
+    def _results(self, res):
+        return dict(zip(self.names, res))
 
-    def _check(self):
-        if self.objs.membership != self._membership:
-            raise RuntimeError('this tracker is stale: objects were added to or removed from the set since it was created; '
-                               'create a new one with objs.tracker()')
-        self.objs._check()
+    def _ref_counts(self):
+        return [len(ob.ref_info['poses']) for ob in self.objs._objects.values()]
 
-    # -------------------------------------------------------------- one step
-    def _full_fn(self, draw=None):
-        predict, c, K = self.objs._predict_device_fn(), self._dev, self.K
+    def _tables(self):
+        return None
+
+    def _groups(self, st):
+        objs = list(self.objs._objects.values())
+        return [ob.tables['views'] for ob in objs], objs[0].tables['tables']['ref_num']
+
+    def _smoother(self):
+        c = self._dev
+        return lambda poses, f32, Ks, ring, count: ops.track_smooth_objects(poses, f32, c['bboxes'], Ks, ring, count,
+                                                                            c['weights'])
+
+    def _detections(self, det, sels):
+        """The set's detections [K*n,4] and selections [(idx, sel_out, logits)] per object -> the tensors a step packs
+        after its state, object by object."""
+        n, parts = det.shape[0] // self.K, []
+        for o in range(self.K):
+            parts += [det[o * n:(o + 1) * n], *sels[o]]
+        return parts
+
+    def _initial(self, st):
+        initial = self.objs._initial_poses_device_fn()
+
+        def fn(frames, cams):
+            poses, det, sels, crop = initial(frames, cams)          # the set's shared detection on the gathered frames
+            return poses, crop, self._detections(det, sels)
+        return fn
+
+    def _verify_fn(self, st, key):
+        return self.objs._verify_fn(key)
+
+    # the graph bodies take the estimator's tables as st= (Tracker's driver passes them by keyword): the set's objects
+    # hold their own, so st is None here
+    def _full_fn(self, draw=None, st=None):
+        predict, smooth = self.objs._predict_device_fn(), self._smoother()
 
         def fn(frames, cams, ring, count, *dt):
-            S = frames.shape[0]
             chain, det, sels, crop = predict(frames, cams)
             poses = chain[-1]
             Ks = cams[:, :9].contiguous()
-            smoothed, avg = ops.track_smooth_objects(poses, chain.shape[0] > 1, c['bboxes'], Ks, ring, count, c['weights'])
+            smoothed, avg = smooth(poses, chain.shape[0] > 1, Ks, ring, count)
             if dt:
                 draw(frames, poses, chain.shape[0] > 1, smoothed, Ks, dt[0])
-            parts = [chain, smoothed, avg, ring, count]
-            for o in range(K):
-                parts += [det[o * S:(o + 1) * S], *sels[o]]
+            parts = [chain, smoothed, avg, ring, count] + self._detections(det, sels)
             packed = torch.cat([t.reshape(-1).to(torch.float64) for t in parts])
             return torch.cat([packed.view(torch.uint8), crop.reshape(-1)]), poses, ring, count
         return fn
 
-    def _refine_fn(self, first_f32, draw=None):
-        objs, iters, c = list(self.objs._objects.values()), self.refine_iter, self._dev
-        views, R = [ob.tables['views'] for ob in objs], objs[0].tables['tables']['ref_num']
+    def _refine_fn(self, first_f32, draw=None, st=None):
+        (views, R), iters, smooth = self._groups(st), self.refine_iter, self._smoother()
         refine = self.est.refiner._refine_warped(128)
 
         def fn(frames, cams, prev, ring, count, *dt):
@@ -964,177 +1003,9 @@ class ObjectTracker:
                 poses = ops.glue_apply_refinements_objects(views, que_pose, que_K, rect, out)
                 chain.append(poses)
             Ks = cams[:, :9].contiguous()
-            smoothed, avg = ops.track_smooth_objects(poses, True, c['bboxes'], Ks, ring, count, c['weights'])
+            smoothed, avg = smooth(poses, True, Ks, ring, count)
             if dt:
                 draw(frames, poses, True, smoothed, Ks, dt[0])
             packed = torch.cat([t.reshape(-1).to(torch.float64) for t in (torch.stack(chain, 0), smoothed, avg, ring, count)])
             return packed.view(torch.uint8), poses, ring, count
         return fn
-
-    def _mixed_fn(self, b, blocks=None, draw=None, S=None):
-        objs, c, K = list(self.objs._objects.values()), self._dev, self.K
-        initial = self.objs._initial_poses_device_fn()
-
-        def init(frames, cams):
-            poses, det, sels, crop = initial(frames, cams)          # the set's shared detection on the gathered frames
-            extras = []
-            for o in range(K):
-                extras += [det[o * b:(o + 1) * b], *sels[o]]
-            return poses, crop, extras
-
-        smooth = lambda poses, Ks, ring, count: ops.track_smooth_objects(poses, True, c['bboxes'], Ks, ring, count, c['weights'])
-        return _mixed_fn(K, S or self.S, b, self.est.cfg['refine_iter'], self.refine_iter, init, [ob.tables['views'] for ob in objs],
-                         objs[0].tables['tables']['ref_num'], self.est.refiner._refine_warped(128), smooth, blocks, draw)
-
-    _partial = Tracker._partial
-
-    def step(self, frames, Ks, out=None, sequences=None):
-        """frames: S uint8 [h,w,3] (of one size or several, row f13; or device frames, row f14, as Tracker.step takes them);
-        Ks: [S,3,3] (shared by all objects); out: drawing destinations as Tracker.step takes them, every object's box
-        drawn on its sequence's frame in object order (each step's result then also holds inter['drawn'] without out=).  Returns {name: (raw poses float32
-        [S,3,4], smoothed poses float64 [S,3,4], inter)}: inter has Tracker.step's keys, and a full-prediction step adds
-        those of ObjectSet.predict (det_score included); a mixed step adds 'reinit' and those entries for the
-        re-initialised sequences, as Tracker.step does.  sequences: step only these sequences, every object on each, as
-        Tracker.step does (row f17); every object's results then hold one row per listed sequence in that order.
-        verify_every (row f20): a verifying refine step adds inter['verify'] to every object's results (its windows
-        detected against that object's references only), and a sequence is re-initialised if any of its objects is
-        judged lost."""
-        self._check()
-        part = None
-        if sequences is not None:
-            part = self._partial(frames, Ks, out, sequences)
-            frames, Ks, out = part.compact(frames), part.compact(Ks), part.compact_out(out)
-            if part.lockstep:
-                return {name: part.results(*r) for name, r in self.step(frames, Ks, out).items()}
-        K, S, est = self.K, self.S if part is None else part.b, self.est
-        if len(frames) != S or len(Ks) != S:
-            raise ValueError(f'step: this tracker follows {S} sequences, got {len(frames)} frames and {len(Ks)} Ks')
-        Ks = np.stack([np.asarray(k) for k in Ks], 0)
-        if Ks.shape != (S, 3, 3):
-            raise ValueError(f'step: Ks must be [{S},3,3], got {Ks.shape}')
-        kind = self._kind() if part is None else part.kind
-        imgs = fr.as_frames(frames, 'step', est.detector)
-        plan = fr.FramePlan(fr.size_pattern(imgs))
-        if plan.mixed:
-            fr.check_frames(imgs, Ks, 'step')
-        stepped = np.arange(self.S) if part is None else part.seq[:part.a]
-        pending, check = self._pending[stepped].copy(), self._verify.due(kind, self._since[stepped])
-        res = self._step_device(imgs, Ks, kind, plan, out, part, check)
-        if part is None:
-            self._pending[:] = False
-        else:
-            self._pending[part.seq] = False
-            res = {name: part.results(*r) for name, r in res.items()}
-        self._verify.advance(self._since, stepped, pending, check)
-        if check:
-            lost = np.any([r[2]['verify']['lost'] for r in res.values()], 0)
-            lost = self._verify.lost_sequences(stepped if part is None else part.sequences, lost)
-            if len(lost):
-                self.reset(lost)
-        return res
-
-    def _step_device(self, imgs, Ks, kind, plan, out=None, part=None, check=False):
-        """One step's graph; part: a partial step (row f17), check: verify (row f20), as in Tracker._step_device."""
-        K, est = self.K, self.est
-        S, pending, f32 = (self.S, self._pending, self._f32) if part is None else (part.b, part.pending, part.f32)
-        rows = (lambda n: n) if part is None else part.name
-        drawer = self._drawer if part is None or self._drawer is None else self._drawer.for_sequences(part.b)
-        full, mixed = kind == 'full', kind == 'mixed'
-        pick = None
-        draw, dt, drawn, named = draw_inputs(drawer, est.detector, plan, out, None if part is None else part.a)
-        dev = est.detector.device
-        if self._prev is None and (part is not None or mixed):
-            self._prev = torch.zeros(K * self.S, 12, dtype=torch.float64, device=dev)
-        wrap, extra = (lambda fn: fn), []
-        if part is not None:
-            wrap = lambda fn: _compact_fn(fn, full)
-        with torch.no_grad():
-            if full:
-                name, fn, fin = fr.stage(est.detector, named(rows('track_full')), wrap(self._full_fn(draw)), imgs, plan)
-            elif not mixed:
-                prev_f32 = bool(f32[0])
-                base, body = f'track_refine{int(prev_f32)}', self._refine_fn(prev_f32, draw)
-                if check:
-                    key = self._verify.key
-                    base, body = V.graph_name(base, key), V.verifying(body, self.objs._verify_fn(key))
-                name, fn, fin = fr.stage(est.detector, named(rows(base)), wrap(body), imgs, plan)
-            else:
-                reinit, b, extra = _mixed_inputs(S, K, pending, f32, est.cfg['refine_iter'], self.refine_iter, dev, plan)
-                if plan.mixed:                   # one graph per size pattern and per-size buckets (row f13)
-                    _, blocks, pick = _size_buckets(reinit, plan)
-                    name, fn = named(rows((plan.key('track_mixed'), tuple(blocks)))), self._mixed_fn(b, blocks, draw, S)
-                else:
-                    name, fn = named(rows(f'track_mixed{b}')), self._mixed_fn(b, draw=draw, S=S)
-                name, fn, fin = fr.bind(est.detector, name, wrap(fn), imgs, plan)
-            if part is not None:
-                state = [self._prev, self._ring, self._count] + part.graph_inputs(dev)
-            else:
-                state = [self._ring, self._count] if full else [self._prev, self._ring, self._count]
-            cams = est.detector._to_dev(glue.cameras(Ks))
-            buf, poses_dev, ring, count = self.stages.run(name, fn, fin + [cams] + state + extra + dt)
-            prev_f32 = bool(f32[0])
-            self._prev = poses_dev.clone()
-            self._ring.copy_(ring)
-            self._count.copy_(count)
-            host = est.detector._to_host(buf)                        # the step's one synchronising read
-        if part is None:
-            self._f32[:] = True
-        else:
-            self._f32[part.seq] = True
-        if not mixed:
-            reinit, b = None, None
-        if check:
-            host, checked = V.split(host, K * S)
-        res = self._decode(host, kind, S, reinit, b, pick, prev_f32, drawn)
-        if check:
-            for o, r in enumerate(res.values()):
-                r[2]['verify'] = {k: v[o * S:(o + 1) * S] for k, v in checked.items()}
-        return res
-
-    def _decode(self, host, kind, S, reinit, b, pick, prev_f32, drawn):
-        K, num, est = self.K, self.num, self.est
-        full, mixed = kind == 'full', kind == 'mixed'
-        n = K * S
-        if mixed:
-            n_chain, qn, m = max(est.cfg['refine_iter'], self.refine_iter) + 1, b, len(reinit)
-        else:
-            n_chain, qn, m = (est.cfg['refine_iter'] if full else self.refine_iter) + 1, S, S
-        pick = slice(0, m) if pick is None else pick             # the gathered row of each re-initialised sequence
-        if full or (mixed and qn):
-            res = est.cfg['ref_resolution']
-            crop_bytes = K * qn * res * res * 3
-            f64 = host[:len(host) - crop_bytes].view(np.float64)
-            crops = host[len(host) - crop_bytes:].reshape(K, qn, res, res, 3)
-        else:
-            f64 = host.view(np.float64)
-        off = 0
-
-        def take(m):
-            nonlocal off
-            off += m
-            return f64[off - m:off]
-        chain = take(n_chain * n * 12).reshape(n_chain, K, S, 3, 4)
-        smoothed = take(n * 12).reshape(K, S, 3, 4)
-        avg = take(n * 16).reshape(K, S, 8, 2)
-        ring_h = take(n * num * 16).reshape(K, S, num, 8, 2).astype(np.float32)
-        count_h = take(n).reshape(K, S).astype(np.int64)
-        res = {}
-        for o, (name, ob) in enumerate(self.objs._objects.items()):
-            refined = [c.astype(np.float32) for c in chain[1:, o]]
-            first = chain[0, o].astype(np.float32) if (kind == 'refine' and prev_f32) else chain[0, o].copy()
-            inter = {'reinit': reinit.astype(np.int64)} if mixed else {}
-            if full or (mixed and qn):
-                d = take(qn * 4).reshape(qn, 4)[pick].astype(np.float32)
-                idx = take(qn)[pick].astype(np.int64)
-                sel_out = take(qn * 2).reshape(qn, 2)[pick].astype(np.float32)
-                logits = take(qn * len(ob.ref_info['poses'])).reshape(qn, -1)[pick].astype(np.float32)
-                inter.update({'det_position': d[:, :2].copy(), 'det_scale_r2q': d[:, 2].copy(), 'det_score': d[:, 3].copy(),
-                              'det_que_img': crops[o, pick].copy(), 'sel_angle_r2q': sel_out[:, 0].copy(), 'sel_scores': logits,
-                              'sel_ref_idx': idx})
-            inter['refine_poses'] = [first] + refined
-            inter['bbox_pts'] = ring_h[o, np.arange(S), count_h[o] - 1].copy()
-            inter['smoothed_pts'] = avg[o].copy()
-            if drawn is not None:
-                inter['drawn'] = drawn
-            res[name] = (refined[-1] if refined else first), smoothed[o].copy(), inter
-        return res
