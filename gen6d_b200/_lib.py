@@ -104,6 +104,8 @@ _SIGNATURES = {
     'g6d_instances_associate_objects_host': [I, I, I, I, I, P, P, P, P, P, D, D, I, P, P, P, P, P, P, P, P, I, P, P, P, P, P, P],
     'g6d_instances_associate_sequences': [I, I, I, I, I, I, P, P, P, P, P, P, D, D, I, P, P, P, P, P, P, P, P, I, P, P, P, P, P, P, P],
     'g6d_instances_associate_sequences_host': [I, I, I, I, I, I, P, P, P, P, P, P, D, D, I, P, P, P, P, P, P, P, P, I, P, P, P, P, P, P],
+    'g6d_instances_verify_update': [I, P, P, I, P, P, P, P, P],
+    'g6d_instances_verify_update_host': [I, P, P, I, P, P, P, P],
     'g6d_nchw_to_nhwc': [P, P, I, I, I, I, I, P],
     'g6d_nhwc_to_nchw': [P, P, I, I, I, I, I, P],
     'g6d_resize_bilinear': [P, P, I, I, I, I, I, I, I, I, P],

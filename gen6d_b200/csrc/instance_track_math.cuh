@@ -10,6 +10,9 @@
 // detection batch of D rows per slot group (det_index[s], -1: the sequence does not detect): the detecting pairs run the
 // association on detection rows g*D + j, the others only set up their refinement, as a refine-only step does.
 //
+// A verifying step (g6d_instances_verify_update, row f21) feeds the same miss rule (track_seen): a live slot judged lost
+// is a track not seen, one judged found a track matched.
+//
 // Layout: K objects with M instance slots each over S sequences; slot group g = m*K + o is instance slot m of object o,
 // and row g*S + s is that slot on sequence s.  A single object (g6d_instances_associate) is K = 1, where g = m and every
 // row index, work row and id is the one of the single-object layout.
@@ -84,6 +87,27 @@ G6D_HD void copy12(double* dst, const double* src) {
     for (int k = 0; k < 12; ++k) dst[k] = src[k];
 }
 
+// Live slot i after a look at its frame: seen (matched to a detection, or judged found by verification) restarts its
+// misses; not seen takes a miss and is dropped past max_misses (live 0, ids -1, misses 0, its id written to dropped[i]).
+G6D_HD void track_seen(long long i, bool seen, int max_misses, int* live, long long* ids, int* misses, long long* dropped) {
+    if (seen) {
+        misses[i] = 0;
+    } else if (++misses[i] > max_misses) {
+        dropped[i] = ids[i];
+        live[i] = 0;
+        ids[i] = -1;
+        misses[i] = 0;
+    }
+}
+
+// The verification update of row i (g6d_instances_verify_update): dropped[i] = -1, then a live slot of a verified row is
+// seen unless judged lost.  Empty slots and unverified rows keep their state.
+G6D_HD void verify_update(long long i, const int* lost, const int* verified, int max_misses, int* live, long long* ids, int* misses,
+                          long long* dropped) {
+    dropped[i] = -1;
+    if (verified[i] && live[i]) track_seen(i, !lost[i], max_misses, live, ids, misses, dropped);
+}
+
 // Everything of sequence s and object o except the new tracks' ids; returns the number of tracks it spawns.  The pair's
 // slot t is row base + t*stride (base = o*S + s, stride = K*S: slot group g = t*K + o) and matches only its object's
 // detection rows, with its object's centre.
@@ -132,14 +156,7 @@ G6D_HD int associate_sequence(int s, int o, const Args& a) {
         a.dropped[i] = -1;
         is_new[t] = false;
         if (!a.live[i]) continue;
-        if (match[t] >= 0) {
-            a.misses[i] = 0;
-        } else if (++a.misses[i] > a.max_misses) {
-            a.dropped[i] = a.ids[i];
-            a.live[i] = 0;
-            a.ids[i] = -1;
-            a.misses[i] = 0;
-        }
+        track_seen(i, match[t] >= 0, a.max_misses, a.live, a.ids, a.misses, a.dropped);
     }
     // work row of slot t: its group's S real rows, then S scratch rows
     auto real_row = [&](int t) { return (long long)(t * a.K + o) * 2 * S + s; };

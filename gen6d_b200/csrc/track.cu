@@ -116,6 +116,20 @@ static int associate_launch(const char* name, const assoc::Args& a, long long* n
     return G6D_OK;
 }
 
+// Verification's slot update: one thread per row.
+__global__ void __launch_bounds__(128) instances_verify_update_kernel(int n, const int* lost, const int* verified, int max_misses, int* live,
+                                                                      long long* ids, int* misses, long long* dropped) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) assoc::verify_update(i, lost, verified, max_misses, live, ids, misses, dropped);
+}
+
+static int verify_update_ok(const char* name, int n, const int* lost, const int* verified, int max_misses, const int* live,
+                            const long long* ids, const int* misses, const long long* dropped) {
+    G6D_REQUIRE(n >= 1 && max_misses >= 0, "%s: need n >= 1 and max_misses >= 0 (got n=%d, max_misses=%d)", name, n, max_misses);
+    G6D_REQUIRE(lost && verified && live && ids && misses && dropped, "%s: null pointer", name);
+    return G6D_OK;
+}
+
 }  // namespace g6d
 
 using namespace g6d;
@@ -262,5 +276,24 @@ extern "C" int g6d_track_smooth_objects_host(const double* poses, int poses_are_
         G6D_REQUIRE(count[i] >= 0 && count[i] <= num, "g6d_track_smooth_objects_host: count[%d] = %d is beyond the ring of %d frames", i,
                     count[i], num);
     for (int i = 0; i < n_rows; ++i) smooth_row_objects(i, rows_per_obj, poses, poses_are_f32, bboxes, Ks, ring, count, num, weights, smoothed, avg_pts);
+    return G6D_OK;
+}
+
+extern "C" int g6d_instances_verify_update(int n, const int* lost, const int* verified, int max_misses, int* live, long long* ids,
+                                           int* misses, long long* dropped, g6d_stream_t stream) {
+    const char* name = "g6d_instances_verify_update";
+    const int rc = verify_update_ok(name, n, lost, verified, max_misses, live, ids, misses, dropped);
+    if (rc != G6D_OK) return rc;
+    instances_verify_update_kernel<<<ceil_div(n, 128), 128, 0, as_stream(stream)>>>(n, lost, verified, max_misses, live, ids, misses,
+                                                                                     dropped);
+    G6D_CHECK_LAUNCH(name);
+    return G6D_OK;
+}
+
+extern "C" int g6d_instances_verify_update_host(int n, const int* lost, const int* verified, int max_misses, int* live, long long* ids,
+                                                int* misses, long long* dropped) {
+    const int rc = verify_update_ok("g6d_instances_verify_update_host", n, lost, verified, max_misses, live, ids, misses, dropped);
+    if (rc != G6D_OK) return rc;
+    for (int i = 0; i < n; ++i) assoc::verify_update(i, lost, verified, max_misses, live, ids, misses, dropped);
     return G6D_OK;
 }

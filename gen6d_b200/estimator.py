@@ -395,10 +395,10 @@ class Gen6DEstimator:
         return instances.inter_of(chain, *parts, rd.crops.reshape(n, res, res, 3), M, qn)
 
     # ------------------------------------------------------------------ checking poses with the detector (row f20)
-    def _verify_fn(self, st, key):
-        """The verification nodes (verify.nodes) of this estimator's object."""
+    def _verify_fn(self, st, key, M=1):
+        """The verification nodes (verify.nodes) of this estimator's object; M: row groups (an instance tracker's slots)."""
         from . import verify
-        return verify.nodes(self, [st['refs']], [self.detector._detect_u8], key)
+        return verify.nodes(self, [st['refs']], [self.detector._detect_u8], key, M)
 
     def verify_poses(self, frames, Ks, poses, lost_score=None, lost_gate=None):
         """Check each pose with the detector on a window around the object (row f20; gen6d_b200/verify.py).  Pose i on
@@ -457,7 +457,7 @@ class Gen6DEstimator:
 
     def instance_tracker(self, num_sequences=1, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
                          min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bbox_3d=None, draw=None,
-                         draw_color=(0, 0, 255), schedule='lockstep'):
+                         draw_color=(0, 0, 255), schedule='lockstep', verify_every=None, lost_score=None, lost_gate=None):
         """An InstanceTracker (gen6d_b200/instance_track.py): every instance of the object, up to `max_instances` per frame,
         followed through `num_sequences` videos in lockstep.  The first step (and the one after reset() / redetect(), and
         every `redetect_every`-th step after the last re-detection) detects predict_instances' instances (min_score,
@@ -468,12 +468,21 @@ class Gen6DEstimator:
         draw_color: as for tracker(); every live slot (track id >= 0) is drawn, in slot order.
         schedule (row f18): 'lockstep' (every sequence re-detects on the same steps), 'per_sequence' (each sequence has its
         own re-detection flag and counter; reset / redetect take sequences, and step takes sequences= to step any subset)
-        or 'staggered' ('per_sequence' with the periodic re-detections spread over the steps; needs redetect_every)."""
+        or 'staggered' ('per_sequence' with the periodic re-detections spread over the steps; needs redetect_every).
+        verify_every (row f21): a step in which a stepped sequence that does not re-detect has taken verify_every steps
+        since its last re-detection, reset(), redetect() or verification also checks the final pose of every slot of
+        every such sequence as verify_poses(lost_score, lost_gate) does, inside the step's graph, and returns the result
+        as inter['verify'] ([S, M] per key; empty slots and re-detecting sequences NaN / not lost).  With a threshold, a
+        live track judged lost takes a miss and is dropped past max_misses as an unmatched track is at a re-detection
+        (inter['verify']['dropped'] lists the ids), one judged found restarts its misses, and every sequence with a lost
+        track re-detects on its next step (detecting(); lockstep: every sequence).  Thresholds None: verify and report,
+        never change a track."""
         from .instance_track import InstanceTracker
         return InstanceTracker(self, num_sequences, max_instances=max_instances, refine_iter=refine_iter,
                                redetect_every=redetect_every, gate=gate, max_misses=max_misses, min_score=min_score, nms_iou=nms_iou,
                                peak_radius=peak_radius, smooth_num=smooth_num, smooth_std=smooth_std, bbox_3d=bbox_3d,
-                               draw=draw, draw_color=draw_color, schedule=schedule)
+                               draw=draw, draw_color=draw_color, schedule=schedule, verify_every=verify_every,
+                               lost_score=lost_score, lost_gate=lost_gate)
 
     def track(self, que_imgs, que_K, **tracker_kwargs):
         """predict.py's loop over one video: que_imgs uint8 [h,w,3] frames of one size, que_K [3,3] (or one per frame).

@@ -44,6 +44,15 @@ records (g6d_det_from_boxes) take the place of the peaks in the same bodies, und
 re-detection step.  Per-sequence schedules: exactly the stepped sequences given boxes re-detect (the mixed step when only
 some do), and their detection counts in the schedule as a detector detection does; a due sequence without boxes is not
 detected and stays due.
+
+Verification (row f21, verify_every=): a step verifies when a stepped sequence that does not re-detect on it has taken
+verify_every steps since its last re-detection, reset, redetect or verification (verify.Schedule.due_rows); refine and
+mixed steps alike.  Its graph is the unchanged step body followed by verify.nodes on the final float32 poses of every slot
+row (M*K*S windows, one detector call per object over its M*S windows) and, with a threshold set,
+g6d_instances_verify_update: a live slot of a verified sequence judged lost takes a miss and is dropped past max_misses
+as the association drops an unmatched track, one judged found restarts its misses.  Everything lands in the same read,
+under verify.graph_name.  The sequences with a lost slot then re-detect on their next step ('lockstep': every sequence),
+so the association can correct a wrong verdict and a track it matches keeps its id.
 """
 import numpy as np
 import torch
@@ -55,6 +64,7 @@ from . import frames as fr
 from . import glue
 from . import instances
 from . import ops
+from . import verify as V
 from .graphs import StageCache
 from .track import (PartialStep, _bucket, _gather_rows, _scatter_rows, _sequences, _size_buckets, check_bbox, draw_inputs,
                     object_bbox, object_bboxes, smoothing_weights)
@@ -175,6 +185,20 @@ def host_associate_objects(det, valid, init, cams, centers, ref_resolution, gate
     return work, flags0, lists, det_slot, spawned, dropped
 
 
+def host_verify_update(lost, verified, max_misses, live, ids, misses):
+    """g6d_instances_verify_update_host on numpy arrays: lost, verified int [n]; live int32, ids int64 and misses int32
+    [n] are updated in place.  Returns dropped int64 [n]."""
+    for a, dt in ((live, np.int32), (ids, np.int64), (misses, np.int32)):
+        if a.dtype != dt or not a.flags.c_contiguous:
+            raise ValueError(f'host_verify_update: the state arrays must be contiguous {dt.__name__} arrays (updated in place)')
+    lost, verified = np.ascontiguousarray(lost, np.int32), np.ascontiguousarray(verified, np.int32)
+    dropped = np.zeros(len(live), np.int64)
+    _lib.check(_lib.lib().g6d_instances_verify_update_host(len(live), lost.ctypes.data, verified.ctypes.data, int(max_misses),
+                                                           live.ctypes.data, ids.ctypes.data, misses.ctypes.data,
+                                                           dropped.ctypes.data), 'g6d_instances_verify_update_host')
+    return dropped
+
+
 def check_det_index(det_index, S, D):
     """ValueError unless det_index [S] holds -1 (the sequence does not detect) or distinct rows j < D, with 0 <= D <= S."""
     det_index = np.asarray(det_index).reshape(-1)
@@ -258,13 +282,16 @@ class InstanceTracker:
     subclass supplies the per-group tables (_groups), the detection (_detection), the id association (_associate) and the
     readback of the selections (_take_selections)."""
 
+    _verify = V.Schedule()           # no verification (row f21)
+
     def __init__(self, est, num_sequences, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
                  min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bbox_3d=None, draw=None,
-                 draw_color=dr.DEFAULT_COLOR, schedule='lockstep'):
+                 draw_color=dr.DEFAULT_COLOR, schedule='lockstep', verify_every=None, lost_score=None, lost_gate=None):
         from .objects import require_device_pipeline
         require_device_pipeline(est, 'instance tracking')
         key = check_args(num_sequences, max_instances, refine_iter, redetect_every, gate, max_misses, min_score, nms_iou,
                          peak_radius, smooth_num, smooth_std, schedule)
+        verify = V.Schedule(verify_every, lost_score, lost_gate)
         if bbox_3d is None:
             bbox_3d = object_bbox(est.refiner.ref_database)
             if bbox_3d is None:
@@ -272,13 +299,14 @@ class InstanceTracker:
         self.bbox = check_bbox(bbox_3d)
         self._gen = est._generation()
         self._setup(est, key, [self.bbox], num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std,
-                    draw, [draw_color], schedule)
+                    draw, [draw_color], schedule, verify)
         center = np.asarray(est.ref_info['center'], np.float64).reshape(1, 3)
         self._dev['centers'] = torch.from_numpy(np.ascontiguousarray(center)).to(est.detector.device)
 
     def _setup(self, est, key, boxes, num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std,
-               draw=None, colors=None, schedule='lockstep'):
-        """The tracker's constants and device state for K = len(boxes) objects with M = key[0] slots each."""
+               draw=None, colors=None, schedule='lockstep', verify=None):
+        """The tracker's constants and device state for K = len(boxes) objects with M = key[0] slots each; verify: a
+        verify.Schedule (row f21)."""
         self.est, self.key, self.schedule = est, key, schedule
         self.K, self.S, self.M, self.refine_iter = len(boxes), int(num_sequences), key[0], int(refine_iter)
         self.redetect_every = None if redetect_every is None else int(redetect_every)
@@ -301,6 +329,9 @@ class InstanceTracker:
         self._pending, self._since = True, 0
         # per-sequence schedules (row f18): each sequence's pending flag and steps since its last detection, on the host
         self._schedule = Schedule(self.S, self.redetect_every, schedule == 'staggered')
+        if verify is not None:
+            self._verify = verify
+        self._vsince = np.zeros(self.S, np.int64)     # steps since the last re-detection / reset / redetect / verification
         # drawing (row f16): every live slot (track id >= 0) of a sequence on its frame, in row (slot group) order
         kinds = self.draw = dr.parse_kinds(draw)
         G = self.M * self.K
@@ -323,6 +354,8 @@ class InstanceTracker:
         st['count'][rows] = 0
         self._pending = True
         self._schedule.pending[slice(None) if sequences is None else seqs] = True
+        if self._verify.every is not None:
+            self._vsince[slice(None) if sequences is None else seqs] = 0
 
     def redetect(self, sequences=None):
         """The next step re-detects: the live tracks are kept and associated with the new detections.  sequences (the
@@ -330,11 +363,16 @@ class InstanceTracker:
         if sequences is None:
             self._pending = True
             self._schedule.pending[:] = True
+            if self._verify.every is not None:
+                self._vsince[:] = 0
             return
         if self.schedule == 'lockstep':
             raise ValueError("redetect(sequences): a lockstep tracker re-detects every sequence together; create it with "
                              "schedule='per_sequence' or 'staggered' to re-detect single sequences")
-        self._schedule.pending[_sequences(self.S, sequences)] = True
+        seqs = _sequences(self.S, sequences)
+        self._schedule.pending[seqs] = True
+        if self._verify.every is not None:
+            self._vsince[seqs] = 0
 
     def detecting(self):
         """bool [S]: the sequences that re-detect on their next step."""
@@ -381,6 +419,10 @@ class InstanceTracker:
         the detected frames)."""
         n = self.M * S
         return [(rd.take(n), rd.take(n * 2), rd.take(n * len(self.est.ref_info['poses'])))]
+
+    def _verify_fn(self, st):
+        """verify.nodes over the M*K slot groups: each group's windows detected against its object's references."""
+        return self.est._verify_fn(st, self._verify.key, self.M)
 
     # -------------------------------------------------------------- the graphs
     def _detect_fn(self, st, draw=None, S=None, boxes=None):
@@ -500,6 +542,27 @@ class InstanceTracker:
             return buf, poses, park, live, ids, misses, next_id, ring, count
         return fn
 
+    def _verifying(self, body, st):
+        """A per-sequence step body (_body's signature) -> its verifying variant (row f21): the body unchanged, then
+        verify.nodes on its final float32 poses of every slot row, whose results are appended to the bytes read.  With a
+        threshold set the variant takes the verified rows (int32 [n], 0: the row's sequence re-detected or pads the batch)
+        as its last input, and g6d_instances_verify_update applies the verdicts to live, ids and misses after the body
+        packed them; its dropped ids go before the verification rows."""
+        nodes, update = self._verify_fn(st), self._verify.resets
+
+        def fn(frames, cams, *args):
+            if update:
+                *args, verified = args
+            outs = body(frames, cams, *args)
+            checked = nodes(frames, cams, outs[1], True)                      # [n, 10]: judge output, lost, window
+            parts = [outs[0]]
+            if update:
+                lost = checked[:, 5].to(torch.int32).contiguous()
+                live, ids, misses = outs[3:6]
+                parts.append(ops.instances_verify_update(lost, verified, self.max_misses, live, ids, misses).view(torch.uint8))
+            return (torch.cat(parts + [checked.reshape(-1).view(torch.uint8)]), *outs[1:])
+        return fn
+
     # -------------------------------------------------------------- one step
     def step(self, frames, Ks, out=None, sequences=None, boxes=None):
         """frames: S uint8 [h,w,3] (of one size or several, row f13; or device frames, row f14, as Tracker.step takes them);
@@ -523,7 +586,12 @@ class InstanceTracker:
         detection; the detector runs no kernel.  Lockstep: every entry must be an array (an empty one: no detections),
         and the step is a re-detection step that restarts the re-detection count.  Per-sequence schedules: exactly the
         sequences given an array re-detect, and each counts as re-detected; a due sequence given None is not detected
-        and stays due (detecting()).  So redetect_every=None with boxes on the first step never runs the detector."""
+        and stays due (detecting()).  So redetect_every=None with boxes on the first step never runs the detector.
+
+        A tracker made with verify_every (row f21) adds inter['verify'] to the steps that verify: verify_poses' keys [S,M]
+        on the step's final poses (empty slots and sequences that re-detected on the step: lost False, NaN), and with a
+        threshold 'dropped', the ids the verdicts removed.  poses, smoothed and track_ids are the step's own; a dropped
+        track's id is -1 from the next step on, and the sequences with a lost track re-detect on their next step."""
         return self._step(frames, Ks, out, sequences, boxes)[0]
 
     def _step(self, frames, Ks, out=None, sequences=None, boxes=None):
@@ -550,6 +618,7 @@ class InstanceTracker:
         res = self._run(frames, Ks, out, 'detect' if detecting else 'refine', boxes=table)
         self._pending = False
         self._since = 1 if detecting else self._since + 1
+        self._mark_lost(res, np.arange(S))
         return res
 
     def _boxes(self, boxes, n):
@@ -559,9 +628,10 @@ class InstanceTracker:
     def _run(self, frames, Ks, out, kind, part=None, det_seq=None, boxes=None):
         """One step's graph and read -> decoded results.  kind: 'detect', 'refine' or 'mixed'; part: a partial step (row
         f17/f18) over its compact batch; det_seq: bool over the batch's sequences, those that re-detect (kind 'mixed');
-        boxes: a boxes.Table of the batch's maps, the detection of a 'detect' or 'mixed' step (row f19)."""
+        boxes: a boxes.Table of the batch's maps, the detection of a 'detect' or 'mixed' step (row f19).  The step
+        verifies (row f21) when the schedule says so; its results then hold inter['verify']."""
         est = self.est
-        S = self.S if part is None else part.b
+        S, stepped, refining, check = self._verify_plan(kind, part, det_seq)
         F = est.cfg['refine_iter']
         if kind != 'refine' and F < 1:
             raise ValueError("instance tracking needs cfg['refine_iter'] >= 1 (a re-detection step smooths float32 poses)")
@@ -573,21 +643,25 @@ class InstanceTracker:
         drawer = self._drawer if part is None or self._drawer is None else self._drawer.for_sequences(part.b)
         draw, dt, drawn, named = draw_inputs(drawer, est.detector, plan, out, None if part is None else part.a)
         dev = est.detector.device
-        det_rows, extra, D = None, [], S
+        up = lambda a, dt_: torch.from_numpy(np.ascontiguousarray(a, dt_)).to(dev)
+        det_rows, extra, D, vin = None, [], S, []
         dbox = tail = None
         if boxes is not None and kind != 'refine':
             dbox = B.Detect(self.M, self.K, boxes.n_maps, boxes.N, B.inv_box_size(est.cfg['ref_resolution']))
             tail = [boxes.upload(est.detector)]
         if kind == 'mixed':
             seq, blocks, det_rows, D, key = plan_mixed(det_seq, plan)
-            up = lambda a, dt_: torch.from_numpy(np.ascontiguousarray(a, dt_)).to(dev)
             extra = [up(seq, np.int64), up(det_rows, np.int32)]
             base, fn = mixed_name(S, key), self._body(stt, 'mixed', S, D, blocks, draw, dbox)
-        elif part is None:
+        elif part is None and not check:
             base = kind
             fn = self._detect_fn(stt, draw, boxes=dbox) if kind == 'detect' else self._refine_fn(stt, draw)
         else:
             base, fn = kind, self._body(stt, kind, S, draw=draw, boxes=dbox)
+        if check:                                  # the verifying variant takes and returns the whole slot state
+            base, fn = V.graph_name(base, self._verify.key), self._verifying(fn, stt)
+            if self._verify.resets:
+                vin = [up(np.tile(refining, self.M * self.K), np.int32)]
         if dbox is not None:
             base, fn = B.graph_name(base, boxes.N), dbox.bind(fn)
         if part is not None:
@@ -597,12 +671,12 @@ class InstanceTracker:
         with torch.no_grad():
             name, fn, fin = fr.stage(est.detector, named(base), fn, imgs, plan)
             cams = est.detector._to_dev(glue.cameras(Ks))
-            if part is None and kind == 'refine':
+            if part is None and kind == 'refine' and not check:
                 outs = self.stages.run(name, fn, fin + [cams, x['prev'], x['park'], x['live'], x['ids'], x['ring'], x['count']] + dt)
                 buf, poses, ring, count = outs
             else:
                 outs = self.stages.run(name, fn, fin + [cams, x['prev'], x['park'], x['live'], x['ids'], x['misses'], self._next_id,
-                                                        x['ring'], x['count']] + extra + dt + (tail or []))
+                                                        x['ring'], x['count']] + extra + dt + vin + (tail or []))
                 buf, poses, park, live, ids, misses, next_id, ring, count = outs
                 for k, v in (('park', park), ('live', live), ('ids', ids), ('misses', misses)):
                     x[k].copy_(v)
@@ -611,11 +685,65 @@ class InstanceTracker:
             x['ring'].copy_(ring)
             x['count'].copy_(count)
             host = est.detector._to_host(buf)                        # the step's one synchronising read
+        if check:
+            host, checked, dropped = self._split_verify(host, self.M * self.K * S)
         res = self._decode(host, kind != 'refine', S, det_rows, D)
         if drawn is not None:
             for r in res:
                 r[3]['drawn'] = drawn
+        if check:
+            self._verify_results(res, checked, dropped, refining, S)
+        self._verify_done(stepped, refining, check)
         return res
+
+    def _verify_plan(self, kind, part=None, det_seq=None):
+        """A step's verification plan (row f21) -> (S: the batch's sequences, stepped: the real ones' tracker indices,
+        refining bool [S]: the batch rows that do not re-detect, padding excluded, check: the step verifies)."""
+        S = self.S if part is None else part.b
+        stepped = np.arange(self.S) if part is None else part.seq[:part.a]
+        refining = np.full(S, kind == 'refine') if det_seq is None else ~np.asarray(det_seq, bool)
+        refining[len(stepped):] = False
+        return S, stepped, refining, self._verify.due_rows(self._vsince[stepped], refining[:len(stepped)])
+
+    def _verify_done(self, stepped, refining, check):
+        """The verification counts after the step: re-detected sequences restart, the others count the step, and a
+        verifying step restarts every stepped sequence."""
+        V.Schedule.advance(self._vsince, stepped, ~refining[:len(stepped)], check)
+
+    def _split_verify(self, host, n):
+        """A verifying step's read -> (the step body's bytes, verify.decode's dict of its n slot rows, the update's dropped
+        int64 [n] or None without a threshold)."""
+        host, checked = V.split(host, n)
+        dropped = None
+        if self._verify.resets:
+            host, dropped = host[:len(host) - n * 8], host[len(host) - n * 8:].view(np.int64)
+        return host, checked, dropped
+
+    def _verify_results(self, res, checked, dropped, refining, S):
+        """inter['verify'] of every object: verify_poses' keys [S, M] in the step's row order, rows of empty slots and of
+        sequences that did not refine (re-detected, or padding) lost False and NaN; 'dropped' (with a threshold) the ids
+        the update removed, ascending."""
+        M, K = self.M, self.K
+        for o, (_, _, ids, inter) in enumerate(res):
+            skip = (ids < 0) | ~refining[:, None]
+            v = {}
+            for k, a in checked.items():
+                a = instances.frame_major(a.reshape(M, K, S, *a.shape[1:])[:, o].reshape(M * S, *a.shape[1:]), M, S)
+                a[skip] = False if a.dtype == bool else np.nan
+                v[k] = a
+            if dropped is not None:
+                v['dropped'] = sorted(int(i) for i in dropped.reshape(M, K, S)[:, o].reshape(-1) if i >= 0)
+            inter['verify'] = v
+
+    def _mark_lost(self, res, seqs):
+        """After a verifying step with a threshold set: every stepped sequence (seqs, the leading rows of the step's
+        batch) with a slot judged lost re-detects on its next step, as redetect([s]) does; a lockstep tracker re-detects
+        together, as redetect() does."""
+        if not self._verify.resets or 'verify' not in res[0][3]:
+            return
+        lost = np.any([r[3]['verify']['lost'][:len(seqs)].any(1) for r in res], 0)
+        if lost.any():
+            self.redetect(None if self.schedule == 'lockstep' else seqs[lost])
 
     def _step_sequences(self, frames, Ks, out, sequences, boxes=None):
         """A step on a per-sequence schedule (row f18): the stepped sequences' plan, one graph, their counters.  boxes (row
@@ -647,6 +775,7 @@ class InstanceTracker:
         det_seq, kind = sch.plan(seqs, n_real, hit)
         res = self._run(frames, Ks, out, kind, None if part is None or part.lockstep else part, det_seq, table)
         sch.advance(seqs[:n_real], det_seq[:n_real])
+        self._mark_lost(res, seqs[:n_real])
         for r in res:
             r[3]['detected'] = det_seq.copy()
         if part is None:
@@ -751,9 +880,12 @@ def _reorder(res, part):
     poses, smoothed, ids, inter = res
     inter = dict(inter)
     dropped = inter.pop('dropped', None)
+    verify_dropped = inter['verify'].pop('dropped', None) if 'verify' in inter else None
     poses, smoothed, inter = part.results(poses, smoothed, inter)
     if dropped is not None:
         inter['dropped'] = dropped
+    if verify_dropped is not None:
+        inter['verify']['dropped'] = verify_dropped
     return poses, smoothed, ids[part.pos], inter
 
 
@@ -764,15 +896,16 @@ class ObjectInstanceTracker(InstanceTracker):
 
     def __init__(self, objs, num_sequences, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
                  min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bboxes=None, draw=None,
-                 draw_colors=None, schedule='lockstep'):
+                 draw_colors=None, schedule='lockstep', verify_every=None, lost_score=None, lost_gate=None):
         key = check_args(num_sequences, max_instances, refine_iter, redetect_every, gate, max_misses, min_score, nms_iou,
                          peak_radius, smooth_num, smooth_std, schedule)
+        verify = V.Schedule(verify_every, lost_score, lost_gate)
         objs._check()
         boxes = object_bboxes(objs, bboxes)
         self.objs, self.names, self.bboxes = objs, objs.names, np.ascontiguousarray(np.stack(boxes, 0))
         self._membership = objs.membership
         self._setup(objs.est, key, boxes, num_sequences, refine_iter, redetect_every, gate, max_misses, smooth_num, smooth_std,
-                    draw, dr.object_colors(self.names, draw_colors), schedule)
+                    draw, dr.object_colors(self.names, draw_colors), schedule, verify)
         centers = np.stack([np.asarray(ob.ref_info['center'], np.float64).reshape(3) for ob in objs._objects.values()], 0)
         self._dev['centers'] = torch.from_numpy(np.ascontiguousarray(centers)).to(self.est.detector.device)
 
@@ -806,6 +939,9 @@ class ObjectInstanceTracker(InstanceTracker):
 
     def _boxes(self, boxes, n):
         return B.for_sequences(boxes, n, 'step', self.est.detector.device, self.names)
+
+    def _verify_fn(self, st):
+        return self.objs._verify_fn(self._verify.key, self.M)
 
     def _take_selections(self, rd, S):
         M, K = self.M, self.K

@@ -330,12 +330,14 @@ class ObjectSet:
                                            valid[:, o], count[o], crops[:, o].reshape(M * qn, res, res, 3), M, qn)
         return out
 
-    def _verify_fn(self, key):
+    def _verify_fn(self, key, M=1):
         """The verification nodes (verify.nodes) of the set's objects, each object's windows detected against its own
-        references: the launches of Gen6DEstimator.verify_poses on an estimator built on that object."""
+        references: the launches of Gen6DEstimator.verify_poses on an estimator built on that object.  M: row groups per
+        object (an instance tracker's slots)."""
         objs = list(self._objects.values())
         det = self.est.detector
-        return verify.nodes(self.est, [ob.tables['refs'] for ob in objs], [partial(det._detect_u8, refs=ob.det) for ob in objs], key)
+        return verify.nodes(self.est, [ob.tables['refs'] for ob in objs], [partial(det._detect_u8, refs=ob.det) for ob in objs], key,
+                            M)
 
     def verify_poses(self, que_imgs, que_Ks, poses, lost_score=None, lost_gate=None):
         """Gen6DEstimator.verify_poses for every object of the set on the same qn frames: poses {name: [qn,3,4]} for every
@@ -382,7 +384,7 @@ class ObjectSet:
 
     def instance_tracker(self, num_sequences=1, max_instances=4, refine_iter=1, redetect_every=None, gate=0.5, max_misses=1,
                          min_score=None, nms_iou=0.3, peak_radius=1, smooth_num=5, smooth_std=2.5, bboxes=None, draw=None,
-                         draw_colors=None, schedule='lockstep'):
+                         draw_colors=None, schedule='lockstep', verify_every=None, lost_score=None, lost_gate=None):
         """An ObjectInstanceTracker (gen6d_b200/instance_track.py): every instance of every object of the set, up to
         `max_instances` per object and frame, followed through `num_sequences` videos in lockstep, with
         Gen6DEstimator.instance_tracker()'s semantics per object (each object's tracks are matched only to its own
@@ -391,12 +393,15 @@ class ObjectSet:
         tracker(); only live slots (track id >= 0) are drawn.
         schedule (row f18): 'lockstep' (every sequence re-detects on the same steps), 'per_sequence' (each sequence has its
         own re-detection flag and counter; reset / redetect take sequences, and step takes sequences= to step any subset)
-        or 'staggered' ('per_sequence' with the periodic re-detections spread over the steps; needs redetect_every)."""
+        or 'staggered' ('per_sequence' with the periodic re-detections spread over the steps; needs redetect_every).
+        verify_every, lost_score, lost_gate: as for Gen6DEstimator.instance_tracker() (row f21), each object's windows
+        detected against its own references; a sequence re-detects when any slot of any object is judged lost."""
         from .instance_track import ObjectInstanceTracker
         return ObjectInstanceTracker(self, num_sequences, max_instances=max_instances, refine_iter=refine_iter,
                                      redetect_every=redetect_every, gate=gate, max_misses=max_misses, min_score=min_score,
                                      nms_iou=nms_iou, peak_radius=peak_radius, smooth_num=smooth_num, smooth_std=smooth_std,
-                                     bboxes=bboxes, draw=draw, draw_colors=draw_colors, schedule=schedule)
+                                     bboxes=bboxes, draw=draw, draw_colors=draw_colors, schedule=schedule,
+                                     verify_every=verify_every, lost_score=lost_score, lost_gate=lost_gate)
 
     def raw_correlation(self, que_imgs):
         """The detector's raw correlation maps for inspection: {name: [scale][level] float32 [qn, H, W, rfn]} (the maps

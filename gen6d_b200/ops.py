@@ -511,6 +511,19 @@ def instances_associate_sequences(det_index, det, valid, init, cams, centers, re
     return work, flags0, lists, det_slot, spawned, dropped
 
 
+def instances_verify_update(lost, verified, max_misses, live, ids, misses):
+    """A verifying instance-tracking step's slot update (g6d_instances_verify_update): lost int32 [n] (verify_judge),
+    verified int32 [n] (0: a row that re-detected this step or pads the batch).  live int32, ids int64 and misses int32 [n]
+    are updated in place.  Returns dropped int64 [n] (-1: none), the association's layout."""
+    n = live.shape[0]
+    if lost.shape != (n,) or verified.shape != (n,) or ids.shape != (n,) or misses.shape != (n,):
+        raise ValueError(f'instances_verify_update: inconsistent shapes for {n} rows')
+    dropped = torch.empty(n, device=live.device, dtype=torch.int64)
+    _call('g6d_instances_verify_update', n, _p(lost, torch.int32), _p(verified, torch.int32), int(max_misses), _p(live, torch.int32),
+          _p(ids, torch.int64), _p(misses, torch.int32), _p(dropped, torch.int64), _stream())
+    return dropped
+
+
 def imagenet_norm(x, out_c=4):
     out = torch.empty(*x.shape[:-1], out_c, device=x.device, dtype=torch.float32)
     _call('g6d_imagenet_norm', _p(x), _p(out), x.numel() // x.shape[-1], x.shape[-1], out_c, _stream())

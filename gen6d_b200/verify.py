@@ -10,7 +10,8 @@ frame and judges the row lost: an invalid record, a score below lost_score, or a
 
 Gen6DEstimator.verify_poses / ObjectSet.verify_poses run this as one captured graph; the trackers' verify_every replays
 a verifying variant of the refine graph (the unchanged refine body, then these nodes, packed into the same read) and
-re-initialise the sequences judged lost (Schedule)."""
+re-initialise the sequences judged lost (Schedule).  The instance trackers' verify_every (row f21) runs the same nodes
+over every slot row, M row groups per object."""
 import math
 
 import numpy as np
@@ -52,20 +53,31 @@ def window_size(est):
     return WINDOW_FACTOR * int(est.cfg['ref_resolution'])
 
 
-def nodes(est, refs, detects, key):
-    """The verification nodes for K objects: fn(frames u8 [qn,h,w,3], cams f64 [qn,20], poses f64 [K*qn,12], poses_are_f32)
-    -> one float64 tensor [K*qn, 10] (judge output, lost, window record).  refs[o]: object o's g6d_glue_refs;
-    detects[o](windows u8 [qn,W,W,3]) -> det [qn,4]: the detector against object o's references only."""
+def nodes(est, refs, detects, key, M=1):
+    """The verification nodes for K objects: fn(frames u8 [qn,h,w,3], cams f64 [qn,20], poses f64 [M*K*qn,12],
+    poses_are_f32) -> one float64 tensor [M*K*qn, 10] (judge output, lost, window record).  Row g*qn + s is row group
+    g = m*K + o (an instance tracker's slot m of object o; M = 1: object o) on frame s.  refs[o]: object o's
+    g6d_glue_refs; detects[o](windows u8 [n,W,W,3]) -> det [n,4]: the detector against object o's references only, run
+    once per object over its M*qn windows.  Each window is cut from its own row's frame: the warp jobs of the object's M
+    groups point into the same frames, so no frame is copied."""
     W, res = window_size(est), float(est.cfg['ref_resolution'])
+    K = len(detects)
+    groups = list(refs) * M                        # group m*K + o: object o's refs
 
     def fn(frames, cams, poses, poses_are_f32):
         qn = frames.shape[0]
-        rec = ops.verify_windows(refs, cams, poses, poses_are_f32)
+        rec = ops.verify_windows(groups, cams, poses, poses_are_f32)
         dets = []
         for o, detect in enumerate(detects):
-            jobs = ops.glue_detection_jobs(rec[o * qn:(o + 1) * qn], frames, W)
-            dets.append(detect(ops.warp_affine_u8(jobs, qn, W, W)))
-        det = dets[0] if len(dets) == 1 else torch.cat(dets, 0)
+            jobs = [ops.glue_detection_jobs(rec[g * qn:(g + 1) * qn], frames, W) for g in range(o, M * K, K)]
+            jobs = jobs[0] if M == 1 else torch.cat(jobs)
+            dets.append(detect(ops.warp_affine_u8(jobs, M * qn, W, W)))
+        if K == 1:
+            det = dets[0]
+        elif M == 1:
+            det = torch.cat(dets, 0)
+        else:                                      # object-major per group -> row order (m*K + o)*qn + s
+            det = torch.stack([d.view(M, qn, 4) for d in dets], 1).reshape(M * K * qn, 4)
         out, lost = ops.verify_judge(rec, det, W, res, *key)
         return torch.cat([out.to(torch.float64), lost.to(torch.float64)[:, None], rec.to(torch.float64)], 1)
     return fn
@@ -118,7 +130,13 @@ class Schedule:
 
     def due(self, kind, since):
         """Does a step of `kind` over sequences with these counts verify?"""
-        return self.every is not None and kind == 'refine' and bool((np.asarray(since) + 1 >= self.every).any())
+        return kind == 'refine' and self.due_rows(since, np.ones(len(np.asarray(since)), bool))
+
+    def due_rows(self, since, refining):
+        """Does a step of any kind verify whose stepped sequences have counts `since`, of which those in `refining` do not
+        re-detect on it?  (The instance trackers, row f21: a step verifies when a refining sequence reaches `every`.)"""
+        since = np.asarray(since)[np.asarray(refining, bool)]
+        return self.every is not None and bool((since + 1 >= self.every).any())
 
     @staticmethod
     def advance(since, seqs, pending, verified):

@@ -387,6 +387,15 @@ int g6d_instances_associate_sequences_host(int S, int K, int M, int F, int r, in
                                            long long* ids, int* misses, long long* next_id, double* park, float* ring, int* count,
                                            int num, double* work, uint8_t* flags0, int* lists, int* det_slot, int* spawned,
                                            long long* dropped);
+/* A verifying instance-tracking step's slot update (row f21), per row i of n = M*K*S (the association's layout):
+ * dropped[i] = -1; then, when verified[i] and live[i], a row judged lost (lost[i] != 0, g6d_verify_judge) takes a miss
+ * and is dropped past max_misses exactly as the association drops an unmatched track (live 0, ids -1, misses 0, its id
+ * in dropped[i]), and a row judged found restarts its misses.  Empty slots and unverified rows (verified[i] == 0: a
+ * sequence that re-detected this step, or a padding row) are untouched.  live, ids and misses are updated in place. */
+int g6d_instances_verify_update(int n, const int* lost, const int* verified, int max_misses, int* live, long long* ids, int* misses,
+                                long long* dropped, g6d_stream_t stream);
+int g6d_instances_verify_update_host(int n, const int* lost, const int* verified, int max_misses, int* live, long long* ids,
+                                     int* misses, long long* dropped);
 /* (x - mean) / std on f32 [n_pixels, in_c] -> [n_pixels, out_c] (in_c, out_c in {3,4})
  * (network/detector.py:189, selector.py:115, refiner.py:65) */
 int g6d_imagenet_norm(const float* in, float* out, long long n_pixels, int in_c, int out_c, g6d_stream_t stream);
